@@ -3,14 +3,15 @@
 
 The reference (kornia-rs) ships its GPU kernels as CUDA-C source strings inside Rust files and JIT-compiles them with
 NVRTC for `compute_XY` with `--fmad=false` (crates/kornia-tensor/src/cuda.rs:675-718).  This script reads those strings
-from /root/reference *where they lie*, compiles each NVRTC translation unit IN MEMORY exactly like the reference does
-(NVRTC, `--gpu-architecture=compute_100 --fmad=false`, nothing else) to `baseline/_ref/ptx/<unit>.ptx`, and records a
+from a kornia-rs checkout (the directory $KORNIA_RS_SRC names) *where they lie*, compiles each NVRTC translation unit
+IN MEMORY exactly like the reference does on an H100
+(NVRTC, `--gpu-architecture=compute_90 --fmad=false`, nothing else) to `baseline/_ref/ptx/<unit>.ptx`, and records a
 manifest (unit -> reference file:line, kernel names).  Only the compiled PTX is kept — the source text is never written
-into the repository tree; `baseline/_ref/` is git-ignored and travels to the GPU box with the snapshot like a built .so,
-where `baseline/ref_gpu.py` loads the PTX through the driver API and launches it with the reference's launch geometry.  Test / measurement infrastructure only: nothing here is
+into the repository tree; `baseline/_ref/` is git-ignored like a built .so.
+`baseline/ref_gpu.py` loads the PTX through the driver API and launches it with the reference's launch geometry.  Test / measurement infrastructure only: nothing here is
 linked into, imported by or shipped with the product library.
 
-Run by `__graft_entry__.build()` whenever /root/reference is present.
+Run by `__graft_entry__.build()` whenever $KORNIA_RS_SRC is set.
 """
 from __future__ import annotations
 
@@ -19,7 +20,7 @@ import os
 import re
 import sys
 
-REF = "/root/reference/crates/kornia-imgproc/src"
+REF = os.path.join(os.environ.get("KORNIA_RS_SRC", ""), "crates", "kornia-imgproc", "src")
 HERE = os.path.dirname(os.path.abspath(__file__))
 OUT = os.path.join(HERE, "_ref")
 
@@ -152,7 +153,7 @@ def nvrtc_ptx(src: str, name: str) -> bytes:
         return r[1:] if len(r) > 2 else (r[1] if len(r) == 2 else None)
 
     prog = ck(nvrtc.nvrtcCreateProgram(src.encode(), f"{name}.cu".encode(), 0, [], []))
-    opts = [b"--gpu-architecture=compute_100", b"--fmad=false"]
+    opts = [b"--gpu-architecture=compute_90", b"--fmad=false"]
     res = nvrtc.nvrtcCompileProgram(prog, len(opts), opts)
     if res[0] != nvrtc.nvrtcResult.NVRTC_SUCCESS:
         n = ck(nvrtc.nvrtcGetProgramLogSize(prog))
@@ -181,7 +182,7 @@ def main() -> int:
             f.write(ptx)
         manifest[u["unit"]] = {"source": f"crates/kornia-imgproc/src/{u['rs']}:{u['line']}", "kernels": u["kernels"]}
     with open(os.path.join(OUT, "manifest.json"), "w") as f:
-        json.dump({"nvrtc_options": ["--gpu-architecture=compute_100", "--fmad=false"], "units": manifest}, f, indent=1)
+        json.dump({"nvrtc_options": ["--gpu-architecture=compute_90", "--fmad=false"], "units": manifest}, f, indent=1)
     print(f"[ref-kernels] {len(manifest)} NVRTC units extracted from {REF} and compiled to PTX under {OUT}")
     return 0
 

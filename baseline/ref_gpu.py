@@ -1,7 +1,7 @@
-"""GPU baseline: the reference's OWN CUDA kernels, run the way the reference runs them, on the same B200.
+"""GPU baseline: the reference's OWN CUDA kernels, run the way the reference runs them, on the same GPU.
 
-`baseline/extract_ref_kernels.py` (run at build time, where /root/reference exists) extracted every NVRTC translation
-unit of the §8 path verbatim and compiled it with the reference's NVRTC options (`compute_100`, `--fmad=false`,
+`baseline/extract_ref_kernels.py` (run at build time when $KORNIA_RS_SRC names a kornia-rs checkout) extracted every NVRTC translation
+unit of the §8 path verbatim and compiled it with the reference's NVRTC options (`compute_90`, `--fmad=false`,
 crates/kornia-tensor/src/cuda.rs:675-718) into `baseline/_ref/ptx/`.  This module loads that PTX through the CUDA
 driver API — the reference's own path: NVRTC PTX -> cuModuleLoadData -> cuLaunchKernel (cudarc) — and launches each
 kernel with the reference's launch geometry:
@@ -15,7 +15,7 @@ kernel with the reference's launch geometry:
   * L1-preferred cache config, best effort (try_compile_with_l1 / prefer_l1_cache)
 
 Measurement and cross-check infrastructure only (bench.py's `vs_ref_gpu` column, tests/test_ref_gpu_kernels.py): the
-product library never sees this file.  Nothing here reads /root/reference at run time.
+product library never sees this file.  Nothing here reads the reference's sources at run time.
 """
 from __future__ import annotations
 

@@ -1,14 +1,16 @@
 #!/usr/bin/env python
 """bench.py — BASELINE.json's metric on BASELINE.json's config, one JSON line on stdout (rank 0).
 
-Workload (N=1): configs[1] — "bilinear resize 3840x2160 -> 1280x720 RGB u8 -> f32, batch=64, 1xB200": the
+Workload (N=1): configs[1] — "bilinear resize 3840x2160 -> 1280x720 RGB u8 -> f32, batch=64, 1xH100": the
 fused u8 HWC -> f32 CHW half-pixel bilinear resize + normalise (resize/fused.rs:147), one launch per step over
 the whole batch.  A "step" = one pass of that hot path over one batch of 64 synthetic frames (LCG pattern,
 seed 0x12345678+n per frame, SURVEY §8(d) cfg 2).  metric = Mpix/s of DESTINATION pixels.
 
   value     whole-job throughput, inputs resident in HBM, CUDA-event timed on the launch stream, K steps
             bracketed by barrier + synchronize, max over ranks.  Each step streams a 1.59 GB source batch (the
-            kernel addresses the 0.53 GB of rows with a non-zero weight) and writes 0.71 GB — far beyond the 126 MB L2.
+            kernel addresses the 0.53 GB of rows with a non-zero weight) and writes 0.71 GB — far beyond the 50 MB L2.
+  --dump-outputs DIR  after the timed steps, rank 0 writes what the last step computed: a fixed sample of the
+            [64,3,720,1280] f32 result (frames DUMP_FRAMES, 44 MB) as DIR/resize_normalize_chw_sample.npy.
   e2e       same metric through the public API with HOST (pinned) images and a host output tensor
             (kb200_resize_normalize_chw_u8_f32_host): per step the upload of the tapped source rows, the kernel and
             the download of the [64,3,720,1280] f32 result, chunked over a 3-stream ring so copies overlap compute.
@@ -42,6 +44,7 @@ SW, SH, DW, DH, BATCH = 3840, 2160, 1280, 720, 64
 IMAGENET_MEAN, IMAGENET_STD = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)
 METRIC, UNIT = "Mpix/s (dst pixels) fused bilinear resize 4K->720p RGB u8->f32 CHW", "Mpix/s"
 WORKLOAD = "configs[1]: fused bilinear resize+normalize 3840x2160->1280x720 RGB u8 HWC -> f32 CHW, batch=64 per GPU"
+DUMP_FRAMES = (0, 21, 42, 63)   # --dump-outputs: 4 of the 64 frames, 4 x 3 x 720 x 1280 f32 = 44 MB
 
 
 # stdout carries exactly ONE JSON line.  Native libraries write banners to fd 1 (NCCL prints its version there when
@@ -74,7 +77,7 @@ def measured_peak_gbs() -> tuple[float, str]:
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 class LcgPattern:
@@ -238,9 +241,8 @@ class CpuArm:
 
 
 def run_reference_arm(args) -> None:
-    """The reference's own CPU implementation of the path (oracle port: the Rust crate cannot be built in this
-    image), all host threads, same config/metric.  One step = a bounded sample (REF_FRAMES frames) of the batch;
-    the timed region lasts >= 2 s whatever --steps says (steps are repeated until it does)."""
+    """The reference's own CPU implementation of the path (oracle port of the Rust crate), all host threads, same
+    config/metric.  One step = a bounded sample (4 frames) of the batch; exactly --steps steps are timed."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
@@ -253,15 +255,11 @@ def run_reference_arm(args) -> None:
 
     for _ in range(max(1, min(args.warmup, 3))):
         step()
-    reps, t0 = 0, time.perf_counter()
-    while True:
-        for _ in range(args.steps):
-            step()
-        reps += 1
-        dt = time.perf_counter() - t0
-        if dt >= 2.0:
-            break
-    nsteps = reps * args.steps
+    t0 = time.perf_counter()
+    for _ in range(args.steps):
+        step()
+    dt = time.perf_counter() - t0
+    nsteps = args.steps
     val = frames * DW * DH * nsteps / 1e6 / dt
     line = {
         "impl": "reference", "metric": METRIC, "value": val, "unit": UNIT, "n_gpus": args.gpus, "steps": args.steps,
@@ -331,7 +329,9 @@ def op_table(kb, dev, peak_gbs: float, quick: bool, n_gpus: int, rank: int) -> d
     """Every hot-path op at N GPUs: each rank runs the op on ITS shard (weak scaling: cfg 3 = 256 frames per GPU,
     cfg 4 = 16 images per GPU, cfg 5 = 64 images per GPU — at N = 8 exactly BASELINE's 128 / 512-image configs), inputs
     from SURVEY §8(d)'s generators, CUDA events on the launch stream, MAX over ranks; Mpix/s is the whole job's.
-    `ref_gpu_ms` / `vs_ref_gpu`: the reference's own CUDA kernels (NVRTC compute_100, fmad=false, 32x8 / 256-thread
+    Each op is timed over a fixed 20 launches after 5 warm-ups (5 / 3 with --quick) whatever --steps says: a step is
+    the headline path, not an op of this table.
+    `ref_gpu_ms` / `vs_ref_gpu`: the reference's own CUDA kernels (NVRTC compute_90, fmad=false, 32x8 / 256-thread
     launches, one launch per image) timed on rank 0 on the SAME buffers."""
     import numpy as np
     import torch
@@ -563,7 +563,12 @@ def main() -> None:
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline sample")
     ap.add_argument("--quick", action="store_true")
     ap.add_argument("--no-e2e", action="store_true", help="tuning sweeps only: skip the host-buffer (e2e) leg; the line then has e2e = null")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write a fixed sample of the last timed step's result to DIR as .npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.impl == "reference" and args.dump_outputs:
+        ap.error("--dump-outputs dumps the GPU path's result; the reference arm has none")
     claim_stdout()
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":
@@ -622,21 +627,11 @@ def main() -> None:
     alg_bytes = BATCH * (SW * SH * 3 * 4 // 9 + DW * DH * 3 * 4)  # 22,118,400 B/frame (SURVEY §8(d) cfg 2)
     ms_launch = e0.elapsed_time(e1) / args.steps
     achieved = alg_bytes / (ms_launch * 1e-3) / 1e9
-    # dram bytes of this kernel from the committed ncu --set full capture — only if the capture was taken from the
-    # kernel source that is running now (hash recorded with it); a stale capture reports null, never a stale number
-    traffic, traffic_src = None, "no ncu capture recorded for the current kernel source"
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tpath):
-        try:
-            import hashlib
+    if args.dump_outputs and rank == 0:
+        import numpy as np
 
-            tj = json.load(open(tpath))
-            cur = hashlib.sha256(open(os.path.join(ROOT, "kornia-rs_b200", "csrc", "resize_fused.cu"), "rb").read()).hexdigest()[:16]
-            if tj.get("fused_resize_cfg2_source_sha16") == cur:
-                traffic = tj.get("fused_resize_cfg2_bytes_per_launch")
-                traffic_src = tj.get("fused_resize_cfg2_capture", "profiles/traffic.json")
-        except Exception:
-            traffic = None
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "resize_normalize_chw_sample.npy"), dst[list(DUMP_FRAMES)].cpu().numpy())
 
     e2e = None
     t_wall1 = time.time()
@@ -652,7 +647,7 @@ def main() -> None:
         def e2e_step():
             kb.imgproc.resize_normalize_to_tensor_u8_to_f32_bilinear(host_src, DW, DH, scale, bias, out=host_dst, pipeline=pipe)
 
-        e2e_steps = max(2, min(args.steps, 10))
+        e2e_steps = args.steps
         for _ in range(2):
             e2e_step()
         torch.cuda.synchronize()
@@ -683,7 +678,7 @@ def main() -> None:
         # config 3 end to end: raw NV12 camera frames in HOST memory -> normalised CHW tensor in HOST memory through
         # Preprocessor.run_raw_host (kb200_preprocess_host): f32, and the reference's f16 output (preprocess.rs:1086) which
         # halves the download — the larger half of the link traffic
-        e2e["config3"] = e2e_config3(kb, dev, st, 16 if args.quick else 64, max(2, min(args.steps, 6)), n_gpus)
+        e2e["config3"] = e2e_config3(kb, dev, st, 16 if args.quick else 64, args.steps, n_gpus)
     clocks = sampler.stop(t_wall0, t_wall1) if sampler else None
     del src, dst
 
@@ -712,11 +707,8 @@ def main() -> None:
             "e2e": e2e,
             "gpu_launches": args.steps,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak_gbs, "unit": "GB/s", "frac": achieved / peak_gbs,
-                         "traffic": traffic, "traffic_source": traffic_src,
-                         "frac_of_traffic": (traffic / (ms_launch * 1e-3) / 1e9 / peak_gbs) if traffic else None,
                          "note": "algorithmic bytes count all four taps per pixel (SURVEY 8(d)); at 3:1 three have weight exactly 0 and are "
-                                 "not fetched, so the bytes moved (traffic) are below the algorithmic bytes and frac can exceed 1; "
-                                 "frac_of_traffic = bytes actually moved / time / peak",
+                                 "not fetched, so the bytes moved are below the algorithmic bytes and frac can exceed 1",
                          "peak_source": peak_src, "kernel": "fused_rows_kernel (resize_fused.cu)",
                          "algorithmic_bytes_per_launch": alg_bytes, "ms_per_launch": ms_launch},
             "clocks": clocks,

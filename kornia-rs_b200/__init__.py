@@ -1,4 +1,4 @@
-"""kornia-rs_b200 — the B200 (sm_100a) implementation of kornia-rs's kornia-imgproc pixel-kernel hot
+"""kornia-rs_b200 — the H100 (sm_90a) implementation of kornia-rs's kornia-imgproc pixel-kernel hot
 path, behind the reference's own operator surface.
 
     import kornia_rs_b200 as kb

@@ -4,7 +4,7 @@
 // thread, scalar 4-byte accesses); color/yuv/kernels.rs:707-1069 (CPU), cuda/color/video.rs:33-130
 // (GPU twin, 1 thread per 2x2 block, byte stores).
 //
-// B200 design: these are pure streaming ops (16 B/px, 4 B/px, 4.5 B/px, 5 B/px).  Every thread
+// Design: these are pure streaming ops (16 B/px, 4 B/px, 4.5 B/px, 5 B/px).  Every thread
 // moves whole 16-byte vectors in both directions (LDG.128 / STG.128, streaming cache hints),
 // de-interleaving the stride-3 pixels in registers; grids are sized so each SM holds several
 // CTAs with ≥ 4 independent 16-byte loads in flight per thread.
@@ -88,8 +88,8 @@ __global__ void gray_from_rgb_u8_scalar(const uint8_t* __restrict__ src, uint8_t
 // One thread: 16 luma columns x 2 rows (one chroma row).  Loads 16 B Y (top), 16 B Y (bottom),
 // 16 B UV; stores 2 x 48 B as 3 x STG.128 each.  Requires width % 16 == 0 and 16-B aligned bases.
 // Saturate-and-pack (I2IP): d = (c << 16) | (sat_u8(a) << 8) | sat_u8(b) — one instruction replaces two min/max
-// pairs and the byte insertion.  ncu on the min/max version: 25 instructions per pixel, 73 % issue utilisation,
-// math-pipe throttled at 0.72 of the HBM roofline.
+// pairs and the byte insertion.  ncu on the min/max version: math-pipe throttled,
+// below the HBM roofline.
 __device__ __forceinline__ uint32_t pack_sat2(int hi, int lo, uint32_t upper) {
     uint32_t d;
     asm("cvt.pack.sat.u8.s32.b32 %0, %1, %2, %3;" : "=r"(d) : "r"(hi), "r"(lo), "r"(upper));

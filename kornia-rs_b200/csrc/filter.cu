@@ -6,7 +6,7 @@
 // cuda/filter.rs:55-110, :515-565 and filter/cuda.rs:106-232 (GPU twin: 2 launches through a DRAM
 // scratch image for a blur, 5 launches / 11 image traversals for sobel).
 //
-// B200 design: ONE kernel per op.  A CTA stages a (TH + ky-1) x (TW + kx-1) pixel tile (zero-filled
+// Design: ONE kernel per op.  A CTA stages a (TH + ky-1) x (TW + kx-1) pixel tile (zero-filled
 // outside the image) in shared memory, runs the H pass into a second shared tile and the V pass
 // straight to global memory — the f32 intermediate never touches HBM (traffic: 1 read + 1 write of
 // the image instead of 2+2; sobel: 1+1 instead of 11).  Sobel runs both gradient filters off the
@@ -136,8 +136,8 @@ __global__ void __launch_bounds__(256) sep_filter_fused_kernel(const float* __re
 // ─────────────────────────────────────────────────────────────────────────────────────────────
 // Row-streaming kernel (the config-4 fast path): C ∈ {1,3,4}, taps ∈ {3,5,7}, (cols*C) % 4 == 0.
 //
-// ncu on the tile kernel above: ~90 instructions per element (K LDS + 2K FP per pass per element, 64-bit
-// index math in the tap loops), issue-bound at 28 % (blur) / 14 % (sobel) of the HBM roofline.  Here:
+// ncu on the tile kernel above: K LDS + 2K FP per pass per element plus 64-bit index math in the tap loops —
+// issue-bound, far below the HBM roofline.  Here:
 //   * work unit = (image, strip of 512*NV floats of a row, chunk of `rows_per_chunk` rows); a CTA walks its
 //     strip top-down.  Each input row segment (strip + 16-B-rounded halo) is copied global -> shared by
 //     the TMA engine (cp.async.bulk 1-D) into an mbarrier ring by a producer warp — every input row is
@@ -216,21 +216,19 @@ struct SobelAcc {
 };
 
 // ─────────────────────────────────────────────────────────────────────────────────────────────
-// Packed (f32x2) vertical pass.
+// Paired vertical pass.
 //
-// ncu history (profiles/r1_filters.md): the first streaming kernel (one float4 per thread, scalar mul+add in both
-// passes, bounds selects in every row) ran 47 warp-instructions per output value at 79 % issue utilisation — 35 %
-// unfused FMUL/FADD, ~25 % mbarrier spin — i.e. issue-bound at 0.75 (blur) / 0.69 (sobel) of the HBM roofline.
-//   * the vertical pass runs on register PAIRS with FFMA2 (sm_100 packed fp32: same lane rate as FFMA — measured
-//     126 vs 118 element-updates/clk/SM, tools/scratch/ffma2_probe.cu — at half the issue slots).  The reference's
-//     unfused `acc += v * k` is kept bit-for-bit: ptxas contracts mul.f32x2 + add.f32x2 into one FFMA2 even under
-//     --fmad=false, so the product is formed as fma2(v, k, -0) and the sum as fma2(p, 1, acc) with -0 and 1 passed
-//     as kernel arguments (opaque to the optimiser): two FFMA2 per tap-pair, each rounding once, = mul then add;
+// ncu history: the first streaming kernel (one float4 per thread, scalar mul+add in both passes, bounds selects in
+// every row) was issue-bound — unfused FMUL/FADD and mbarrier spin took most of the issue slots.
+//   * the vertical pass runs on register PAIRS (fma2_rn, kb200_common.cuh: one scalar FFMA per lane on sm_90).  The
+//     reference's unfused `acc += v * k` is kept bit-for-bit: the product is formed as fma2(v, k, -0) and the sum as
+//     fma2(p, 1, acc) with -0 and 1 passed as kernel arguments (opaque to the optimiser), each rounding once, = mul
+//     then add;
 //   * the first tap of every accumulation is a single fma(v, k, +0) (== round(v*k) + 0, signed zeros included);
 //   * the horizontal pass stays scalar: with C = 3 the tap pairs of neighbouring outputs alternate between even
 //     and odd register offsets, and an unaligned pair costs more moves than the packed op saves;
 //   * NV = 1 is what ships: two columns per thread (NV = 2) halve the per-row bookkeeping but need 77-93 registers,
-//     which caps the SM at 4 CTAs / 20 warps and measured 6 % slower than NV = 1 at 6-7 CTAs (56 registers).
+//     which caps the SM at 4 CTAs / 20 warps.
 template <int NV> struct SS2 {
     static constexpr int COLS4 = 128;               // consumer threads
     static constexpr int EW = COLS4 * 4 * NV;       // floats per strip
@@ -241,7 +239,7 @@ template <int NV> struct SS2 {
 typedef unsigned long long ss_u64;
 __device__ __forceinline__ ss_u64 ss_pack(float a, float b) { ss_u64 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
 __device__ __forceinline__ void ss_unpack(ss_u64 v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ ss_u64 ss_fma2(ss_u64 a, ss_u64 b, ss_u64 c) { ss_u64 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
+__device__ __forceinline__ ss_u64 ss_fma2(ss_u64 a, ss_u64 b, ss_u64 c) { return fma2_rn(a, b, c); }
 
 // exact two-rounding helpers on pairs (see header): NZ = (-0,-0), ONE = (1,1), both opaque run-time values
 struct PairConst { ss_u64 nz, one, zero; };
@@ -408,7 +406,7 @@ __global__ void __launch_bounds__(SS2<NV>::THREADS) sep_filter_stream2_kernel(co
                                 const ss_u64 m = pair_add(pair_mul(gx, gx, pc), pair_mul(gy, gy, pc), pc);   // gx*gx + gy*gy, unfused
                                 float m0, m1;
                                 ss_unpack(m, m0, m1);
-                                pair_sqrt_rn(m0, m1, &o[2 * h], &o[2 * h + 1]);     // == sqrtf on both, 12 instructions per pair (pair_math.cuh)
+                                pair_sqrt_rn(m0, m1, &o[2 * h], &o[2 * h + 1]);     // == sqrtf on both (pair_math.cuh)
                             } else {
                                 ss_u64 acc = ss_fma2(winA[(s + 1) % KY][v][h], kyp[0], pc.zero);   // == 0 + w*k
 #pragma unroll
@@ -449,9 +447,10 @@ static int launch_sep_stream2(cudaStream_t s, const float* src, float* dst, cons
     P.rowlen = cols * C; P.rows = rows; P.batch = batch;
     P.strips = (P.rowlen + G::EW - 1) / G::EW;
     P.slot_floats = G::EW + HL + HR;
-    // B200 sweep (profiles/r1_filters.md): blur is best at 6 CTAs x 4 stages, sobel (fewer bytes per instruction) at 7 x 3
-    const uint32_t stages = (tune_stages >= 2 && tune_stages <= G::MAX_STAGES) ? (uint32_t)tune_stages : (SOBEL ? 3u : 4u);
-    const int per_sm = tune_ctas > 0 ? tune_ctas : (SOBEL ? 7 : 6);
+    // H100 sweep (16 x 4K f32, CTAs 3..10 x stages 2..6): blur is best at 6 CTAs x 4 stages, sobel at 4 x 4 (its
+    // neighbours within 1 %; the 7 x 3 of the previous target is slower here).  Knobs ss.ctas / ss.stages re-sweep them.
+    const uint32_t stages = (tune_stages >= 2 && tune_stages <= G::MAX_STAGES) ? (uint32_t)tune_stages : 4u;
+    const int per_sm = tune_ctas > 0 ? tune_ctas : (SOBEL ? 4 : 6);
     const size_t smem = (size_t)P.slot_floats * 4 * stages;
     auto kern = sep_filter_stream2_kernel<C, KX, KY, SOBEL, NV>;
     if (smem > 40 * 1024) {
@@ -466,7 +465,7 @@ static int launch_sep_stream2(cudaStream_t s, const float* src, float* dst, cons
     }
     const size_t ctas = (size_t)device_info().sm_count * std::min(per_sm, resident);
     // chunk height: ~12 units per CTA keeps the persistent grid balanced (a search that traded balance against the
-    // KY-1 halo rows per chunk measured 8-13 % slower on B200: long chunks leave the ragged last strip's CTAs idle);
+    // KY-1 halo rows per chunk measured slower: long chunks leave the ragged last strip's CTAs idle);
     // at least 32 rows so the halo re-reads stay near 10 %
     const int tune_rc = knob(KNOB_SS_RC);
     const size_t total = (size_t)P.strips * batch * rows;

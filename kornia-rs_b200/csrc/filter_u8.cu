@@ -112,7 +112,7 @@ __global__ void __launch_bounds__(256) blur_u8_tile_kernel(const uint8_t* __rest
 
 // ── word-granular variant ────────────────────────────────────────────────────────────────────
 // ncu-free arithmetic on the kernel above: ~15 LSU operations per output byte (byte gathers, one LDS.U8 per tap per
-// byte, byte stores) against 1.5 B of DRAM traffic per byte — LSU-bound at 0.12 of the roofline.  Here every access is
+// byte, byte stores) against 1.5 B of DRAM traffic per byte — LSU-bound, far below the roofline.  Here every access is
 // a 32-bit word and four bytes are filtered at once in two 16-bit lanes per register:
 //   e = w & 0x00FF00FF, o = (w >> 8) & 0x00FF00FF;  acc_e += e * k, acc_o += o * k
 // A lane never overflows: Σ byte·k <= 255 · Σk = 255 · 256 < 2^16 (the host checks Σk <= 256), and the Q8 rounding
@@ -230,7 +230,7 @@ __global__ void __launch_bounds__(256) blur_u8_tile_w_kernel(const uint8_t* __re
 
 // ── row-streaming variant (round 2) ───────────────────────────────────────────────────────────
 // The tile kernel above pays two block-wide phase changes, a (64+K-1)^2 / 64^2 halo and a shared-memory round trip of the
-// intermediate per tile: 0.23 of the roofline.  This is the u8 twin of sep_filter_stream2 (filter.cu): a unit is
+// intermediate per tile.  This is the u8 twin of sep_filter_stream2 (filter.cu): a unit is
 // (image, strip of 128*NV words of a row, chunk of rows); every source row span is copied ONCE global -> shared by the
 // TMA engine (cp.async.bulk, mbarrier ring, producer lane; rows clamped = the reference's replicate border in y); a
 // consumer thread owns NV word columns: the H pass reads the words around its column (compile-time funnel shifts per tap,
@@ -329,7 +329,7 @@ __global__ void __launch_bounds__(U8S_THREADS) blur_u8_stream_kernel(const uint8
         const bool rpatch = last_word < U8S_CT * NV && ((last_word % U8S_CT) >> 5) == (int)(tid >> 5);   // ... its last word (warp-uniform)
         // K-deep register window of H-pass results, oldest first.  The row loop is NOT unrolled: rotating the window costs
         // (K-1)*NV register moves per row, whereas K unrolled copies of the row step made the kernel ~40 KB of code that
-        // missed the instruction cache on every lap (ncu: no-instruction stalls, icache requests 45-79 % of peak).
+        // missed the instruction cache on every lap (ncu: no-instruction stalls).
         // Q8 path: the window keeps each H result SPLIT into its even and odd bytes (two 16-bit lanes per register: exactly the
         // operand form of the V pass), so the V pass is ten IMADs and one PRMT per word — no byte extraction (the kernel is bound
         // by the ALU pipe: LOP / PRMT / SHF).  The binomial path (K = 3) keeps packed bytes in win alone.
@@ -441,8 +441,8 @@ static int launch_blur_u8_stream(cudaStream_t s, const uint8_t* src, uint8_t* ds
     const int per_sm = std::min(resident, knob(KNOB_C) > 0 ? knob(KNOB_C) : 8);
     const size_t ctas = (size_t)device_info().sm_count * per_sm;
     const size_t total = (size_t)P.strips * batch * rows;
-    // rows per chunk: every chunk re-reads K-1 halo rows, so long chunks when there is enough work for ~4 units per CTA (16 x 4K:
-    // 32 rows 0.384 ms, 128 rows 0.368 ms), short ones otherwise
+    // rows per chunk: every chunk re-reads K-1 halo rows, so long chunks when there is enough work for ~4 units per CTA,
+    // short ones otherwise
     uint32_t rc = knob(KNOB_D) > 0 ? (uint32_t)knob(KNOB_D) : (uint32_t)std::min<size_t>(128, std::max<size_t>(32, total / (ctas * 4)));
     rc = std::min(rc, rows);
     P.rows_per_chunk = rc;

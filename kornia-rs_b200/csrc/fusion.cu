@@ -6,7 +6,7 @@
 //   Normalize (:592-620)          v * scale[c] + bias[c]
 //   RgbToGray (:624-642)          0.299 x + 0.587 y + 0.114 z, replicated to the three lanes
 //   WriteChwF32 / WriteC1F32 (:645-690)  three planes / the .x lane
-// There is no runtime compiler in this library (everything is AOT sm_100a code), so the composable shapes are compiled
+// There is no runtime compiler in this library (everything is AOT sm_90a code), so the composable shapes are compiled
 // ahead of time as template instantiations of one kernel: map chains {}, {N}, {G}, {N,G}, {G,N} x sinks {CHW, C1} — every
 // chain the vocabulary can express without repeating a stage.  Same contract as the engine: f32 register flow between
 // stages (NOT bit-equal to running the ops through u8 buffers, fusion.rs:21-27), parameters in the constant bank, batch

@@ -2,7 +2,7 @@
 //
 // The reference's fused resize (`resize_normalize_to_tensor_u8_to_f32_bilinear`, resize/fused.rs:147) takes host
 // images and writes a host tensor.  A drop-in for that call therefore has to move the frames over PCIe, and at 4K the
-// link — not the kernel — sets the rate (a 64-frame 4K batch is 1.59 GB in, 0.71 GB out; the kernel needs 0.24 ms).
+// link — not the kernel — sets the rate (a 64-frame 4K batch is 1.59 GB in, 0.71 GB out; the kernel needs < 1 ms).
 // Two things keep the link busy and lightly loaded:
 //
 //   * a ring of `depth` streams, each owning a device source and destination staging buffer: chunk i's upload, kernel

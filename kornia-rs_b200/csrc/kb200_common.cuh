@@ -1,6 +1,6 @@
-// kb200_common.cuh — shared host/device helpers of libkornia_b200.so (sm_100a only).
+// kb200_common.cuh — shared host/device helpers of libkornia_b200.so (sm_90a only).
 //
-// Compile contract (see __graft_entry__.build): -gencode arch=compute_100a,code=sm_100a
+// Compile contract (see __graft_entry__.build): -gencode arch=compute_90a,code=sm_90a
 // -fmad=false.  The reference JIT-compiles every kernel with fmad=false
 // (crates/kornia-tensor/src/cuda.rs:675-718) so that `a*b + c` in kernel source rounds twice,
 // exactly like the Rust CPU code; we keep that rule for the whole library and write fmaf()
@@ -108,6 +108,20 @@ __device__ __forceinline__ void stg_stream_u4(uint4* p, uint4 v) {
 }
 __device__ __forceinline__ void stg_stream_f1(float* p, float v) {
     asm volatile("st.global.L1::no_allocate.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
+}
+
+// Lane-wise fma.rn on two floats held as one 64-bit pair {lo, hi}.  sm_90 has no packed FP32 instruction, so each lane
+// is one scalar FFMA; every lane rounds once, exactly like fmaf.  The pair form keeps the callers' register layout.
+__device__ __forceinline__ unsigned long long fma2_rn(unsigned long long a, unsigned long long b, unsigned long long c) {
+    float a0, a1, b0, b1, c0, c1, r0, r1;
+    asm("mov.b64 {%0, %1}, %2;" : "=f"(a0), "=f"(a1) : "l"(a));
+    asm("mov.b64 {%0, %1}, %2;" : "=f"(b0), "=f"(b1) : "l"(b));
+    asm("mov.b64 {%0, %1}, %2;" : "=f"(c0), "=f"(c1) : "l"(c));
+    asm("fma.rn.f32 %0, %1, %2, %3;" : "=f"(r0) : "f"(a0), "f"(b0), "f"(c0));
+    asm("fma.rn.f32 %0, %1, %2, %3;" : "=f"(r1) : "f"(a1), "f"(b1), "f"(c1));
+    unsigned long long r;
+    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(r0), "f"(r1));
+    return r;
 }
 
 // byte `i` (0..3) of a 32-bit word -> exact float, through the 2^23 mantissa trick:

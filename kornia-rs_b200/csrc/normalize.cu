@@ -4,7 +4,7 @@
 // Reference: normalize.rs:56-87, :123-146, :191-222, :235-263 (+ scalar leaf :407-421, AVX2 leaf with
 // fmadd on the npixels&~7 bulk), core.rs:42-67.
 //
-// B200 design: streaming kernels over flat arrays with lane-contiguous 16-byte vector accesses in both
+// Design: streaming kernels over flat arrays with lane-contiguous 16-byte vector accesses in both
 // directions (the channel phase of a vector is (index % 3), loop-invariant per thread); reductions use
 // per-thread integer accumulators, warp shuffles and one atomic per CTA, so `std_mean`'s sums are
 // exact integers independent of the order of accumulation (= the reference's f64 folds, which are
@@ -36,8 +36,8 @@ __global__ void __launch_bounds__(256) normalize_mean_std_c3_vec(const float4* _
         v.x = __fdiv_rn(v.x - ma, sa); v.y = __fdiv_rn(v.y - mb, sb); v.z = __fdiv_rn(v.z - mc, sc); v.w = __fdiv_rn(v.w - ma, sa);
         return v;
     };
-    // four independent 16-B loads in flight per thread: ncu on the one-load loop showed 96 % occupancy, 34 % issue and
-    // a long-scoreboard stall of 40 cycles per instruction — 32 KB in flight per SM is short of bandwidth x latency
+    // four independent 16-B loads in flight per thread: ncu on the one-load loop showed full occupancy, low issue and
+    // long-scoreboard stalls — one 16-B load per thread in flight per SM is short of bandwidth x latency
     for (; q + 3 * stride < nvec; q += 4 * stride) {
         const float4 a = ldg_stream_f4(src + q), b = ldg_stream_f4(src + q + stride), c = ldg_stream_f4(src + q + 2 * stride),
                      d = ldg_stream_f4(src + q + 3 * stride);

@@ -184,8 +184,7 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
 // ── NV12 identity fast path (config 3a: 1080p NV12 → [N,3,1080,1920], scale 1, no pad) ─────────────────────
 // When scale_x == scale_y == 1 and pad == 0, sx = (float)ox / 1.0f = ox exactly, so ax = ay = 0 and the
 // bilinear (and the nearest) sample is the decoded tap (ox, oy) itself — bit-for-bit (see the header note).
-// The generic kernel spends ~150 instructions per pixel here and reaches 21 % of the HBM roofline (ncu: issue-
-// bound).  This kernel is a pure streaming decode:
+// The generic kernel is issue-bound here, far below the HBM roofline (ncu).  This kernel is a pure streaming decode:
 //   * one thread = 8 luma columns x 2 rows (one chroma row): 3 x LDG.64 in, 12 x STG.128 out (f32) — a warp
 //     reads 256 contiguous bytes per plane row and writes 1 KB contiguous per output plane row;
 //   * the chroma terms (CUB*u+half, CUG*u+CVG*v+half, CVR*v+half) are computed once per 2x2 block;
@@ -215,7 +214,7 @@ __device__ __forceinline__ float norm_int_px(int r, float m, float is) { return 
 // One thread = 4 luma columns x 2 rows.  Every warp-level access is lane-contiguous: 3 x LDG.32 (128 B per
 // warp), 6 x STG.128 (512 contiguous bytes per warp per plane row).  [The first version gave each thread 8
 // columns = two STG.128 per plane row; each store instruction then wrote only half of every 32-B sector and
-// ncu showed 2x the write sectors at L2 (lts__t_sectors_srcunit_tex_op_write) with l1tex at 86 %.]
+// ncu showed 2x the write sectors at L2 (lts__t_sectors_srcunit_tex_op_write).]
 template <bool F16, bool PTRS>
 __global__ void __launch_bounds__(128) preprocess_nv12_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                        const __grid_constant__ PreFrames fr, void* __restrict__ dst,
@@ -257,8 +256,8 @@ __global__ void __launch_bounds__(128) preprocess_nv12_identity_kernel(const __g
 }
 
 // ── NV12 general path (config 3b: 1080p NV12 → letterboxed 640x640, and every other NV12 geometry) ──────────
-// ncu on the generic kernel for config 3b: 89 % issue-slot utilisation, ~250 instructions per output pixel (format
-// switch, integer div/mod for (ox, oy), byte-granular everything), DRAM at 20 %.  This kernel is NV12-only:
+// ncu on the generic kernel for config 3b: issue-bound (format switch, integer div/mod for (ox, oy), byte-granular
+// everything), DRAM mostly idle.  This kernel is NV12-only:
 //   * one thread = 4 consecutive destination pixels of one row; the row comes from blockIdx.y (no div/mod);
 //     pad rows and pad pixels store a host-precomputed normalised pad value; 3 lane-contiguous STG.128 per thread;
 //   * taps are fetched only when their weight is non-zero (exact, see the header) — at integer scale ratios

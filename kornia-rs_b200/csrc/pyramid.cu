@@ -7,7 +7,7 @@
 // intermediate value is rounded to its storage type (f32 / u16 / u8) before the second pass, so computing it on the fly
 // gives the same bits and the kernels below are single-pass: no scratch, one launch per level for the whole batch.
 //
-// B200 notes: these are small stencil kernels (each level is 1/4 of the previous one); a thread produces one destination
+// Notes: these are small stencil kernels (each level is 1/4 of the previous one); a thread produces one destination
 // pixel (pyrdown) or the 2x2 destination block of one source pixel (pyrup) for all channels; neighbouring threads share
 // their taps through L1.  Batch = grid.z.
 #include "kb200_common.cuh"

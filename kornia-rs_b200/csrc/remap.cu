@@ -148,7 +148,7 @@ KB200_API int kb200_remap_f32_c3(kb200_stream_t stream, const float* src, size_t
     cudaStream_t s = as_stream(stream);
     if (interp == KB200_INTERP_BILINEAR) {
         // round 2: the lean bilinear gather of the warps, coordinates from the maps (warp.cu) — four rows per thread, interior
-        // fast path, TMA tile stores: 0.90 -> see profiles/ for the measured time per 16 x 4K
+        // fast path, TMA tile stores
         int st = KB200_OK;
         if (launch_remap_lean(s, src, dst, map_x, map_y, sw, sh, dw, dh, batch, &st)) return st;
     }
@@ -171,7 +171,7 @@ KB200_API int kb200_remap_u8(kb200_stream_t stream, const uint8_t* src, size_t s
     dim3 grid(img_fast ? batch : nblk, img_fast ? nblk : batch);
     cudaStream_t s = as_stream(stream);
     const bool bil = interp == KB200_INTERP_BILINEAR;
-    // word taps measured neutral-to-slower for remap (0.751 -> 0.773 ms, 16 x 4K): off unless knob b = 2
+    // word taps measured neutral-to-slower for remap: off unless knob b = 2
     const bool aligned = C == 3 && knob(KNOB_B) != 1 && (reinterpret_cast<uintptr_t>(src) & 3u) == 0 && (batch == 1 || ((size_t)sw * sh * 3) % 4 == 0);
     const bool words = aligned && knob(KNOB_B) == 2;
 #define KB200_REMAP_U8(CC)                                                                                         \

@@ -12,7 +12,7 @@
 //   Lanczos resize separable: per-axis tables (tap base + six normalised weights per destination index, lanczos.rs:59-92),
 //                  H pass into an f32 intermediate of dst_w x src_h, then V pass, both fmaf chains (lanczos.rs:187-236).
 //
-// B200 notes.  These are the reference's "quality" samplers: 16 / 36 taps per pixel, compute-heavier and rarely on a
+// Notes.  These are the reference's "quality" samplers: 16 / 36 taps per pixel, compute-heavier and rarely on a
 // camera pipeline's critical path.  Thread per destination pixel with batch = grid.z; the tables of the separable
 // Lanczos resize are built ON THE DEVICE by a small table kernel with the host code's own expression trees (same IEEE
 // operations -> same bits as the reference's host-built tables), into the caller's scratch buffer — nothing is

@@ -124,8 +124,8 @@ __device__ __forceinline__ void bilinear_tap_q14(uint32_t i, double scale, uint3
 // ── u8 kernels of resize_fast_u8_aa (resize/mod.rs:283-410) ──────────────────────────────────
 // Thread per destination pixel (pyrup: per 2x2 destination block) with byte loads: a warp's pixels read one
 // contiguous byte run per source row and L1 turns the byte loads into whole sectors.  A variant that gave each thread
-// four consecutive destination BYTES (one STG.32) and re-evaluated the per-pixel setup per byte measured 1.5-1.8x
-// slower on B200: these kernels are bound by instructions per pixel, not by the byte stores.
+// four consecutive destination BYTES (one STG.32) and re-evaluated the per-pixel setup per byte measured
+// slower: these kernels are bound by instructions per pixel, not by the byte stores.
 
 // resize/kernels.rs:64-75: dst = (a + b + c + d + 2) >> 2 per channel
 __global__ void __launch_bounds__(256) pyrdown_2x_rgb_u8_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst,
@@ -142,8 +142,7 @@ __global__ void __launch_bounds__(256) pyrdown_2x_rgb_u8_kernel(const uint8_t* _
 }
 
 // Word-granular pyrdown: a thread produces 4 destination pixels (12 bytes = 3 words) from 2 x 24 source bytes read as
-// 6 + 6 aligned words — 15 memory instructions per 4 pixels instead of 60 (the byte version is LSU-bound at 0.48 of the
-// roofline).  Needs sw % 8 == 0 (row = whole 24-byte groups, 4-byte aligned) and 4-byte aligned bases.
+// 6 + 6 aligned words — 15 memory instructions per 4 pixels instead of 60 (the byte version is LSU-bound).  Needs sw % 8 == 0 (row = whole 24-byte groups, 4-byte aligned) and 4-byte aligned bases.
 __global__ void __launch_bounds__(256) pyrdown_2x_rgb_u8_w4_kernel(const uint32_t* __restrict__ src, uint32_t* __restrict__ dst, uint32_t sw,
                                                                    uint32_t sh, uint32_t dw, uint32_t dh) {
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;   // group of 4 destination pixels

@@ -186,12 +186,10 @@ KB200_API void kb200_resize_row_plan(uint32_t src_h, uint32_t dst_h, uint32_t* p
 // ─────────────────────────────────────────────────────────────────────────────────────────────
 // Row-span staged kernel (the config-2 fast path).
 //
-// ncu history (profiles/r1_cfg2_fused_resize.md): the gather kernel above executes 170 warp-instructions per output
-// pixel at 79 % issue-slot utilisation with DRAM at 60 % — instruction-bound.  A first staged kernel (TMA row spans,
-// one destination column per thread) reached 100 instructions/pixel and 0.71-0.90 of the roofline but was still
-// issue-bound: ~45 of those instructions were per-ROW bookkeeping repeated for a single pixel.  The kernel below keeps
-// the staging scheme and spreads that bookkeeping over several pixels per thread (35 instructions/pixel in point
-// mode; issue utilisation 35 %; DRAM-bound at ~90 % of the measured copy bandwidth):
+// ncu history: the gather kernel above is instruction-bound.  A first staged kernel (TMA row spans, one destination
+// column per thread) cut the instructions per pixel but was still issue-bound: ~45 of those instructions were per-ROW bookkeeping repeated for a single pixel.  The kernel below keeps
+// the staging scheme and spreads that bookkeeping over several pixels per thread (point mode is
+// DRAM-bound):
 //
 //   * work unit = (image, column tile of TW destination columns, chunk of RC destination rows); CTAs are
 //     persistent and walk their units with carry arithmetic (no integer division in the loop).
@@ -510,10 +508,9 @@ int launch_fused_resize_rows(cudaStream_t s, const uint8_t* src, float* dst, con
     const bool xz = yz && axis_weights_all_zero(p.dw, p.sw, p.scale_x);
     const bool box2x = (p.sw == 2 * p.dw && p.sh == 2 * p.dh);
     const int mode = box2x ? FR_BOX : (xz ? FR_POINT : (yz ? FR_YZERO : FR_GENERAL));
-    // columns per thread: least padding in the last tile; among near-equals prefer 2, then 3, 1, 4, 5 — the B200 sweep
-    // (profiles/r1_cfg2_fused_resize.md) has 2 columns/thread ahead: enough amortisation, many producers.  The general
-    // mode (two source rows and a full lerp per pixel) is heavier per pixel: it accepts up to 10 % tile padding to keep
-    // >= 2 columns per thread (round-2 sweep, 4K -> 1600x900: npx 1 0.130 ms, npx 2 0.104 ms at 4 CTAs x 4 stages).
+    // columns per thread: least padding in the last tile; among near-equals prefer 2, then 3, 1, 4, 5 — 2 columns/thread
+    // give enough amortisation and many producers.  The general mode (two source rows and a full lerp per pixel) is
+    // heavier per pixel: it accepts up to 10 % tile padding to keep >= 2 columns per thread.
     int npx = 1;
     {
         static const int order[5] = {2, 3, 1, 4, 5};
@@ -533,9 +530,10 @@ int launch_fused_resize_rows(cudaStream_t s, const uint8_t* src, float* dst, con
     slot = (slot + 127u) & ~127u;
     slot = std::min(slot, (row_bytes + 16u + 127u) & ~127u);  // +16: the 3-word tap read may run 8 B past the span
     const uint32_t stage_bytes = slot * ((mode == FR_GENERAL || mode == FR_BOX) ? 2u : 1u);
-    // Ring sizing: the sweep's optimum keeps ~36 KB of source rows in flight per SM (about bandwidth x latency for the
-    // whole GPU); deeper rings or more CTAs than that cost 5-8 % (queueing in the memory system), fewer starve.
-    uint32_t stages = tune_stages >= 2 && tune_stages <= FR_MAX_STAGES ? (uint32_t)tune_stages : (mode == FR_GENERAL ? 4u : 3u);
+    // Ring sizing: ~36 KB of source rows in flight per SM (about bandwidth x latency for the whole GPU); the general mode
+    // runs 4 CTAs x 3 stages.  H100 sweep (npx 1..3 x stages 3/4/6 x CTAs 2..8): the point / box / general defaults are
+    // within 3 % of the best configuration (general: 4 stages was 5 % slower than 3).  Knobs fr.* re-sweep them.
+    uint32_t stages = tune_stages >= 2 && tune_stages <= FR_MAX_STAGES ? (uint32_t)tune_stages : 3u;
     int per_sm = tune_ctas > 0 ? tune_ctas : (mode == FR_GENERAL ? 4 : (int)std::lround(36.0 * 1024.0 / ((double)stages * stage_bytes)));
     per_sm = std::max(2, std::min(per_sm, 8));
     while (per_sm > 2 && (size_t)per_sm * ((size_t)stages * stage_bytes + 1024) > 200 * 1024) --per_sm;

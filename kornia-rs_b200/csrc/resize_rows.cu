@@ -1,4 +1,4 @@
-// resize_rows.cu — f32 HWC C=3 bilinear resize (a1), row-streaming design for B200.
+// resize_rows.cu — f32 HWC C=3 bilinear resize (a1), row-streaming design.
 //
 // Reference: resize/mod.rs:114-207 (CPU `resize`), interpolation/bilinear.rs:16-66, GPU twin cuda/resize.rs:97-235.
 // The reference's GPU kernel is one thread per destination pixel with 12 scalar `__ldg` taps at a 12-byte lane stride
@@ -261,8 +261,8 @@ int launch_resize_rows_f32(int mode, cudaStream_t s, const float* src, float* ds
     P.stages = stages;
     int resident = npx == 1 ? rr_occupancy<1>(mode, smem) : (npx == 2 ? rr_occupancy<2>(mode, smem) : rr_occupancy<3>(mode, smem));
     if (resident < 1) return KB200_OK;
-    // ~48-64 KB of row copies in flight per SM is enough to cover the HBM latency (resize_fused.cu sweep: ~36 KB for byte
-    // rows); more CTAs than that only queue in the memory system
+    // ~64 KB of row copies in flight per SM covers the HBM latency; more CTAs than that only queue in the memory system
+    // (knobs rs.npx / rs.stages / rs.ctas re-sweep the choice)
     int per_sm = (int)std::lround(64.0 * 1024.0 / (double)(stage_bytes * stages));
     per_sm = std::max(2, std::min(per_sm, 8));
     if (knob(KNOB_RS_CTAS) > 0) per_sm = knob(KNOB_RS_CTAS);

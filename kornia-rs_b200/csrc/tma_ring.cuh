@@ -1,4 +1,4 @@
-// tma_ring.cuh — mbarrier + 1-D bulk-copy (TMA) helpers shared by the row-streaming kernels (sm_100a).
+// tma_ring.cuh — mbarrier + 1-D bulk-copy (TMA) helpers shared by the row-streaming kernels (sm_90a).
 //
 // Pattern (resize_rows.cu, warp_stream.cu; the same scheme as fused_rows in resize_fused.cu): a producer lane issues
 // `cp.async.bulk` global -> shared copies (SASS UBLKCP) of row spans into a ring of stages, completion is counted on the

@@ -1,7 +1,7 @@
 // u8_sampler.cuh — the Q10 bilinear blend of the u8 warps / remap (warp/common.rs:14-181) with WORD-granular taps.
 //
 // The byte version issues 12 `LDG.U8` per RGB pixel (4 taps x 3 channels); ncu on the round-1 kernels showed them bound
-// by LSU instructions, far from DRAM (0.12-0.17 of the roofline).  The two taps of a row are six consecutive bytes, so
+// by LSU instructions, far from DRAM.  The two taps of a row are six consecutive bytes, so
 // three aligned 32-bit words per row cover them: 6 `LDG.32` + two funnel shifts per row instead of 12 byte loads.  The
 // arithmetic is unchanged — `(top*fy1 + bot*fy + 2^19) >> 20` with `top = p0*fx1 + p1*fx` — and bit-exact.
 #pragma once
@@ -40,7 +40,7 @@ __device__ __forceinline__ bool q10_blend_c3_words(const uint8_t* __restrict__ i
     return true;
 }
 
-// Interior form (round 2, second pass).  ncu on the u8 warps: 188 instructions per pixel at 89 % issue utilisation — the
+// Interior form (round 2, second pass).  ncu on the u8 warps: issue-bound — the
 // clamps, the +1-tap selects, the window test and the two-stage blend run for every pixel although only the image border
 // needs them.  For a pixel whose taps (xi, yi) .. (xi+1, yi+1) are all inside and yi + 2 < sh (so both 12-byte windows stay
 // inside the image: the callers' fast predicate), the sampler is: 6 LDG.32, 4 funnel shifts (the shifter uses the low five

@@ -1,8 +1,7 @@
 // warp_stream.cu — row-streaming warp_affine / warp_perspective (f32 HWC C=3) for gentle maps (config 5).
 //
 // Reference: cuda/warp_perspective.rs:51-167, cuda/warp_affine.rs:74-230 (one thread per destination pixel, 12 scattered
-// `__ldg` taps).  ncu on our own gather kernels (profiles/r1_summary.md) showed that design bound by memory LATENCY at
-// ~0.7 of the roofline: a thread brings in 12 new bytes per pixel, so ~25 KB of unique bytes are in flight per SM.  Here
+// `__ldg` taps).  ncu on our own gather kernels showed that design bound by memory LATENCY: a thread brings in 12 new bytes per pixel, so ~25 KB of unique bytes are in flight per SM.  Here
 // the source is streamed instead of gathered:
 //
 //   * work unit = (image, tile of TW = 128*NPX destination columns, chunk of destination rows); persistent CTAs.

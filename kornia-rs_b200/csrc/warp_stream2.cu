@@ -6,9 +6,8 @@
 // leaner.  Here:
 //   * a thread owns ONE destination column and processes TWO destination rows per step (the schedule is computed per
 //     row pair, ws_pair_need), so mbarrier traffic, the named barrier and the row copy-out are paid once per two pixels;
-//   * the two pixels are computed as a PAIR on FFMA2 (`fma.rn.f32x2`): every `a*b` is fma2(a, b, -0) and every `a+b` is
-//     fma2(a, 1, b) with -0 / 1 opaque kernel arguments — the reference's unfused, twice-rounded arithmetic at half the
-//     issue slots (ptxas would contract a packed mul+add even under --fmad=false; see DESIGN.md lesson 6);
+//   * the two pixels are computed as a PAIR (fma2_rn, kb200_common.cuh): every `a*b` is fma2(a, b, -0) and every `a+b`
+//     is fma2(a, 1, b) with -0 / 1 opaque kernel arguments — the reference's unfused, twice-rounded arithmetic;
 //   * an interior pixel whose 2x2 footprint is resident takes its 12 taps as `LDS.32` at immediate offsets from TWO
 //     32-bit shared-memory addresses (row y0 and row y0+1 of the ring) — no 64-bit address arithmetic, no per-tap select;
 //   * everything else (image border pixels where a +1 neighbour is missing, a tap outside the resident band or span)
@@ -24,7 +23,7 @@ namespace kb200 {
 typedef unsigned long long ws_u64;
 __device__ __forceinline__ ws_u64 ws_pack(float a, float b) { ws_u64 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
 __device__ __forceinline__ void ws_unpack(ws_u64 v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ ws_u64 ws_fma2(ws_u64 a, ws_u64 b, ws_u64 c) { ws_u64 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
+__device__ __forceinline__ ws_u64 ws_fma2(ws_u64 a, ws_u64 b, ws_u64 c) { return fma2_rn(a, b, c); }
 struct WsConst { ws_u64 nz, one; };
 __device__ __forceinline__ ws_u64 ws_mul(ws_u64 a, ws_u64 b, const WsConst& c) { return ws_fma2(a, b, c.nz); }
 __device__ __forceinline__ ws_u64 ws_add(ws_u64 a, ws_u64 b, const WsConst& c) { return ws_fma2(a, c.one, b); }

@@ -85,8 +85,8 @@ def _node_of_cpu(cpu: int) -> int | None:
 def bind_to_gpu_numa(index: int) -> dict:
     """Pin this process (threads created later inherit it) to the CPUs of the GPU's NUMA node and prefer that node for
     memory, BEFORE any pinned host buffer is allocated: page-locked staging memory is then first-touched on the socket
-    the GPU's PCIe root belongs to, so host<->device copies never cross the inter-socket link.  Round-1 measurement:
-    without this, 4 ranks sharing a socket ran their e2e step at 27 ms instead of 15 ms (SCALE_r01).
+    the GPU's PCIe root belongs to, so host<->device copies never cross the inter-socket link (ranks sharing a socket
+    otherwise slow each other's e2e step).
     Returns what was done (reported by bench.py); every step is best effort."""
     info = {"gpu": index, "cpus": None, "node": None, "mempolicy": None}
     cpus = gpu_cpu_affinity(index)

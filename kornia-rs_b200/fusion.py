@@ -1,4 +1,4 @@
-"""cuda/fusion.rs — the fusion engine's stage vocabulary and `FusedPipeline`, over pre-instantiated sm_100a kernels.
+"""cuda/fusion.rs — the fusion engine's stage vocabulary and `FusedPipeline`, over pre-instantiated sm_90a kernels.
 
     from kornia_rs_b200.fusion import FusedPipeline, ReadU8RgbBilinear, Normalize, RgbToGray, WriteChwF32, WriteC1F32
     pipe = FusedPipeline.build([ReadU8RgbBilinear(sw, sh, dw, dh), Normalize(scale, bias), RgbToGray(), WriteC1F32()], dw, dh)

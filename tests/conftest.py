@@ -2,7 +2,7 @@
 
 `-m "not gpu"` = oracle vs the reference's golden vectors, host logic, C-ABI symbol
 checks (runs anywhere).  `-m gpu` = parity tests proper: the CUDA path called through
-the C-ABI vs the oracle (needs a B200).
+the C-ABI vs the oracle (needs an H100).
 """
 import os
 import sys
@@ -15,7 +15,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_sessionstart(session):

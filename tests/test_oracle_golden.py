@@ -1,9 +1,9 @@
 """Pins the CPU oracle against the reference's OWN known-answer tests.
 
 Every test cites the reference test it transcribes (paths relative to
-/root/reference/crates/kornia-imgproc/src).  The Rust reference cannot run here (no cargo), so
+kornia-rs's crates/kornia-imgproc/src).  The Rust reference cannot run here (no cargo), so
 these vectors — plus the cv2 fixtures the reference declares byte-parity with — are what makes the
-oracle "pinned" (SURVEY §8(c)).  CPU only: no GPU, no /root/reference access at run time.
+oracle "pinned" (SURVEY §8(c)).  CPU only: no GPU, no access to the reference's sources at run time.
 """
 import os
 
