@@ -69,6 +69,12 @@ pub mod ffi {
         pub fn kb200_resize_normalize_chw_u8_f32(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut f32, dst_len: usize,
                                                  src_w: u32, src_h: u32, dst_w: u32, dst_h: u32, batch: u32, scale: *const f32,
                                                  bias: *const f32, leaf: c_int) -> c_int;
+        pub fn kb200_resize_normalize_chw_u8_f16(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u16, dst_len: usize,
+                                                 src_w: u32, src_h: u32, dst_w: u32, dst_h: u32, batch: u32, scale: *const f32,
+                                                 bias: *const f32, leaf: c_int) -> c_int;
+        pub fn kb200_resize_normalize_chw_u8_bf16(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u16, dst_len: usize,
+                                                  src_w: u32, src_h: u32, dst_w: u32, dst_h: u32, batch: u32, scale: *const f32,
+                                                  bias: *const f32, leaf: c_int) -> c_int;
         pub fn kb200_resize_row_plan(src_h: u32, dst_h: u32, period: *mut u32, first: *mut u32, keep: *mut u32);
         pub fn kb200_resize_normalize_chw_u8_f32_rows(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut f32, dst_len: usize,
                                                       src_w: u32, src_h: u32, dst_w: u32, dst_h: u32, batch: u32, scale: *const f32,
@@ -79,6 +85,10 @@ pub mod ffi {
         pub fn kb200_host_pipeline_last_transfer(pipeline: *const kb200_host_pipeline, h2d_bytes: *mut u64, d2h_bytes: *mut u64) -> c_int;
         pub fn kb200_host_register(ptr: *mut c_void, bytes: usize) -> c_int;
         pub fn kb200_host_unregister(ptr: *mut c_void) -> c_int;
+        pub fn kb200_resize_normalize_chw_u8_host(pipeline: *mut kb200_host_pipeline, stream: *mut c_void, host_src: *const u8,
+                                                  src_len: usize, host_dst: *mut c_void, dst_len: usize, src_w: u32, src_h: u32,
+                                                  dst_w: u32, dst_h: u32, batch: u32, scale: *const f32, bias: *const f32,
+                                                  leaf: c_int, out_format: c_int) -> c_int;
         pub fn kb200_resize_normalize_chw_u8_f32_host(pipeline: *mut kb200_host_pipeline, stream: *mut c_void, host_src: *const u8,
                                                       src_len: usize, host_dst: *mut f32, dst_len: usize, src_w: u32, src_h: u32,
                                                       dst_w: u32, dst_h: u32, batch: u32, scale: *const f32, bias: *const f32,
@@ -198,6 +208,12 @@ fn bind(ctx: &Arc<CudaContext>) -> Result<(), Kb200Error> {
 pub const LEAF_SCALAR: c_int = 0;
 pub const LEAF_X86_AVX2_FMA: c_int = 1;
 pub const LEAF_NEON: c_int = 2;
+
+/// `out_format` of `kb200_resize_normalize_chw_u8_host` (kb200_out_format): the CHW element type.  16-bit values are the
+/// f32 result rounded once to nearest-even, stored as their raw bits.
+pub const OUT_F32: c_int = 0;
+pub const OUT_F16: c_int = 1;
+pub const OUT_BF16: c_int = 2;
 
 /// `PixelMapping` of cuda/resize.rs:441.
 #[derive(Debug, Clone, Copy, PartialEq, Eq)]
@@ -326,6 +342,37 @@ impl HostPipeline {
             ffi::kb200_resize_normalize_chw_u8_f32_host(self.raw, stream.cu_stream() as *mut c_void, src.as_ptr(), src.len(),
                                                         dst.as_mut_ptr(), dst.len(), src_size.0, src_size.1, dst_size.0, dst_size.1,
                                                         batch, scale.as_ptr(), bias.as_ptr(), LEAF_X86_AVX2_FMA)
+        })
+    }
+
+    /// Same as `resize_normalize_u8_to_f32`, `dst` holding IEEE binary16 bits: RNE of the f32 result (an extension beyond
+    /// the reference, which writes f32 only).  The download moves half the bytes.
+    #[allow(clippy::too_many_arguments)]
+    pub fn resize_normalize_u8_to_f16(
+        &mut self, stream: &Arc<CudaStream>, src: &[u8], src_size: (u32, u32), dst: &mut [u16], dst_size: (u32, u32), batch: u32,
+        scale: &[f32; 3], bias: &[f32; 3],
+    ) -> Result<(), Kb200Error> {
+        self.resize_normalize_u8_to_16bit(stream, src, src_size, dst, dst_size, batch, scale, bias, OUT_F16)
+    }
+
+    /// Same as `resize_normalize_u8_to_f16`, `dst` holding bfloat16 bits.
+    #[allow(clippy::too_many_arguments)]
+    pub fn resize_normalize_u8_to_bf16(
+        &mut self, stream: &Arc<CudaStream>, src: &[u8], src_size: (u32, u32), dst: &mut [u16], dst_size: (u32, u32), batch: u32,
+        scale: &[f32; 3], bias: &[f32; 3],
+    ) -> Result<(), Kb200Error> {
+        self.resize_normalize_u8_to_16bit(stream, src, src_size, dst, dst_size, batch, scale, bias, OUT_BF16)
+    }
+
+    #[allow(clippy::too_many_arguments)]
+    fn resize_normalize_u8_to_16bit(
+        &mut self, stream: &Arc<CudaStream>, src: &[u8], src_size: (u32, u32), dst: &mut [u16], dst_size: (u32, u32), batch: u32,
+        scale: &[f32; 3], bias: &[f32; 3], out_format: c_int,
+    ) -> Result<(), Kb200Error> {
+        check(unsafe {
+            ffi::kb200_resize_normalize_chw_u8_host(self.raw, stream.cu_stream() as *mut c_void, src.as_ptr(), src.len(),
+                                                    dst.as_mut_ptr() as *mut c_void, dst.len(), src_size.0, src_size.1, dst_size.0,
+                                                    dst_size.1, batch, scale.as_ptr(), bias.as_ptr(), LEAF_X86_AVX2_FMA, out_format)
         })
     }
 

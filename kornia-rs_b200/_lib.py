@@ -16,6 +16,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libkornia_b200.so")
 OK = 0
 ERR_INVALID_ARGUMENT, ERR_SLICE_TOO_SMALL, ERR_SINGULAR_MATRIX, ERR_UNSUPPORTED = -1, -2, -3, -4
 ERR_CUDA, ERR_INVALID_KERNEL, ERR_DIMS_TOO_LARGE, ERR_INVALID_SOURCE = -5, -6, -7, -8
+OUT_F32, OUT_F16, OUT_BF16 = 0, 1, 2   # kb200_out_format
 
 
 class PreprocessDesc(C.Structure):
@@ -57,6 +58,8 @@ def _declare(l: C.CDLL) -> None:
         "kb200_pyrdown_u8": ([vp, vp, sz, vp, sz, u32, u32, u32, u32], i),
         "kb200_pyrup_u8": ([vp, vp, sz, vp, sz, u32, u32, u32, u32], i),
         "kb200_resize_normalize_chw_u8_f32": ([vp, vp, sz, vp, sz, u32, u32, u32, u32, u32, fp, fp, i], i),
+        "kb200_resize_normalize_chw_u8_f16": ([vp, vp, sz, vp, sz, u32, u32, u32, u32, u32, fp, fp, i], i),
+        "kb200_resize_normalize_chw_u8_bf16": ([vp, vp, sz, vp, sz, u32, u32, u32, u32, u32, fp, fp, i], i),
         "kb200_resize_row_plan": ([u32, u32, C.POINTER(u32), C.POINTER(u32), C.POINTER(u32)], None),
         "kb200_resize_normalize_chw_u8_f32_rows": ([vp, vp, sz, vp, sz, u32, u32, u32, u32, u32, fp, fp, i, u32, u32, u32], i),
         "kb200_host_pipeline_create": ([i, sz, sz, i, C.POINTER(vp)], i),
@@ -64,6 +67,7 @@ def _declare(l: C.CDLL) -> None:
         "kb200_host_pipeline_last_transfer": ([vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)], i),
         "kb200_host_register": ([vp, sz], i),
         "kb200_host_unregister": ([vp], i),
+        "kb200_resize_normalize_chw_u8_host": ([vp, vp, vp, sz, vp, sz, u32, u32, u32, u32, u32, fp, fp, i, i], i),
         "kb200_resize_normalize_chw_u8_f32_host": ([vp, vp, vp, sz, vp, sz, u32, u32, u32, u32, u32, fp, fp, i], i),
         "kb200_resize_bilinear_u8": ([vp, vp, sz, vp, sz, u32, u32, u32, u32, u32, u32], i),
         "kb200_resize_fast_u8": ([vp, vp, sz, vp, sz, u32, u32, u32, u32, u32, u32, i], i),

@@ -111,14 +111,16 @@ KB200_API int kb200_host_unregister(void* ptr) {
     return KB200_OK;
 }
 
-KB200_API int kb200_resize_normalize_chw_u8_f32_host(kb200_host_pipeline* pipe, kb200_stream_t stream,
-                                                     const uint8_t* host_src, size_t src_len, float* host_dst,
-                                                     size_t dst_len, uint32_t sw, uint32_t sh, uint32_t dw, uint32_t dh,
-                                                     uint32_t batch, const float scale[3], const float bias[3], int leaf) {
+KB200_API int kb200_resize_normalize_chw_u8_host(kb200_host_pipeline* pipe, kb200_stream_t stream, const uint8_t* host_src,
+                                                 size_t src_len, void* host_dst, size_t dst_len, uint32_t sw, uint32_t sh,
+                                                 uint32_t dw, uint32_t dh, uint32_t batch, const float scale[3],
+                                                 const float bias[3], int leaf, int out_format) {
     KB200_TRY(check_ptr("pipeline", pipe));
     KB200_TRY(check_ptr("src", host_src)); KB200_TRY(check_ptr("dst", host_dst));
     KB200_TRY(check_ptr("scale", scale)); KB200_TRY(check_ptr("bias", bias));
     if (leaf < 0 || leaf > 2) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown cpu leaf %d", leaf);
+    if (out_format != KB200_OUT_F32 && out_format != KB200_OUT_F16 && out_format != KB200_OUT_BF16)
+        return fail(KB200_ERR_INVALID_ARGUMENT, "unknown output format %d", out_format);
     if (batch == 0) return fail(KB200_ERR_INVALID_ARGUMENT, "batch must be non-zero");
     KB200_TRY(check_slice("src", src_len, (size_t)sw * sh * 3 * batch));
     KB200_TRY(check_slice("dst", dst_len, (size_t)dw * dh * 3 * batch));
@@ -132,7 +134,7 @@ KB200_API int kb200_resize_normalize_chw_u8_f32_host(kb200_host_pipeline* pipe, 
     const size_t row_bytes = (size_t)sw * 3;
     const size_t src_frame_dev = row_bytes * p.src_rows;          // compacted frame in the staging buffer
     const size_t src_frame_host = row_bytes * sh;
-    const size_t dst_frame = (size_t)dw * dh * 3 * sizeof(float);
+    const size_t dst_frame = (size_t)dw * dh * 3 * (out_format == KB200_OUT_F32 ? sizeof(float) : sizeof(uint16_t));
     const size_t per_chunk = std::min<size_t>(std::min(pipe->src_bytes / src_frame_dev, pipe->dst_bytes / dst_frame), 65535);
     if (per_chunk == 0)
         return fail(KB200_ERR_INVALID_ARGUMENT, "pipeline staging (%zu B src, %zu B dst) is smaller than one frame (%zu B, %zu B)",
@@ -157,8 +159,11 @@ KB200_API int kb200_resize_normalize_chw_u8_f32_host(kb200_host_pipeline* pipe, 
             KB200_CUDA(cudaMemcpy2DAsync(pipe->src[k], row_bytes * p.row_k, hs + row_bytes * p.row_f, row_bytes * p.row_p,
                                          row_bytes * p.row_k, (size_t)n * (sh / p.row_p), cudaMemcpyHostToDevice, s));
         }
-        KB200_TRY(launch_fused_resize(s, pipe->src[k], reinterpret_cast<float*>(pipe->dst[k]), p, n));
-        KB200_CUDA(cudaMemcpyAsync(host_dst + (size_t)f0 * dw * dh * 3, pipe->dst[k], dst_frame * n, cudaMemcpyDeviceToHost, s));
+        if (out_format == KB200_OUT_F32) KB200_TRY(launch_fused_resize(s, pipe->src[k], reinterpret_cast<float*>(pipe->dst[k]), p, n));
+        else if (out_format == KB200_OUT_F16) KB200_TRY(launch_fused_resize(s, pipe->src[k], reinterpret_cast<__half*>(pipe->dst[k]), p, n));
+        else KB200_TRY(launch_fused_resize(s, pipe->src[k], reinterpret_cast<__nv_bfloat16*>(pipe->dst[k]), p, n));
+        KB200_CUDA(cudaMemcpyAsync(static_cast<uint8_t*>(host_dst) + (size_t)f0 * dst_frame, pipe->dst[k], dst_frame * n,
+                                   cudaMemcpyDeviceToHost, s));
         pipe->h2d_bytes += src_frame_dev * n;
         pipe->d2h_bytes += dst_frame * n;
         f0 += n;
@@ -170,6 +175,13 @@ KB200_API int kb200_resize_normalize_chw_u8_f32_host(kb200_host_pipeline* pipe, 
     return KB200_OK;
 }
 
+KB200_API int kb200_resize_normalize_chw_u8_f32_host(kb200_host_pipeline* pipe, kb200_stream_t stream,
+                                                     const uint8_t* host_src, size_t src_len, float* host_dst,
+                                                     size_t dst_len, uint32_t sw, uint32_t sh, uint32_t dw, uint32_t dh,
+                                                     uint32_t batch, const float scale[3], const float bias[3], int leaf) {
+    return kb200_resize_normalize_chw_u8_host(pipe, stream, host_src, src_len, host_dst, dst_len, sw, sh, dw, dh, batch, scale, bias,
+                                              leaf, KB200_OUT_F32);
+}
 
 // Host-buffer form of Preprocessor::run_raw_batch (preprocess.rs:1234; the reference's Python Preprocessor pins and
 // uploads camera frames itself, kornia-py/src/cuda_ext/mod.rs:700-760): `batch` raw frames at host_base + i*frame_stride

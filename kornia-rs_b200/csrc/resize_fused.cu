@@ -1,4 +1,4 @@
-// resize_fused.cu — fused u8 HWC → f32 CHW bilinear resize + normalize (a2; BASELINE config 2).
+// resize_fused.cu — fused u8 HWC → f32 / f16 / bf16 CHW bilinear resize + normalize (a2; BASELINE config 2).
 //
 // Reference: resize/fused.rs:147-228 (general bilinear, half-pixel, non-antialiased), scalar leaf
 // :273-318, AVX2+FMA leaf :414-497 (FMA form on the dst_w&~7 bulk, scalar form on the tail),
@@ -7,6 +7,10 @@
 // `fma_bulk` = number of leading destination columns whose arithmetic is the reference's FMA leaf;
 // columns ≥ fma_bulk use the scalar (mul, add) leaf — so the output is bit-identical to what the
 // reference produces on the chosen CPU (x86 AVX2+FMA: bulk = dst_w & ~7, or & ~15 on the 2x path).
+//
+// 16-bit outputs (an extension: the reference writes f32 only): every kernel is templated on the output element type
+// and computes the f32 value exactly as the f32 instantiation does; only the store differs, one round-to-nearest-even
+// conversion (fused_out) of that value.  So out16 == RNE(out_f32) for every mode, leaf and column.
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
@@ -30,16 +34,23 @@ __device__ __forceinline__ float fused_lerp(float a, float b, float c, float d, 
     return val * sc + bi;
 }
 
+// The one place the output type enters the arithmetic: f32 is stored as computed, a 16-bit type is the hardware RNE
+// conversion of it (overflow -> inf, subnormals and the sign of zero kept, NaN -> NaN).
+template <typename T> __device__ __forceinline__ T fused_out(float v);
+template <> __device__ __forceinline__ float fused_out<float>(float v) { return v; }
+template <> __device__ __forceinline__ __half fused_out<__half>(float v) { return __float2half_rn(v); }
+template <> __device__ __forceinline__ __nv_bfloat16 fused_out<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+
 // Generic path: any size / alignment.  One thread per destination pixel, batch = grid.z.
-template <bool BOX2X>
-__global__ void __launch_bounds__(256) fused_resize_gather_kernel(const uint8_t* __restrict__ src, float* __restrict__ dst,
+template <typename T, bool BOX2X>
+__global__ void __launch_bounds__(256) fused_resize_gather_kernel(const uint8_t* __restrict__ src, T* __restrict__ dst,
                                                                   const __grid_constant__ FusedParams p) {
     const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x >= p.dw || y >= p.dh) return;
     const uint8_t* s = src + (size_t)blockIdx.z * p.sw * p.src_rows * 3;
     const size_t plane = (size_t)p.dw * p.dh;
-    float* d = dst + (size_t)blockIdx.z * plane * 3 + (size_t)y * p.dw + x;
+    T* d = dst + (size_t)blockIdx.z * plane * 3 + (size_t)y * p.dw + x;
     const bool fused = x < p.fma_bulk;
     if (BOX2X) {  // resize/fused.rs:528-559
         const uint8_t* r0 = s + ((size_t)(2 * y) * p.sw + 2 * x) * 3;
@@ -48,7 +59,7 @@ __global__ void __launch_bounds__(256) fused_resize_gather_kernel(const uint8_t*
         for (int c = 0; c < 3; ++c) {
             const uint32_t sum = (uint32_t)r0[c] + r0[3 + c] + r1[c] + r1[3 + c];
             const float s4 = p.scale[c] * 0.25f;
-            d[c * plane] = fused ? fmaf((float)sum, s4, p.bias[c]) : (float)sum * s4 + p.bias[c];
+            d[c * plane] = fused_out<T>(fused ? fmaf((float)sum, s4, p.bias[c]) : (float)sum * s4 + p.bias[c]);
         }
         return;
     }
@@ -66,11 +77,12 @@ __global__ void __launch_bounds__(256) fused_resize_gather_kernel(const uint8_t*
     for (int c = 0; c < 3; ++c) {
         const float a = (float)row0[x0 * 3 + c], b = (float)row0[x1 * 3 + c];
         const float cc = (float)row1[x0 * 3 + c], dd = (float)row1[x1 * 3 + c];
-        d[c * plane] = fused_lerp(a, b, cc, dd, wx, wy, p.scale[c], p.bias[c], fused);
+        d[c * plane] = fused_out<T>(fused_lerp(a, b, cc, dd, wx, wy, p.scale[c], p.bias[c], fused));
     }
 }
 
-int launch_fused_resize_rows(cudaStream_t s, const uint8_t* src, float* dst, const FusedParams& p, uint32_t batch, bool* handled);
+template <typename T>
+int launch_fused_resize_rows(cudaStream_t s, const uint8_t* src, T* dst, const FusedParams& p, uint32_t batch, bool* handled);
 
 FusedParams make_fused_params(uint32_t sw, uint32_t sh, uint32_t dw, uint32_t dh, const float scale[3], const float bias[3], int leaf) {
     FusedParams p;
@@ -109,7 +121,8 @@ void resize_row_plan(uint32_t sh, uint32_t dh, uint32_t* period, uint32_t* first
     *period = P; *first = lo; *keep = hi - lo + 1;
 }
 
-int launch_fused_resize(cudaStream_t s, const uint8_t* src, float* dst, const FusedParams& p, uint32_t batch) {
+template <typename T>
+int launch_fused_resize(cudaStream_t s, const uint8_t* src, T* dst, const FusedParams& p, uint32_t batch) {
     const bool box2x = (p.sw == 2 * p.dw && p.sh == 2 * p.dh);
     {
         bool handled = false;
@@ -117,21 +130,23 @@ int launch_fused_resize(cudaStream_t s, const uint8_t* src, float* dst, const Fu
         if (handled) return KB200_OK;
     }
     dim3 block(32, 8), grid(div_up(p.dw, 32), div_up(p.dh, 8), batch);
-    if (box2x) fused_resize_gather_kernel<true><<<grid, block, 0, s>>>(src, dst, p);
-    else fused_resize_gather_kernel<false><<<grid, block, 0, s>>>(src, dst, p);
+    if (box2x) fused_resize_gather_kernel<T, true><<<grid, block, 0, s>>>(src, dst, p);
+    else fused_resize_gather_kernel<T, false><<<grid, block, 0, s>>>(src, dst, p);
     return check_launch("fused_resize_gather_kernel");
 }
+template int launch_fused_resize<float>(cudaStream_t, const uint8_t*, float*, const FusedParams&, uint32_t);
+template int launch_fused_resize<__half>(cudaStream_t, const uint8_t*, __half*, const FusedParams&, uint32_t);
+template int launch_fused_resize<__nv_bfloat16>(cudaStream_t, const uint8_t*, __nv_bfloat16*, const FusedParams&, uint32_t);
 
 }  // namespace kb200
 
 using namespace kb200;
 
-extern "C" {
-
-KB200_API int kb200_resize_normalize_chw_u8_f32(kb200_stream_t stream, const uint8_t* src, size_t src_len,
-                                                float* dst, size_t dst_len, uint32_t sw, uint32_t sh, uint32_t dw,
-                                                uint32_t dh, uint32_t batch, const float scale[3],
-                                                const float bias[3], int leaf) {
+// Device-buffer entry points: one validation for every output type (dst_len counts elements).
+template <typename T>
+static int resize_normalize_chw(kb200_stream_t stream, const uint8_t* src, size_t src_len, T* dst, size_t dst_len, uint32_t sw,
+                                uint32_t sh, uint32_t dw, uint32_t dh, uint32_t batch, const float scale[3], const float bias[3],
+                                int leaf) {
     KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
     KB200_TRY(check_ptr("scale", scale)); KB200_TRY(check_ptr("bias", bias));
     if (leaf < 0 || leaf > 2) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown cpu leaf %d", leaf);
@@ -143,6 +158,30 @@ KB200_API int kb200_resize_normalize_chw_u8_f32(kb200_stream_t stream, const uin
     if (dw == 0 || dh == 0 || sw == 0 || sh == 0) return KB200_OK;  // resize/fused.rs:184-186: empty is a no-op
     FusedParams p = make_fused_params(sw, sh, dw, dh, scale, bias, leaf);
     return launch_fused_resize(as_stream(stream), src, dst, p, batch);
+}
+
+extern "C" {
+
+KB200_API int kb200_resize_normalize_chw_u8_f32(kb200_stream_t stream, const uint8_t* src, size_t src_len,
+                                                float* dst, size_t dst_len, uint32_t sw, uint32_t sh, uint32_t dw,
+                                                uint32_t dh, uint32_t batch, const float scale[3],
+                                                const float bias[3], int leaf) {
+    return resize_normalize_chw(stream, src, src_len, dst, dst_len, sw, sh, dw, dh, batch, scale, bias, leaf);
+}
+
+KB200_API int kb200_resize_normalize_chw_u8_f16(kb200_stream_t stream, const uint8_t* src, size_t src_len,
+                                                uint16_t* dst, size_t dst_len, uint32_t sw, uint32_t sh, uint32_t dw,
+                                                uint32_t dh, uint32_t batch, const float scale[3],
+                                                const float bias[3], int leaf) {
+    return resize_normalize_chw(stream, src, src_len, reinterpret_cast<__half*>(dst), dst_len, sw, sh, dw, dh, batch, scale, bias, leaf);
+}
+
+KB200_API int kb200_resize_normalize_chw_u8_bf16(kb200_stream_t stream, const uint8_t* src, size_t src_len,
+                                                 uint16_t* dst, size_t dst_len, uint32_t sw, uint32_t sh, uint32_t dw,
+                                                 uint32_t dh, uint32_t batch, const float scale[3],
+                                                 const float bias[3], int leaf) {
+    return resize_normalize_chw(stream, src, src_len, reinterpret_cast<__nv_bfloat16*>(dst), dst_len, sw, sh, dw, dh, batch, scale,
+                                bias, leaf);
 }
 
 KB200_API int kb200_resize_normalize_chw_u8_f32_rows(kb200_stream_t stream, const uint8_t* src, size_t src_len,
@@ -205,7 +244,8 @@ KB200_API void kb200_resize_row_plan(uint32_t src_h, uint32_t dst_h, uint32_t* p
 //   * taps are read as three aligned 32-bit words per source row and funnel-shifted into place; a byte becomes a
 //     float with one PRMT into the mantissa of 2^23; `b - a` is formed on the biased values (exact) and only the
 //     base taps are unbiased (one FADD).
-//   * stores: a warp writes 32 consecutive floats of one channel plane = one full 128-B line.
+//   * stores: a warp writes 32 consecutive values of one channel plane = one full 128-B line (f32), or two full
+//     32-B sectors (f16 / bf16: element alignment is all a store needs).
 //
 // Arithmetic is identical to the gather kernel (and therefore to the reference leaf selected).
 namespace kb200 {
@@ -354,8 +394,8 @@ __device__ __forceinline__ void fr_pixel(const uint8_t* __restrict__ rp, uint32_
     else          { q0 = v[0] * s0 + o0;     q1 = v[1] * s1 + o1;     q2 = v[2] * s2 + o2; }       // :317
 }
 
-template <int NPX, int MODE, bool ALLFMA>
-__global__ void __launch_bounds__(FR_THREADS) fused_rows_kernel(const uint8_t* __restrict__ src, float* __restrict__ dst,
+template <typename T, int NPX, int MODE, bool ALLFMA>
+__global__ void __launch_bounds__(FR_THREADS) fused_rows_kernel(const uint8_t* __restrict__ src, T* __restrict__ dst,
                                                                 const __grid_constant__ FusedRowsParams R) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     __shared__ __align__(8) uint64_t full_bar[FR_MAX_STAGES];
@@ -439,9 +479,9 @@ __global__ void __launch_bounds__(FR_THREADS) fused_rows_kernel(const uint8_t* _
             fm |= (x < p.fma_bulk ? 1u : 0u) << j;
         }
         const uint32_t y_first = w.cy * P.rows_per_chunk, y_end = min(y_first + P.rows_per_chunk, p.dh);
-        float* out0 = dst + (size_t)w.img * plane * 3 + (size_t)y_first * p.dw + dx0 + tid;
-        float* out1 = out0 + plane;
-        float* out2 = out1 + plane;
+        T* out0 = dst + (size_t)w.img * plane * 3 + (size_t)y_first * p.dw + dx0 + tid;
+        T* out1 = out0 + plane;
+        T* out2 = out1 + plane;
         for (uint32_t dy = y_first; dy < y_end; ++dy) {
             mbar_wait(&full_bar[stage], phase);
             const uint8_t* sbase = smem_raw + (size_t)stage * R.stage_bytes;
@@ -450,7 +490,7 @@ __global__ void __launch_bounds__(FR_THREADS) fused_rows_kernel(const uint8_t* _
             for (int j = 0; j < NPX; ++j) {
                 float q0, q1, q2;
                 fr_pixel<MODE>(sbase + off[j], P.slot_bytes, shft[j], wx[j], wy, ALLFMA || ((fm >> j) & 1u), s0, s1, s2, o0, o1, o2, q0, q1, q2);
-                if ((act >> j) & 1u) { out0[j * FR_CT] = q0; out1[j * FR_CT] = q1; out2[j * FR_CT] = q2; }
+                if ((act >> j) & 1u) { out0[j * FR_CT] = fused_out<T>(q0); out1[j * FR_CT] = fused_out<T>(q1); out2[j * FR_CT] = fused_out<T>(q2); }
             }
             out0 += p.dw; out1 += p.dw; out2 += p.dw;
             __syncwarp();
@@ -472,8 +512,8 @@ static bool axis_weights_all_zero(uint32_t dst_len, uint32_t src_len, float scal
     return true;
 }
 
-template <int NPX, int MODE>
-static cudaError_t fr_launch(bool allfma, unsigned grid, size_t smem, cudaStream_t s, const uint8_t* src, float* dst, const FusedRowsParams& R) {
+template <typename T, int NPX, int MODE>
+static cudaError_t fr_launch(bool allfma, unsigned grid, size_t smem, cudaStream_t s, const uint8_t* src, T* dst, const FusedRowsParams& R) {
     auto go = [&](auto kern) -> cudaError_t {
         if (smem > 40 * 1024) {
             cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -482,21 +522,23 @@ static cudaError_t fr_launch(bool allfma, unsigned grid, size_t smem, cudaStream
         kern<<<grid, FR_THREADS, smem, s>>>(src, dst, R);
         return cudaSuccess;
     };
-    return allfma ? go(fused_rows_kernel<NPX, MODE, true>) : go(fused_rows_kernel<NPX, MODE, false>);
+    return allfma ? go(fused_rows_kernel<T, NPX, MODE, true>) : go(fused_rows_kernel<T, NPX, MODE, false>);
 }
 
-template <int MODE>
-static cudaError_t fr_launch_npx(int npx, bool allfma, unsigned grid, size_t smem, cudaStream_t s, const uint8_t* src, float* dst, const FusedRowsParams& R) {
+template <typename T, int MODE>
+static cudaError_t fr_launch_npx(int npx, bool allfma, unsigned grid, size_t smem, cudaStream_t s, const uint8_t* src, T* dst, const FusedRowsParams& R) {
     switch (npx) {
-        case 1: return fr_launch<1, MODE>(allfma, grid, smem, s, src, dst, R);
-        case 2: return fr_launch<2, MODE>(allfma, grid, smem, s, src, dst, R);
-        case 3: return fr_launch<3, MODE>(allfma, grid, smem, s, src, dst, R);
-        case 4: return fr_launch<4, MODE>(allfma, grid, smem, s, src, dst, R);
-        default: return fr_launch<5, MODE>(allfma, grid, smem, s, src, dst, R);
+        case 1: return fr_launch<T, 1, MODE>(allfma, grid, smem, s, src, dst, R);
+        case 2: return fr_launch<T, 2, MODE>(allfma, grid, smem, s, src, dst, R);
+        case 3: return fr_launch<T, 3, MODE>(allfma, grid, smem, s, src, dst, R);
+        case 4: return fr_launch<T, 4, MODE>(allfma, grid, smem, s, src, dst, R);
+        default: return fr_launch<T, 5, MODE>(allfma, grid, smem, s, src, dst, R);
     }
 }
 
-int launch_fused_resize_rows(cudaStream_t s, const uint8_t* src, float* dst, const FusedParams& p, uint32_t batch, bool* handled) {
+// Geometry, mode, npx, ring depth and CTA count depend on the source side only: the same for every output type.
+template <typename T>
+int launch_fused_resize_rows(cudaStream_t s, const uint8_t* src, T* dst, const FusedParams& p, uint32_t batch, bool* handled) {
     *handled = false;
     const uint32_t row_bytes = p.sw * 3u;
     // TMA 1-D bulk copies need 16-B aligned rows; very strong downscales have sparse taps (the span would be
@@ -567,14 +609,17 @@ int launch_fused_resize_rows(cudaStream_t s, const uint8_t* src, float* dst, con
     P.dimg = g / P.chunks_y;
     const bool allfma = p.fma_bulk >= p.dw;
     cudaError_t e;
-    if (mode == FR_POINT) e = fr_launch_npx<FR_POINT>(npx, allfma, grid, smem, s, src, dst, R);
-    else if (mode == FR_YZERO) e = fr_launch_npx<FR_YZERO>(npx, allfma, grid, smem, s, src, dst, R);
-    else if (mode == FR_BOX) e = fr_launch_npx<FR_BOX>(npx, allfma, grid, smem, s, src, dst, R);
-    else e = fr_launch_npx<FR_GENERAL>(npx, allfma, grid, smem, s, src, dst, R);
+    if (mode == FR_POINT) e = fr_launch_npx<T, FR_POINT>(npx, allfma, grid, smem, s, src, dst, R);
+    else if (mode == FR_YZERO) e = fr_launch_npx<T, FR_YZERO>(npx, allfma, grid, smem, s, src, dst, R);
+    else if (mode == FR_BOX) e = fr_launch_npx<T, FR_BOX>(npx, allfma, grid, smem, s, src, dst, R);
+    else e = fr_launch_npx<T, FR_GENERAL>(npx, allfma, grid, smem, s, src, dst, R);
     if (e != cudaSuccess) return fail(KB200_ERR_CUDA, "cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
     KB200_TRY(check_launch("fused_rows_kernel"));
     *handled = true;
     return KB200_OK;
 }
+template int launch_fused_resize_rows<float>(cudaStream_t, const uint8_t*, float*, const FusedParams&, uint32_t, bool*);
+template int launch_fused_resize_rows<__half>(cudaStream_t, const uint8_t*, __half*, const FusedParams&, uint32_t, bool*);
+template int launch_fused_resize_rows<__nv_bfloat16>(cudaStream_t, const uint8_t*, __nv_bfloat16*, const FusedParams&, uint32_t, bool*);
 
 }  // namespace kb200

@@ -194,6 +194,12 @@ def _pipeline_for(pipeline: HostPipeline | None) -> HostPipeline:
     return _default_pipelines[idx]
 
 
+# output dtype -> (device entry point, kb200_out_format of the host-buffer form; f32 keeps its own host entry point)
+_CHW_OUT = {torch.float32: ("kb200_resize_normalize_chw_u8_f32", None),
+            torch.float16: ("kb200_resize_normalize_chw_u8_f16", _lib.OUT_F16),
+            torch.bfloat16: ("kb200_resize_normalize_chw_u8_bf16", _lib.OUT_BF16)}
+
+
 def resize_normalize_to_tensor_u8_to_f32_bilinear(src, dst_w: int, dst_h: int, scale, bias, out: torch.Tensor | None = None,
                                                   leaf: int = DEFAULT_LEAF, pipeline: HostPipeline | None = None) -> torch.Tensor:
     """resize/fused.rs:147 — u8 HWC (or NHWC) → f32 CHW ([N,3,dst_h,dst_w]) bilinear (half-pixel, non-AA)
@@ -202,6 +208,26 @@ def resize_normalize_to_tensor_u8_to_f32_bilinear(src, dst_w: int, dst_h: int, s
     Device images run the kernel in place.  HOST images (the reference operator's own signature) go through a
     `HostPipeline`: chunked upload → kernel → download on the GPU, enqueued on the current stream of the pipeline's
     device — synchronise that stream before reading `out`.  There is no CPU implementation."""
+    return _resize_normalize_chw("resize_normalize_to_tensor_u8_to_f32_bilinear", src, dst_w, dst_h, scale, bias, torch.float32, out,
+                                 leaf, pipeline)
+
+
+def resize_normalize_to_tensor_u8_bilinear(src, dst_w: int, dst_h: int, scale, bias, dtype: torch.dtype, out: torch.Tensor | None = None,
+                                           leaf: int = DEFAULT_LEAF, pipeline: HostPipeline | None = None) -> torch.Tensor:
+    """`resize_normalize_to_tensor_u8_to_f32_bilinear` with the CHW output in `dtype`: torch.float32, torch.float16 or
+    torch.bfloat16.  A 16-bit value is the f32 result rounded once to nearest-even — bit-identical to calling the f32
+    operator and then `.to(dtype)`, without writing and re-reading the f32 tensor.  (An extension: the reference writes
+    f32 only.)  Device and host sources as for the f32 operator; an `out` it allocates for a host source is pinned."""
+    if dtype not in _CHW_OUT:
+        raise ImageError.DtypeMismatch("torch.float32, torch.float16 or torch.bfloat16", dtype)
+    if out is not None and out.dtype != dtype:
+        raise ImageError.DtypeMismatch(dtype, out.dtype)
+    return _resize_normalize_chw("resize_normalize_to_tensor_u8_bilinear", src, dst_w, dst_h, scale, bias, dtype, out, leaf, pipeline)
+
+
+def _resize_normalize_chw(op: str, src, dst_w: int, dst_h: int, scale, bias, dtype: torch.dtype, out: torch.Tensor | None, leaf: int,
+                          pipeline: HostPipeline | None) -> torch.Tensor:
+    fn, out_format = _CHW_OUT[dtype]
     t = src.data if isinstance(src, Image) else src
     if t.dtype != torch.uint8:
         raise ImageError.DtypeMismatch(torch.uint8, t.dtype)
@@ -214,29 +240,33 @@ def resize_normalize_to_tensor_u8_to_f32_bilinear(src, dst_w: int, dst_h: int, s
         raise ImageError.InvalidChannelShape(t.numel(), n * sh * sw * 3)
     if not t.is_cuda:
         if not torch.cuda.is_available():
-            raise ImageError.HostPathNotBuilt("resize_normalize_to_tensor_u8_to_f32_bilinear")
+            raise ImageError.HostPathNotBuilt(op)
         if out is None:
-            out = torch.empty((n, 3, dst_h, dst_w), dtype=torch.float32, pin_memory=True)
+            out = torch.empty((n, 3, dst_h, dst_w), dtype=dtype, pin_memory=True)
         elif out.is_cuda:
             raise ImageError.MixedResidency()
-        if out.dtype != torch.float32 or not out.is_contiguous() or out.numel() != n * 3 * dst_h * dst_w:
+        if out.dtype != dtype or not out.is_contiguous() or out.numel() != n * 3 * dst_h * dst_w:
             raise ImageError.InvalidChannelShape(out.numel(), n * 3 * dst_h * dst_w)
         pipe = _pipeline_for(pipeline)
         _lib.set_device(pipe.device.index)
-        _check(_lib.lib().kb200_resize_normalize_chw_u8_f32_host(pipe._h, _stream(pipe.device), t.data_ptr(), t.numel(), out.data_ptr(),
-                                                                out.numel(), sw, sh, dst_w, dst_h, n, _lib.f3(scale), _lib.f3(bias), leaf))
+        args = (pipe._h, _stream(pipe.device), t.data_ptr(), t.numel(), out.data_ptr(), out.numel(), sw, sh, dst_w, dst_h, n,
+                _lib.f3(scale), _lib.f3(bias), leaf)
+        if out_format is None:
+            _check(_lib.lib().kb200_resize_normalize_chw_u8_f32_host(*args))
+        else:
+            _check(_lib.lib().kb200_resize_normalize_chw_u8_host(*args, out_format))
         return out
     if out is None:
-        out = torch.empty((n, 3, dst_h, dst_w), dtype=torch.float32, device=t.device)
+        out = torch.empty((n, 3, dst_h, dst_w), dtype=dtype, device=t.device)
     else:
         if out.device != t.device:
             raise ImageError.DeviceMismatch() if out.is_cuda else ImageError.MixedResidency()
-        if out.dtype != torch.float32 or not out.is_contiguous() or out.numel() != n * 3 * dst_h * dst_w:
+        if out.dtype != dtype or not out.is_contiguous() or out.numel() != n * 3 * dst_h * dst_w:
             raise ImageError.InvalidChannelShape(out.numel(), n * 3 * dst_h * dst_w)
     dev = t.device
     _lib.set_device(dev.index)
-    _check(_lib.lib().kb200_resize_normalize_chw_u8_f32(_stream(dev), t.data_ptr(), t.numel(), out.data_ptr(), out.numel(),
-                                                       sw, sh, dst_w, dst_h, n, _lib.f3(scale), _lib.f3(bias), leaf))
+    _check(getattr(_lib.lib(), fn)(_stream(dev), t.data_ptr(), t.numel(), out.data_ptr(), out.numel(),
+                                   sw, sh, dst_w, dst_h, n, _lib.f3(scale), _lib.f3(bias), leaf))
     return out
 
 
