@@ -69,14 +69,19 @@ def f32_then_cast(kb, src, dw, dh, scale, bias, dtype, **kw):
     (384, 216, 128, 72, "fused_rows_kernel"),      # 3:1 -> FR_POINT
     (384, 216, 192, 108, "fused_rows_kernel"),     # 2:1 -> FR_BOX
     (384, 216, 160, 90, "fused_rows_kernel"),      # 2.4:1 -> FR_GENERAL
-    (384, 216, 384, 72, "fused_rows_kernel"),      # y 3:1, x 1:1 -> FR_YZERO (x general)
+    (384, 216, 384, 72, "fused_rows_kernel"),      # y 3:1, x 1:1 -> FR_POINT (a 1:1 axis has all-zero weights too)
+    (384, 216, 160, 72, "fused_rows_kernel"),      # y 3:1, x 2.4:1 -> FR_YZERO (x general)
     (383, 216, 128, 72, "fused_resize_gather_kernel"),   # row_bytes % 16 != 0 -> gather fallback
     (3840, 40, 512, 20, "fused_resize_gather_kernel"),   # scale_x > 6 -> gather fallback
 ])
 @pytest.mark.parametrize("leaf", [0, 1])
 @pytest.mark.parametrize("dtype", HALF)
 def test_half_modes_named(kb, oracle, dev, sw, sh, dw, dh, kernel, leaf, dtype):
+    from test_gpu_variants import NAMED_FUSED_MODES
+    from test_launch_shapes import fused_schedule
+
     n = 2
+    assert fused_schedule(sw, sh, dw, dh, n, torch.cuda.get_device_properties(dev).multi_processor_count).mode == NAMED_FUSED_MODES[(sw, sh, dw, dh)]
     src = np.stack([oracle.pattern_u8(sw * sh * 3, 77 + i).reshape(sh, sw, 3) for i in range(n)])
     scale, bias = scale_bias(oracle, kb)
     s = cu(src, dev)

@@ -215,17 +215,26 @@ def test_full_size_config3b_nv12_letterbox640(kb, oracle, dev, f16):
 
 
 # ── fused resize: every mode of fused_rows + the gather fallback, with the kernel named ─────
+# the mode each geometry below must reach, checked with the host mirror of the dispatcher (test_launch_shapes.fused_schedule)
+NAMED_FUSED_MODES = {(384, 216, 128, 72): "POINT", (384, 216, 192, 108): "BOX", (384, 216, 160, 90): "GENERAL", (384, 216, 384, 72): "POINT",
+                     (384, 216, 160, 72): "YZERO", (383, 216, 128, 72): "gather", (3840, 40, 512, 20): "gather"}
+
+
 @pytest.mark.parametrize("sw,sh,dw,dh,kernel", [
     (384, 216, 128, 72, "fused_rows_kernel"),      # 3:1 -> FR_POINT
     (384, 216, 192, 108, "fused_rows_kernel"),     # 2:1 -> FR_BOX
     (384, 216, 160, 90, "fused_rows_kernel"),      # 2.4:1 -> FR_GENERAL
-    (384, 216, 384, 72, "fused_rows_kernel"),      # y 3:1, x 1:1 -> FR_YZERO (x general)
+    (384, 216, 384, 72, "fused_rows_kernel"),      # y 3:1, x 1:1 -> FR_POINT (a 1:1 axis has all-zero weights too)
+    (384, 216, 160, 72, "fused_rows_kernel"),      # y 3:1, x 2.4:1 -> FR_YZERO (x general)
     (383, 216, 128, 72, "fused_resize_gather_kernel"),   # row_bytes % 16 != 0 -> gather fallback
     (3840, 40, 512, 20, "fused_resize_gather_kernel"),   # scale_x > 6 -> gather fallback
 ])
 @pytest.mark.parametrize("leaf", [0, 1])
 def test_fused_resize_modes_named(kb, oracle, dev, sw, sh, dw, dh, kernel, leaf):
+    from test_launch_shapes import fused_schedule
+
     n = 2
+    assert fused_schedule(sw, sh, dw, dh, n, torch.cuda.get_device_properties(dev).multi_processor_count).mode == NAMED_FUSED_MODES[(sw, sh, dw, dh)]
     src = np.stack([oracle.pattern_u8(sw * sh * 3, 77 + i).reshape(sh, sw, 3) for i in range(n)])
     scale, bias = oracle.normalize_params_from_mean_std(kb.IMAGENET_MEAN, kb.IMAGENET_STD)
     out = kb.imgproc.resize_normalize_to_tensor_u8_to_f32_bilinear(cu(src, dev), dw, dh, scale, bias, leaf=leaf)
