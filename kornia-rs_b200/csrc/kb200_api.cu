@@ -33,7 +33,7 @@ static const char*& last_kernel_ref() {
 
 static std::atomic<int> g_knobs[KNOB_COUNT];
 static const char* const g_knob_names[KNOB_COUNT] = {
-    "fr.npx", "fr.stages", "fr.ctas", "ss.stages", "ss.ctas", "ss.rc", "warp.pf", "warp.path",
+    "fr.npx", "fr.stages", "fr.ctas", "fr.rows", "ss.stages", "ss.ctas", "ss.rc", "warp.pf", "warp.path",
     "ws.stages", "ws.ctas", "ws.rc", "ws.npx", "rs.stages", "rs.ctas", "rs.npx", "a", "b", "c", "d"};
 int knob(Knob k) { return g_knobs[k].load(std::memory_order_relaxed); }
 

@@ -28,7 +28,8 @@ int check_launch(const char* what);  // cudaGetLastError() -> KB200_ERR_CUDA; re
 // Developer tuning knobs (kb200_debug_set_knob): process-wide integers the launchers consult instead of the
 // environment.  0 = "use the built-in choice".  Product code never needs them; sweeps and tests do.
 enum Knob {
-    KNOB_FR_NPX = 0, KNOB_FR_STAGES, KNOB_FR_CTAS,          // fused_rows (resize_fused.cu)
+    KNOB_FR_NPX = 0, KNOB_FR_STAGES, KNOB_FR_CTAS,          // fused_rows (resize_fused.cu), tiled schedule
+    KNOB_FR_ROWS,                                           // fused_rows point mode: 1 tiled, 2 full-row kernel
     KNOB_SS_STAGES, KNOB_SS_CTAS, KNOB_SS_RC,               // sep_filter_stream2 (filter.cu)
     KNOB_WARP_PF, KNOB_WARP_PATH,                           // warp.cu: prefetch rows (-1 = off); forced path (1 gather, 2 tiled, 3 stream)
     KNOB_WS_STAGES, KNOB_WS_CTAS, KNOB_WS_RC, KNOB_WS_NPX,  // warp_stream
