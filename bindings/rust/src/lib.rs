@@ -134,6 +134,8 @@ pub mod ffi {
         pub fn kb200_gray_from_rgb_u8(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, npixels: usize) -> c_int;
         pub fn kb200_rgb_from_nv12_u8(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, width: u32, height: u32, batch: u32) -> c_int;
         pub fn kb200_rgb_from_yuyv_u8(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, width: u32, height: u32, batch: u32) -> c_int;
+        pub fn kb200_rgb_from_yuv420_u8(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, width: u32, height: u32, batch: u32, layout: c_int) -> c_int;
+        pub fn kb200_rgb_from_yuv422_u8(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, width: u32, height: u32, batch: u32, layout: c_int) -> c_int;
         pub fn kb200_normalize_mean_std_f32(stream: *mut c_void, src: *const f32, dst: *mut f32, npixels: usize, channels: u32, mean: *const f32, std: *const f32) -> c_int;
         pub fn kb200_normalize_rgb_u8_f32(stream: *mut c_void, src: *const u8, dst: *mut f32, npixels: usize, scale: *const f32, offset: *const f32, leaf: c_int) -> c_int;
         pub fn kb200_find_min_max_f32(stream: *mut c_void, src: *const f32, n: usize, minmax_dev: *mut f32) -> c_int;
@@ -214,6 +216,29 @@ pub const LEAF_NEON: c_int = 2;
 pub const OUT_F32: c_int = 0;
 pub const OUT_F16: c_int = 1;
 pub const OUT_BF16: c_int = 2;
+
+/// `fmt` of `kb200_preprocess_desc` (kb200_src_fmt).  Codes 5-9 go beyond the reference's `SourceFormat`.
+pub const FMT_RGB: i32 = 0;
+pub const FMT_BGR: i32 = 1;
+pub const FMT_GRAY: i32 = 2;
+pub const FMT_NV12: i32 = 3;
+pub const FMT_YUYV: i32 = 4;
+pub const FMT_NV21: i32 = 5;
+pub const FMT_I420: i32 = 6;
+pub const FMT_YV12: i32 = 7;
+pub const FMT_UYVY: i32 = 8;
+pub const FMT_YVYU: i32 = 9;
+
+/// `layout` of `kb200_rgb_from_yuv420_u8` (kb200_yuv420_layout): the chroma after the Y plane.
+pub const YUV420_NV12: c_int = 0;
+pub const YUV420_NV21: c_int = 1;
+pub const YUV420_I420: c_int = 2;
+pub const YUV420_YV12: c_int = 3;
+
+/// `layout` of `kb200_rgb_from_yuv422_u8` (kb200_yuv422_layout): the byte order of each 2-pixel word.
+pub const YUV422_YUYV: c_int = 0;
+pub const YUV422_UYVY: c_int = 1;
+pub const YUV422_YVYU: c_int = 2;
 
 /// `PixelMapping` of cuda/resize.rs:441.
 #[derive(Debug, Clone, Copy, PartialEq, Eq)]

@@ -1,4 +1,5 @@
-// color.cu — gray_from_rgb (f32, u8) and the BT.601-limited Q20 video decoders (NV12, YUYV).
+// color.cu — gray_from_rgb (f32, u8) and the BT.601-limited Q20 video decoders (4:2:0: NV12, NV21, I420, YV12;
+// 4:2:2: YUYV, UYVY, YVYU).
 //
 // Reference: color/gray/kernels.rs (CPU), cuda/color/gray.rs:17-68 (GPU twin, 1 px or 4 px per
 // thread, scalar 4-byte accesses); color/yuv/kernels.rs:707-1069 (CPU), cuda/color/video.rs:33-130
@@ -130,8 +131,12 @@ __device__ __forceinline__ void store_rgb48_coalesced(uint4* __restrict__ warp_d
     stg_stream_u4(warp_dst + lane, a); stg_stream_u4(warp_dst + 32 + lane, b); stg_stream_u4(warp_dst + 64 + lane, c);
 }
 
-__global__ void __launch_bounds__(128) rgb_from_nv12_vec16(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst,
-                                                           uint32_t width, uint32_t height, size_t frame_bytes) {
+// One thread: 16 luma columns x 2 rows (one chroma row) — 16 B Y (top), 16 B Y (bottom) and the 8 chroma pairs: one
+// 16-B load of the interleaved row (NV12 / NV21), or 8 B of the U plane and 8 B of the V plane (I420 / YV12; with
+// width % 16 == 0 both planes and every thread's offset in them are 8-B aligned).
+template <int L>
+__global__ void __launch_bounds__(128) rgb_from_yuv420_vec16(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst,
+                                                             uint32_t width, uint32_t height, size_t frame_bytes) {
     __shared__ uint4 stage[4][96];
     const uint32_t gx = blockIdx.x * blockDim.x + threadIdx.x;  // 16-column group
     const uint32_t cy = blockIdx.y;                             // chroma row
@@ -143,18 +148,30 @@ __global__ void __launch_bounds__(128) rgb_from_nv12_vec16(const uint8_t* __rest
     const uint8_t* frame = src + (size_t)blockIdx.z * frame_bytes;
     uint8_t* out = dst + (size_t)blockIdx.z * (size_t)width * height * 3;
     const size_t x = (size_t)gx * 16;
-    uint4 yt = make_uint4(0, 0, 0, 0), yb = yt, uv = yt;
+    uint4 yt = make_uint4(0, 0, 0, 0), yb = yt, uv = yt;   // planar layouts: uv = {U bytes 0-7, V bytes 0-7}
     if (active) {
         yt = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + (size_t)(2 * cy) * width + x));
         yb = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + (size_t)(2 * cy + 1) * width + x));
-        uv = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + (size_t)width * height + (size_t)cy * width + x));
+        if (yuv420_planar(L)) {
+            const size_t c = (size_t)cy * (width / 2) + x / 2;
+            const uint2 u = ldg_stream_u2(reinterpret_cast<const uint2*>(frame + yuv420_u_plane(L, width, height) + c));
+            const uint2 v = ldg_stream_u2(reinterpret_cast<const uint2*>(frame + yuv420_v_plane(L, width, height) + c));
+            uv = make_uint4(u.x, u.y, v.x, v.y);
+        } else {
+            uv = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + (size_t)width * height + (size_t)cy * width + x));
+        }
     }
     const uint32_t uvw[4] = {uv.x, uv.y, uv.z, uv.w};
     ChromaTerms ct[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
-        const uint32_t pair = (uvw[k >> 1] >> (16 * (k & 1))) & 0xFFFFu;
-        ct[k] = chroma_terms((int)(pair & 0xFFu), (int)(pair >> 8));
+        if (yuv420_planar(L)) {
+            ct[k] = chroma_terms((int)((uvw[k >> 2] >> (8 * (k & 3))) & 0xFFu), (int)((uvw[2 + (k >> 2)] >> (8 * (k & 3))) & 0xFFu));
+        } else {
+            const uint32_t pair = (uvw[k >> 1] >> (16 * (k & 1))) & 0xFFFFu;
+            if (L == YUV420_NV21) ct[k] = chroma_terms((int)(pair >> 8), (int)(pair & 0xFFu));
+            else ct[k] = chroma_terms((int)(pair & 0xFFu), (int)(pair >> 8));
+        }
     }
     uint4 o[3];
     const uint32_t ytw[4] = {yt.x, yt.y, yt.z, yt.w};
@@ -175,14 +192,21 @@ __global__ void __launch_bounds__(128) rgb_from_nv12_vec16(const uint8_t* __rest
 }
 
 // Generic fallback (any even width / unaligned buffers): one thread per 2x2 block.
-__global__ void rgb_from_nv12_generic(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, uint32_t width,
-                                      uint32_t height, size_t frame_bytes) {
+template <int L>
+__global__ void rgb_from_yuv420_generic(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, uint32_t width,
+                                        uint32_t height, size_t frame_bytes) {
     const uint32_t cx = blockIdx.x * blockDim.x + threadIdx.x, cy = blockIdx.y * blockDim.y + threadIdx.y;
     if (cx >= width / 2 || cy >= height / 2) return;
     const uint8_t* frame = src + (size_t)blockIdx.z * frame_bytes;
     uint8_t* out = dst + (size_t)blockIdx.z * (size_t)width * height * 3;
-    const uint8_t* uvp = frame + (size_t)width * height + (size_t)cy * width + 2 * cx;
-    const ChromaTerms ct = chroma_terms(uvp[0], uvp[1]);
+    ChromaTerms ct;
+    if (yuv420_planar(L)) {
+        const size_t c = (size_t)cy * (width / 2) + cx;
+        ct = chroma_terms(frame[yuv420_u_plane(L, width, height) + c], frame[yuv420_v_plane(L, width, height) + c]);
+    } else {
+        const uint8_t* uvp = frame + (size_t)width * height + (size_t)cy * width + 2 * cx;
+        ct = L == YUV420_NV21 ? chroma_terms(uvp[1], uvp[0]) : chroma_terms(uvp[0], uvp[1]);
+    }
 #pragma unroll
     for (int dy = 0; dy < 2; ++dy)
 #pragma unroll
@@ -197,15 +221,24 @@ __global__ void rgb_from_nv12_generic(const uint8_t* __restrict__ src, uint8_t* 
 // ── YUYV → RGB8 ─────────────────────────────────────────────────────────────────────────────
 // One thread: 16 px = 32 B in (2 x LDG.128), 48 B out (3 x STG.128).  Flat over the whole batch
 // (rows are independent and tight), requires total px % 16 == 0 and aligned bases.
-__device__ __forceinline__ void yuyv_decode16(const uint4& A, const uint4& B, uint4 o[3]) {
-    const uint32_t g4[8] = {A.x, A.y, A.z, A.w, B.x, B.y, B.z, B.w};  // each word: Y0 U Y1 V
+// 4:2:2 layouts (kb200_yuv422_layout): each 2-px group is one 32-bit word; Yuv422Bytes<L> gives the byte of Y0, Y1,
+// U and V in it.  YUYV = Y0 U Y1 V, UYVY = U Y0 V Y1, YVYU = Y0 V Y1 U.
+static constexpr int YUV422_YUYV = KB200_YUV422_YUYV, YUV422_UYVY = KB200_YUV422_UYVY, YUV422_YVYU = KB200_YUV422_YVYU;
+template <int L> struct Yuv422Bytes { static constexpr int y0 = 0, y1 = 2, u = 1, v = 3; };
+template <> struct Yuv422Bytes<YUV422_UYVY> { static constexpr int y0 = 1, y1 = 3, u = 0, v = 2; };
+template <> struct Yuv422Bytes<YUV422_YVYU> { static constexpr int y0 = 0, y1 = 2, u = 3, v = 1; };
+
+template <int L>
+__device__ __forceinline__ void yuv422_decode16(const uint4& A, const uint4& B, uint4 o[3]) {
+    using P = Yuv422Bytes<L>;
+    const uint32_t g4[8] = {A.x, A.y, A.z, A.w, B.x, B.y, B.z, B.w};  // each word: one 2-px group
     uint32_t yw[4];
     ChromaTerms ct[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
         const uint32_t w = g4[k];
-        ct[k] = chroma_terms((int)((w >> 8) & 0xFFu), (int)(w >> 24));
-        const uint32_t ypair = __byte_perm(w, 0, 0x4420);   // {Y0, Y1, 0, 0}
+        ct[k] = chroma_terms((int)((w >> (8 * P::u)) & 0xFFu), (int)((w >> (8 * P::v)) & 0xFFu));
+        const uint32_t ypair = __byte_perm(w, 0, 0x4400 | (P::y1 << 4) | P::y0);   // {Y0, Y1, 0, 0}
         if (k & 1) yw[k >> 1] |= ypair << 16; else yw[k >> 1] = ypair;
     }
     pack_rgb16(yw, ct, o);
@@ -214,8 +247,9 @@ __device__ __forceinline__ void yuyv_decode16(const uint4& A, const uint4& B, ui
 // A warp owns 32 consecutive 16-px groups = 1024 B in, 1536 B out, both contiguous: the loads are issued
 // lane-contiguous (2 x LDG.128 per lane over the warp's run) and handed to their owners through shared memory, the
 // stores go back through it (store_rgb48_coalesced) — every global access instruction covers whole 128-B lines.
-__global__ void __launch_bounds__(256) rgb_from_yuyv_vec16(const uint4* __restrict__ src, uint4* __restrict__ dst,
-                                                           size_t ngroups) {
+template <int L>
+__global__ void __launch_bounds__(256) rgb_from_yuv422_vec16(const uint4* __restrict__ src, uint4* __restrict__ dst,
+                                                             size_t ngroups) {
     __shared__ uint4 stage[8][96];
     const uint32_t lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
     const size_t stride = (size_t)gridDim.x * blockDim.x;
@@ -228,26 +262,28 @@ __global__ void __launch_bounds__(256) rgb_from_yuyv_vec16(const uint4* __restri
             __syncwarp();
             const uint4 A = st[2 * lane], B = st[2 * lane + 1];
             __syncwarp();
-            yuyv_decode16(A, B, o);
+            yuv422_decode16<L>(A, B, o);
             store_rgb48_coalesced(dst + 3 * q0, st, lane, o);
         } else if (q0 + lane < ngroups) {   // ragged tail warp
             const size_t q = q0 + lane;
-            yuyv_decode16(ldg_stream_u4(src + 2 * q), ldg_stream_u4(src + 2 * q + 1), o);
+            yuv422_decode16<L>(ldg_stream_u4(src + 2 * q), ldg_stream_u4(src + 2 * q + 1), o);
             stg_stream_u4(dst + 3 * q, o[0]); stg_stream_u4(dst + 3 * q + 1, o[1]); stg_stream_u4(dst + 3 * q + 2, o[2]);
         }
     }
 }
 
-__global__ void rgb_from_yuyv_generic(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, size_t first_group,
-                                      size_t ngroups) {
+template <int L>
+__global__ void rgb_from_yuv422_generic(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, size_t first_group,
+                                        size_t ngroups) {
+    using P = Yuv422Bytes<L>;
     const size_t g = first_group + (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= ngroups) return;
     const uint8_t* s = src + 4 * g;
-    const ChromaTerms ct = chroma_terms(s[1], s[3]);
+    const ChromaTerms ct = chroma_terms(s[P::u], s[P::v]);
     int r, gg, b;
-    decode_rgb(yy_term(s[0]), ct, r, gg, b);
+    decode_rgb(yy_term(s[P::y0]), ct, r, gg, b);
     dst[6 * g] = (uint8_t)r; dst[6 * g + 1] = (uint8_t)gg; dst[6 * g + 2] = (uint8_t)b;
-    decode_rgb(yy_term(s[2]), ct, r, gg, b);
+    decode_rgb(yy_term(s[P::y1]), ct, r, gg, b);
     dst[6 * g + 3] = (uint8_t)r; dst[6 * g + 4] = (uint8_t)gg; dst[6 * g + 5] = (uint8_t)b;
 }
 
@@ -256,6 +292,32 @@ static inline unsigned stream_grid(size_t items, unsigned block, unsigned ctas_p
     const size_t cap = (size_t)device_info().sm_count * ctas_per_sm;
     return (unsigned)std::max<size_t>(1, std::min(want, cap));
 }
+
+// The kernels of each layout, indexed by kb200_yuv420_layout / kb200_yuv422_layout, and the names they report through
+// kb200_last_kernel().
+struct Yuv420Kernels {
+    const char* layout;
+    void (*vec16)(const uint8_t*, uint8_t*, uint32_t, uint32_t, size_t);
+    void (*generic)(const uint8_t*, uint8_t*, uint32_t, uint32_t, size_t);
+    const char *vec16_name, *generic_name;
+};
+static const Yuv420Kernels YUV420_KERNELS[4] = {
+    {"NV12", rgb_from_yuv420_vec16<YUV420_NV12>, rgb_from_yuv420_generic<YUV420_NV12>, "rgb_from_nv12_vec16", "rgb_from_nv12_generic"},
+    {"NV21", rgb_from_yuv420_vec16<YUV420_NV21>, rgb_from_yuv420_generic<YUV420_NV21>, "rgb_from_nv21_vec16", "rgb_from_nv21_generic"},
+    {"I420", rgb_from_yuv420_vec16<YUV420_I420>, rgb_from_yuv420_generic<YUV420_I420>, "rgb_from_i420_vec16", "rgb_from_i420_generic"},
+    {"YV12", rgb_from_yuv420_vec16<YUV420_YV12>, rgb_from_yuv420_generic<YUV420_YV12>, "rgb_from_yv12_vec16", "rgb_from_yv12_generic"},
+};
+struct Yuv422Kernels {
+    const char* layout;
+    void (*vec16)(const uint4*, uint4*, size_t);
+    void (*generic)(const uint8_t*, uint8_t*, size_t, size_t);
+    const char *vec16_name, *generic_name;
+};
+static const Yuv422Kernels YUV422_KERNELS[3] = {
+    {"YUYV", rgb_from_yuv422_vec16<YUV422_YUYV>, rgb_from_yuv422_generic<YUV422_YUYV>, "rgb_from_yuyv_vec16", "rgb_from_yuyv_generic"},
+    {"UYVY", rgb_from_yuv422_vec16<YUV422_UYVY>, rgb_from_yuv422_generic<YUV422_UYVY>, "rgb_from_uyvy_vec16", "rgb_from_uyvy_generic"},
+    {"YVYU", rgb_from_yuv422_vec16<YUV422_YVYU>, rgb_from_yuv422_generic<YUV422_YVYU>, "rgb_from_yvyu_vec16", "rgb_from_yvyu_generic"},
+};
 
 // ── RGB8 → YUYV / NV12 encode (SURVEY §8(f) #4) ─────────────────────────────────────────────
 // color/yuv/kernels.rs:1223-1252: Q8 BT.601 limited — Y = ((66R + 129G + 25B + 128) >> 8) + 16,
@@ -353,11 +415,13 @@ KB200_API int kb200_gray_from_rgb_u8(kb200_stream_t stream, const uint8_t* src, 
     return KB200_OK;
 }
 
-KB200_API int kb200_rgb_from_nv12_u8(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst,
-                                     size_t dst_len, uint32_t width, uint32_t height, uint32_t batch) {
+KB200_API int kb200_rgb_from_yuv420_u8(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst,
+                                       size_t dst_len, uint32_t width, uint32_t height, uint32_t batch, int layout) {
     KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
+    if (layout < KB200_YUV420_NV12 || layout > KB200_YUV420_YV12) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown 4:2:0 layout %d", layout);
+    const Yuv420Kernels& k = YUV420_KERNELS[layout];
     KB200_TRY(check_geometry(width, height, width, height, batch));
-    if ((width & 1u) || (height & 1u)) return fail(KB200_ERR_INVALID_ARGUMENT, "NV12 needs even dimensions, got %ux%u", width, height);
+    if ((width & 1u) || (height & 1u)) return fail(KB200_ERR_INVALID_ARGUMENT, "%s needs even dimensions, got %ux%u", k.layout, width, height);
     if (batch > 65535u) return fail(KB200_ERR_INVALID_ARGUMENT, "batch %u exceeds 65535", batch);
     const size_t frame = (size_t)width * height * 3 / 2, out_frame = (size_t)width * height * 3;
     KB200_TRY(check_slice("src", src_len, frame * batch)); KB200_TRY(check_slice("dst", dst_len, out_frame * batch));
@@ -366,19 +430,21 @@ KB200_API int kb200_rgb_from_nv12_u8(kb200_stream_t stream, const uint8_t* src, 
         const unsigned groups = width / 16;
         const unsigned bx = groups >= 128 ? 128 : 32 * ((groups + 31) / 32);
         dim3 grid(div_up(groups, bx), height / 2, batch);
-        rgb_from_nv12_vec16<<<grid, bx, 0, s>>>(src, dst, width, height, frame);
-        return check_launch("rgb_from_nv12_vec16");
+        k.vec16<<<grid, bx, 0, s>>>(src, dst, width, height, frame);
+        return check_launch(k.vec16_name);
     }
     dim3 block(32, 8), grid(div_up(width / 2, 32), div_up(height / 2, 8), batch);
-    rgb_from_nv12_generic<<<grid, block, 0, s>>>(src, dst, width, height, frame);
-    return check_launch("rgb_from_nv12_generic");
+    k.generic<<<grid, block, 0, s>>>(src, dst, width, height, frame);
+    return check_launch(k.generic_name);
 }
 
-KB200_API int kb200_rgb_from_yuyv_u8(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst,
-                                     size_t dst_len, uint32_t width, uint32_t height, uint32_t batch) {
+KB200_API int kb200_rgb_from_yuv422_u8(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst,
+                                       size_t dst_len, uint32_t width, uint32_t height, uint32_t batch, int layout) {
     KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
+    if (layout < KB200_YUV422_YUYV || layout > KB200_YUV422_YVYU) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown 4:2:2 layout %d", layout);
+    const Yuv422Kernels& k = YUV422_KERNELS[layout];
     KB200_TRY(check_geometry(width, height, width, height, batch));
-    if (width & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "YUYV needs an even width, got %u", width);
+    if (width & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "%s needs an even width, got %u", k.layout, width);
     const size_t npx = (size_t)width * height * batch;
     KB200_TRY(check_slice("src", src_len, npx * 2)); KB200_TRY(check_slice("dst", dst_len, npx * 3));
     cudaStream_t s = as_stream(stream);
@@ -387,17 +453,26 @@ KB200_API int kb200_rgb_from_yuyv_u8(kb200_stream_t stream, const uint8_t* src, 
     if (aligned16(src) && aligned16(dst)) {
         const size_t n16 = npx / 16;
         if (n16) {
-            rgb_from_yuyv_vec16<<<stream_grid(n16, 256, 8), 256, 0, s>>>(reinterpret_cast<const uint4*>(src),
-                                                                        reinterpret_cast<uint4*>(dst), n16);
-            KB200_TRY(check_launch("rgb_from_yuyv_vec16"));
+            k.vec16<<<stream_grid(n16, 256, 8), 256, 0, s>>>(reinterpret_cast<const uint4*>(src), reinterpret_cast<uint4*>(dst), n16);
+            KB200_TRY(check_launch(k.vec16_name));
         }
         done = n16 * 8;
     }
     if (done < ngroups2) {
-        rgb_from_yuyv_generic<<<div_up(ngroups2 - done, 256), 256, 0, s>>>(src, dst, done, ngroups2);
-        KB200_TRY(check_launch("rgb_from_yuyv_generic"));
+        k.generic<<<div_up(ngroups2 - done, 256), 256, 0, s>>>(src, dst, done, ngroups2);
+        KB200_TRY(check_launch(k.generic_name));
     }
     return KB200_OK;
+}
+
+KB200_API int kb200_rgb_from_nv12_u8(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst,
+                                     size_t dst_len, uint32_t width, uint32_t height, uint32_t batch) {
+    return kb200_rgb_from_yuv420_u8(stream, src, src_len, dst, dst_len, width, height, batch, KB200_YUV420_NV12);
+}
+
+KB200_API int kb200_rgb_from_yuyv_u8(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst,
+                                     size_t dst_len, uint32_t width, uint32_t height, uint32_t batch) {
+    return kb200_rgb_from_yuv422_u8(stream, src, src_len, dst, dst_len, width, height, batch, KB200_YUV422_YUYV);
 }
 
 

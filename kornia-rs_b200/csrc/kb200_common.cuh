@@ -85,6 +85,15 @@ inline unsigned div_up(size_t a, size_t b) { return (unsigned)((a + b - 1) / b);
 // ── device helpers ──────────────────────────────────────────────────────────────────────────
 #ifdef __CUDACC__
 
+// 4:2:0 layouts (kb200_yuv420_layout): one tight w*h*3/2 buffer, Y plane first.  NV12 / NV21 interleave the chroma
+// (U V / V U) at a w-byte row stride; I420 / YV12 store two (w/2 x h/2) planes, U then V / V then U.
+static constexpr int YUV420_NV12 = KB200_YUV420_NV12, YUV420_NV21 = KB200_YUV420_NV21, YUV420_I420 = KB200_YUV420_I420,
+                     YUV420_YV12 = KB200_YUV420_YV12;
+__host__ __device__ constexpr bool yuv420_planar(int L) { return L == YUV420_I420 || L == YUV420_YV12; }
+// byte offsets of the U and V planes of a planar frame (w, h even)
+__host__ __device__ inline size_t yuv420_u_plane(int L, size_t w, size_t h) { return L == YUV420_I420 ? w * h : w * h + w * h / 4; }
+__host__ __device__ inline size_t yuv420_v_plane(int L, size_t w, size_t h) { return L == YUV420_I420 ? w * h + w * h / 4 : w * h; }
+
 // Streaming (read-once / write-once) vector accesses: keep L1 for the gather taps.
 __device__ __forceinline__ float4 ldg_stream_f4(const float4* p) {
     float4 v;

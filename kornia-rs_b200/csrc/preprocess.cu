@@ -1,6 +1,7 @@
 // preprocess.cu — the fused camera preprocess (a12; BASELINE config 3): raw frame (RGB/BGR/RGBA/
-// Gray/NV12/YUYV, tight or pitched) → letterbox/stretch resample → (v/255 - mean) * inv_std →
-// planar CHW f32 or f16, for a whole batch in ONE launch.
+// Gray/NV12/YUYV, tight or pitched; beyond the reference also NV21/I420/YV12/UYVY/YVYU) → letterbox/stretch
+// resample → (v/255 - mean) * inv_std → planar CHW f32 or f16, for a whole batch in ONE launch.
+// The 4:2:0 formats share the NV12 kernels (templated on the chroma layout); the 4:2:2 formats take the generic kernel.
 //
 // Reference: preprocess.rs:430-647 (the CUDA source string — the specification of this path; there
 // is no CPU implementation for the camera formats), launch seam :1324-1372, batch loop :1277-1280
@@ -70,9 +71,33 @@ __device__ __forceinline__ void yuv_to_rgbf(int yv, int u, int v, float px[3]) {
     px[0] = (float)r; px[1] = (float)g; px[2] = (float)b;
 }
 
+// fmt 5-9, the YUV layouts beyond the reference's SourceFormat: the chroma addressing of the standalone decoders (color.cu)
+__device__ __forceinline__ void fetch_px_yuv_ext(const uint8_t* __restrict__ src, int x, int y, const kb200_preprocess_desc& d,
+                                                 float px[3]) {
+    if (d.fmt == KB200_FMT_UYVY || d.fmt == KB200_FMT_YVYU) {
+        const uint8_t* grp = src + (long long)y * d.src_pitch + (x >> 1) * 4;
+        if (d.fmt == KB200_FMT_UYVY) yuv_to_rgbf(grp[(x & 1) ? 3 : 1], grp[0], grp[2], px);   // U Y0 V Y1
+        else yuv_to_rgbf(grp[(x & 1) ? 2 : 0], grp[3], grp[1], px);                           // Y0 V Y1 U
+        return;
+    }
+    const int yv = src[(long long)y * d.src_w + x];
+    if (d.fmt == KB200_FMT_NV21) {
+        const uint8_t* vu = src + (long long)d.src_w * d.src_h + (long long)(y >> 1) * d.src_w + (x >> 1) * 2;
+        yuv_to_rgbf(yv, vu[1], vu[0], px);
+    } else {
+        const int L = d.fmt == KB200_FMT_I420 ? YUV420_I420 : YUV420_YV12;
+        const size_t c = (size_t)(y >> 1) * (d.src_w >> 1) + (x >> 1);
+        yuv_to_rgbf(yv, src[yuv420_u_plane(L, d.src_w, d.src_h) + c], src[yuv420_v_plane(L, d.src_w, d.src_h) + c], px);
+    }
+}
+
+// EXT_YUV: the frame is one of fmt 5-9 (a separate instantiation, so the kernels of fmt 0-4 are unchanged by them)
+template <bool EXT_YUV>
 __device__ __forceinline__ void fetch_px(const uint8_t* __restrict__ src, int x, int y, const kb200_preprocess_desc& d,
                                          float px[3]) {  // :510-530
-    if (d.fmt <= 1) {
+    if (EXT_YUV) {
+        fetch_px_yuv_ext(src, x, y, d, px);
+    } else if (d.fmt <= 1) {
         const uint8_t* p = src + (long long)y * d.src_pitch + x * d.src_bpp;
         if (d.fmt == 0) { px[0] = (float)p[0]; px[1] = (float)p[1]; px[2] = (float)p[2]; }
         else { px[0] = (float)p[2]; px[1] = (float)p[1]; px[2] = (float)p[0]; }
@@ -100,7 +125,7 @@ __device__ __forceinline__ float pre_lanczos_w(float dd) {
 }
 
 // SAMP: kb200_interp — 0 nearest, 1 bilinear, 3 Lanczos-3 (6x6 taps, clamp-to-edge, weights renormalised by their sum)
-template <bool F16, int SAMP, bool PTRS>
+template <bool F16, int SAMP, bool PTRS, bool EXT_YUV>
 __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                  const __grid_constant__ PreFrames fr, void* __restrict__ dst,
                                                                  uint32_t frame0) {
@@ -127,7 +152,7 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
                     const float w = wy * pre_lanczos_w(sx - (float)xi);
                     const int xc = min(max(xi, 0), d.src_w - 1);
                     float t[3];
-                    fetch_px(src, xc, yc, d, t);
+                    fetch_px<EXT_YUV>(src, xc, yc, d, t);
                     acc0 += w * t[0]; acc1 += w * t[1]; acc2 += w * t[2];
                     wsum += w;
                 }
@@ -139,12 +164,12 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
             const int x1 = min(x0 + 1, d.src_w - 1), y1 = min(y0 + 1, d.src_h - 1);
             x0 = max(x0, 0); y0 = max(y0, 0);
             float t00[3], t10[3], t01[3], t11[3];
-            fetch_px(src, x0, y0, d, t00);
+            fetch_px<EXT_YUV>(src, x0, y0, d, t00);
             const bool need_x = ax != 0.0f, need_y = ay != 0.0f;
-            if (need_x) fetch_px(src, x1, y0, d, t10);
+            if (need_x) fetch_px<EXT_YUV>(src, x1, y0, d, t10);
             if (need_y) {
-                fetch_px(src, x0, y1, d, t01);
-                if (need_x) fetch_px(src, x1, y1, d, t11);
+                fetch_px<EXT_YUV>(src, x0, y1, d, t01);
+                if (need_x) fetch_px<EXT_YUV>(src, x1, y1, d, t11);
             }
 #pragma unroll
             for (int c = 0; c < 3; ++c) {
@@ -159,7 +184,7 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
         } else {
             const int xn = min(max((int)roundf(sx), 0), d.src_w - 1);
             const int yn = min(max((int)roundf(sy), 0), d.src_h - 1);
-            fetch_px(src, xn, yn, d, px);
+            fetch_px<EXT_YUV>(src, xn, yn, d, px);
         }
     } else {
         px[0] = d.pad_value; px[1] = d.pad_value; px[2] = d.pad_value;
@@ -215,10 +240,12 @@ __device__ __forceinline__ float norm_int_px(int r, float m, float is) { return 
 // warp), 6 x STG.128 (512 contiguous bytes per warp per plane row).  [The first version gave each thread 8
 // columns = two STG.128 per plane row; each store instruction then wrote only half of every 32-B sector and
 // ncu showed 2x the write sectors at L2 (lts__t_sectors_srcunit_tex_op_write).]
-template <bool F16, bool PTRS>
-__global__ void __launch_bounds__(128) preprocess_nv12_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
-                                                                       const __grid_constant__ PreFrames fr, void* __restrict__ dst,
-                                                                       uint32_t frame0, uint32_t groups_per_row, uint32_t items) {
+// The other 4:2:0 layouts (L, kb200_yuv420_layout) take this kernel too: NV21 loads the same 4 chroma bytes and swaps
+// each pair; I420 / YV12 load 2 U bytes and 2 V bytes (LDG.16 each; w % 4 == 0 keeps them 2-B aligned).
+template <bool F16, bool PTRS, int L>
+__global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
+                                                                         const __grid_constant__ PreFrames fr, void* __restrict__ dst,
+                                                                         uint32_t frame0, uint32_t groups_per_row, uint32_t items) {
     const uint32_t item = blockIdx.x * blockDim.x + threadIdx.x;
     if (item >= items) return;
     const uint32_t rp = item / groups_per_row, g = item - rp * groups_per_row;
@@ -228,10 +255,23 @@ __global__ void __launch_bounds__(128) preprocess_nv12_identity_kernel(const __g
     const uint32_t x = g * 4u;
     const uint32_t y0w = __ldg(reinterpret_cast<const uint32_t*>(src + (size_t)(2u * rp) * w + x));
     const uint32_t y1w = __ldg(reinterpret_cast<const uint32_t*>(src + (size_t)(2u * rp + 1u) * w + x));
-    const uint32_t uvw = __ldg(reinterpret_cast<const uint32_t*>(src + (size_t)w * h + (size_t)rp * w + x));
     ChromaTerms ct[2];
-    ct[0] = chroma_terms((int)(uvw & 0xFFu), (int)((uvw >> 8) & 0xFFu));
-    ct[1] = chroma_terms((int)((uvw >> 16) & 0xFFu), (int)(uvw >> 24));
+    if (yuv420_planar(L)) {
+        const size_t c = (size_t)rp * (w / 2u) + x / 2u;
+        const uint32_t u2 = __ldg(reinterpret_cast<const unsigned short*>(src + yuv420_u_plane(L, w, h) + c));
+        const uint32_t v2 = __ldg(reinterpret_cast<const unsigned short*>(src + yuv420_v_plane(L, w, h) + c));
+        ct[0] = chroma_terms((int)(u2 & 0xFFu), (int)(v2 & 0xFFu));
+        ct[1] = chroma_terms((int)(u2 >> 8), (int)(v2 >> 8));
+    } else {
+        const uint32_t uvw = __ldg(reinterpret_cast<const uint32_t*>(src + (size_t)w * h + (size_t)rp * w + x));
+        if (L == YUV420_NV21) {
+            ct[0] = chroma_terms((int)((uvw >> 8) & 0xFFu), (int)(uvw & 0xFFu));
+            ct[1] = chroma_terms((int)(uvw >> 24), (int)((uvw >> 16) & 0xFFu));
+        } else {
+            ct[0] = chroma_terms((int)(uvw & 0xFFu), (int)((uvw >> 8) & 0xFFu));
+            ct[1] = chroma_terms((int)((uvw >> 16) & 0xFFu), (int)(uvw >> 24));
+        }
+    }
     const size_t plane = (size_t)w * h;
     const size_t base = (size_t)(frame0 + f) * 3 * plane + (size_t)(2u * rp) * w + x;
     const float m0 = d.mean[0], m1 = d.mean[1], m2 = d.mean[2], i0 = d.inv_std[0], i1 = d.inv_std[1], i2 = d.inv_std[2];
@@ -269,19 +309,27 @@ struct Nv12Args {
     uint32_t groups;    // ceil(dst_w / 4)
 };
 
-__device__ __forceinline__ void nv12_tap(const uint8_t* __restrict__ src, int x, int y, int w, int h, int rgb[3]) {
+// One decoded tap of a 4:2:0 frame in layout L (kb200_yuv420_layout): the kernel below serves all four layouts.
+template <int L>
+__device__ __forceinline__ void yuv420_tap(const uint8_t* __restrict__ src, int x, int y, int w, int h, int rgb[3]) {
     const int yv = __ldg(src + (size_t)y * w + x);
-    const uint32_t uv = __ldg(reinterpret_cast<const unsigned short*>(src + (size_t)w * h + (size_t)(y >> 1) * w + (x >> 1) * 2));
-    const ChromaTerms t = chroma_terms((int)(uv & 0xFFu), (int)(uv >> 8));
+    ChromaTerms t;
+    if (yuv420_planar(L)) {
+        const size_t c = (size_t)(y >> 1) * (w >> 1) + (x >> 1);
+        t = chroma_terms(__ldg(src + yuv420_u_plane(L, w, h) + c), __ldg(src + yuv420_v_plane(L, w, h) + c));
+    } else {
+        const uint32_t uv = __ldg(reinterpret_cast<const unsigned short*>(src + (size_t)w * h + (size_t)(y >> 1) * w + (x >> 1) * 2));
+        t = L == YUV420_NV21 ? chroma_terms((int)(uv >> 8), (int)(uv & 0xFFu)) : chroma_terms((int)(uv & 0xFFu), (int)(uv >> 8));
+    }
     decode_rgb(yy_term(yv), t, rgb[0], rgb[1], rgb[2]);
 }
 
 static constexpr int NV12_ROWS = 8;  // destination rows per thread: the x-side of the sampler is computed once for all of them
 
-template <bool F16, bool BILINEAR, bool PTRS>
-__global__ void __launch_bounds__(128) preprocess_nv12_kernel(const __grid_constant__ kb200_preprocess_desc d,
-                                                              const __grid_constant__ PreFrames fr, const __grid_constant__ Nv12Args na,
-                                                              void* __restrict__ dst, uint32_t frame0) {
+template <bool F16, bool BILINEAR, bool PTRS, int L>
+__global__ void __launch_bounds__(128) preprocess_yuv420_kernel(const __grid_constant__ kb200_preprocess_desc d,
+                                                                const __grid_constant__ PreFrames fr, const __grid_constant__ Nv12Args na,
+                                                                void* __restrict__ dst, uint32_t frame0) {
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= na.groups) return;
     const uint32_t f = blockIdx.z;
@@ -337,17 +385,17 @@ __global__ void __launch_bounds__(128) preprocess_nv12_kernel(const __grid_const
             for (int j = 0; j < 4; ++j) {
                 if (!xin[j]) { o[0][j] = na.pad_norm[0]; o[1][j] = na.pad_norm[1]; o[2][j] = na.pad_norm[2]; continue; }
                 int t00[3];
-                nv12_tap(src, xa[j], y0, w, h, t00);
+                yuv420_tap<L>(src, xa[j], y0, w, h, t00);
                 const bool need_x = BILINEAR && ax[j] != 0.0f;
                 float px[3];
                 if (!need_x && !need_y) {  // the sample IS the decoded tap (exact, see header)
                     px[0] = (float)t00[0]; px[1] = (float)t00[1]; px[2] = (float)t00[2];
                 } else {
                     int t10[3] = {0, 0, 0}, t01[3] = {0, 0, 0}, t11[3] = {0, 0, 0};
-                    if (need_x) nv12_tap(src, xb[j], y0, w, h, t10);
+                    if (need_x) yuv420_tap<L>(src, xb[j], y0, w, h, t10);
                     if (need_y) {
-                        nv12_tap(src, xa[j], y1, w, h, t01);
-                        if (need_x) nv12_tap(src, xb[j], y1, w, h, t11);
+                        yuv420_tap<L>(src, xa[j], y1, w, h, t01);
+                        if (need_x) yuv420_tap<L>(src, xb[j], y1, w, h, t11);
                     }
 #pragma unroll
                     for (int c = 0; c < 3; ++c) {
@@ -373,8 +421,23 @@ __global__ void __launch_bounds__(128) preprocess_nv12_kernel(const __grid_const
     }
 }
 
+// fmt -> kb200_yuv420_layout, or -1 for the formats that are not 4:2:0
+static int yuv420_layout(int fmt) {
+    switch (fmt) {
+        case KB200_FMT_NV12: return YUV420_NV12;
+        case KB200_FMT_NV21: return YUV420_NV21;
+        case KB200_FMT_I420: return YUV420_I420;
+        case KB200_FMT_YV12: return YUV420_YV12;
+        default: return -1;
+    }
+}
+static bool is_yuv422(int fmt) { return fmt == KB200_FMT_YUYV || fmt == KB200_FMT_UYVY || fmt == KB200_FMT_YVYU; }
+// SourceFormat names, in the validation messages
+static const char* const FMT_NAMES[10] = {"Rgb8", "Bgr8", "Gray8", "Nv12", "Yuyv", "Nv21", "I420", "Yv12", "Uyvy", "Yvyu"};
+static const char* const YUV420_UPPER[4] = {"NV12", "NV21", "I420", "YV12"};
+
 static size_t src_bytes(const kb200_preprocess_desc& d) {
-    const size_t chroma = d.fmt == KB200_FMT_NV12 ? (size_t)d.src_w * d.src_h / 2 : 0;
+    const size_t chroma = yuv420_layout(d.fmt) >= 0 ? (size_t)d.src_w * d.src_h / 2 : 0;
     return (size_t)d.src_pitch * d.src_h + chroma;
 }
 
@@ -384,28 +447,59 @@ static int validate_desc(const kb200_preprocess_desc* dp) {
     if (d.src_w <= 0 || d.src_h <= 0 || d.dst_w <= 0 || d.dst_h <= 0)
         return fail(KB200_ERR_INVALID_ARGUMENT, "image dimensions must be non-zero");
     if ((long long)d.dst_w * d.dst_h > 0x7FFFFFFFll) return fail(KB200_ERR_DIMS_TOO_LARGE, "dimensions exceed the 32-bit CUDA kernel index limit");  // :1336-1339
-    if (d.fmt < 0 || d.fmt > 4) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown source format code %d", d.fmt);
+    if (d.fmt < 0 || d.fmt > KB200_FMT_YVYU) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown source format code %d", d.fmt);
     if (d.sampling != KB200_INTERP_NEAREST && d.sampling != KB200_INTERP_BILINEAR && d.sampling != KB200_INTERP_LANCZOS)
         return fail(KB200_ERR_UNSUPPORTED, "unsupported sampling mode %d (expected Nearest, Bilinear or Lanczos)", d.sampling);  // preprocess.rs:1044-1051
     if (d.fmt <= 1 && d.src_bpp != 3 && d.src_bpp != 4) return fail(KB200_ERR_UNSUPPORTED, "unsupported source channel count %d (expected 3 or 4)", d.src_bpp);
     // SourceFormat::dims_ok :188-195 ; pitch covers a row (PitchedSurface::validate :829-842)
-    if (d.fmt == KB200_FMT_NV12 && ((d.src_w | d.src_h) & 1)) return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for Nv12 at %dx%d (even dimensions required)", d.src_w, d.src_h);
-    if (d.fmt == KB200_FMT_YUYV && (d.src_w & 1)) return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for Yuyv at %dx%d (even width required)", d.src_w, d.src_h);
-    const int bpp = d.fmt <= 1 ? d.src_bpp : (d.fmt == KB200_FMT_YUYV ? 2 : 1);
+    const int l420 = yuv420_layout(d.fmt);
+    if (l420 >= 0 && ((d.src_w | d.src_h) & 1)) return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s at %dx%d (even dimensions required)", FMT_NAMES[d.fmt], d.src_w, d.src_h);
+    if (is_yuv422(d.fmt) && (d.src_w & 1)) return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s at %dx%d (even width required)", FMT_NAMES[d.fmt], d.src_w, d.src_h);
+    const int bpp = d.fmt <= 1 ? d.src_bpp : (is_yuv422(d.fmt) ? 2 : 1);
     if ((long long)d.src_pitch < (long long)d.src_w * bpp) return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface (need pitch >= width*channels and len >= pitch*height)");
-    if (d.fmt == KB200_FMT_NV12 && d.src_pitch != d.src_w) return fail(KB200_ERR_INVALID_SOURCE, "NV12 frames must be tightly packed (pitch == width)");
+    if (l420 >= 0 && d.src_pitch != d.src_w) return fail(KB200_ERR_INVALID_SOURCE, "%s frames must be tightly packed (pitch == width)", YUV420_UPPER[l420]);
     if (!(d.scale_x > 0.0f) || !(d.scale_y > 0.0f)) return fail(KB200_ERR_INVALID_ARGUMENT, "scale must be positive");
     return KB200_OK;
 }
+
+// The 4:2:0 fast kernels of layout L, for one launch of <= 256 frames.
+template <bool F16, int L>
+static void launch_yuv420_fast(cudaStream_t s, bool identity, bool bil, const kb200_preprocess_desc& d, const PreFrames& fr, bool ptrs,
+                               const Nv12Args& nv, void* dst, uint32_t f0, uint32_t nb, uint32_t id_groups, size_t id_items) {
+    if (identity) {
+        dim3 grid(div_up(id_items, 128), nb);
+        if (ptrs) preprocess_yuv420_identity_kernel<F16, true, L><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
+        else preprocess_yuv420_identity_kernel<F16, false, L><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
+        return;
+    }
+    dim3 grid(div_up(nv.groups, 128), div_up((size_t)d.dst_h, NV12_ROWS), nb);
+#define KB200_YUV420_LAUNCH(BIL, PT) preprocess_yuv420_kernel<F16, BIL, PT, L><<<grid, 128, 0, s>>>(d, fr, nv, dst, f0)
+    if (bil) { if (ptrs) KB200_YUV420_LAUNCH(true, true); else KB200_YUV420_LAUNCH(true, false); }
+    else     { if (ptrs) KB200_YUV420_LAUNCH(false, true); else KB200_YUV420_LAUNCH(false, false); }
+#undef KB200_YUV420_LAUNCH
+}
+
+template <bool F16, bool PTRS, bool EXT_YUV>
+static void launch_generic(cudaStream_t s, dim3 grid, int sampling, const kb200_preprocess_desc& d, const PreFrames& fr, void* dst, uint32_t f0) {
+    if (sampling == KB200_INTERP_LANCZOS) preprocess_generic_kernel<F16, KB200_INTERP_LANCZOS, PTRS, EXT_YUV><<<grid, 256, 0, s>>>(d, fr, dst, f0);
+    else if (sampling == KB200_INTERP_BILINEAR) preprocess_generic_kernel<F16, KB200_INTERP_BILINEAR, PTRS, EXT_YUV><<<grid, 256, 0, s>>>(d, fr, dst, f0);
+    else preprocess_generic_kernel<F16, KB200_INTERP_NEAREST, PTRS, EXT_YUV><<<grid, 256, 0, s>>>(d, fr, dst, f0);
+}
+
+// kb200_last_kernel() names of the 4:2:0 fast kernels, by layout
+static const char* const YUV420_IDENTITY_NAMES[4] = {"preprocess_nv12_identity_kernel", "preprocess_nv21_identity_kernel",
+                                                     "preprocess_i420_identity_kernel", "preprocess_yv12_identity_kernel"};
+static const char* const YUV420_FAST_NAMES[4] = {"preprocess_nv12_kernel", "preprocess_nv21_kernel", "preprocess_i420_kernel", "preprocess_yv12_kernel"};
 
 template <bool F16>
 static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, const uint8_t* const* frames,
                              const uint8_t* base, size_t stride, uint32_t batch, void* dst) {
     const int pixels = d.dst_w * d.dst_h;
     const bool bil = d.sampling == KB200_INTERP_BILINEAR, lanczos = d.sampling == KB200_INTERP_LANCZOS;
-    // identity fast path: NV12, scale 1, no pad, same size, 8-column vectors possible
+    const int l420 = yuv420_layout(d.fmt);
+    // identity fast path: a 4:2:0 format, scale 1, no pad, same size, 8-column vectors possible
     // (Lanczos always takes the generic kernel: its off-centre weights at integer coordinates are sinf(k*pi) != 0 exactly)
-    bool identity = !lanczos && d.fmt == KB200_FMT_NV12 && d.scale_x == 1.0f && d.scale_y == 1.0f && d.pad_x == 0.0f && d.pad_y == 0.0f &&
+    bool identity = !lanczos && l420 >= 0 && d.scale_x == 1.0f && d.scale_y == 1.0f && d.pad_x == 0.0f && d.pad_y == 0.0f &&
                     d.dst_w == d.src_w && d.dst_h == d.src_h && (d.src_w % 4) == 0 && aligned16(dst);
     if (identity) {
         if (frames) { for (uint32_t k = 0; k < batch; ++k) identity = identity && ((reinterpret_cast<uintptr_t>(frames[k]) & 3u) == 0); }
@@ -414,8 +508,9 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
     const uint32_t id_groups = (uint32_t)d.src_w / 4u;
     const size_t id_items = (size_t)id_groups * ((size_t)d.src_h / 2);
     if (id_items > 0x7FFFFFFFull) identity = false;
-    // NV12 general fast path: vector stores need dst_w % 4 == 0 and a 16-B (f32) / 8-B (f16) aligned destination
-    const bool nv12_fast = !lanczos && d.fmt == KB200_FMT_NV12 && (d.dst_w % 4) == 0 && aligned16(dst) && d.dst_h <= 65535 * NV12_ROWS;
+    // 4:2:0 general fast path: vector stores need dst_w % 4 == 0 and a 16-B (f32) / 8-B (f16) aligned destination
+    const bool yuv420_fast = !lanczos && l420 >= 0 && (d.dst_w % 4) == 0 && aligned16(dst) && d.dst_h <= 65535 * NV12_ROWS;
+    const bool ext_yuv = d.fmt >= KB200_FMT_NV21;
     Nv12Args nv{};
     nv.groups = (uint32_t)(d.dst_w + 3) / 4u;
     for (int c = 0; c < 3; ++c) nv.pad_norm[c] = (d.pad_value / 255.0f - d.mean[c]) * d.inv_std[c];  // BODY :610-612 on the host (f32, unfused)
@@ -424,32 +519,20 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
         PreFrames fr{};
         fr.base = base; fr.stride = stride;
         if (frames) for (uint32_t k = 0; k < nb; ++k) fr.ptr[k] = frames[f0 + k];
-        if (identity) {
-            dim3 grid(div_up(id_items, 128), nb);
-            if (frames) preprocess_nv12_identity_kernel<F16, true><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
-            else preprocess_nv12_identity_kernel<F16, false><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
-            KB200_TRY(check_launch("preprocess_nv12_identity_kernel"));
-            continue;
-        }
-        if (nv12_fast) {
-            dim3 grid(div_up(nv.groups, 128), div_up((size_t)d.dst_h, NV12_ROWS), nb);
-#define KB200_NV12_LAUNCH(BIL, PT) preprocess_nv12_kernel<F16, BIL, PT><<<grid, 128, 0, s>>>(d, fr, nv, dst, f0)
-            if (bil) { if (frames) KB200_NV12_LAUNCH(true, true); else KB200_NV12_LAUNCH(true, false); }
-            else     { if (frames) KB200_NV12_LAUNCH(false, true); else KB200_NV12_LAUNCH(false, false); }
-#undef KB200_NV12_LAUNCH
-            KB200_TRY(check_launch("preprocess_nv12_kernel"));
+        if (identity || yuv420_fast) {
+            const bool p = frames != nullptr;
+            switch (l420) {
+                case YUV420_NV12: launch_yuv420_fast<F16, YUV420_NV12>(s, identity, bil, d, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                case YUV420_NV21: launch_yuv420_fast<F16, YUV420_NV21>(s, identity, bil, d, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                case YUV420_I420: launch_yuv420_fast<F16, YUV420_I420>(s, identity, bil, d, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                default: launch_yuv420_fast<F16, YUV420_YV12>(s, identity, bil, d, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+            }
+            KB200_TRY(check_launch(identity ? YUV420_IDENTITY_NAMES[l420] : YUV420_FAST_NAMES[l420]));
             continue;
         }
         dim3 grid(div_up(pixels, 256), nb);
-        if (frames) {
-            if (lanczos) preprocess_generic_kernel<F16, KB200_INTERP_LANCZOS, true><<<grid, 256, 0, s>>>(d, fr, dst, f0);
-            else if (bil) preprocess_generic_kernel<F16, KB200_INTERP_BILINEAR, true><<<grid, 256, 0, s>>>(d, fr, dst, f0);
-            else preprocess_generic_kernel<F16, KB200_INTERP_NEAREST, true><<<grid, 256, 0, s>>>(d, fr, dst, f0);
-        } else {
-            if (lanczos) preprocess_generic_kernel<F16, KB200_INTERP_LANCZOS, false><<<grid, 256, 0, s>>>(d, fr, dst, f0);
-            else if (bil) preprocess_generic_kernel<F16, KB200_INTERP_BILINEAR, false><<<grid, 256, 0, s>>>(d, fr, dst, f0);
-            else preprocess_generic_kernel<F16, KB200_INTERP_NEAREST, false><<<grid, 256, 0, s>>>(d, fr, dst, f0);
-        }
+        if (frames) { if (ext_yuv) launch_generic<F16, true, true>(s, grid, d.sampling, d, fr, dst, f0); else launch_generic<F16, true, false>(s, grid, d.sampling, d, fr, dst, f0); }
+        else        { if (ext_yuv) launch_generic<F16, false, true>(s, grid, d.sampling, d, fr, dst, f0); else launch_generic<F16, false, false>(s, grid, d.sampling, d, fr, dst, f0); }
         KB200_TRY(check_launch("preprocess_generic_kernel"));
     }
     return KB200_OK;

@@ -528,37 +528,61 @@ def _raw_frames(src, what: str) -> torch.Tensor:
     return t
 
 
-def rgb_from_nv12(src, dst: Image) -> None:
-    """color/yuv/mod.rs:235 — `src`: u8 tensor holding, per frame, w*h Y bytes then w*h/2 interleaved UV
-    bytes ([len] or [N,len]); BT.601 limited, Q20, bit-exact."""
-    t = _raw_frames(src, "rgb_from_nv12")
+YUV420_NV12, YUV420_NV21, YUV420_I420, YUV420_YV12 = 0, 1, 2, 3   # kb200_yuv420_layout
+YUV422_YUYV, YUV422_UYVY, YUV422_YVYU = 0, 1, 2                   # kb200_yuv422_layout
+
+
+def _rgb_from_yuv(src, dst: Image, what: str, bytes_num: int, bytes_den: int, fn_name: str, *layout) -> None:
+    """The video decoders: `src` holds N tight frames of w*h*bytes_num/bytes_den bytes; `layout` is the extra argument of
+    the layout-generic entry points (none for the NV12 / YUYV ones)."""
+    t = _raw_frames(src, what)
     if not dst.is_device:
         raise ImageError.MixedResidency()
     if t.device != dst.device:
         raise ImageError.DeviceMismatch()
     _expect_dtype(dst, torch.uint8, "dst")
     w, h, n = dst.cols(), dst.rows(), dst.batch
-    need = w * h * 3 // 2 * n
+    need = w * h * bytes_num // bytes_den * n
     if dst.num_channels() != 3 or t.numel() != need:
         raise ImageError.InvalidImageSize(t.numel(), 1, need, 1)  # check_dst_size, color/yuv/mod.rs:186-207
     _lib.set_device(t.device.index)
-    _check(_lib.lib().kb200_rgb_from_nv12_u8(_stream(t.device), t.data_ptr(), t.numel(), dst.data.data_ptr(), dst.numel(), w, h, n))
+    _check(getattr(_lib.lib(), fn_name)(_stream(t.device), t.data_ptr(), t.numel(), dst.data.data_ptr(), dst.numel(), w, h, n, *layout))
+
+
+def rgb_from_nv12(src, dst: Image) -> None:
+    """color/yuv/mod.rs:235 — `src`: u8 tensor holding, per frame, w*h Y bytes then w*h/2 interleaved UV
+    bytes ([len] or [N,len]); BT.601 limited, Q20, bit-exact."""
+    _rgb_from_yuv(src, dst, "rgb_from_nv12", 3, 2, "kb200_rgb_from_nv12_u8")
+
+
+def rgb_from_nv21(src, dst: Image) -> None:
+    """Like rgb_from_nv12, with the chroma pairs stored V U (the Android camera default)."""
+    _rgb_from_yuv(src, dst, "rgb_from_nv21", 3, 2, "kb200_rgb_from_yuv420_u8", YUV420_NV21)
+
+
+def rgb_from_i420(src, dst: Image) -> None:
+    """Like rgb_from_nv12, with the chroma in two (w/2 x h/2) planes after the Y plane: U, then V (yuv420p)."""
+    _rgb_from_yuv(src, dst, "rgb_from_i420", 3, 2, "kb200_rgb_from_yuv420_u8", YUV420_I420)
+
+
+def rgb_from_yv12(src, dst: Image) -> None:
+    """Like rgb_from_i420, with the V plane before the U plane."""
+    _rgb_from_yuv(src, dst, "rgb_from_yv12", 3, 2, "kb200_rgb_from_yuv420_u8", YUV420_YV12)
 
 
 def rgb_from_yuyv(src, dst: Image) -> None:
     """color/yuv/mod.rs:209 (impl_packed422!, Yuyv)."""
-    t = _raw_frames(src, "rgb_from_yuyv")
-    if not dst.is_device:
-        raise ImageError.MixedResidency()
-    if t.device != dst.device:
-        raise ImageError.DeviceMismatch()
-    _expect_dtype(dst, torch.uint8, "dst")
-    w, h, n = dst.cols(), dst.rows(), dst.batch
-    need = w * h * 2 * n
-    if dst.num_channels() != 3 or t.numel() != need:
-        raise ImageError.InvalidImageSize(t.numel(), 1, need, 1)
-    _lib.set_device(t.device.index)
-    _check(_lib.lib().kb200_rgb_from_yuyv_u8(_stream(t.device), t.data_ptr(), t.numel(), dst.data.data_ptr(), dst.numel(), w, h, n))
+    _rgb_from_yuv(src, dst, "rgb_from_yuyv", 2, 1, "kb200_rgb_from_yuyv_u8")
+
+
+def rgb_from_uyvy(src, dst: Image) -> None:
+    """Like rgb_from_yuyv, with each pixel pair stored `U Y0 V Y1`."""
+    _rgb_from_yuv(src, dst, "rgb_from_uyvy", 2, 1, "kb200_rgb_from_yuv422_u8", YUV422_UYVY)
+
+
+def rgb_from_yvyu(src, dst: Image) -> None:
+    """Like rgb_from_yuyv, with each pixel pair stored `Y0 V Y1 U`."""
+    _rgb_from_yuv(src, dst, "rgb_from_yvyu", 2, 1, "kb200_rgb_from_yuv422_u8", YUV422_YVYU)
 
 
 def _encode(op: str, fn_name: str, src: Image, dst: torch.Tensor, bytes_per_px_num: int, bytes_per_px_den: int, need_even_h: bool) -> None:

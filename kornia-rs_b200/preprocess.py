@@ -46,24 +46,39 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
     Gray8 = "gray8"
     Nv12 = "nv12"
     Yuyv = "yuyv"
+    # Beyond the reference's SourceFormat: the other 4:2:0 layouts (tight w*h*3/2 frames, like Nv12) and 4:2:2 layouts
+    # (w*h*2, like Yuyv).  Each decodes to exactly what its byte-repacked Nv12 / Yuyv twin decodes to.
+    Nv21 = "nv21"
+    I420 = "i420"
+    Yv12 = "yv12"
+    Uyvy = "uyvy"
+    Yvyu = "yvyu"
 
     def fmt_code(self) -> int:  # :153-161
-        return {"rgb8": 0, "rgba8": 0, "bgr8": 1, "bgra8": 1, "gray8": 2, "nv12": 3, "yuyv": 4}[self.value]
+        return {"rgb8": 0, "rgba8": 0, "bgr8": 1, "bgra8": 1, "gray8": 2, "nv12": 3, "yuyv": 4,
+                "nv21": 5, "i420": 6, "yv12": 7, "uyvy": 8, "yvyu": 9}[self.value]
 
     def bpp(self) -> int:  # :164-171
-        return {"rgb8": 3, "bgr8": 3, "rgba8": 4, "bgra8": 4, "gray8": 1, "nv12": 1, "yuyv": 2}[self.value]
+        return {"rgb8": 3, "bgr8": 3, "rgba8": 4, "bgra8": 4, "gray8": 1, "nv12": 1, "yuyv": 2,
+                "nv21": 1, "i420": 1, "yv12": 1, "uyvy": 2, "yvyu": 2}[self.value]
 
     def pitch(self, w: int) -> int:
         return w * self.bpp()
 
+    def is_yuv420(self) -> bool:
+        return self in (SourceFormat.Nv12, SourceFormat.Nv21, SourceFormat.I420, SourceFormat.Yv12)
+
+    def is_yuv422(self) -> bool:
+        return self in (SourceFormat.Yuyv, SourceFormat.Uyvy, SourceFormat.Yvyu)
+
     def buffer_len(self, w: int, h: int) -> int:  # :177-186
-        chroma = w * h // 2 if self is SourceFormat.Nv12 else 0
+        chroma = w * h // 2 if self.is_yuv420() else 0
         return self.pitch(w) * h + chroma
 
     def dims_ok(self, w: int, h: int) -> bool:  # :188-195
-        if self is SourceFormat.Nv12:
+        if self.is_yuv420():
             return w % 2 == 0 and h % 2 == 0
-        if self is SourceFormat.Yuyv:
+        if self.is_yuv422():
             return w % 2 == 0
         return True
 
@@ -73,7 +88,8 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
     @staticmethod
     def from_name(name: str):  # :221-233
         table = {"rgb": "Rgb8", "rgb8": "Rgb8", "bgr": "Bgr8", "bgr8": "Bgr8", "rgba": "Rgba8", "rgba8": "Rgba8",
-                 "bgra": "Bgra8", "bgra8": "Bgra8", "gray": "Gray8", "gray8": "Gray8", "nv12": "Nv12", "yuyv": "Yuyv"}
+                 "bgra": "Bgra8", "bgra8": "Bgra8", "gray": "Gray8", "gray8": "Gray8", "nv12": "Nv12", "yuyv": "Yuyv",
+                 "nv21": "Nv21", "i420": "I420", "yv12": "Yv12", "uyvy": "Uyvy", "yvyu": "Yvyu"}
         key = table.get(name.lower())
         return None if key is None else SourceFormat[key]
 
