@@ -1,7 +1,9 @@
 // preprocess.cu — the fused camera preprocess (a12; BASELINE config 3): raw frame (RGB/BGR/RGBA/
-// Gray/NV12/YUYV, tight or pitched; beyond the reference also NV21/I420/YV12/UYVY/YVYU) → letterbox/stretch
-// resample → (v/255 - mean) * inv_std → planar CHW f32 or f16, for a whole batch in ONE launch.
+// Gray/NV12/YUYV, tight or pitched; beyond the reference also NV21/I420/YV12/UYVY/YVYU and the Bayer mosaics) →
+// letterbox/stretch resample → (v/255 - mean) * inv_std → planar CHW f32 or f16, for a whole batch in ONE launch.
 // The 4:2:0 formats share the NV12 kernels (templated on the chroma layout); the 4:2:2 formats take the generic kernel.
+// A Bayer tap is the demosaiced pixel at the tap's coordinate (bayer.cuh); Bayer frames take the generic kernel, except
+// the identity geometry, which has its own fast kernel.
 //
 // Reference: preprocess.rs:430-647 (the CUDA source string — the specification of this path; there
 // is no CPU implementation for the camera formats), launch seam :1324-1372, batch loop :1277-1280
@@ -17,6 +19,7 @@
 // integer scales (1080p NV12 → 1080p CHW, config 3a) that removes 3 of the 4 decodes per pixel.
 #include <cuda_fp16.h>
 
+#include "bayer.cuh"
 #include "kb200_common.cuh"
 
 namespace kb200 {
@@ -91,11 +94,18 @@ __device__ __forceinline__ void fetch_px_yuv_ext(const uint8_t* __restrict__ src
     }
 }
 
-// EXT_YUV: the frame is one of fmt 5-9 (a separate instantiation, so the kernels of fmt 0-4 are unchanged by them)
-template <bool EXT_YUV>
+// Which formats an instantiation of the generic kernel serves: the reference's (fmt 0-4), the YUV layouts beyond them
+// (fmt 5-9) or the Bayer mosaics (fmt 16-19).  Separate instantiations, so the kernels of fmt 0-4 are unchanged by the others.
+static constexpr int SRC_BASE = 0, SRC_EXT_YUV = 1, SRC_BAYER = 2;
+
+template <int EXT>
 __device__ __forceinline__ void fetch_px(const uint8_t* __restrict__ src, int x, int y, const kb200_preprocess_desc& d,
                                          float px[3]) {  // :510-530
-    if (EXT_YUV) {
+    if (EXT == SRC_BAYER) {
+        int rgb[3];
+        bayer_px(src, (size_t)d.src_pitch, d.src_w, d.src_h, x, y, d.fmt - KB200_FMT_BAYER_RGGB, rgb);
+        px[0] = (float)rgb[0]; px[1] = (float)rgb[1]; px[2] = (float)rgb[2];
+    } else if (EXT == SRC_EXT_YUV) {
         fetch_px_yuv_ext(src, x, y, d, px);
     } else if (d.fmt <= 1) {
         const uint8_t* p = src + (long long)y * d.src_pitch + x * d.src_bpp;
@@ -125,7 +135,7 @@ __device__ __forceinline__ float pre_lanczos_w(float dd) {
 }
 
 // SAMP: kb200_interp — 0 nearest, 1 bilinear, 3 Lanczos-3 (6x6 taps, clamp-to-edge, weights renormalised by their sum)
-template <bool F16, int SAMP, bool PTRS, bool EXT_YUV>
+template <bool F16, int SAMP, bool PTRS, int EXT>
 __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                  const __grid_constant__ PreFrames fr, void* __restrict__ dst,
                                                                  uint32_t frame0) {
@@ -152,7 +162,7 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
                     const float w = wy * pre_lanczos_w(sx - (float)xi);
                     const int xc = min(max(xi, 0), d.src_w - 1);
                     float t[3];
-                    fetch_px<EXT_YUV>(src, xc, yc, d, t);
+                    fetch_px<EXT>(src, xc, yc, d, t);
                     acc0 += w * t[0]; acc1 += w * t[1]; acc2 += w * t[2];
                     wsum += w;
                 }
@@ -164,12 +174,12 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
             const int x1 = min(x0 + 1, d.src_w - 1), y1 = min(y0 + 1, d.src_h - 1);
             x0 = max(x0, 0); y0 = max(y0, 0);
             float t00[3], t10[3], t01[3], t11[3];
-            fetch_px<EXT_YUV>(src, x0, y0, d, t00);
+            fetch_px<EXT>(src, x0, y0, d, t00);
             const bool need_x = ax != 0.0f, need_y = ay != 0.0f;
-            if (need_x) fetch_px<EXT_YUV>(src, x1, y0, d, t10);
+            if (need_x) fetch_px<EXT>(src, x1, y0, d, t10);
             if (need_y) {
-                fetch_px<EXT_YUV>(src, x0, y1, d, t01);
-                if (need_x) fetch_px<EXT_YUV>(src, x1, y1, d, t11);
+                fetch_px<EXT>(src, x0, y1, d, t01);
+                if (need_x) fetch_px<EXT>(src, x1, y1, d, t11);
             }
 #pragma unroll
             for (int c = 0; c < 3; ++c) {
@@ -184,7 +194,7 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
         } else {
             const int xn = min(max((int)roundf(sx), 0), d.src_w - 1);
             const int yn = min(max((int)roundf(sy), 0), d.src_h - 1);
-            fetch_px<EXT_YUV>(src, xn, yn, d, px);
+            fetch_px<EXT>(src, xn, yn, d, px);
         }
     } else {
         px[0] = d.pad_value; px[1] = d.pad_value; px[2] = d.pad_value;
@@ -293,6 +303,53 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const _
         nv12_store4<F16>(dst, o + plane, g4);
         nv12_store4<F16>(dst, o + 2 * plane, b4);
     }
+}
+
+// ── Bayer identity fast path (the config-3a shape from a Bayer mosaic: scale 1, no pad, same size) ──────────────
+// As for 4:2:0, the sample is the demosaiced pixel (ox, oy) itself.  One thread = 4 columns x 2 output rows (the row
+// pairs of bayer_row_pairs): 4 lane-contiguous LDG.32 of the rows ya-1 .. ya+2 plus shuffled halos (bayer_load_rows),
+// 6 to 12 lane-contiguous 4-pixel stores per thread (nv12_store4).  Requires w % 4 == 0 and 4-B aligned rows.
+template <bool F16, bool PTRS, int P>
+__global__ void __launch_bounds__(128) preprocess_bayer_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
+                                                                        const __grid_constant__ PreFrames fr, void* __restrict__ dst,
+                                                                        uint32_t frame0, uint32_t groups_per_row, uint32_t items) {
+    const uint32_t item = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool active = item < items;                         // the lanes past the end still take part in the shuffles
+    const uint32_t it = active ? item : items - 1;
+    const uint32_t rp = it / groups_per_row, g = it - rp * groups_per_row;
+    const uint32_t w = (uint32_t)d.src_w, h = (uint32_t)d.src_h;
+    const uint32_t f = blockIdx.y;
+    const uint8_t* src = PTRS ? fr.ptr[f] : fr.base + (size_t)(frame0 + f) * fr.stride;
+    const uint32_t x = g * 4u, ya = 1u + 2u * rp, yb = ya + 1u;
+    uint32_t rows[4][1];
+    int hl[4], hr[4];
+    bayer_load_rows<1>(src, (size_t)d.src_pitch, w, h, x, ya, threadIdx.x & 31u, [](const uint8_t* p, uint32_t v[1]) {
+        v[0] = __ldg(reinterpret_cast<const uint32_t*>(p));
+    }, rows, hl, hr);
+    if (!active) return;
+    const bool left_edge = x == 0, right_edge = x + 4u == w;
+    const size_t plane = (size_t)w * h;
+    const size_t base = (size_t)(frame0 + f) * 3 * plane + x;
+    const float m0 = d.mean[0], m1 = d.mean[1], m2 = d.mean[2], i0 = d.inv_std[0], i1 = d.inv_std[1], i2 = d.inv_std[2];
+    float r4[4], g4[4], b4[4];
+    auto store_row = [&](uint32_t y) {
+        const size_t o = base + (size_t)y * w;
+        nv12_store4<F16>(dst, o, r4);
+        nv12_store4<F16>(dst, o + plane, g4);
+        nv12_store4<F16>(dst, o + 2 * plane, b4);
+    };
+    int r[4], gg[4], b[4];
+    bayer_row<P, 1, 1>(rows[0], rows[1], rows[2], hl, hr, left_edge, right_edge, r, gg, b);   // ya is odd
+#pragma unroll
+    for (int i = 0; i < 4; ++i) { r4[i] = norm_int_px(r[i], m0, i0); g4[i] = norm_int_px(gg[i], m1, i1); b4[i] = norm_int_px(b[i], m2, i2); }
+    store_row(ya);
+    if (ya == 1u) store_row(0);
+    if (yb == h - 1u) { store_row(yb); return; }
+    bayer_row<P, 0, 1>(rows[1], rows[2], rows[3], hl + 1, hr + 1, left_edge, right_edge, r, gg, b);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) { r4[i] = norm_int_px(r[i], m0, i0); g4[i] = norm_int_px(gg[i], m1, i1); b4[i] = norm_int_px(b[i], m2, i2); }
+    store_row(yb);
+    if (yb == h - 2u) store_row(h - 1u);
 }
 
 // ── NV12 general path (config 3b: 1080p NV12 → letterboxed 640x640, and every other NV12 geometry) ──────────
@@ -432,8 +489,10 @@ static int yuv420_layout(int fmt) {
     }
 }
 static bool is_yuv422(int fmt) { return fmt == KB200_FMT_YUYV || fmt == KB200_FMT_UYVY || fmt == KB200_FMT_YVYU; }
+static bool is_bayer(int fmt) { return fmt >= KB200_FMT_BAYER_RGGB && fmt <= KB200_FMT_BAYER_GBRG; }
 // SourceFormat names, in the validation messages
 static const char* const FMT_NAMES[10] = {"Rgb8", "Bgr8", "Gray8", "Nv12", "Yuyv", "Nv21", "I420", "Yv12", "Uyvy", "Yvyu"};
+static const char* const BAYER_NAMES[4] = {"BayerRggb", "BayerBggr", "BayerGrbg", "BayerGbrg"};
 static const char* const YUV420_UPPER[4] = {"NV12", "NV21", "I420", "YV12"};
 
 static size_t src_bytes(const kb200_preprocess_desc& d) {
@@ -447,7 +506,7 @@ static int validate_desc(const kb200_preprocess_desc* dp) {
     if (d.src_w <= 0 || d.src_h <= 0 || d.dst_w <= 0 || d.dst_h <= 0)
         return fail(KB200_ERR_INVALID_ARGUMENT, "image dimensions must be non-zero");
     if ((long long)d.dst_w * d.dst_h > 0x7FFFFFFFll) return fail(KB200_ERR_DIMS_TOO_LARGE, "dimensions exceed the 32-bit CUDA kernel index limit");  // :1336-1339
-    if (d.fmt < 0 || d.fmt > KB200_FMT_YVYU) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown source format code %d", d.fmt);
+    if (d.fmt < 0 || (d.fmt > KB200_FMT_YVYU && !is_bayer(d.fmt))) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown source format code %d", d.fmt);
     if (d.sampling != KB200_INTERP_NEAREST && d.sampling != KB200_INTERP_BILINEAR && d.sampling != KB200_INTERP_LANCZOS)
         return fail(KB200_ERR_UNSUPPORTED, "unsupported sampling mode %d (expected Nearest, Bilinear or Lanczos)", d.sampling);  // preprocess.rs:1044-1051
     if (d.fmt <= 1 && d.src_bpp != 3 && d.src_bpp != 4) return fail(KB200_ERR_UNSUPPORTED, "unsupported source channel count %d (expected 3 or 4)", d.src_bpp);
@@ -455,6 +514,8 @@ static int validate_desc(const kb200_preprocess_desc* dp) {
     const int l420 = yuv420_layout(d.fmt);
     if (l420 >= 0 && ((d.src_w | d.src_h) & 1)) return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s at %dx%d (even dimensions required)", FMT_NAMES[d.fmt], d.src_w, d.src_h);
     if (is_yuv422(d.fmt) && (d.src_w & 1)) return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s at %dx%d (even width required)", FMT_NAMES[d.fmt], d.src_w, d.src_h);
+    if (is_bayer(d.fmt) && (d.src_w < 3 || d.src_h < 3))
+        return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s at %dx%d (at least 3x3 required)", BAYER_NAMES[d.fmt - KB200_FMT_BAYER_RGGB], d.src_w, d.src_h);
     const int bpp = d.fmt <= 1 ? d.src_bpp : (is_yuv422(d.fmt) ? 2 : 1);
     if ((long long)d.src_pitch < (long long)d.src_w * bpp) return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface (need pitch >= width*channels and len >= pitch*height)");
     if (l420 >= 0 && d.src_pitch != d.src_w) return fail(KB200_ERR_INVALID_SOURCE, "%s frames must be tightly packed (pitch == width)", YUV420_UPPER[l420]);
@@ -479,17 +540,36 @@ static void launch_yuv420_fast(cudaStream_t s, bool identity, bool bil, const kb
 #undef KB200_YUV420_LAUNCH
 }
 
-template <bool F16, bool PTRS, bool EXT_YUV>
+// The Bayer identity kernel of pattern P, for one launch of <= 256 frames.
+template <bool F16, int P>
+static void launch_bayer_identity(cudaStream_t s, const kb200_preprocess_desc& d, const PreFrames& fr, bool ptrs, void* dst, uint32_t f0,
+                                  uint32_t nb, uint32_t id_groups, size_t id_items) {
+    dim3 grid(div_up(id_items, 128), nb);
+    if (ptrs) preprocess_bayer_identity_kernel<F16, true, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
+    else preprocess_bayer_identity_kernel<F16, false, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
+}
+
+template <bool F16, bool PTRS, int EXT>
 static void launch_generic(cudaStream_t s, dim3 grid, int sampling, const kb200_preprocess_desc& d, const PreFrames& fr, void* dst, uint32_t f0) {
-    if (sampling == KB200_INTERP_LANCZOS) preprocess_generic_kernel<F16, KB200_INTERP_LANCZOS, PTRS, EXT_YUV><<<grid, 256, 0, s>>>(d, fr, dst, f0);
-    else if (sampling == KB200_INTERP_BILINEAR) preprocess_generic_kernel<F16, KB200_INTERP_BILINEAR, PTRS, EXT_YUV><<<grid, 256, 0, s>>>(d, fr, dst, f0);
-    else preprocess_generic_kernel<F16, KB200_INTERP_NEAREST, PTRS, EXT_YUV><<<grid, 256, 0, s>>>(d, fr, dst, f0);
+    if (sampling == KB200_INTERP_LANCZOS) preprocess_generic_kernel<F16, KB200_INTERP_LANCZOS, PTRS, EXT><<<grid, 256, 0, s>>>(d, fr, dst, f0);
+    else if (sampling == KB200_INTERP_BILINEAR) preprocess_generic_kernel<F16, KB200_INTERP_BILINEAR, PTRS, EXT><<<grid, 256, 0, s>>>(d, fr, dst, f0);
+    else preprocess_generic_kernel<F16, KB200_INTERP_NEAREST, PTRS, EXT><<<grid, 256, 0, s>>>(d, fr, dst, f0);
+}
+
+template <bool F16, bool PTRS>
+static void launch_generic_for(int ext, cudaStream_t s, dim3 grid, int sampling, const kb200_preprocess_desc& d, const PreFrames& fr, void* dst,
+                               uint32_t f0) {
+    if (ext == SRC_BAYER) launch_generic<F16, PTRS, SRC_BAYER>(s, grid, sampling, d, fr, dst, f0);
+    else if (ext == SRC_EXT_YUV) launch_generic<F16, PTRS, SRC_EXT_YUV>(s, grid, sampling, d, fr, dst, f0);
+    else launch_generic<F16, PTRS, SRC_BASE>(s, grid, sampling, d, fr, dst, f0);
 }
 
 // kb200_last_kernel() names of the 4:2:0 fast kernels, by layout
 static const char* const YUV420_IDENTITY_NAMES[4] = {"preprocess_nv12_identity_kernel", "preprocess_nv21_identity_kernel",
                                                      "preprocess_i420_identity_kernel", "preprocess_yv12_identity_kernel"};
 static const char* const YUV420_FAST_NAMES[4] = {"preprocess_nv12_kernel", "preprocess_nv21_kernel", "preprocess_i420_kernel", "preprocess_yv12_kernel"};
+static const char* const BAYER_IDENTITY_NAMES[4] = {"preprocess_bayer_rggb_identity_kernel", "preprocess_bayer_bggr_identity_kernel",
+                                                    "preprocess_bayer_grbg_identity_kernel", "preprocess_bayer_gbrg_identity_kernel"};
 
 template <bool F16>
 static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, const uint8_t* const* frames,
@@ -497,20 +577,21 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
     const int pixels = d.dst_w * d.dst_h;
     const bool bil = d.sampling == KB200_INTERP_BILINEAR, lanczos = d.sampling == KB200_INTERP_LANCZOS;
     const int l420 = yuv420_layout(d.fmt);
-    // identity fast path: a 4:2:0 format, scale 1, no pad, same size, 8-column vectors possible
+    const bool bayer = is_bayer(d.fmt);
+    // identity fast path: a 4:2:0 or Bayer format, scale 1, no pad, same size, 8-column vectors possible
     // (Lanczos always takes the generic kernel: its off-centre weights at integer coordinates are sinf(k*pi) != 0 exactly)
-    bool identity = !lanczos && l420 >= 0 && d.scale_x == 1.0f && d.scale_y == 1.0f && d.pad_x == 0.0f && d.pad_y == 0.0f &&
-                    d.dst_w == d.src_w && d.dst_h == d.src_h && (d.src_w % 4) == 0 && aligned16(dst);
+    bool identity = !lanczos && (l420 >= 0 || bayer) && d.scale_x == 1.0f && d.scale_y == 1.0f && d.pad_x == 0.0f && d.pad_y == 0.0f &&
+                    d.dst_w == d.src_w && d.dst_h == d.src_h && (d.src_w % 4) == 0 && (d.src_pitch % 4) == 0 && aligned16(dst);
     if (identity) {
         if (frames) { for (uint32_t k = 0; k < batch; ++k) identity = identity && ((reinterpret_cast<uintptr_t>(frames[k]) & 3u) == 0); }
         else identity = ((reinterpret_cast<uintptr_t>(base) & 3u) == 0) && (stride % 4 == 0);
     }
     const uint32_t id_groups = (uint32_t)d.src_w / 4u;
-    const size_t id_items = (size_t)id_groups * ((size_t)d.src_h / 2);
+    const size_t id_items = (size_t)id_groups * (bayer ? bayer_row_pairs((uint32_t)d.src_h) : (size_t)d.src_h / 2);
     if (id_items > 0x7FFFFFFFull) identity = false;
     // 4:2:0 general fast path: vector stores need dst_w % 4 == 0 and a 16-B (f32) / 8-B (f16) aligned destination
     const bool yuv420_fast = !lanczos && l420 >= 0 && (d.dst_w % 4) == 0 && aligned16(dst) && d.dst_h <= 65535 * NV12_ROWS;
-    const bool ext_yuv = d.fmt >= KB200_FMT_NV21;
+    const int ext = bayer ? SRC_BAYER : d.fmt >= KB200_FMT_NV21 ? SRC_EXT_YUV : SRC_BASE;
     Nv12Args nv{};
     nv.groups = (uint32_t)(d.dst_w + 3) / 4u;
     for (int c = 0; c < 3; ++c) nv.pad_norm[c] = (d.pad_value / 255.0f - d.mean[c]) * d.inv_std[c];  // BODY :610-612 on the host (f32, unfused)
@@ -519,8 +600,18 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
         PreFrames fr{};
         fr.base = base; fr.stride = stride;
         if (frames) for (uint32_t k = 0; k < nb; ++k) fr.ptr[k] = frames[f0 + k];
+        const bool p = frames != nullptr;
+        if (identity && bayer) {
+            switch (d.fmt) {
+                case KB200_FMT_BAYER_RGGB: launch_bayer_identity<F16, KB200_BAYER_RGGB>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
+                case KB200_FMT_BAYER_BGGR: launch_bayer_identity<F16, KB200_BAYER_BGGR>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
+                case KB200_FMT_BAYER_GRBG: launch_bayer_identity<F16, KB200_BAYER_GRBG>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
+                default: launch_bayer_identity<F16, KB200_BAYER_GBRG>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
+            }
+            KB200_TRY(check_launch(BAYER_IDENTITY_NAMES[d.fmt - KB200_FMT_BAYER_RGGB]));
+            continue;
+        }
         if (identity || yuv420_fast) {
-            const bool p = frames != nullptr;
             switch (l420) {
                 case YUV420_NV12: launch_yuv420_fast<F16, YUV420_NV12>(s, identity, bil, d, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
                 case YUV420_NV21: launch_yuv420_fast<F16, YUV420_NV21>(s, identity, bil, d, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
@@ -531,8 +622,8 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
             continue;
         }
         dim3 grid(div_up(pixels, 256), nb);
-        if (frames) { if (ext_yuv) launch_generic<F16, true, true>(s, grid, d.sampling, d, fr, dst, f0); else launch_generic<F16, true, false>(s, grid, d.sampling, d, fr, dst, f0); }
-        else        { if (ext_yuv) launch_generic<F16, false, true>(s, grid, d.sampling, d, fr, dst, f0); else launch_generic<F16, false, false>(s, grid, d.sampling, d, fr, dst, f0); }
+        if (p) launch_generic_for<F16, true>(ext, s, grid, d.sampling, d, fr, dst, f0);
+        else launch_generic_for<F16, false>(ext, s, grid, d.sampling, d, fr, dst, f0);
         KB200_TRY(check_launch("preprocess_generic_kernel"));
     }
     return KB200_OK;

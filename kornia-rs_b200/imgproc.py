@@ -11,6 +11,7 @@ host operands raise `ImageError(UnsupportedDevice)`.
 from __future__ import annotations
 
 import ctypes as C
+import enum
 from typing import Sequence
 
 import torch
@@ -583,6 +584,22 @@ def rgb_from_uyvy(src, dst: Image) -> None:
 def rgb_from_yvyu(src, dst: Image) -> None:
     """Like rgb_from_yuyv, with each pixel pair stored `Y0 V Y1 U`."""
     _rgb_from_yuv(src, dst, "rgb_from_yvyu", 2, 1, "kb200_rgb_from_yuv422_u8", YUV422_YVYU)
+
+
+class BayerPattern(enum.IntEnum):
+    """kb200_bayer_pattern: the 2x2 quad of a Bayer mosaic read row-major (RGGB: the top-left pixel is R).  OpenCV names
+    the same patterns by another pair of the quad: RGGB = COLOR_BayerBG2RGB, BGGR = COLOR_BayerRG2RGB,
+    GRBG = COLOR_BayerGB2RGB, GBRG = COLOR_BayerGR2RGB."""
+    RGGB = 0
+    BGGR = 1
+    GRBG = 2
+    GBRG = 3
+
+
+def rgb_from_bayer(src, dst: Image, pattern: BayerPattern) -> None:
+    """8-bit Bayer mosaic -> RGB8, bilinear demosaic bit-identical to OpenCV's cvtColor(COLOR_Bayer??2RGB) (an extension
+    beyond the reference).  `src`: u8 device tensor holding N tight frames of w*h bytes (w, h >= 3)."""
+    _rgb_from_yuv(src, dst, "rgb_from_bayer", 1, 1, "kb200_rgb_from_bayer_u8", int(BayerPattern(pattern)))
 
 
 def _encode(op: str, fn_name: str, src: Image, dst: torch.Tensor, bytes_per_px_num: int, bytes_per_px_den: int, need_even_h: bool) -> None:

@@ -2,7 +2,7 @@
 
 Built once via `Preprocessor.builder()…build_cuda()`, then applied to any number of frames of any
 resolution: the target H/W is read from the destination tensor each call.  Camera formats
-(NV12 / YUYV / Gray) go through `run_raw*`; colour decode is fused into the resample taps.  Unlike the
+(NV12 / YUYV / Gray, the other YUV layouts and the Bayer mosaics) go through `run_raw*`; colour decode is fused into the resample taps.  Unlike the
 reference (one launch per frame, preprocess.rs:1277-1280) a batch is ONE launch.
 
 Only the CUDA preprocessor exists here (`build()` = the reference's CPU preprocessor is out of scope:
@@ -53,14 +53,22 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
     Yv12 = "yv12"
     Uyvy = "uyvy"
     Yvyu = "yvyu"
+    # Beyond the reference too: 8-bit Bayer mosaics (one byte per pixel, w*h like Gray8, at least 3x3), named by their
+    # 2x2 quad read row-major.  A tap is the bilinear demosaic of OpenCV's cvtColor(COLOR_Bayer??2RGB) at that pixel.
+    BayerRggb = "bayer_rggb"
+    BayerBggr = "bayer_bggr"
+    BayerGrbg = "bayer_grbg"
+    BayerGbrg = "bayer_gbrg"
 
     def fmt_code(self) -> int:  # :153-161
         return {"rgb8": 0, "rgba8": 0, "bgr8": 1, "bgra8": 1, "gray8": 2, "nv12": 3, "yuyv": 4,
-                "nv21": 5, "i420": 6, "yv12": 7, "uyvy": 8, "yvyu": 9}[self.value]
+                "nv21": 5, "i420": 6, "yv12": 7, "uyvy": 8, "yvyu": 9,
+                "bayer_rggb": 16, "bayer_bggr": 17, "bayer_grbg": 18, "bayer_gbrg": 19}[self.value]
 
     def bpp(self) -> int:  # :164-171
         return {"rgb8": 3, "bgr8": 3, "rgba8": 4, "bgra8": 4, "gray8": 1, "nv12": 1, "yuyv": 2,
-                "nv21": 1, "i420": 1, "yv12": 1, "uyvy": 2, "yvyu": 2}[self.value]
+                "nv21": 1, "i420": 1, "yv12": 1, "uyvy": 2, "yvyu": 2,
+                "bayer_rggb": 1, "bayer_bggr": 1, "bayer_grbg": 1, "bayer_gbrg": 1}[self.value]
 
     def pitch(self, w: int) -> int:
         return w * self.bpp()
@@ -71,6 +79,9 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
     def is_yuv422(self) -> bool:
         return self in (SourceFormat.Yuyv, SourceFormat.Uyvy, SourceFormat.Yvyu)
 
+    def is_bayer(self) -> bool:
+        return self.value.startswith("bayer_")
+
     def buffer_len(self, w: int, h: int) -> int:  # :177-186
         chroma = w * h // 2 if self.is_yuv420() else 0
         return self.pitch(w) * h + chroma
@@ -80,6 +91,8 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
             return w % 2 == 0 and h % 2 == 0
         if self.is_yuv422():
             return w % 2 == 0
+        if self.is_bayer():
+            return w >= 3 and h >= 3
         return True
 
     def interleaved(self) -> bool:  # :211-216
@@ -89,7 +102,8 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
     def from_name(name: str):  # :221-233
         table = {"rgb": "Rgb8", "rgb8": "Rgb8", "bgr": "Bgr8", "bgr8": "Bgr8", "rgba": "Rgba8", "rgba8": "Rgba8",
                  "bgra": "Bgra8", "bgra8": "Bgra8", "gray": "Gray8", "gray8": "Gray8", "nv12": "Nv12", "yuyv": "Yuyv",
-                 "nv21": "Nv21", "i420": "I420", "yv12": "Yv12", "uyvy": "Uyvy", "yvyu": "Yvyu"}
+                 "nv21": "Nv21", "i420": "I420", "yv12": "Yv12", "uyvy": "Uyvy", "yvyu": "Yvyu",
+                 "bayer_rggb": "BayerRggb", "bayer_bggr": "BayerBggr", "bayer_grbg": "BayerGrbg", "bayer_gbrg": "BayerGbrg"}
         key = table.get(name.lower())
         return None if key is None else SourceFormat[key]
 
