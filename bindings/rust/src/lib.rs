@@ -137,6 +137,7 @@ pub mod ffi {
         pub fn kb200_rgb_from_yuv420_u8(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, width: u32, height: u32, batch: u32, layout: c_int) -> c_int;
         pub fn kb200_rgb_from_yuv422_u8(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, width: u32, height: u32, batch: u32, layout: c_int) -> c_int;
         pub fn kb200_rgb_from_bayer_u8(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, width: u32, height: u32, batch: u32, pattern: c_int) -> c_int;
+        pub fn kb200_rgb_from_bayer_u16(stream: *mut c_void, src: *const u16, src_len: usize, dst: *mut u16, dst_len: usize, width: u32, height: u32, batch: u32, pattern: c_int) -> c_int;
         pub fn kb200_normalize_mean_std_f32(stream: *mut c_void, src: *const f32, dst: *mut f32, npixels: usize, channels: u32, mean: *const f32, std: *const f32) -> c_int;
         pub fn kb200_normalize_rgb_u8_f32(stream: *mut c_void, src: *const u8, dst: *mut f32, npixels: usize, scale: *const f32, offset: *const f32, leaf: c_int) -> c_int;
         pub fn kb200_find_min_max_f32(stream: *mut c_void, src: *const f32, n: usize, minmax_dev: *mut f32) -> c_int;
@@ -218,7 +219,7 @@ pub const OUT_F32: c_int = 0;
 pub const OUT_F16: c_int = 1;
 pub const OUT_BF16: c_int = 2;
 
-/// `fmt` of `kb200_preprocess_desc` (kb200_src_fmt).  Codes 5-9 and 16-19 go beyond the reference's `SourceFormat`.
+/// `fmt` of `kb200_preprocess_desc` (kb200_src_fmt).  Codes 5-9, 16-19 and 32-47 go beyond the reference's `SourceFormat`.
 pub const FMT_RGB: i32 = 0;
 pub const FMT_BGR: i32 = 1;
 pub const FMT_GRAY: i32 = 2;
@@ -233,6 +234,13 @@ pub const FMT_BAYER_RGGB: i32 = 16;
 pub const FMT_BAYER_BGGR: i32 = 17;
 pub const FMT_BAYER_GRBG: i32 = 18;
 pub const FMT_BAYER_GBRG: i32 = 19;
+/// 10- to 16-bit Bayer mosaics (one LSB-aligned u16 per sample): `FMT_BAYER16_BASE + 4 * k + pattern`, k = 0..3 for
+/// 10, 12, 14 and 16 bits.
+pub const FMT_BAYER16_BASE: i32 = 32;
+pub const FMT_BAYER_RGGB10: i32 = 32;
+pub const FMT_BAYER_RGGB12: i32 = 36;
+pub const FMT_BAYER_RGGB14: i32 = 40;
+pub const FMT_BAYER_RGGB16: i32 = 44;
 
 /// `pattern` of `kb200_rgb_from_bayer_u8` (kb200_bayer_pattern): the mosaic's 2x2 quad read row-major.
 pub const BAYER_RGGB: c_int = 0;

@@ -1,8 +1,8 @@
-// bayer.cuh — bilinear demosaic of 8-bit Bayer mosaics, shared by the standalone decoder (color.cu) and the camera
-// preprocess (preprocess.cu).
+// bayer.cuh — bilinear demosaic of Bayer mosaics, 8-bit or 16-bit samples, shared by the standalone decoders
+// (color.cu) and the camera preprocess (preprocess.cu).
 //
 // An extension beyond the reference, pinned to OpenCV: bit-identical to cv2.cvtColor(raw, COLOR_Bayer??2RGB)
-// (checked against cv2 4.13, tests/golden/bayer_cv2.npz).  A pattern (kb200_bayer_pattern) is named by its 2x2 quad
+// (checked against cv2 4.13 on 8-bit and 16-bit mosaics, tests/golden/bayer_cv2.npz and bayer16_cv2.npz).  A pattern (kb200_bayer_pattern) is named by its 2x2 quad
 // read row-major: RGGB means the top-left pixel is R.  cv2's codes are offset from these names:
 //     RGGB <-> COLOR_BayerBG2RGB, BGGR <-> COLOR_BayerRG2RGB, GRBG <-> COLOR_BayerGB2RGB, GBRG <-> COLOR_BayerGR2RGB.
 //
@@ -21,7 +21,7 @@ namespace kb200 {
 __host__ __device__ constexpr int bayer_rx(int P) { return (P == KB200_BAYER_BGGR || P == KB200_BAYER_GRBG) ? 1 : 0; }
 __host__ __device__ constexpr int bayer_ry(int P) { return (P == KB200_BAYER_BGGR || P == KB200_BAYER_GBRG) ? 1 : 0; }
 
-// The demosaiced colour of a centre pixel of column parity px, row parity py: c the centre byte, n s w e its edge
+// The demosaiced colour of a centre pixel of column parity px, row parity py: c the centre sample, n s w e its edge
 // neighbours, d the sum of its diagonal neighbours.  With P, px and py known at compile time this is two sums.
 __device__ __forceinline__ void bayer_demosaic(int P, int px, int py, int c, int n, int s, int w, int e, int d, int& r, int& g, int& b) {
     const int rx = bayer_rx(P), ry = bayer_ry(P);
@@ -36,56 +36,70 @@ __device__ __forceinline__ void bayer_demosaic(int P, int px, int py, int c, int
     }
 }
 
-// Output pixel (x, y) of a frame at `src` with row pitch `pitch`: nine byte loads around the clamped centre.
-__device__ __forceinline__ void bayer_px(const uint8_t* __restrict__ src, size_t pitch, int w, int h, int x, int y, int P, int rgb[3]) {
+// Output pixel (x, y) of a frame at `src` with row pitch `pitch` (in samples): nine sample loads around the clamped
+// centre.  T = uint8_t (8-bit mosaics) or uint16_t (10- to 16-bit mosaics, one LSB-aligned word per sample): every sum
+// is an int, so 4 * 65535 + 2 fits.
+template <typename T>
+__device__ __forceinline__ void bayer_px(const T* __restrict__ src, size_t pitch, int w, int h, int x, int y, int P, int rgb[3]) {
     const int cx = min(max(x, 1), w - 2), cy = min(max(y, 1), h - 2);
-    const uint8_t* up = src + (size_t)(cy - 1) * pitch + cx;
-    const uint8_t* mid = up + pitch;
-    const uint8_t* dn = mid + pitch;
+    const T* up = src + (size_t)(cy - 1) * pitch + cx;
+    const T* mid = up + pitch;
+    const T* dn = mid + pitch;
     const int d = (int)__ldg(up - 1) + (int)__ldg(up + 1) + (int)__ldg(dn - 1) + (int)__ldg(dn + 1);
     bayer_demosaic(P, cx & 1, cy & 1, __ldg(mid), __ldg(up), __ldg(dn), __ldg(mid - 1), __ldg(mid + 1), d, rgb[0], rgb[1], rgb[2]);
 }
 
-// Byte j of a row segment of NW words, j = -1 and j = 4*NW being the halo bytes left and right of it.
-template <int NW>
-__device__ __forceinline__ int bayer_seg_byte(const uint32_t w[NW], int left, int right, int j) {
-    return j < 0 ? left : j >= 4 * NW ? right : (int)((w[j >> 2] >> (8 * (j & 3))) & 0xFFu);
+// Samples of type T per 32-bit word of a row segment, and their width in bits.
+template <typename T> __host__ __device__ constexpr int bayer_per_word() { return 4 / (int)sizeof(T); }
+template <typename T> __host__ __device__ constexpr int bayer_bits() { return 8 * (int)sizeof(T); }
+
+// Sample j of a row segment of NW words, j = -1 and j = S*NW (S samples per word) being the halo samples left and
+// right of it.
+template <int NW, typename T = uint8_t>
+__device__ __forceinline__ int bayer_seg_sample(const uint32_t w[NW], int left, int right, int j) {
+    constexpr int S = bayer_per_word<T>(), B = bayer_bits<T>();
+    constexpr uint32_t M = (1u << B) - 1u;
+    return j < 0 ? left : j >= S * NW ? right : (int)((w[j / S] >> (B * (j % S))) & M);
 }
 
-// The 4*NW demosaiced pixels of one row segment of the fast kernels: row parity PY, the segment starting at an even
-// column.  n / c / s: the segments of the rows above, at and below; hl / hr: their halo bytes (above, at, below).
+// The S*NW demosaiced pixels of one row segment of the fast kernels: row parity PY, the segment starting at an even
+// column.  n / c / s: the segments of the rows above, at and below; hl / hr: their halo samples (above, at, below).
 // left_edge / right_edge: the segment holds column 0 / w-1, which copy columns 1 / w-2.
-template <int P, int PY, int NW>
+template <int P, int PY, int NW, typename T = uint8_t>
 __device__ __forceinline__ void bayer_row(const uint32_t n[NW], const uint32_t c[NW], const uint32_t s[NW], const int hl[3], const int hr[3],
-                                          bool left_edge, bool right_edge, int r[4 * NW], int g[4 * NW], int b[4 * NW]) {
+                                          bool left_edge, bool right_edge, int r[bayer_per_word<T>() * NW],
+                                          int g[bayer_per_word<T>() * NW], int b[bayer_per_word<T>() * NW]) {
+    constexpr int N = bayer_per_word<T>() * NW;
 #pragma unroll
-    for (int j = 0; j < 4 * NW; ++j) {
-        const int d = bayer_seg_byte<NW>(n, hl[0], hr[0], j - 1) + bayer_seg_byte<NW>(n, hl[0], hr[0], j + 1) +
-                      bayer_seg_byte<NW>(s, hl[2], hr[2], j - 1) + bayer_seg_byte<NW>(s, hl[2], hr[2], j + 1);
-        bayer_demosaic(P, j & 1, PY, bayer_seg_byte<NW>(c, hl[1], hr[1], j), bayer_seg_byte<NW>(n, hl[0], hr[0], j),
-                       bayer_seg_byte<NW>(s, hl[2], hr[2], j), bayer_seg_byte<NW>(c, hl[1], hr[1], j - 1),
-                       bayer_seg_byte<NW>(c, hl[1], hr[1], j + 1), d, r[j], g[j], b[j]);
+    for (int j = 0; j < N; ++j) {
+        const int d = bayer_seg_sample<NW, T>(n, hl[0], hr[0], j - 1) + bayer_seg_sample<NW, T>(n, hl[0], hr[0], j + 1) +
+                      bayer_seg_sample<NW, T>(s, hl[2], hr[2], j - 1) + bayer_seg_sample<NW, T>(s, hl[2], hr[2], j + 1);
+        bayer_demosaic(P, j & 1, PY, bayer_seg_sample<NW, T>(c, hl[1], hr[1], j), bayer_seg_sample<NW, T>(n, hl[0], hr[0], j),
+                       bayer_seg_sample<NW, T>(s, hl[2], hr[2], j), bayer_seg_sample<NW, T>(c, hl[1], hr[1], j - 1),
+                       bayer_seg_sample<NW, T>(c, hl[1], hr[1], j + 1), d, r[j], g[j], b[j]);
     }
-    constexpr int L = 4 * NW - 1;
+    constexpr int L = N - 1;
     if (left_edge) { r[0] = r[1]; g[0] = g[1]; b[0] = b[1]; }
     if (right_edge) { r[L] = r[L - 1]; g[L] = g[L - 1]; b[L] = b[L - 1]; }
 }
 
 // Loads the four rows ya-1 .. ya+2 of a lane's NW-word segment at column x (row index clamped to h-1: row ya+2 = h
-// when h is odd is never used), and the halo byte on each side of it.  The halos come from the neighbouring lanes'
-// words by shuffle; the warp's edge lanes load theirs.  Every lane of the warp must call; a lane whose neighbour holds
-// another row pair's segment has its halo there at column -1 or w, which the border copy never reads.
-template <int NW, typename LOAD>
-__device__ __forceinline__ void bayer_load_rows(const uint8_t* __restrict__ frame, size_t pitch, uint32_t w, uint32_t h, uint32_t x,
+// when h is odd is never used), and the halo sample on each side of it.  `pitch` is in samples.  The halos come from
+// the neighbouring lanes' words by shuffle; the warp's edge lanes load theirs.  Every lane of the warp must call; a lane
+// whose neighbour holds another row pair's segment has its halo there at column -1 or w, which the border copy never reads.
+template <int NW, typename T, typename LOAD>
+__device__ __forceinline__ void bayer_load_rows(const T* __restrict__ frame, size_t pitch, uint32_t w, uint32_t h, uint32_t x,
                                                 uint32_t ya, uint32_t lane, LOAD load, uint32_t rows[4][NW], int hl[4], int hr[4]) {
+    constexpr int S = bayer_per_word<T>(), B = bayer_bits<T>();
+    constexpr uint32_t M = (1u << B) - 1u;
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-        const uint8_t* row = frame + (size_t)min(ya - 1 + k, h - 1) * pitch;
+        const T* row = frame + (size_t)min(ya - 1 + k, h - 1) * pitch;
         load(row + x, rows[k]);
-        hl[k] = (int)(__shfl_up_sync(0xFFFFFFFFu, rows[k][NW - 1], 1) >> 24);
-        hr[k] = (int)(__shfl_down_sync(0xFFFFFFFFu, rows[k][0], 1) & 0xFFu);
+        hl[k] = (int)(__shfl_up_sync(0xFFFFFFFFu, rows[k][NW - 1], 1) >> (32 - B));
+        hr[k] = (int)(__shfl_down_sync(0xFFFFFFFFu, rows[k][0], 1) & M);
         if (lane == 0 && x > 0) hl[k] = __ldg(row + x - 1);
-        if (lane == 31 && x + 4 * NW < w) hr[k] = __ldg(row + x + 4 * NW);
+        if (lane == 31 && x + S * NW < w) hr[k] = __ldg(row + x + S * NW);
     }
 }
 

@@ -1,9 +1,11 @@
 // preprocess.cu — the fused camera preprocess (a12; BASELINE config 3): raw frame (RGB/BGR/RGBA/
-// Gray/NV12/YUYV, tight or pitched; beyond the reference also NV21/I420/YV12/UYVY/YVYU and the Bayer mosaics) →
+// Gray/NV12/YUYV, tight or pitched; beyond the reference also NV21/I420/YV12/UYVY/YVYU and the 8- and 16-bit Bayer
+// mosaics) →
 // letterbox/stretch resample → (v/255 - mean) * inv_std → planar CHW f32 or f16, for a whole batch in ONE launch.
 // The 4:2:0 formats share the NV12 kernels (templated on the chroma layout); the 4:2:2 formats take the generic kernel.
 // A Bayer tap is the demosaiced pixel at the tap's coordinate (bayer.cuh); Bayer frames take the generic kernel, except
-// the identity geometry, which has its own fast kernel.
+// the identity geometry, which has its own fast kernel.  A 16-bit Bayer tap is normalised against the white level
+// W = 2^bits - 1 of its format: (px / W - mean) * inv_std, px / W the IEEE quotient.
 //
 // Reference: preprocess.rs:430-647 (the CUDA source string — the specification of this path; there
 // is no CPU implementation for the camera formats), launch seam :1324-1372, batch loop :1277-1280
@@ -95,13 +97,23 @@ __device__ __forceinline__ void fetch_px_yuv_ext(const uint8_t* __restrict__ src
 }
 
 // Which formats an instantiation of the generic kernel serves: the reference's (fmt 0-4), the YUV layouts beyond them
-// (fmt 5-9) or the Bayer mosaics (fmt 16-19).  Separate instantiations, so the kernels of fmt 0-4 are unchanged by the others.
-static constexpr int SRC_BASE = 0, SRC_EXT_YUV = 1, SRC_BAYER = 2;
+// (fmt 5-9), the 8-bit Bayer mosaics (fmt 16-19) or the 16-bit ones (fmt 32-47).  Separate instantiations, so the
+// kernels of fmt 0-4 are unchanged by the others.
+static constexpr int SRC_BASE = 0, SRC_EXT_YUV = 1, SRC_BAYER = 2, SRC_BAYER16 = 3;
+
+// fmt 32-47 = 32 + 4*k + kb200_bayer_pattern, k = 0..3 for 10, 12, 14 and 16 bits per sample
+__host__ __device__ inline int bayer16_pattern(int fmt) { return (fmt - KB200_FMT_BAYER_RGGB10) & 3; }
+__host__ __device__ inline int bayer16_bits(int fmt) { return 10 + 2 * ((fmt - KB200_FMT_BAYER_RGGB10) >> 2); }
+__host__ __device__ inline float bayer16_white(int fmt) { return (float)((1u << bayer16_bits(fmt)) - 1u); }
 
 template <int EXT>
 __device__ __forceinline__ void fetch_px(const uint8_t* __restrict__ src, int x, int y, const kb200_preprocess_desc& d,
                                          float px[3]) {  // :510-530
-    if (EXT == SRC_BAYER) {
+    if (EXT == SRC_BAYER16) {   // src_pitch is in bytes and even
+        int rgb[3];
+        bayer_px(reinterpret_cast<const uint16_t*>(src), (size_t)d.src_pitch / 2, d.src_w, d.src_h, x, y, bayer16_pattern(d.fmt), rgb);
+        px[0] = (float)rgb[0]; px[1] = (float)rgb[1]; px[2] = (float)rgb[2];
+    } else if (EXT == SRC_BAYER) {
         int rgb[3];
         bayer_px(src, (size_t)d.src_pitch, d.src_w, d.src_h, x, y, d.fmt - KB200_FMT_BAYER_RGGB, rgb);
         px[0] = (float)rgb[0]; px[1] = (float)rgb[1]; px[2] = (float)rgb[2];
@@ -200,7 +212,10 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
         px[0] = d.pad_value; px[1] = d.pad_value; px[2] = d.pad_value;
     }
     float q0, q1, q2;
-    if (inside && SAMP != KB200_INTERP_LANCZOS) { q0 = div255_exact(px[0]); q1 = div255_exact(px[1]); q2 = div255_exact(px[2]); }
+    if (EXT == SRC_BAYER16 && inside) {   // px / W: taps up to 65535 and Lanczos overshoot, so the IEEE division
+        const float wl = bayer16_white(d.fmt);
+        q0 = __fdiv_rn(px[0], wl); q1 = __fdiv_rn(px[1], wl); q2 = __fdiv_rn(px[2], wl);
+    } else if (inside && SAMP != KB200_INTERP_LANCZOS) { q0 = div255_exact(px[0]); q1 = div255_exact(px[1]); q2 = div255_exact(px[2]); }
     else if (inside) { q0 = __fdiv_rn(px[0], 255.0f); q1 = __fdiv_rn(px[1], 255.0f); q2 = __fdiv_rn(px[2], 255.0f); }  // Lanczos overshoots [0, 255]
     else { q0 = __fdiv_rn(px[0], 255.0f); q1 = q0; q2 = q0; }  // pad_value is caller-supplied: plain IEEE division
     const float o0 = (q0 - d.mean[0]) * d.inv_std[0];
@@ -352,6 +367,61 @@ __global__ void __launch_bounds__(128) preprocess_bayer_identity_kernel(const __
     if (yb == h - 2u) store_row(h - 1u);
 }
 
+// ── 16-bit Bayer identity fast path (the config-3a shape from a 10- to 16-bit mosaic) ─────────────────────────
+// The 8-bit kernel above on 2-byte samples: one thread = 4 columns x 2 output rows, 4 lane-contiguous LDG.64 of the rows
+// ya-1 .. ya+2 (256 contiguous bytes per warp and row) plus shuffled halo samples, the same 6 to 12 lane-contiguous
+// 4-pixel stores.  px / W is the IEEE division (W = bayer16_white(fmt)).  Requires w % 4 == 0 and 8-B aligned rows.
+template <bool F16, bool PTRS, int P>
+__global__ void __launch_bounds__(128) preprocess_bayer16_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
+                                                                          const __grid_constant__ PreFrames fr, void* __restrict__ dst,
+                                                                          uint32_t frame0, uint32_t groups_per_row, uint32_t items) {
+    const uint32_t item = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool active = item < items;                         // the lanes past the end still take part in the shuffles
+    const uint32_t it = active ? item : items - 1;
+    const uint32_t rp = it / groups_per_row, g = it - rp * groups_per_row;
+    const uint32_t w = (uint32_t)d.src_w, h = (uint32_t)d.src_h;
+    const uint32_t f = blockIdx.y;
+    const uint16_t* src = reinterpret_cast<const uint16_t*>(PTRS ? fr.ptr[f] : fr.base + (size_t)(frame0 + f) * fr.stride);
+    const uint32_t x = g * 4u, ya = 1u + 2u * rp, yb = ya + 1u;
+    uint32_t rows[4][2];
+    int hl[4], hr[4];
+    bayer_load_rows<2>(src, (size_t)d.src_pitch / 2, w, h, x, ya, threadIdx.x & 31u, [](const uint16_t* p, uint32_t v[2]) {
+        const uint2 q = __ldg(reinterpret_cast<const uint2*>(p));
+        v[0] = q.x; v[1] = q.y;
+    }, rows, hl, hr);
+    if (!active) return;
+    const bool left_edge = x == 0, right_edge = x + 4u == w;
+    const size_t plane = (size_t)w * h;
+    const size_t base = (size_t)(frame0 + f) * 3 * plane + x;
+    const float wl = bayer16_white(d.fmt);
+    const float m0 = d.mean[0], m1 = d.mean[1], m2 = d.mean[2], i0 = d.inv_std[0], i1 = d.inv_std[1], i2 = d.inv_std[2];
+    float r4[4], g4[4], b4[4];
+    auto store_row = [&](uint32_t y) {
+        const size_t o = base + (size_t)y * w;
+        nv12_store4<F16>(dst, o, r4);
+        nv12_store4<F16>(dst, o + plane, g4);
+        nv12_store4<F16>(dst, o + 2 * plane, b4);
+    };
+    auto norm = [&](const int r[4], const int gg[4], const int b[4]) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            r4[i] = (__fdiv_rn((float)r[i], wl) - m0) * i0;
+            g4[i] = (__fdiv_rn((float)gg[i], wl) - m1) * i1;
+            b4[i] = (__fdiv_rn((float)b[i], wl) - m2) * i2;
+        }
+    };
+    int r[4], gg[4], b[4];
+    bayer_row<P, 1, 2, uint16_t>(rows[0], rows[1], rows[2], hl, hr, left_edge, right_edge, r, gg, b);   // ya is odd
+    norm(r, gg, b);
+    store_row(ya);
+    if (ya == 1u) store_row(0);
+    if (yb == h - 1u) { store_row(yb); return; }
+    bayer_row<P, 0, 2, uint16_t>(rows[1], rows[2], rows[3], hl + 1, hr + 1, left_edge, right_edge, r, gg, b);
+    norm(r, gg, b);
+    store_row(yb);
+    if (yb == h - 2u) store_row(h - 1u);
+}
+
 // ── NV12 general path (config 3b: 1080p NV12 → letterboxed 640x640, and every other NV12 geometry) ──────────
 // ncu on the generic kernel for config 3b: issue-bound (format switch, integer div/mod for (ox, oy), byte-granular
 // everything), DRAM mostly idle.  This kernel is NV12-only:
@@ -490,6 +560,7 @@ static int yuv420_layout(int fmt) {
 }
 static bool is_yuv422(int fmt) { return fmt == KB200_FMT_YUYV || fmt == KB200_FMT_UYVY || fmt == KB200_FMT_YVYU; }
 static bool is_bayer(int fmt) { return fmt >= KB200_FMT_BAYER_RGGB && fmt <= KB200_FMT_BAYER_GBRG; }
+static bool is_bayer16(int fmt) { return fmt >= KB200_FMT_BAYER_RGGB10 && fmt <= KB200_FMT_BAYER_GBRG16; }
 // SourceFormat names, in the validation messages
 static const char* const FMT_NAMES[10] = {"Rgb8", "Bgr8", "Gray8", "Nv12", "Yuyv", "Nv21", "I420", "Yv12", "Uyvy", "Yvyu"};
 static const char* const BAYER_NAMES[4] = {"BayerRggb", "BayerBggr", "BayerGrbg", "BayerGbrg"};
@@ -506,7 +577,7 @@ static int validate_desc(const kb200_preprocess_desc* dp) {
     if (d.src_w <= 0 || d.src_h <= 0 || d.dst_w <= 0 || d.dst_h <= 0)
         return fail(KB200_ERR_INVALID_ARGUMENT, "image dimensions must be non-zero");
     if ((long long)d.dst_w * d.dst_h > 0x7FFFFFFFll) return fail(KB200_ERR_DIMS_TOO_LARGE, "dimensions exceed the 32-bit CUDA kernel index limit");  // :1336-1339
-    if (d.fmt < 0 || (d.fmt > KB200_FMT_YVYU && !is_bayer(d.fmt))) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown source format code %d", d.fmt);
+    if (d.fmt < 0 || (d.fmt > KB200_FMT_YVYU && !is_bayer(d.fmt) && !is_bayer16(d.fmt))) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown source format code %d", d.fmt);
     if (d.sampling != KB200_INTERP_NEAREST && d.sampling != KB200_INTERP_BILINEAR && d.sampling != KB200_INTERP_LANCZOS)
         return fail(KB200_ERR_UNSUPPORTED, "unsupported sampling mode %d (expected Nearest, Bilinear or Lanczos)", d.sampling);  // preprocess.rs:1044-1051
     if (d.fmt <= 1 && d.src_bpp != 3 && d.src_bpp != 4) return fail(KB200_ERR_UNSUPPORTED, "unsupported source channel count %d (expected 3 or 4)", d.src_bpp);
@@ -516,7 +587,15 @@ static int validate_desc(const kb200_preprocess_desc* dp) {
     if (is_yuv422(d.fmt) && (d.src_w & 1)) return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s at %dx%d (even width required)", FMT_NAMES[d.fmt], d.src_w, d.src_h);
     if (is_bayer(d.fmt) && (d.src_w < 3 || d.src_h < 3))
         return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s at %dx%d (at least 3x3 required)", BAYER_NAMES[d.fmt - KB200_FMT_BAYER_RGGB], d.src_w, d.src_h);
-    const int bpp = d.fmt <= 1 ? d.src_bpp : (is_yuv422(d.fmt) ? 2 : 1);
+    if (is_bayer16(d.fmt)) {   // SourceFormat names: BayerRggb10 ... BayerGbrg16
+        const char* name = BAYER_NAMES[bayer16_pattern(d.fmt)];
+        const int bits = bayer16_bits(d.fmt);
+        if (d.src_w < 3 || d.src_h < 3)
+            return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s%d at %dx%d (at least 3x3 required)", name, bits, d.src_w, d.src_h);
+        if (d.src_pitch & 1)
+            return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface for %s%d (pitch %d is odd: rows of 16-bit samples must start 2-byte aligned)", name, bits, d.src_pitch);
+    }
+    const int bpp = d.fmt <= 1 ? d.src_bpp : (is_yuv422(d.fmt) || is_bayer16(d.fmt) ? 2 : 1);
     if ((long long)d.src_pitch < (long long)d.src_w * bpp) return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface (need pitch >= width*channels and len >= pitch*height)");
     if (l420 >= 0 && d.src_pitch != d.src_w) return fail(KB200_ERR_INVALID_SOURCE, "%s frames must be tightly packed (pitch == width)", YUV420_UPPER[l420]);
     if (!(d.scale_x > 0.0f) || !(d.scale_y > 0.0f)) return fail(KB200_ERR_INVALID_ARGUMENT, "scale must be positive");
@@ -549,6 +628,15 @@ static void launch_bayer_identity(cudaStream_t s, const kb200_preprocess_desc& d
     else preprocess_bayer_identity_kernel<F16, false, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
 }
 
+// The 16-bit Bayer identity kernel of pattern P, for one launch of <= 256 frames.
+template <bool F16, int P>
+static void launch_bayer16_identity(cudaStream_t s, const kb200_preprocess_desc& d, const PreFrames& fr, bool ptrs, void* dst, uint32_t f0,
+                                    uint32_t nb, uint32_t id_groups, size_t id_items) {
+    dim3 grid(div_up(id_items, 128), nb);
+    if (ptrs) preprocess_bayer16_identity_kernel<F16, true, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
+    else preprocess_bayer16_identity_kernel<F16, false, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
+}
+
 template <bool F16, bool PTRS, int EXT>
 static void launch_generic(cudaStream_t s, dim3 grid, int sampling, const kb200_preprocess_desc& d, const PreFrames& fr, void* dst, uint32_t f0) {
     if (sampling == KB200_INTERP_LANCZOS) preprocess_generic_kernel<F16, KB200_INTERP_LANCZOS, PTRS, EXT><<<grid, 256, 0, s>>>(d, fr, dst, f0);
@@ -559,7 +647,8 @@ static void launch_generic(cudaStream_t s, dim3 grid, int sampling, const kb200_
 template <bool F16, bool PTRS>
 static void launch_generic_for(int ext, cudaStream_t s, dim3 grid, int sampling, const kb200_preprocess_desc& d, const PreFrames& fr, void* dst,
                                uint32_t f0) {
-    if (ext == SRC_BAYER) launch_generic<F16, PTRS, SRC_BAYER>(s, grid, sampling, d, fr, dst, f0);
+    if (ext == SRC_BAYER16) launch_generic<F16, PTRS, SRC_BAYER16>(s, grid, sampling, d, fr, dst, f0);
+    else if (ext == SRC_BAYER) launch_generic<F16, PTRS, SRC_BAYER>(s, grid, sampling, d, fr, dst, f0);
     else if (ext == SRC_EXT_YUV) launch_generic<F16, PTRS, SRC_EXT_YUV>(s, grid, sampling, d, fr, dst, f0);
     else launch_generic<F16, PTRS, SRC_BASE>(s, grid, sampling, d, fr, dst, f0);
 }
@@ -570,6 +659,8 @@ static const char* const YUV420_IDENTITY_NAMES[4] = {"preprocess_nv12_identity_k
 static const char* const YUV420_FAST_NAMES[4] = {"preprocess_nv12_kernel", "preprocess_nv21_kernel", "preprocess_i420_kernel", "preprocess_yv12_kernel"};
 static const char* const BAYER_IDENTITY_NAMES[4] = {"preprocess_bayer_rggb_identity_kernel", "preprocess_bayer_bggr_identity_kernel",
                                                     "preprocess_bayer_grbg_identity_kernel", "preprocess_bayer_gbrg_identity_kernel"};
+static const char* const BAYER16_IDENTITY_NAMES[4] = {"preprocess_bayer16_rggb_identity_kernel", "preprocess_bayer16_bggr_identity_kernel",
+                                                      "preprocess_bayer16_grbg_identity_kernel", "preprocess_bayer16_gbrg_identity_kernel"};
 
 template <bool F16>
 static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, const uint8_t* const* frames,
@@ -577,21 +668,23 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
     const int pixels = d.dst_w * d.dst_h;
     const bool bil = d.sampling == KB200_INTERP_BILINEAR, lanczos = d.sampling == KB200_INTERP_LANCZOS;
     const int l420 = yuv420_layout(d.fmt);
-    const bool bayer = is_bayer(d.fmt);
+    const bool bayer = is_bayer(d.fmt), bayer16 = is_bayer16(d.fmt);
     // identity fast path: a 4:2:0 or Bayer format, scale 1, no pad, same size, 8-column vectors possible
-    // (Lanczos always takes the generic kernel: its off-centre weights at integer coordinates are sinf(k*pi) != 0 exactly)
-    bool identity = !lanczos && (l420 >= 0 || bayer) && d.scale_x == 1.0f && d.scale_y == 1.0f && d.pad_x == 0.0f && d.pad_y == 0.0f &&
-                    d.dst_w == d.src_w && d.dst_h == d.src_h && (d.src_w % 4) == 0 && (d.src_pitch % 4) == 0 && aligned16(dst);
+    // (Lanczos always takes the generic kernel: its off-centre weights at integer coordinates are sinf(k*pi) != 0 exactly).
+    // A thread loads 4 samples per row: 4 B aligned rows and frames, 8 B for 16-bit Bayer.
+    const uint32_t row_align = bayer16 ? 8u : 4u;
+    bool identity = !lanczos && (l420 >= 0 || bayer || bayer16) && d.scale_x == 1.0f && d.scale_y == 1.0f && d.pad_x == 0.0f && d.pad_y == 0.0f &&
+                    d.dst_w == d.src_w && d.dst_h == d.src_h && (d.src_w % 4) == 0 && (d.src_pitch % row_align) == 0 && aligned16(dst);
     if (identity) {
-        if (frames) { for (uint32_t k = 0; k < batch; ++k) identity = identity && ((reinterpret_cast<uintptr_t>(frames[k]) & 3u) == 0); }
-        else identity = ((reinterpret_cast<uintptr_t>(base) & 3u) == 0) && (stride % 4 == 0);
+        if (frames) { for (uint32_t k = 0; k < batch; ++k) identity = identity && ((reinterpret_cast<uintptr_t>(frames[k]) & (row_align - 1)) == 0); }
+        else identity = ((reinterpret_cast<uintptr_t>(base) & (row_align - 1)) == 0) && (stride % row_align == 0);
     }
     const uint32_t id_groups = (uint32_t)d.src_w / 4u;
-    const size_t id_items = (size_t)id_groups * (bayer ? bayer_row_pairs((uint32_t)d.src_h) : (size_t)d.src_h / 2);
+    const size_t id_items = (size_t)id_groups * (bayer || bayer16 ? bayer_row_pairs((uint32_t)d.src_h) : (size_t)d.src_h / 2);
     if (id_items > 0x7FFFFFFFull) identity = false;
     // 4:2:0 general fast path: vector stores need dst_w % 4 == 0 and a 16-B (f32) / 8-B (f16) aligned destination
     const bool yuv420_fast = !lanczos && l420 >= 0 && (d.dst_w % 4) == 0 && aligned16(dst) && d.dst_h <= 65535 * NV12_ROWS;
-    const int ext = bayer ? SRC_BAYER : d.fmt >= KB200_FMT_NV21 ? SRC_EXT_YUV : SRC_BASE;
+    const int ext = bayer16 ? SRC_BAYER16 : bayer ? SRC_BAYER : d.fmt >= KB200_FMT_NV21 ? SRC_EXT_YUV : SRC_BASE;
     Nv12Args nv{};
     nv.groups = (uint32_t)(d.dst_w + 3) / 4u;
     for (int c = 0; c < 3; ++c) nv.pad_norm[c] = (d.pad_value / 255.0f - d.mean[c]) * d.inv_std[c];  // BODY :610-612 on the host (f32, unfused)
@@ -609,6 +702,16 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
                 default: launch_bayer_identity<F16, KB200_BAYER_GBRG>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
             }
             KB200_TRY(check_launch(BAYER_IDENTITY_NAMES[d.fmt - KB200_FMT_BAYER_RGGB]));
+            continue;
+        }
+        if (identity && bayer16) {
+            switch (bayer16_pattern(d.fmt)) {
+                case KB200_BAYER_RGGB: launch_bayer16_identity<F16, KB200_BAYER_RGGB>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
+                case KB200_BAYER_BGGR: launch_bayer16_identity<F16, KB200_BAYER_BGGR>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
+                case KB200_BAYER_GRBG: launch_bayer16_identity<F16, KB200_BAYER_GRBG>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
+                default: launch_bayer16_identity<F16, KB200_BAYER_GBRG>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
+            }
+            KB200_TRY(check_launch(BAYER16_IDENTITY_NAMES[bayer16_pattern(d.fmt)]));
             continue;
         }
         if (identity || yuv420_fast) {
@@ -644,9 +747,15 @@ static int preprocess_entry(kb200_stream_t stream, const kb200_preprocess_desc* 
     KB200_TRY(check_ptr("dst", dst));
     if (batch == 0) return fail(KB200_ERR_INVALID_ARGUMENT, "batch must be non-zero");
     const size_t need = src_bytes(*desc);
+    const bool bayer16 = is_bayer16(desc->fmt);   // 16-bit samples: every frame must start 2-byte aligned
+    if (bayer16 && !frames && ((reinterpret_cast<uintptr_t>(base) & 1u) || (batch > 1 && (stride & 1u))))
+        return fail(KB200_ERR_INVALID_SOURCE, "%s%d frames must start 2-byte aligned (base %p, stride %zu)", BAYER_NAMES[bayer16_pattern(desc->fmt)],
+                    bayer16_bits(desc->fmt), (const void*)base, stride);
     if (frames) {
         for (uint32_t i = 0; i < batch; ++i) {
             if (!frames[i]) return fail(KB200_ERR_INVALID_ARGUMENT, "null frame pointer at index %u", i);
+            if (bayer16 && (reinterpret_cast<uintptr_t>(frames[i]) & 1u))
+                return fail(KB200_ERR_INVALID_SOURCE, "%s%d frame %u is not 2-byte aligned", BAYER_NAMES[bayer16_pattern(desc->fmt)], bayer16_bits(desc->fmt), i);
             if (frame_len && frame_len[i] < need)  // InvalidRawSource{got,need}, preprocess.rs:1287-1300
                 return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source at %dx%d (got %zu bytes, need %zu)", desc->src_w, desc->src_h, frame_len[i], need);
         }

@@ -101,7 +101,7 @@ class ImageSize:
     height: int
 
 
-_TYPESTR = {torch.float32: "<f4", torch.float16: "<f2", torch.uint8: "|u1", torch.float64: "<f8"}
+_TYPESTR = {torch.float32: "<f4", torch.float16: "<f2", torch.uint8: "|u1", torch.float64: "<f8", torch.uint16: "<u2"}
 
 
 class Image:

@@ -602,6 +602,32 @@ def rgb_from_bayer(src, dst: Image, pattern: BayerPattern) -> None:
     _rgb_from_yuv(src, dst, "rgb_from_bayer", 1, 1, "kb200_rgb_from_bayer_u8", int(BayerPattern(pattern)))
 
 
+def rgb_from_bayer16(src, dst: Image, pattern: BayerPattern) -> None:
+    """10- to 16-bit Bayer mosaic -> RGB with 16-bit channels: the demosaic of rgb_from_bayer on the 16-bit values
+    (cv2.cvtColor gives the same bits on uint16 mosaics).  `src`: uint16 device tensor holding N tight frames of w*h
+    samples, each an LSB-aligned little-endian word (V4L2's unpacked SRGGB10 ... SGBRG16); `dst`: a uint16 Image
+    [N, h, w, 3].  The bit depth plays no part: the output is the same whatever it is."""
+    code = int(BayerPattern(pattern))
+    t = src.data if isinstance(src, Image) else src
+    if not t.is_cuda:
+        raise ImageError.HostPathNotBuilt("rgb_from_bayer16")
+    if t.dtype != torch.uint16:
+        raise ImageError.DtypeMismatch(torch.uint16, t.dtype)
+    if not t.is_contiguous():
+        raise ImageError.ImageDataNotContiguous()
+    if not dst.is_device:
+        raise ImageError.MixedResidency()
+    if t.device != dst.device:
+        raise ImageError.DeviceMismatch()
+    _expect_dtype(dst, torch.uint16, "dst")
+    w, h, n = dst.cols(), dst.rows(), dst.batch
+    need = w * h * n
+    if dst.num_channels() != 3 or t.numel() != need:
+        raise ImageError.InvalidImageSize(t.numel(), 1, need, 1)
+    _lib.set_device(t.device.index)
+    _check(_lib.lib().kb200_rgb_from_bayer_u16(_stream(t.device), t.data_ptr(), t.numel(), dst.data.data_ptr(), dst.numel(), w, h, n, code))
+
+
 def _encode(op: str, fn_name: str, src: Image, dst: torch.Tensor, bytes_per_px_num: int, bytes_per_px_den: int, need_even_h: bool) -> None:
     if not src.is_device:
         raise ImageError.HostPathNotBuilt(op)

@@ -2,7 +2,7 @@
 
 Built once via `Preprocessor.builder()…build_cuda()`, then applied to any number of frames of any
 resolution: the target H/W is read from the destination tensor each call.  Camera formats
-(NV12 / YUYV / Gray, the other YUV layouts and the Bayer mosaics) go through `run_raw*`; colour decode is fused into the resample taps.  Unlike the
+(NV12 / YUYV / Gray, the other YUV layouts and the 8- to 16-bit Bayer mosaics) go through `run_raw*`; colour decode is fused into the resample taps.  Unlike the
 reference (one launch per frame, preprocess.rs:1277-1280) a batch is ONE launch.
 
 Only the CUDA preprocessor exists here (`build()` = the reference's CPU preprocessor is out of scope:
@@ -38,6 +38,9 @@ class ResizeMode(enum.Enum):  # preprocess.rs:67
     Stretch = 1
 
 
+_BAYER_PATTERNS = ("rggb", "bggr", "grbg", "gbrg")   # kb200_bayer_pattern order
+
+
 class SourceFormat(enum.Enum):  # preprocess.rs:130
     Rgb8 = "rgb8"
     Bgr8 = "bgr8"
@@ -59,13 +62,36 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
     BayerBggr = "bayer_bggr"
     BayerGrbg = "bayer_grbg"
     BayerGbrg = "bayer_gbrg"
+    # 10- to 16-bit Bayer mosaics: one little-endian 16-bit word per sample, the value in its low bits (V4L2's unpacked
+    # SRGGB10 ... SGBRG16), rows of 2*w bytes.  The demosaic is the 8-bit one on the 16-bit values; the bit depth sets
+    # only the white level W = 2^bits - 1 a tap is normalised by, (px / W - mean) * inv_std.  pad_value stays 0..255.
+    BayerRggb10 = "bayer_rggb10"
+    BayerBggr10 = "bayer_bggr10"
+    BayerGrbg10 = "bayer_grbg10"
+    BayerGbrg10 = "bayer_gbrg10"
+    BayerRggb12 = "bayer_rggb12"
+    BayerBggr12 = "bayer_bggr12"
+    BayerGrbg12 = "bayer_grbg12"
+    BayerGbrg12 = "bayer_gbrg12"
+    BayerRggb14 = "bayer_rggb14"
+    BayerBggr14 = "bayer_bggr14"
+    BayerGrbg14 = "bayer_grbg14"
+    BayerGbrg14 = "bayer_gbrg14"
+    BayerRggb16 = "bayer_rggb16"
+    BayerBggr16 = "bayer_bggr16"
+    BayerGrbg16 = "bayer_grbg16"
+    BayerGbrg16 = "bayer_gbrg16"
 
     def fmt_code(self) -> int:  # :153-161
+        if self.is_bayer16():   # 32 + 4*k + pattern, k = 0..3 for 10, 12, 14, 16 bits
+            return 32 + 4 * ((self.bit_depth() - 10) // 2) + _BAYER_PATTERNS.index(self.value[6:10])
         return {"rgb8": 0, "rgba8": 0, "bgr8": 1, "bgra8": 1, "gray8": 2, "nv12": 3, "yuyv": 4,
                 "nv21": 5, "i420": 6, "yv12": 7, "uyvy": 8, "yvyu": 9,
                 "bayer_rggb": 16, "bayer_bggr": 17, "bayer_grbg": 18, "bayer_gbrg": 19}[self.value]
 
     def bpp(self) -> int:  # :164-171
+        if self.is_bayer16():
+            return 2
         return {"rgb8": 3, "bgr8": 3, "rgba8": 4, "bgra8": 4, "gray8": 1, "nv12": 1, "yuyv": 2,
                 "nv21": 1, "i420": 1, "yv12": 1, "uyvy": 2, "yvyu": 2,
                 "bayer_rggb": 1, "bayer_bggr": 1, "bayer_grbg": 1, "bayer_gbrg": 1}[self.value]
@@ -81,6 +107,16 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
 
     def is_bayer(self) -> bool:
         return self.value.startswith("bayer_")
+
+    def is_bayer16(self) -> bool:
+        """A Bayer format of 16-bit samples (10 to 16 bits per pixel)."""
+        return self.is_bayer() and len(self.value) > 10
+
+    def bit_depth(self) -> int | None:
+        """Bits per sample of a Bayer format (8 for the byte mosaics), None for the other formats."""
+        if not self.is_bayer():
+            return None
+        return int(self.value[10:]) if self.is_bayer16() else 8
 
     def buffer_len(self, w: int, h: int) -> int:  # :177-186
         chroma = w * h // 2 if self.is_yuv420() else 0
@@ -104,6 +140,7 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
                  "bgra": "Bgra8", "bgra8": "Bgra8", "gray": "Gray8", "gray8": "Gray8", "nv12": "Nv12", "yuyv": "Yuyv",
                  "nv21": "Nv21", "i420": "I420", "yv12": "Yv12", "uyvy": "Uyvy", "yvyu": "Yvyu",
                  "bayer_rggb": "BayerRggb", "bayer_bggr": "BayerBggr", "bayer_grbg": "BayerGrbg", "bayer_gbrg": "BayerGbrg"}
+        table.update({f"bayer_{p}{b}": f"Bayer{p.capitalize()}{b}" for p in _BAYER_PATTERNS for b in (10, 12, 14, 16)})
         key = table.get(name.lower())
         return None if key is None else SourceFormat[key]
 
@@ -361,7 +398,7 @@ class Preprocessor:
                      f16: bool = False, pipeline=None) -> torch.Tensor:
         """HOST camera frames in, HOST tensor out — what the reference's Python `Preprocessor` does around its kernel (pinned
         staging, upload, launch: kornia-py/src/cuda_ext/mod.rs:700-760), as one call: `host_frames` is a [N, frame_bytes] uint8
-        host tensor (page-locked for overlap), the result a [N,3,H,W] f32 / f16 host tensor (pinned when allocated here).
+        host tensor, or [N, w*h] uint16 for the 16-bit Bayer formats (page-locked for overlap), the result a [N,3,H,W] f32 / f16 host tensor (pinned when allocated here).
         Chunks ride a `HostPipeline` ring: upload -> ONE fused launch per chunk -> download.  Enqueue-only: synchronise the
         current stream of the pipeline's device before reading the result."""
         from . import imgproc
@@ -369,9 +406,9 @@ class Preprocessor:
         t = host_frames
         if t.is_cuda:
             raise PreprocessError("NotDeviceImage", "run_raw_host takes host frames; use run_raw_batch / run_raw_strided for device frames")
-        if t.dtype != torch.uint8 or t.dim() != 2 or not t.is_contiguous():
-            raise PreprocessError("InvalidRawSource", "host frames must be a contiguous [N, frame_bytes] uint8 tensor")
-        n, stride = t.shape
+        if t.dtype not in (torch.uint8, torch.uint16) or t.dim() != 2 or not t.is_contiguous():
+            raise PreprocessError("InvalidRawSource", "host frames must be a contiguous [N, frame_bytes] uint8 or [N, samples] uint16 tensor")
+        n, stride = t.shape[0], t.shape[1] * t.element_size()   # bytes
         self._validate_raw(stride, src_w, src_h)
         dw, dh = dst_size
         want = torch.float16 if f16 else torch.float32
@@ -383,7 +420,7 @@ class Preprocessor:
         desc = self._desc(src_w, src_h, fmt.pitch(src_w), fmt.bpp(), fmt.fmt_code(), dw, dh)
         pipe = imgproc._pipeline_for(pipeline)
         _lib.set_device(pipe.device.index)
-        st = _lib.lib().kb200_preprocess_host(pipe._h, torch.cuda.current_stream(pipe.device).cuda_stream, C.byref(desc), t.data_ptr(), t.numel(),
+        st = _lib.lib().kb200_preprocess_host(pipe._h, torch.cuda.current_stream(pipe.device).cuda_stream, C.byref(desc), t.data_ptr(), n * stride,
                                              stride, n, out.data_ptr(), out.numel(), 1 if f16 else 0)
         if st != _lib.OK:
             kind = {_lib.ERR_INVALID_SOURCE: "InvalidRawSource"}.get(st, "Cuda")
@@ -392,10 +429,12 @@ class Preprocessor:
 
     def run_raw_strided(self, base: torch.Tensor, frame_stride: int, batch: int, src_w: int, src_h: int,
                         dst: torch.Tensor, f16: bool = False) -> None:
-        """Frames at `base + i*frame_stride` bytes (a capture ring buffer): no pointer table."""
+        """Frames at `base + i*frame_stride` bytes (a capture ring buffer): no pointer table.  `base` may be uint8 or, for
+        the 16-bit Bayer formats, uint16: its length is counted in bytes."""
         self._validate_dst(dst, batch, f16)
         fmt = self._fmt
-        self._validate_raw(min(frame_stride, base.numel()) if batch > 1 else base.numel(), src_w, src_h)
+        nbytes = base.numel() * base.element_size()
+        self._validate_raw(min(frame_stride, nbytes) if batch > 1 else nbytes, src_w, src_h)
         desc = self._desc(src_w, src_h, fmt.pitch(src_w), fmt.bpp(), fmt.fmt_code(), dst.shape[3], dst.shape[2])
         if not base.is_cuda:
             raise PreprocessError("NotDeviceImage", "CUDA preprocessor requires a device-resident source image")
@@ -403,7 +442,7 @@ class Preprocessor:
         _lib.set_device(dev.index)
         l = _lib.lib()
         fn = l.kb200_preprocess_strided_f16 if f16 else l.kb200_preprocess_strided_f32
-        st = fn(torch.cuda.current_stream(dev).cuda_stream, C.byref(desc), base.data_ptr(), base.numel(), frame_stride, batch,
+        st = fn(torch.cuda.current_stream(dev).cuda_stream, C.byref(desc), base.data_ptr(), nbytes, frame_stride, batch,
                 dst.data_ptr(), dst.numel())
         if st != _lib.OK:
             kind = {_lib.ERR_INVALID_SOURCE: "InvalidRawSource"}.get(st, "Cuda")
