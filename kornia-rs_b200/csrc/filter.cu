@@ -191,17 +191,17 @@ template <int K> struct SobelTaps;
 template <> struct SobelTaps<3> { static constexpr int D[3] = {-1, 0, 1}; static constexpr int S[3] = {1, 2, 1}; };
 template <> struct SobelTaps<5> { static constexpr int D[5] = {-1, -2, 0, 2, 1}; static constexpr int S[5] = {1, 4, 6, 4, 1}; };
 
-// acc + v*k for a compile-time integer tap, bit-identical to the reference's unfused `acc += v * k`:
-//   k == 0      : v*0 = ±0 and acc + ±0 = acc (acc is never -0: every accumulation starts from +0.0) — skipped;
-//   |k| = 2^n   : the product is exact, so one FFMA (single rounding of acc + v*k) equals mul-then-add;
-//   otherwise   : mul, then add.
-// (Finite inputs, like the zero-halo argument in the file header.)
+// acc + v*k for a compile-time integer tap, bit-identical to the reference's unfused `acc += v * k` for every v:
+//   k == 0      : one FFMA, acc + v*0 with the product exact — acc for finite v (acc is never -0: every accumulation
+//                 starts from +0.0), NaN for v = ±inf or NaN, like the reference's 0 * inf;
+//   k == ±1     : the product is v itself, so acc ± v;
+//   otherwise   : mul, then add.  (An FFMA would be exact for |k| = 2^n only while v*k does not overflow: the
+//                 reference's product rounds to inf first, the fused sum may come back into range.)
 template <int KV>
 __device__ __forceinline__ float acc_tap(float acc, float v) {
-    if (KV == 0) return acc;
+    if (KV == 0) return fmaf(v, 0.0f, acc);
     if (KV == 1) return acc + v;
     if (KV == -1) return acc - v;
-    if ((KV & (KV - 1)) == 0 || ((-KV) & (-KV - 1)) == 0) return fmaf(v, (float)KV, acc);
     return acc + v * (float)KV;
 }
 template <int K, bool DERIV, int T>
@@ -209,7 +209,7 @@ struct SobelAcc {
     template <typename F>
     __device__ __forceinline__ static float run(float acc, F&& get) {
         constexpr int kv = DERIV ? SobelTaps<K>::D[T] : SobelTaps<K>::S[T];
-        acc = acc_tap<kv>(acc, kv == 0 ? 0.0f : get(T));
+        acc = acc_tap<kv>(acc, get(T));
         if constexpr (T + 1 < K) return SobelAcc<K, DERIV, T + 1>::run(acc, get);
         else return acc;
     }
@@ -249,8 +249,8 @@ __device__ __forceinline__ ss_u64 pair_add(ss_u64 a, ss_u64 b, const PairConst& 
 // acc + v*k on pairs for a compile-time integer tap (same case analysis as acc_tap above)
 template <int KV>
 __device__ __forceinline__ ss_u64 pair_acc_tap(ss_u64 acc, ss_u64 v, const PairConst& c) {
-    if (KV == 0) return acc;
-    if ((KV & (KV - 1)) == 0 || ((-KV) & (-KV - 1)) == 0) return ss_fma2(v, ss_pack((float)KV, (float)KV), acc);  // exact product: one rounding == two
+    if (KV == 0) return ss_fma2(v, c.zero, acc);                                                 // acc, or NaN for inf / NaN v
+    if (KV == 1 || KV == -1) return ss_fma2(v, ss_pack((float)KV, (float)KV), acc);              // product v or -v: one rounding == two
     return pair_add(acc, pair_mul(v, ss_pack((float)KV, (float)KV), c), c);
 }
 template <int K, bool DERIV, int T>
@@ -258,7 +258,7 @@ struct SobelAccPair {
     template <typename F>
     __device__ __forceinline__ static ss_u64 run(ss_u64 acc, const PairConst& c, F&& get) {
         constexpr int kv = DERIV ? SobelTaps<K>::D[T] : SobelTaps<K>::S[T];
-        if constexpr (kv != 0) acc = pair_acc_tap<kv>(acc, get(T), c);
+        acc = pair_acc_tap<kv>(acc, get(T), c);
         if constexpr (T + 1 < K) return SobelAccPair<K, DERIV, T + 1>::run(acc, c, get);
         else return acc;
     }

@@ -67,7 +67,11 @@ __global__ void __launch_bounds__(256) resize_f32_c3_kernel(const float* __restr
     const float w[4] = {gy * gx, gy * tx.f, ty.f * gx, ty.f * tx.f};          // taps (x0,y0) (x1,y0) (x0,y1) (x1,y1)
     const float* r0 = s + (size_t)ty.i0 * sw * 3;
     const float* r1 = s + (size_t)ty.i1 * sw * 3;
-    const float* tap[4] = {r0 + tx.i0 * 3u, r0 + tx.i1 * 3u, r1 + tx.i0 * 3u, r1 + tx.i1 * 3u};
+    // the reference's sampler (interpolation/bilinear.rs) replicates the top-left tap for a missing neighbour: the x1 and y1
+    // taps clamp onto it, and the diagonal tap is the top-left one when either axis is clamped (its weight is 0 there, but
+    // 0 * inf must be the reference's)
+    const bool diag = tx.i1 != tx.i0 && ty.i1 != ty.i0;
+    const float* tap[4] = {r0 + tx.i0 * 3u, r0 + tx.i1 * 3u, r1 + tx.i0 * 3u, diag ? r1 + tx.i1 * 3u : r0 + tx.i0 * 3u};
     const float mean[3] = {mean0, mean1, mean2}, inv[3] = {is0, is1, is2};
 #pragma unroll
     for (int k = 0; k < 3; ++k) {

@@ -86,6 +86,7 @@ __global__ void __launch_bounds__(RR_THREADS) resize_rows_f32_kernel(const float
     __shared__ __align__(8) uint64_t full_bar[RR_MAX_STAGES];
     __shared__ __align__(8) uint64_t empty_bar[RR_MAX_STAGES];
     __shared__ float fy_s[RR_MAX_STAGES];
+    __shared__ uint32_t ycl_s[RR_MAX_STAGES];   // y1 == y0: the last source row, the second staged row repeats the first
     constexpr uint32_t TW = RR_CT * NPX;
     constexpr uint32_t OUT_FLOATS = TW * 3u;                      // one destination row of the tile
     const uint32_t tid = threadIdx.x;
@@ -122,6 +123,7 @@ __global__ void __launch_bounds__(RR_THREADS) resize_rows_f32_kernel(const float
                 rr_axis(dy, P.ay, P.by, P.sh, &y0, &y1, &fy);
                 float* sbase = ring + (size_t)stage * stage_floats;
                 fy_s[stage] = fy;   // before the arrive(release): covered by the consumers' acquire on `full`
+                ycl_s[stage] = y1 == y0;
                 tma::mbar_expect_tx(&full_bar[stage], bytes * 2u);
                 tma::load_1d(sbase, frame + (size_t)y0 * P.row_floats, bytes, &full_bar[stage]);
                 tma::load_1d(sbase + P.slot_floats, frame + (size_t)y1 * P.row_floats, bytes, &full_bar[stage]);
@@ -157,6 +159,7 @@ __global__ void __launch_bounds__(RR_THREADS) resize_rows_f32_kernel(const float
             const float* r0 = ring + (size_t)stage * stage_floats;
             const float* r1 = r0 + P.slot_floats;
             const float fy = fy_s[stage], gy = 1.0f - fy;
+            const bool ycl = ycl_s[stage] != 0u;
             float* orow = rr_smem + obuf * OUT_FLOATS;
 #pragma unroll
             for (int j = 0; j < NPX; ++j) {
@@ -165,7 +168,9 @@ __global__ void __launch_bounds__(RR_THREADS) resize_rows_f32_kernel(const float
                 const float* p00 = r0 + o0[j];
                 const float* p10 = r0 + o1[j];
                 const float* p01 = r1 + o0[j];
-                const float* p11 = r1 + o1[j];
+                // the reference's sampler takes the top-left tap for the diagonal when either axis is clamped (weight 0, but
+                // 0 * inf must be the reference's); x1 == x0 and y1 == y0 only when clamped at the last column / row
+                const float* p11 = (o1[j] == o0[j] || ycl) ? p00 : r1 + o1[j];
                 float c[3];
 #pragma unroll
                 for (int k = 0; k < 3; ++k) c[k] = w00 * p00[k] + w10 * p10[k] + w01 * p01[k] + w11 * p11[k];
