@@ -1,5 +1,7 @@
 // bayer.cuh — bilinear demosaic of Bayer mosaics, 8-bit or 16-bit samples, shared by the standalone decoders
-// (color.cu) and the camera preprocess (preprocess.cu).
+// (color.cu: rgb_from_bayer_vec<T, P>, rgb_from_bayer_generic<T, P>) and the camera preprocess (preprocess.cu:
+// preprocess_bayer_identity_kernel<F16, PTRS, T, P> and the Bayer taps of the generic kernel).  Everything here is
+// generic over the sample type T; BayerSample<T> holds the few facts of T the kernels above it need.
 //
 // An extension beyond the reference, pinned to OpenCV: bit-identical to cv2.cvtColor(raw, COLOR_Bayer??2RGB)
 // (checked against cv2 4.13 on 8-bit and 16-bit mosaics, tests/golden/bayer_cv2.npz and bayer16_cv2.npz).  A pattern (kb200_bayer_pattern) is named by its 2x2 quad
@@ -48,6 +50,13 @@ __device__ __forceinline__ void bayer_px(const T* __restrict__ src, size_t pitch
     const int d = (int)__ldg(up - 1) + (int)__ldg(up + 1) + (int)__ldg(dn - 1) + (int)__ldg(dn + 1);
     bayer_demosaic(P, cx & 1, cy & 1, __ldg(mid), __ldg(up), __ldg(dn), __ldg(mid - 1), __ldg(mid + 1), d, rgb[0], rgb[1], rgb[2]);
 }
+
+// The sample types: uint8_t (8-bit mosaics) and uint16_t (10- to 16-bit).  VEC_COLS: columns per 16-byte vector, the
+// row segment of a decoder thread.  ID_WORDS: 32-bit words per 4-sample load of the preprocess identity kernel
+// (LDG.32 / LDG.64), and ID_ALIGN: the row and frame alignment in bytes that load needs.
+template <typename T> struct BayerSample;
+template <> struct BayerSample<uint8_t> { static constexpr uint32_t VEC_COLS = 16, ID_WORDS = 1, ID_ALIGN = 4; };
+template <> struct BayerSample<uint16_t> { static constexpr uint32_t VEC_COLS = 8, ID_WORDS = 2, ID_ALIGN = 8; };
 
 // Samples of type T per 32-bit word of a row segment, and their width in bits.
 template <typename T> __host__ __device__ constexpr int bayer_per_word() { return 4 / (int)sizeof(T); }

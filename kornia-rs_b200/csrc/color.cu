@@ -288,154 +288,81 @@ __global__ void rgb_from_yuv422_generic(const uint8_t* __restrict__ src, uint8_t
     dst[6 * g + 3] = (uint8_t)r; dst[6 * g + 4] = (uint8_t)gg; dst[6 * g + 5] = (uint8_t)b;
 }
 
-// ── Bayer → RGB8 (bilinear demosaic, bayer.cuh) ─────────────────────────────────────────────
-// 16 demosaiced pixels of one row (bayer_row) -> 48 RGB bytes.
-template <int P, int PY>
-__device__ __forceinline__ void bayer_row16(const uint32_t n[4], const uint32_t c[4], const uint32_t s[4], const int hl[3], const int hr[3],
+// ── Bayer → RGB (bilinear demosaic, bayer.cuh): 8-bit mosaics to RGB8, 10- to 16-bit ones to RGB16 ───────────────
+// The S = BayerSample<T>::VEC_COLS demosaiced pixels of one row (bayer_row) -> 48 RGB bytes, the interleaved samples
+// r0 g0 b0 r1 g1 b1 ...: 16 pixels as saturated bytes, or 8 pixels as 16-bit words (every result is <= 65535: no
+// saturation).  Either way a thread stores 48 B per row, so the same coalesced store serves both.
+template <typename T, int P, int PY>
+__device__ __forceinline__ void bayer_row48(const uint32_t n[4], const uint32_t c[4], const uint32_t s[4], const int hl[3], const int hr[3],
                                             bool left_edge, bool right_edge, uint4 o[3]) {
-    int r[16], g[16], b[16];
-    bayer_row<P, PY, 4>(n, c, s, hl, hr, left_edge, right_edge, r, g, b);
+    int rgb[3][BayerSample<T>::VEC_COLS];
+    bayer_row<P, PY, 4, T>(n, c, s, hl, hr, left_edge, right_edge, rgb[0], rgb[1], rgb[2]);
+    auto sample = [&](int a) { return rgb[a % 3][a / 3]; };   // output sample a of the row
     uint32_t w[12];
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {  // 4 px -> 12 bytes = 3 words: r0 g0 b0 r1 | g1 b1 r2 g2 | b2 r3 g3 b3
-        const int q = 4 * k;
-        w[3 * k] = pack_sat4(r[q], g[q], b[q], r[q + 1]);
-        w[3 * k + 1] = pack_sat4(g[q + 1], b[q + 1], r[q + 2], g[q + 2]);
-        w[3 * k + 2] = pack_sat4(b[q + 2], r[q + 3], g[q + 3], b[q + 3]);
+    for (int m = 0; m < 12; ++m) {
+        if constexpr (sizeof(T) == 1) w[m] = pack_sat4(sample(4 * m), sample(4 * m + 1), sample(4 * m + 2), sample(4 * m + 3));
+        else w[m] = (uint32_t)sample(2 * m) | ((uint32_t)sample(2 * m + 1) << 16);
     }
     o[0] = make_uint4(w[0], w[1], w[2], w[3]);
     o[1] = make_uint4(w[4], w[5], w[6], w[7]);
     o[2] = make_uint4(w[8], w[9], w[10], w[11]);
 }
 
-// One thread: 16 columns x 2 output rows, ya = 1 + 2 * blockIdx.y and ya + 1 (bayer_row_pairs).  Loads the rows ya-1 ..
-// ya+2 of its 16 columns as four LDG.128 plus shuffled halos (bayer_load_rows) and stores through
-// store_rgb48_coalesced.  Requires width % 16 == 0 and 16-B aligned bases.
-template <int P>
-__global__ void __launch_bounds__(128) rgb_from_bayer_vec16(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, uint32_t width,
-                                                            uint32_t height) {
+// One thread: S = BayerSample<T>::VEC_COLS columns (one 16-B vector per row) x 2 output rows, ya = 1 + 2 * blockIdx.y
+// and ya + 1 (bayer_row_pairs).  Loads the rows ya-1 .. ya+2 of its S columns as four lane-contiguous LDG.128 plus
+// shuffled halos (bayer_load_rows) and stores 48 B per row through store_rgb48_coalesced (three lane-contiguous STG.128
+// per warp and row).  Requires width % S == 0 and 16-B aligned bases, so every row of source and output starts 16-B aligned.
+template <typename T, int P>
+__global__ void __launch_bounds__(128) rgb_from_bayer_vec(const T* __restrict__ src, T* __restrict__ dst, uint32_t width, uint32_t height) {
+    constexpr uint32_t S = BayerSample<T>::VEC_COLS;
     __shared__ uint4 stage[4][96];
-    const uint32_t gx = blockIdx.x * blockDim.x + threadIdx.x;  // 16-column group
+    const uint32_t gx = blockIdx.x * blockDim.x + threadIdx.x;  // S-column group
     const uint32_t lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
     const uint32_t gx0 = gx - lane;                             // first group of this warp
-    if (gx0 * 16 >= width) return;                              // whole warp out of the row
-    const bool full_warp = (gx0 + 32) * 16 <= width;
-    const bool active = gx * 16 < width;
-    const uint32_t x = gx * 16;
+    if (gx0 * S >= width) return;                               // whole warp out of the row
+    const bool full_warp = (gx0 + 32) * S <= width;
+    const bool active = gx * S < width;
+    const uint32_t x = gx * S;
     const uint32_t ya = 1 + 2 * blockIdx.y, yb = ya + 1;
-    const uint8_t* frame = src + (size_t)blockIdx.z * width * height;
-    uint8_t* out = dst + (size_t)blockIdx.z * width * height * 3;
+    const T* frame = src + (size_t)blockIdx.z * width * height;
+    T* out = dst + (size_t)blockIdx.z * width * height * 3;
     uint32_t rows[4][4];
     int hl[4], hr[4];
-    bayer_load_rows<4>(frame, width, width, height, x, ya, lane, [&](const uint8_t* p, uint32_t v[4]) {
+    bayer_load_rows<4>(frame, width, width, height, x, ya, lane, [&](const T* p, uint32_t v[4]) {
         const uint4 q = active ? ldg_stream_u4(reinterpret_cast<const uint4*>(p)) : make_uint4(0, 0, 0, 0);
         v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
     }, rows, hl, hr);
-    const bool left_edge = x == 0, right_edge = x + 16 == width;
+    const bool left_edge = x == 0, right_edge = x + S == width;
     auto store_row = [&](uint32_t y, const uint4 o[3]) {
-        uint4* d = reinterpret_cast<uint4*>(out + ((size_t)y * width + (size_t)gx0 * 16) * 3);   // this warp's run of row y
+        uint4* d = reinterpret_cast<uint4*>(out + ((size_t)y * width + (size_t)gx0 * S) * 3);   // this warp's run of row y
         if (full_warp) store_rgb48_coalesced(d, stage[wid], lane, o);
         else if (active) { stg_stream_u4(d + 3 * lane, o[0]); stg_stream_u4(d + 3 * lane + 1, o[1]); stg_stream_u4(d + 3 * lane + 2, o[2]); }
     };
     uint4 oa[3];
-    bayer_row16<P, 1>(rows[0], rows[1], rows[2], hl, hr, left_edge, right_edge, oa);   // ya is odd
+    bayer_row48<T, P, 1>(rows[0], rows[1], rows[2], hl, hr, left_edge, right_edge, oa);   // ya is odd
     store_row(ya, oa);
     if (ya == 1) store_row(0, oa);
     if (yb == height - 1) {
         store_row(yb, oa);
     } else {
         uint4 ob[3];
-        bayer_row16<P, 0>(rows[1], rows[2], rows[3], hl + 1, hr + 1, left_edge, right_edge, ob);
+        bayer_row48<T, P, 0>(rows[1], rows[2], rows[3], hl + 1, hr + 1, left_edge, right_edge, ob);
         store_row(yb, ob);
         if (yb == height - 2) store_row(height - 1, ob);
     }
 }
 
-// Generic fallback (any width, any alignment): one thread per pixel, nine byte loads.
-template <int P>
-__global__ void rgb_from_bayer_generic(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, uint32_t width, uint32_t height) {
+// Generic fallback (any width, any base aligned to T): one thread per pixel, nine sample loads.
+template <typename T, int P>
+__global__ void rgb_from_bayer_generic(const T* __restrict__ src, T* __restrict__ dst, uint32_t width, uint32_t height) {
     const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x >= width || y >= height) return;
     const size_t frame = (size_t)width * height;
     int rgb[3];
     bayer_px(src + blockIdx.z * frame, width, (int)width, (int)height, (int)x, (int)y, P, rgb);
-    uint8_t* o = dst + (blockIdx.z * frame + (size_t)y * width + x) * 3;
-    o[0] = (uint8_t)rgb[0]; o[1] = (uint8_t)rgb[1]; o[2] = (uint8_t)rgb[2];
-}
-
-// ── 16-bit Bayer → RGB16 (10- to 16-bit mosaics, one LSB-aligned word per sample; bayer.cuh) ─────────────────
-// 8 demosaiced pixels of one row (bayer_row over 16-bit samples) -> 24 RGB words = 48 bytes, the payload the 8-bit
-// kernel stores per thread, so the same coalesced store serves both.  Every result is <= 65535: no saturation.
-template <int P, int PY>
-__device__ __forceinline__ void bayer16_row8(const uint32_t n[4], const uint32_t c[4], const uint32_t s[4], const int hl[3], const int hr[3],
-                                             bool left_edge, bool right_edge, uint4 o[3]) {
-    int rgb[3][8];
-    bayer_row<P, PY, 4, uint16_t>(n, c, s, hl, hr, left_edge, right_edge, rgb[0], rgb[1], rgb[2]);
-    uint32_t w[12];
-#pragma unroll
-    for (int m = 0; m < 12; ++m) {   // word m holds output samples 2m and 2m+1 of r0 g0 b0 r1 g1 b1 ...
-        const int a = 2 * m, b = 2 * m + 1;
-        w[m] = (uint32_t)rgb[a % 3][a / 3] | ((uint32_t)rgb[b % 3][b / 3] << 16);
-    }
-    o[0] = make_uint4(w[0], w[1], w[2], w[3]);
-    o[1] = make_uint4(w[4], w[5], w[6], w[7]);
-    o[2] = make_uint4(w[8], w[9], w[10], w[11]);
-}
-
-// One thread: 8 columns x 2 output rows (bayer_row_pairs).  Loads the rows ya-1 .. ya+2 of its 8 columns as four
-// lane-contiguous LDG.128 plus shuffled halo samples (bayer_load_rows) and stores 48 B per row through
-// store_rgb48_coalesced (three lane-contiguous STG.128 per warp and row).  Requires width % 8 == 0 and 16-B aligned
-// bases, so every row of source (2*width B) and output (6*width B) starts 16-B aligned.
-template <int P>
-__global__ void __launch_bounds__(128) rgb_from_bayer16_vec8(const uint16_t* __restrict__ src, uint16_t* __restrict__ dst, uint32_t width,
-                                                             uint32_t height) {
-    __shared__ uint4 stage[4][96];
-    const uint32_t gx = blockIdx.x * blockDim.x + threadIdx.x;  // 8-column group
-    const uint32_t lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
-    const uint32_t gx0 = gx - lane;                             // first group of this warp
-    if (gx0 * 8 >= width) return;                               // whole warp out of the row
-    const bool full_warp = (gx0 + 32) * 8 <= width;
-    const bool active = gx * 8 < width;
-    const uint32_t x = gx * 8;
-    const uint32_t ya = 1 + 2 * blockIdx.y, yb = ya + 1;
-    const uint16_t* frame = src + (size_t)blockIdx.z * width * height;
-    uint16_t* out = dst + (size_t)blockIdx.z * width * height * 3;
-    uint32_t rows[4][4];
-    int hl[4], hr[4];
-    bayer_load_rows<4>(frame, width, width, height, x, ya, lane, [&](const uint16_t* p, uint32_t v[4]) {
-        const uint4 q = active ? ldg_stream_u4(reinterpret_cast<const uint4*>(p)) : make_uint4(0, 0, 0, 0);
-        v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
-    }, rows, hl, hr);
-    const bool left_edge = x == 0, right_edge = x + 8 == width;
-    auto store_row = [&](uint32_t y, const uint4 o[3]) {
-        uint4* d = reinterpret_cast<uint4*>(out + ((size_t)y * width + (size_t)gx0 * 8) * 3);   // this warp's run of row y
-        if (full_warp) store_rgb48_coalesced(d, stage[wid], lane, o);
-        else if (active) { stg_stream_u4(d + 3 * lane, o[0]); stg_stream_u4(d + 3 * lane + 1, o[1]); stg_stream_u4(d + 3 * lane + 2, o[2]); }
-    };
-    uint4 oa[3];
-    bayer16_row8<P, 1>(rows[0], rows[1], rows[2], hl, hr, left_edge, right_edge, oa);   // ya is odd
-    store_row(ya, oa);
-    if (ya == 1) store_row(0, oa);
-    if (yb == height - 1) {
-        store_row(yb, oa);
-    } else {
-        uint4 ob[3];
-        bayer16_row8<P, 0>(rows[1], rows[2], rows[3], hl + 1, hr + 1, left_edge, right_edge, ob);
-        store_row(yb, ob);
-        if (yb == height - 2) store_row(height - 1, ob);
-    }
-}
-
-// Generic fallback (any width, any 2-B aligned base): one thread per pixel, nine sample loads.
-template <int P>
-__global__ void rgb_from_bayer16_generic(const uint16_t* __restrict__ src, uint16_t* __restrict__ dst, uint32_t width, uint32_t height) {
-    const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
-    if (x >= width || y >= height) return;
-    const size_t frame = (size_t)width * height;
-    int rgb[3];
-    bayer_px(src + blockIdx.z * frame, width, (int)width, (int)height, (int)x, (int)y, P, rgb);
-    uint16_t* o = dst + (blockIdx.z * frame + (size_t)y * width + x) * 3;
-    o[0] = (uint16_t)rgb[0]; o[1] = (uint16_t)rgb[1]; o[2] = (uint16_t)rgb[2];
+    T* o = dst + (blockIdx.z * frame + (size_t)y * width + x) * 3;
+    o[0] = (T)rgb[0]; o[1] = (T)rgb[1]; o[2] = (T)rgb[2];
 }
 
 static inline unsigned stream_grid(size_t items, unsigned block, unsigned ctas_per_sm) {
@@ -469,29 +396,52 @@ static const Yuv422Kernels YUV422_KERNELS[3] = {
     {"UYVY", rgb_from_yuv422_vec16<YUV422_UYVY>, rgb_from_yuv422_generic<YUV422_UYVY>, "rgb_from_uyvy_vec16", "rgb_from_uyvy_generic"},
     {"YVYU", rgb_from_yuv422_vec16<YUV422_YVYU>, rgb_from_yuv422_generic<YUV422_YVYU>, "rgb_from_yvyu_vec16", "rgb_from_yvyu_generic"},
 };
+// The Bayer kernels of each sample type, indexed by kb200_bayer_pattern.
+static const char* const BAYER_PATTERNS[4] = {"RGGB", "BGGR", "GRBG", "GBRG"};
+template <typename T>
 struct BayerKernels {
-    const char* pattern;
-    void (*vec16)(const uint8_t*, uint8_t*, uint32_t, uint32_t);
-    void (*generic)(const uint8_t*, uint8_t*, uint32_t, uint32_t);
-    const char *vec16_name, *generic_name;
+    void (*vec)(const T*, T*, uint32_t, uint32_t);
+    void (*generic)(const T*, T*, uint32_t, uint32_t);
+    const char *vec_name, *generic_name;
 };
-static const BayerKernels BAYER_KERNELS[4] = {
-    {"RGGB", rgb_from_bayer_vec16<KB200_BAYER_RGGB>, rgb_from_bayer_generic<KB200_BAYER_RGGB>, "rgb_from_bayer_rggb_vec16", "rgb_from_bayer_rggb_generic"},
-    {"BGGR", rgb_from_bayer_vec16<KB200_BAYER_BGGR>, rgb_from_bayer_generic<KB200_BAYER_BGGR>, "rgb_from_bayer_bggr_vec16", "rgb_from_bayer_bggr_generic"},
-    {"GRBG", rgb_from_bayer_vec16<KB200_BAYER_GRBG>, rgb_from_bayer_generic<KB200_BAYER_GRBG>, "rgb_from_bayer_grbg_vec16", "rgb_from_bayer_grbg_generic"},
-    {"GBRG", rgb_from_bayer_vec16<KB200_BAYER_GBRG>, rgb_from_bayer_generic<KB200_BAYER_GBRG>, "rgb_from_bayer_gbrg_vec16", "rgb_from_bayer_gbrg_generic"},
+static const BayerKernels<uint8_t> BAYER_KERNELS_U8[4] = {
+    {rgb_from_bayer_vec<uint8_t, KB200_BAYER_RGGB>, rgb_from_bayer_generic<uint8_t, KB200_BAYER_RGGB>, "rgb_from_bayer_rggb_vec16", "rgb_from_bayer_rggb_generic"},
+    {rgb_from_bayer_vec<uint8_t, KB200_BAYER_BGGR>, rgb_from_bayer_generic<uint8_t, KB200_BAYER_BGGR>, "rgb_from_bayer_bggr_vec16", "rgb_from_bayer_bggr_generic"},
+    {rgb_from_bayer_vec<uint8_t, KB200_BAYER_GRBG>, rgb_from_bayer_generic<uint8_t, KB200_BAYER_GRBG>, "rgb_from_bayer_grbg_vec16", "rgb_from_bayer_grbg_generic"},
+    {rgb_from_bayer_vec<uint8_t, KB200_BAYER_GBRG>, rgb_from_bayer_generic<uint8_t, KB200_BAYER_GBRG>, "rgb_from_bayer_gbrg_vec16", "rgb_from_bayer_gbrg_generic"},
 };
-struct Bayer16Kernels {
-    void (*vec8)(const uint16_t*, uint16_t*, uint32_t, uint32_t);
-    void (*generic)(const uint16_t*, uint16_t*, uint32_t, uint32_t);
-    const char *vec8_name, *generic_name;
+static const BayerKernels<uint16_t> BAYER_KERNELS_U16[4] = {
+    {rgb_from_bayer_vec<uint16_t, KB200_BAYER_RGGB>, rgb_from_bayer_generic<uint16_t, KB200_BAYER_RGGB>, "rgb_from_bayer16_rggb_vec", "rgb_from_bayer16_rggb_generic"},
+    {rgb_from_bayer_vec<uint16_t, KB200_BAYER_BGGR>, rgb_from_bayer_generic<uint16_t, KB200_BAYER_BGGR>, "rgb_from_bayer16_bggr_vec", "rgb_from_bayer16_bggr_generic"},
+    {rgb_from_bayer_vec<uint16_t, KB200_BAYER_GRBG>, rgb_from_bayer_generic<uint16_t, KB200_BAYER_GRBG>, "rgb_from_bayer16_grbg_vec", "rgb_from_bayer16_grbg_generic"},
+    {rgb_from_bayer_vec<uint16_t, KB200_BAYER_GBRG>, rgb_from_bayer_generic<uint16_t, KB200_BAYER_GBRG>, "rgb_from_bayer16_gbrg_vec", "rgb_from_bayer16_gbrg_generic"},
 };
-static const Bayer16Kernels BAYER16_KERNELS[4] = {
-    {rgb_from_bayer16_vec8<KB200_BAYER_RGGB>, rgb_from_bayer16_generic<KB200_BAYER_RGGB>, "rgb_from_bayer16_rggb_vec", "rgb_from_bayer16_rggb_generic"},
-    {rgb_from_bayer16_vec8<KB200_BAYER_BGGR>, rgb_from_bayer16_generic<KB200_BAYER_BGGR>, "rgb_from_bayer16_bggr_vec", "rgb_from_bayer16_bggr_generic"},
-    {rgb_from_bayer16_vec8<KB200_BAYER_GRBG>, rgb_from_bayer16_generic<KB200_BAYER_GRBG>, "rgb_from_bayer16_grbg_vec", "rgb_from_bayer16_grbg_generic"},
-    {rgb_from_bayer16_vec8<KB200_BAYER_GBRG>, rgb_from_bayer16_generic<KB200_BAYER_GBRG>, "rgb_from_bayer16_gbrg_vec", "rgb_from_bayer16_gbrg_generic"},
-};
+
+// The demosaic behind kb200_rgb_from_bayer_u8 / _u16 (pointers already checked): the fast kernel when every row is whole
+// 16-B vectors, the one-thread-per-pixel kernel otherwise.  Lengths are in samples.
+template <typename T>
+static int launch_rgb_from_bayer(const BayerKernels<T> (&table)[4], kb200_stream_t stream, const T* src, size_t src_len, T* dst,
+                                 size_t dst_len, uint32_t width, uint32_t height, uint32_t batch, int pattern) {
+    if (pattern < KB200_BAYER_RGGB || pattern > KB200_BAYER_GBRG) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown Bayer pattern %d", pattern);
+    const BayerKernels<T>& k = table[pattern];
+    KB200_TRY(check_geometry(width, height, width, height, batch));
+    if (width < 3 || height < 3) return fail(KB200_ERR_INVALID_ARGUMENT, "Bayer %s needs at least 3x3 pixels, got %ux%u", BAYER_PATTERNS[pattern], width, height);
+    if (batch > 65535u) return fail(KB200_ERR_INVALID_ARGUMENT, "batch %u exceeds 65535", batch);
+    const size_t frame = (size_t)width * height;
+    KB200_TRY(check_slice("src", src_len, frame * batch)); KB200_TRY(check_slice("dst", dst_len, frame * 3 * batch));
+    cudaStream_t s = as_stream(stream);
+    constexpr uint32_t S = BayerSample<T>::VEC_COLS;
+    if ((width % S) == 0 && aligned16(src) && aligned16(dst) && bayer_row_pairs(height) <= 65535u) {
+        const unsigned groups = width / S;
+        const unsigned bx = groups >= 128 ? 128 : 32 * ((groups + 31) / 32);
+        dim3 grid(div_up(groups, bx), bayer_row_pairs(height), batch);
+        k.vec<<<grid, bx, 0, s>>>(src, dst, width, height);
+        return check_launch(k.vec_name);
+    }
+    dim3 block(32, 8), grid(div_up(width, 32), div_up(height, 8), batch);
+    k.generic<<<grid, block, 0, s>>>(src, dst, width, height);
+    return check_launch(k.generic_name);
+}
 
 // ── RGB8 → YUYV / NV12 encode (SURVEY §8(f) #4) ─────────────────────────────────────────────
 // color/yuv/kernels.rs:1223-1252: Q8 BT.601 limited — Y = ((66R + 129G + 25B + 128) >> 8) + 16,
@@ -652,24 +602,7 @@ KB200_API int kb200_rgb_from_yuyv_u8(kb200_stream_t stream, const uint8_t* src, 
 KB200_API int kb200_rgb_from_bayer_u8(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst,
                                       size_t dst_len, uint32_t width, uint32_t height, uint32_t batch, int pattern) {
     KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
-    if (pattern < KB200_BAYER_RGGB || pattern > KB200_BAYER_GBRG) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown Bayer pattern %d", pattern);
-    const BayerKernels& k = BAYER_KERNELS[pattern];
-    KB200_TRY(check_geometry(width, height, width, height, batch));
-    if (width < 3 || height < 3) return fail(KB200_ERR_INVALID_ARGUMENT, "Bayer %s needs at least 3x3 pixels, got %ux%u", k.pattern, width, height);
-    if (batch > 65535u) return fail(KB200_ERR_INVALID_ARGUMENT, "batch %u exceeds 65535", batch);
-    const size_t frame = (size_t)width * height;
-    KB200_TRY(check_slice("src", src_len, frame * batch)); KB200_TRY(check_slice("dst", dst_len, frame * 3 * batch));
-    cudaStream_t s = as_stream(stream);
-    if ((width % 16u) == 0 && aligned16(src) && aligned16(dst) && bayer_row_pairs(height) <= 65535u) {
-        const unsigned groups = width / 16;
-        const unsigned bx = groups >= 128 ? 128 : 32 * ((groups + 31) / 32);
-        dim3 grid(div_up(groups, bx), bayer_row_pairs(height), batch);
-        k.vec16<<<grid, bx, 0, s>>>(src, dst, width, height);
-        return check_launch(k.vec16_name);
-    }
-    dim3 block(32, 8), grid(div_up(width, 32), div_up(height, 8), batch);
-    k.generic<<<grid, block, 0, s>>>(src, dst, width, height);
-    return check_launch(k.generic_name);
+    return launch_rgb_from_bayer(BAYER_KERNELS_U8, stream, src, src_len, dst, dst_len, width, height, batch, pattern);
 }
 
 KB200_API int kb200_rgb_from_bayer_u16(kb200_stream_t stream, const uint16_t* src, size_t src_len, uint16_t* dst,
@@ -677,25 +610,7 @@ KB200_API int kb200_rgb_from_bayer_u16(kb200_stream_t stream, const uint16_t* sr
     KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
     if (reinterpret_cast<uintptr_t>(src) & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "'src' is not 2-byte aligned (16-bit samples)");
     if (reinterpret_cast<uintptr_t>(dst) & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "'dst' is not 2-byte aligned (16-bit samples)");
-    if (pattern < KB200_BAYER_RGGB || pattern > KB200_BAYER_GBRG) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown Bayer pattern %d", pattern);
-    const Bayer16Kernels& k = BAYER16_KERNELS[pattern];
-    KB200_TRY(check_geometry(width, height, width, height, batch));
-    if (width < 3 || height < 3)
-        return fail(KB200_ERR_INVALID_ARGUMENT, "Bayer %s needs at least 3x3 pixels, got %ux%u", BAYER_KERNELS[pattern].pattern, width, height);
-    if (batch > 65535u) return fail(KB200_ERR_INVALID_ARGUMENT, "batch %u exceeds 65535", batch);
-    const size_t frame = (size_t)width * height;   // samples
-    KB200_TRY(check_slice("src", src_len, frame * batch)); KB200_TRY(check_slice("dst", dst_len, frame * 3 * batch));
-    cudaStream_t s = as_stream(stream);
-    if ((width % 8u) == 0 && aligned16(src) && aligned16(dst) && bayer_row_pairs(height) <= 65535u) {
-        const unsigned groups = width / 8;
-        const unsigned bx = groups >= 128 ? 128 : 32 * ((groups + 31) / 32);
-        dim3 grid(div_up(groups, bx), bayer_row_pairs(height), batch);
-        k.vec8<<<grid, bx, 0, s>>>(src, dst, width, height);
-        return check_launch(k.vec8_name);
-    }
-    dim3 block(32, 8), grid(div_up(width, 32), div_up(height, 8), batch);
-    k.generic<<<grid, block, 0, s>>>(src, dst, width, height);
-    return check_launch(k.generic_name);
+    return launch_rgb_from_bayer(BAYER_KERNELS_U16, stream, src, src_len, dst, dst_len, width, height, batch, pattern);
 }
 
 

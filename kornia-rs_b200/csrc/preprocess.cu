@@ -21,6 +21,8 @@
 // integer scales (1080p NV12 → 1080p CHW, config 3a) that removes 3 of the 4 decodes per pixel.
 #include <cuda_fp16.h>
 
+#include <type_traits>
+
 #include "bayer.cuh"
 #include "kb200_common.cuh"
 
@@ -105,17 +107,16 @@ static constexpr int SRC_BASE = 0, SRC_EXT_YUV = 1, SRC_BAYER = 2, SRC_BAYER16 =
 __host__ __device__ inline int bayer16_pattern(int fmt) { return (fmt - KB200_FMT_BAYER_RGGB10) & 3; }
 __host__ __device__ inline int bayer16_bits(int fmt) { return 10 + 2 * ((fmt - KB200_FMT_BAYER_RGGB10) >> 2); }
 __host__ __device__ inline float bayer16_white(int fmt) { return (float)((1u << bayer16_bits(fmt)) - 1u); }
+// kb200_bayer_pattern of a Bayer format: fmt 16-19 (8-bit samples) = 16 + pattern, fmt 32-47 (16-bit) as above
+__host__ __device__ inline int bayer_pattern(int fmt, bool bayer16) { return bayer16 ? bayer16_pattern(fmt) : fmt - KB200_FMT_BAYER_RGGB; }
 
 template <int EXT>
 __device__ __forceinline__ void fetch_px(const uint8_t* __restrict__ src, int x, int y, const kb200_preprocess_desc& d,
                                          float px[3]) {  // :510-530
-    if (EXT == SRC_BAYER16) {   // src_pitch is in bytes and even
+    if (EXT == SRC_BAYER || EXT == SRC_BAYER16) {   // src_pitch is in bytes (even for 16-bit samples)
+        using T = std::conditional_t<EXT == SRC_BAYER16, uint16_t, uint8_t>;
         int rgb[3];
-        bayer_px(reinterpret_cast<const uint16_t*>(src), (size_t)d.src_pitch / 2, d.src_w, d.src_h, x, y, bayer16_pattern(d.fmt), rgb);
-        px[0] = (float)rgb[0]; px[1] = (float)rgb[1]; px[2] = (float)rgb[2];
-    } else if (EXT == SRC_BAYER) {
-        int rgb[3];
-        bayer_px(src, (size_t)d.src_pitch, d.src_w, d.src_h, x, y, d.fmt - KB200_FMT_BAYER_RGGB, rgb);
+        bayer_px(reinterpret_cast<const T*>(src), (size_t)d.src_pitch / sizeof(T), d.src_w, d.src_h, x, y, bayer_pattern(d.fmt, EXT == SRC_BAYER16), rgb);
         px[0] = (float)rgb[0]; px[1] = (float)rgb[1]; px[2] = (float)rgb[2];
     } else if (EXT == SRC_EXT_YUV) {
         fetch_px_yuv_ext(src, x, y, d, px);
@@ -322,29 +323,37 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const _
 
 // ── Bayer identity fast path (the config-3a shape from a Bayer mosaic: scale 1, no pad, same size) ──────────────
 // As for 4:2:0, the sample is the demosaiced pixel (ox, oy) itself.  One thread = 4 columns x 2 output rows (the row
-// pairs of bayer_row_pairs): 4 lane-contiguous LDG.32 of the rows ya-1 .. ya+2 plus shuffled halos (bayer_load_rows),
-// 6 to 12 lane-contiguous 4-pixel stores per thread (nv12_store4).  Requires w % 4 == 0 and 4-B aligned rows.
-template <bool F16, bool PTRS, int P>
+// pairs of bayer_row_pairs): 4 lane-contiguous loads of the rows ya-1 .. ya+2 (LDG.32 of 8-bit samples, LDG.64 of 16-bit
+// ones: BayerSample<T>::ID_WORDS) plus shuffled halos (bayer_load_rows), 6 to 12 lane-contiguous 4-pixel stores per
+// thread (nv12_store4).  Requires w % 4 == 0 and rows aligned to BayerSample<T>::ID_ALIGN.
+template <bool F16, bool PTRS, typename T, int P>
 __global__ void __launch_bounds__(128) preprocess_bayer_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                         const __grid_constant__ PreFrames fr, void* __restrict__ dst,
                                                                         uint32_t frame0, uint32_t groups_per_row, uint32_t items) {
+    constexpr uint32_t NW = BayerSample<T>::ID_WORDS;
     const uint32_t item = blockIdx.x * blockDim.x + threadIdx.x;
     const bool active = item < items;                         // the lanes past the end still take part in the shuffles
     const uint32_t it = active ? item : items - 1;
     const uint32_t rp = it / groups_per_row, g = it - rp * groups_per_row;
     const uint32_t w = (uint32_t)d.src_w, h = (uint32_t)d.src_h;
     const uint32_t f = blockIdx.y;
-    const uint8_t* src = PTRS ? fr.ptr[f] : fr.base + (size_t)(frame0 + f) * fr.stride;
+    const T* src = reinterpret_cast<const T*>(PTRS ? fr.ptr[f] : fr.base + (size_t)(frame0 + f) * fr.stride);
     const uint32_t x = g * 4u, ya = 1u + 2u * rp, yb = ya + 1u;
-    uint32_t rows[4][1];
+    uint32_t rows[4][NW];
     int hl[4], hr[4];
-    bayer_load_rows<1>(src, (size_t)d.src_pitch, w, h, x, ya, threadIdx.x & 31u, [](const uint8_t* p, uint32_t v[1]) {
-        v[0] = __ldg(reinterpret_cast<const uint32_t*>(p));
+    bayer_load_rows<NW>(src, (size_t)d.src_pitch / sizeof(T), w, h, x, ya, threadIdx.x & 31u, [](const T* p, uint32_t v[NW]) {
+        if constexpr (NW == 1) {
+            v[0] = __ldg(reinterpret_cast<const uint32_t*>(p));
+        } else {
+            const uint2 q = __ldg(reinterpret_cast<const uint2*>(p));
+            v[0] = q.x; v[1] = q.y;
+        }
     }, rows, hl, hr);
     if (!active) return;
     const bool left_edge = x == 0, right_edge = x + 4u == w;
     const size_t plane = (size_t)w * h;
     const size_t base = (size_t)(frame0 + f) * 3 * plane + x;
+    [[maybe_unused]] const float wl = bayer16_white(d.fmt);   // the white level W of a 16-bit format
     const float m0 = d.mean[0], m1 = d.mean[1], m2 = d.mean[2], i0 = d.inv_std[0], i1 = d.inv_std[1], i2 = d.inv_std[2];
     float r4[4], g4[4], b4[4];
     auto store_row = [&](uint32_t y) {
@@ -353,70 +362,26 @@ __global__ void __launch_bounds__(128) preprocess_bayer_identity_kernel(const __
         nv12_store4<F16>(dst, o + plane, g4);
         nv12_store4<F16>(dst, o + 2 * plane, b4);
     };
-    int r[4], gg[4], b[4];
-    bayer_row<P, 1, 1>(rows[0], rows[1], rows[2], hl, hr, left_edge, right_edge, r, gg, b);   // ya is odd
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { r4[i] = norm_int_px(r[i], m0, i0); g4[i] = norm_int_px(gg[i], m1, i1); b4[i] = norm_int_px(b[i], m2, i2); }
-    store_row(ya);
-    if (ya == 1u) store_row(0);
-    if (yb == h - 1u) { store_row(yb); return; }
-    bayer_row<P, 0, 1>(rows[1], rows[2], rows[3], hl + 1, hr + 1, left_edge, right_edge, r, gg, b);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { r4[i] = norm_int_px(r[i], m0, i0); g4[i] = norm_int_px(gg[i], m1, i1); b4[i] = norm_int_px(b[i], m2, i2); }
-    store_row(yb);
-    if (yb == h - 2u) store_row(h - 1u);
-}
-
-// ── 16-bit Bayer identity fast path (the config-3a shape from a 10- to 16-bit mosaic) ─────────────────────────
-// The 8-bit kernel above on 2-byte samples: one thread = 4 columns x 2 output rows, 4 lane-contiguous LDG.64 of the rows
-// ya-1 .. ya+2 (256 contiguous bytes per warp and row) plus shuffled halo samples, the same 6 to 12 lane-contiguous
-// 4-pixel stores.  px / W is the IEEE division (W = bayer16_white(fmt)).  Requires w % 4 == 0 and 8-B aligned rows.
-template <bool F16, bool PTRS, int P>
-__global__ void __launch_bounds__(128) preprocess_bayer16_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
-                                                                          const __grid_constant__ PreFrames fr, void* __restrict__ dst,
-                                                                          uint32_t frame0, uint32_t groups_per_row, uint32_t items) {
-    const uint32_t item = blockIdx.x * blockDim.x + threadIdx.x;
-    const bool active = item < items;                         // the lanes past the end still take part in the shuffles
-    const uint32_t it = active ? item : items - 1;
-    const uint32_t rp = it / groups_per_row, g = it - rp * groups_per_row;
-    const uint32_t w = (uint32_t)d.src_w, h = (uint32_t)d.src_h;
-    const uint32_t f = blockIdx.y;
-    const uint16_t* src = reinterpret_cast<const uint16_t*>(PTRS ? fr.ptr[f] : fr.base + (size_t)(frame0 + f) * fr.stride);
-    const uint32_t x = g * 4u, ya = 1u + 2u * rp, yb = ya + 1u;
-    uint32_t rows[4][2];
-    int hl[4], hr[4];
-    bayer_load_rows<2>(src, (size_t)d.src_pitch / 2, w, h, x, ya, threadIdx.x & 31u, [](const uint16_t* p, uint32_t v[2]) {
-        const uint2 q = __ldg(reinterpret_cast<const uint2*>(p));
-        v[0] = q.x; v[1] = q.y;
-    }, rows, hl, hr);
-    if (!active) return;
-    const bool left_edge = x == 0, right_edge = x + 4u == w;
-    const size_t plane = (size_t)w * h;
-    const size_t base = (size_t)(frame0 + f) * 3 * plane + x;
-    const float wl = bayer16_white(d.fmt);
-    const float m0 = d.mean[0], m1 = d.mean[1], m2 = d.mean[2], i0 = d.inv_std[0], i1 = d.inv_std[1], i2 = d.inv_std[2];
-    float r4[4], g4[4], b4[4];
-    auto store_row = [&](uint32_t y) {
-        const size_t o = base + (size_t)y * w;
-        nv12_store4<F16>(dst, o, r4);
-        nv12_store4<F16>(dst, o + plane, g4);
-        nv12_store4<F16>(dst, o + 2 * plane, b4);
-    };
+    // 8-bit: px / 255 by the exact 3-instruction form (norm_int_px); 16-bit: px / W, the IEEE division
     auto norm = [&](const int r[4], const int gg[4], const int b[4]) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-            r4[i] = (__fdiv_rn((float)r[i], wl) - m0) * i0;
-            g4[i] = (__fdiv_rn((float)gg[i], wl) - m1) * i1;
-            b4[i] = (__fdiv_rn((float)b[i], wl) - m2) * i2;
+            if constexpr (sizeof(T) == 1) {
+                r4[i] = norm_int_px(r[i], m0, i0); g4[i] = norm_int_px(gg[i], m1, i1); b4[i] = norm_int_px(b[i], m2, i2);
+            } else {
+                r4[i] = (__fdiv_rn((float)r[i], wl) - m0) * i0;
+                g4[i] = (__fdiv_rn((float)gg[i], wl) - m1) * i1;
+                b4[i] = (__fdiv_rn((float)b[i], wl) - m2) * i2;
+            }
         }
     };
     int r[4], gg[4], b[4];
-    bayer_row<P, 1, 2, uint16_t>(rows[0], rows[1], rows[2], hl, hr, left_edge, right_edge, r, gg, b);   // ya is odd
+    bayer_row<P, 1, NW, T>(rows[0], rows[1], rows[2], hl, hr, left_edge, right_edge, r, gg, b);   // ya is odd
     norm(r, gg, b);
     store_row(ya);
     if (ya == 1u) store_row(0);
     if (yb == h - 1u) { store_row(yb); return; }
-    bayer_row<P, 0, 2, uint16_t>(rows[1], rows[2], rows[3], hl + 1, hr + 1, left_edge, right_edge, r, gg, b);
+    bayer_row<P, 0, NW, T>(rows[1], rows[2], rows[3], hl + 1, hr + 1, left_edge, right_edge, r, gg, b);
     norm(r, gg, b);
     store_row(yb);
     if (yb == h - 2u) store_row(h - 1u);
@@ -619,22 +584,13 @@ static void launch_yuv420_fast(cudaStream_t s, bool identity, bool bil, const kb
 #undef KB200_YUV420_LAUNCH
 }
 
-// The Bayer identity kernel of pattern P, for one launch of <= 256 frames.
-template <bool F16, int P>
+// The Bayer identity kernel of sample type T and pattern P, for one launch of <= 256 frames.
+template <bool F16, typename T, int P>
 static void launch_bayer_identity(cudaStream_t s, const kb200_preprocess_desc& d, const PreFrames& fr, bool ptrs, void* dst, uint32_t f0,
                                   uint32_t nb, uint32_t id_groups, size_t id_items) {
     dim3 grid(div_up(id_items, 128), nb);
-    if (ptrs) preprocess_bayer_identity_kernel<F16, true, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
-    else preprocess_bayer_identity_kernel<F16, false, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
-}
-
-// The 16-bit Bayer identity kernel of pattern P, for one launch of <= 256 frames.
-template <bool F16, int P>
-static void launch_bayer16_identity(cudaStream_t s, const kb200_preprocess_desc& d, const PreFrames& fr, bool ptrs, void* dst, uint32_t f0,
-                                    uint32_t nb, uint32_t id_groups, size_t id_items) {
-    dim3 grid(div_up(id_items, 128), nb);
-    if (ptrs) preprocess_bayer16_identity_kernel<F16, true, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
-    else preprocess_bayer16_identity_kernel<F16, false, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
+    if (ptrs) preprocess_bayer_identity_kernel<F16, true, T, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
+    else preprocess_bayer_identity_kernel<F16, false, T, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
 }
 
 template <bool F16, bool PTRS, int EXT>
@@ -657,10 +613,12 @@ static void launch_generic_for(int ext, cudaStream_t s, dim3 grid, int sampling,
 static const char* const YUV420_IDENTITY_NAMES[4] = {"preprocess_nv12_identity_kernel", "preprocess_nv21_identity_kernel",
                                                      "preprocess_i420_identity_kernel", "preprocess_yv12_identity_kernel"};
 static const char* const YUV420_FAST_NAMES[4] = {"preprocess_nv12_kernel", "preprocess_nv21_kernel", "preprocess_i420_kernel", "preprocess_yv12_kernel"};
-static const char* const BAYER_IDENTITY_NAMES[4] = {"preprocess_bayer_rggb_identity_kernel", "preprocess_bayer_bggr_identity_kernel",
-                                                    "preprocess_bayer_grbg_identity_kernel", "preprocess_bayer_gbrg_identity_kernel"};
-static const char* const BAYER16_IDENTITY_NAMES[4] = {"preprocess_bayer16_rggb_identity_kernel", "preprocess_bayer16_bggr_identity_kernel",
-                                                      "preprocess_bayer16_grbg_identity_kernel", "preprocess_bayer16_gbrg_identity_kernel"};
+// ... and of the Bayer identity kernels, by sample width (8-bit, 16-bit) and pattern
+static const char* const BAYER_IDENTITY_NAMES[2][4] = {
+    {"preprocess_bayer_rggb_identity_kernel", "preprocess_bayer_bggr_identity_kernel", "preprocess_bayer_grbg_identity_kernel",
+     "preprocess_bayer_gbrg_identity_kernel"},
+    {"preprocess_bayer16_rggb_identity_kernel", "preprocess_bayer16_bggr_identity_kernel", "preprocess_bayer16_grbg_identity_kernel",
+     "preprocess_bayer16_gbrg_identity_kernel"}};
 
 template <bool F16>
 static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, const uint8_t* const* frames,
@@ -668,19 +626,20 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
     const int pixels = d.dst_w * d.dst_h;
     const bool bil = d.sampling == KB200_INTERP_BILINEAR, lanczos = d.sampling == KB200_INTERP_LANCZOS;
     const int l420 = yuv420_layout(d.fmt);
-    const bool bayer = is_bayer(d.fmt), bayer16 = is_bayer16(d.fmt);
+    const bool bayer16 = is_bayer16(d.fmt), bayer = bayer16 || is_bayer(d.fmt);   // bayer: any Bayer mosaic
     // identity fast path: a 4:2:0 or Bayer format, scale 1, no pad, same size, 8-column vectors possible
     // (Lanczos always takes the generic kernel: its off-centre weights at integer coordinates are sinf(k*pi) != 0 exactly).
-    // A thread loads 4 samples per row: 4 B aligned rows and frames, 8 B for 16-bit Bayer.
-    const uint32_t row_align = bayer16 ? 8u : 4u;
-    bool identity = !lanczos && (l420 >= 0 || bayer || bayer16) && d.scale_x == 1.0f && d.scale_y == 1.0f && d.pad_x == 0.0f && d.pad_y == 0.0f &&
+    // A thread loads 4 samples per row, so rows and frames are aligned to that load: 4 B for 4:2:0 and 8-bit Bayer, 8 B
+    // for 16-bit Bayer.
+    const uint32_t row_align = bayer16 ? BayerSample<uint16_t>::ID_ALIGN : BayerSample<uint8_t>::ID_ALIGN;
+    bool identity = !lanczos && (l420 >= 0 || bayer) && d.scale_x == 1.0f && d.scale_y == 1.0f && d.pad_x == 0.0f && d.pad_y == 0.0f &&
                     d.dst_w == d.src_w && d.dst_h == d.src_h && (d.src_w % 4) == 0 && (d.src_pitch % row_align) == 0 && aligned16(dst);
     if (identity) {
         if (frames) { for (uint32_t k = 0; k < batch; ++k) identity = identity && ((reinterpret_cast<uintptr_t>(frames[k]) & (row_align - 1)) == 0); }
         else identity = ((reinterpret_cast<uintptr_t>(base) & (row_align - 1)) == 0) && (stride % row_align == 0);
     }
     const uint32_t id_groups = (uint32_t)d.src_w / 4u;
-    const size_t id_items = (size_t)id_groups * (bayer || bayer16 ? bayer_row_pairs((uint32_t)d.src_h) : (size_t)d.src_h / 2);
+    const size_t id_items = (size_t)id_groups * (bayer ? bayer_row_pairs((uint32_t)d.src_h) : (size_t)d.src_h / 2);
     if (id_items > 0x7FFFFFFFull) identity = false;
     // 4:2:0 general fast path: vector stores need dst_w % 4 == 0 and a 16-B (f32) / 8-B (f16) aligned destination
     const bool yuv420_fast = !lanczos && l420 >= 0 && (d.dst_w % 4) == 0 && aligned16(dst) && d.dst_h <= 65535 * NV12_ROWS;
@@ -695,23 +654,19 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
         if (frames) for (uint32_t k = 0; k < nb; ++k) fr.ptr[k] = frames[f0 + k];
         const bool p = frames != nullptr;
         if (identity && bayer) {
-            switch (d.fmt) {
-                case KB200_FMT_BAYER_RGGB: launch_bayer_identity<F16, KB200_BAYER_RGGB>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
-                case KB200_FMT_BAYER_BGGR: launch_bayer_identity<F16, KB200_BAYER_BGGR>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
-                case KB200_FMT_BAYER_GRBG: launch_bayer_identity<F16, KB200_BAYER_GRBG>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
-                default: launch_bayer_identity<F16, KB200_BAYER_GBRG>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
-            }
-            KB200_TRY(check_launch(BAYER_IDENTITY_NAMES[d.fmt - KB200_FMT_BAYER_RGGB]));
-            continue;
-        }
-        if (identity && bayer16) {
-            switch (bayer16_pattern(d.fmt)) {
-                case KB200_BAYER_RGGB: launch_bayer16_identity<F16, KB200_BAYER_RGGB>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
-                case KB200_BAYER_BGGR: launch_bayer16_identity<F16, KB200_BAYER_BGGR>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
-                case KB200_BAYER_GRBG: launch_bayer16_identity<F16, KB200_BAYER_GRBG>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
-                default: launch_bayer16_identity<F16, KB200_BAYER_GBRG>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
-            }
-            KB200_TRY(check_launch(BAYER16_IDENTITY_NAMES[bayer16_pattern(d.fmt)]));
+            const int pattern = bayer_pattern(d.fmt, bayer16);
+            auto launch = [&](auto sample) {   // the kernel of pattern `pattern` for samples of the type of `sample`
+                using T = decltype(sample);
+                switch (pattern) {
+                    case KB200_BAYER_RGGB: launch_bayer_identity<F16, T, KB200_BAYER_RGGB>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
+                    case KB200_BAYER_BGGR: launch_bayer_identity<F16, T, KB200_BAYER_BGGR>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
+                    case KB200_BAYER_GRBG: launch_bayer_identity<F16, T, KB200_BAYER_GRBG>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
+                    default: launch_bayer_identity<F16, T, KB200_BAYER_GBRG>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
+                }
+            };
+            if (bayer16) launch(uint16_t{});
+            else launch(uint8_t{});
+            KB200_TRY(check_launch(BAYER_IDENTITY_NAMES[bayer16][pattern]));
             continue;
         }
         if (identity || yuv420_fast) {

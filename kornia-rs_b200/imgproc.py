@@ -518,12 +518,12 @@ def gray_from_rgb(src: Image, dst: Image, leaf: int = LEAF_SCALAR) -> None:
         raise ImageError.DtypeMismatch(src.dtype, dst.dtype)
 
 
-def _raw_frames(src, what: str) -> torch.Tensor:
+def _raw_frames(src, what: str, dtype: torch.dtype) -> torch.Tensor:
     t = src.data if isinstance(src, Image) else src
     if not t.is_cuda:
         raise ImageError.HostPathNotBuilt(what)
-    if t.dtype != torch.uint8:
-        raise ImageError.DtypeMismatch(torch.uint8, t.dtype)
+    if t.dtype != dtype:
+        raise ImageError.DtypeMismatch(dtype, t.dtype)
     if not t.is_contiguous():
         raise ImageError.ImageDataNotContiguous()
     return t
@@ -533,15 +533,16 @@ YUV420_NV12, YUV420_NV21, YUV420_I420, YUV420_YV12 = 0, 1, 2, 3   # kb200_yuv420
 YUV422_YUYV, YUV422_UYVY, YUV422_YVYU = 0, 1, 2                   # kb200_yuv422_layout
 
 
-def _rgb_from_yuv(src, dst: Image, what: str, bytes_num: int, bytes_den: int, fn_name: str, *layout) -> None:
-    """The video decoders: `src` holds N tight frames of w*h*bytes_num/bytes_den bytes; `layout` is the extra argument of
-    the layout-generic entry points (none for the NV12 / YUYV ones)."""
-    t = _raw_frames(src, what)
+def _rgb_from_yuv(src, dst: Image, what: str, bytes_num: int, bytes_den: int, fn_name: str, *layout,
+                  dtype: torch.dtype = torch.uint8) -> None:
+    """The video and Bayer decoders: `src` holds N tight frames of w*h*bytes_num/bytes_den samples of `dtype`, the dtype
+    of `dst` too; `layout` is the extra argument of the layout-generic entry points (none for the NV12 / YUYV ones)."""
+    t = _raw_frames(src, what, dtype)
     if not dst.is_device:
         raise ImageError.MixedResidency()
     if t.device != dst.device:
         raise ImageError.DeviceMismatch()
-    _expect_dtype(dst, torch.uint8, "dst")
+    _expect_dtype(dst, dtype, "dst")
     w, h, n = dst.cols(), dst.rows(), dst.batch
     need = w * h * bytes_num // bytes_den * n
     if dst.num_channels() != 3 or t.numel() != need:
@@ -607,25 +608,7 @@ def rgb_from_bayer16(src, dst: Image, pattern: BayerPattern) -> None:
     (cv2.cvtColor gives the same bits on uint16 mosaics).  `src`: uint16 device tensor holding N tight frames of w*h
     samples, each an LSB-aligned little-endian word (V4L2's unpacked SRGGB10 ... SGBRG16); `dst`: a uint16 Image
     [N, h, w, 3].  The bit depth plays no part: the output is the same whatever it is."""
-    code = int(BayerPattern(pattern))
-    t = src.data if isinstance(src, Image) else src
-    if not t.is_cuda:
-        raise ImageError.HostPathNotBuilt("rgb_from_bayer16")
-    if t.dtype != torch.uint16:
-        raise ImageError.DtypeMismatch(torch.uint16, t.dtype)
-    if not t.is_contiguous():
-        raise ImageError.ImageDataNotContiguous()
-    if not dst.is_device:
-        raise ImageError.MixedResidency()
-    if t.device != dst.device:
-        raise ImageError.DeviceMismatch()
-    _expect_dtype(dst, torch.uint16, "dst")
-    w, h, n = dst.cols(), dst.rows(), dst.batch
-    need = w * h * n
-    if dst.num_channels() != 3 or t.numel() != need:
-        raise ImageError.InvalidImageSize(t.numel(), 1, need, 1)
-    _lib.set_device(t.device.index)
-    _check(_lib.lib().kb200_rgb_from_bayer_u16(_stream(t.device), t.data_ptr(), t.numel(), dst.data.data_ptr(), dst.numel(), w, h, n, code))
+    _rgb_from_yuv(src, dst, "rgb_from_bayer16", 1, 1, "kb200_rgb_from_bayer_u16", int(BayerPattern(pattern)), dtype=torch.uint16)
 
 
 def _encode(op: str, fn_name: str, src: Image, dst: torch.Tensor, bytes_per_px_num: int, bytes_per_px_den: int, need_even_h: bool) -> None:
