@@ -138,6 +138,7 @@ pub mod ffi {
         pub fn kb200_rgb_from_yuv422_u8(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, width: u32, height: u32, batch: u32, layout: c_int) -> c_int;
         pub fn kb200_rgb_from_bayer_u8(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, width: u32, height: u32, batch: u32, pattern: c_int) -> c_int;
         pub fn kb200_rgb_from_bayer_u16(stream: *mut c_void, src: *const u16, src_len: usize, dst: *mut u16, dst_len: usize, width: u32, height: u32, batch: u32, pattern: c_int) -> c_int;
+        pub fn kb200_rgb_from_bayer_packed(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u16, dst_len: usize, width: u32, height: u32, batch: u32, pattern: c_int, bits: c_int) -> c_int;
         pub fn kb200_normalize_mean_std_f32(stream: *mut c_void, src: *const f32, dst: *mut f32, npixels: usize, channels: u32, mean: *const f32, std: *const f32) -> c_int;
         pub fn kb200_normalize_rgb_u8_f32(stream: *mut c_void, src: *const u8, dst: *mut f32, npixels: usize, scale: *const f32, offset: *const f32, leaf: c_int) -> c_int;
         pub fn kb200_find_min_max_f32(stream: *mut c_void, src: *const f32, n: usize, minmax_dev: *mut f32) -> c_int;
@@ -241,6 +242,12 @@ pub const FMT_BAYER_RGGB10: i32 = 32;
 pub const FMT_BAYER_RGGB12: i32 = 36;
 pub const FMT_BAYER_RGGB14: i32 = 40;
 pub const FMT_BAYER_RGGB16: i32 = 44;
+/// The 10-, 12- and 14-bit mosaics MIPI CSI-2 packed (V4L2's SRGGB10P ... SGBRG14P, w * bits / 8 bytes per row):
+/// `FMT_BAYER_PACKED_BASE + 4 * k + pattern`, k = 0..2 for 10, 12 and 14 bits.
+pub const FMT_BAYER_PACKED_BASE: i32 = 64;
+pub const FMT_BAYER_RGGB10P: i32 = 64;
+pub const FMT_BAYER_RGGB12P: i32 = 68;
+pub const FMT_BAYER_RGGB14P: i32 = 72;
 
 /// `pattern` of `kb200_rgb_from_bayer_u8` (kb200_bayer_pattern): the mosaic's 2x2 quad read row-major.
 pub const BAYER_RGGB: c_int = 0;

@@ -1,7 +1,9 @@
-// bayer.cuh — bilinear demosaic of Bayer mosaics, 8-bit or 16-bit samples, shared by the standalone decoders
-// (color.cu: rgb_from_bayer_vec<T, P>, rgb_from_bayer_generic<T, P>) and the camera preprocess (preprocess.cu:
-// preprocess_bayer_identity_kernel<F16, PTRS, T, P> and the Bayer taps of the generic kernel).  Everything here is
-// generic over the sample type T; BayerSample<T> holds the few facts of T the kernels above it need.
+// bayer.cuh — bilinear demosaic of Bayer mosaics, 8-bit, 16-bit or MIPI-packed 10/12/14-bit samples, shared by the
+// standalone decoders (color.cu: rgb_from_bayer_vec<T, P>, rgb_from_bayer_generic<T, P>) and the camera preprocess
+// (preprocess.cu: preprocess_bayer_identity_kernel<F16, PTRS, T, P> and the Bayer taps of the generic kernel).  Everything
+// here is generic over the sample type T; BayerSample<T> holds the few facts of T the kernels above it need.  Packed
+// samples (T = BayerPacked<BITS>) only change the loads: they are unpacked into the words of the 16-bit kernels
+// (bayer_unpack, bayer_load_rows_packed, bayer_px_packed), and everything after that is the uint16_t path.
 //
 // An extension beyond the reference, pinned to OpenCV: bit-identical to cv2.cvtColor(raw, COLOR_Bayer??2RGB)
 // (checked against cv2 4.13 on 8-bit and 16-bit mosaics, tests/golden/bayer_cv2.npz and bayer16_cv2.npz).  A pattern (kb200_bayer_pattern) is named by its 2x2 quad
@@ -51,12 +53,76 @@ __device__ __forceinline__ void bayer_px(const T* __restrict__ src, size_t pitch
     bayer_demosaic(P, cx & 1, cy & 1, __ldg(mid), __ldg(up), __ldg(dn), __ldg(mid - 1), __ldg(mid + 1), d, rgb[0], rgb[1], rgb[2]);
 }
 
-// The sample types: uint8_t (8-bit mosaics) and uint16_t (10- to 16-bit).  VEC_COLS: columns per 16-byte vector, the
-// row segment of a decoder thread.  ID_WORDS: 32-bit words per 4-sample load of the preprocess identity kernel
-// (LDG.32 / LDG.64), and ID_ALIGN: the row and frame alignment in bytes that load needs.
+// MIPI CSI-2 packed samples of BITS = 10, 12 or 14 bits (V4L2's SRGGB10P ... SGBRG14P).  Each row is packed on its own
+// in groups of G = 4, 2, 4 samples in GB = 5, 3, 7 bytes: the first G bytes hold the high 8 bits of each sample, the
+// rest the low BITS - 8 bits of sample j at bit (BITS - 8) * j of their little-endian word.  A tag type: no value of it
+// is ever read, it only selects the packed loaders below.
+template <int BITS> struct BayerPacked {};
+__host__ __device__ constexpr int bayer_packed_group(int bits) { return bits == 12 ? 2 : 4; }
+__host__ __device__ constexpr int bayer_packed_group_bytes(int bits) { return bayer_packed_group(bits) * bits / 8; }
+
+// The sample types: uint8_t (8-bit mosaics), uint16_t (10- to 16-bit) and BayerPacked<BITS>.  VEC_COLS: columns per
+// decoder thread (one 16-byte vector of uint8_t / uint16_t samples).  ID_WORDS: 32-bit words per 4-sample load of the
+// preprocess identity kernel (LDG.32 / LDG.64), and ID_ALIGN: the row and frame alignment in bytes that load needs.
+// Word: the sample type of the unpacked words the demosaic reads (bayer_row) and of the decoder's output.  PACKED_BITS:
+// the packing's bits per sample, 0 for the unpacked types.
 template <typename T> struct BayerSample;
-template <> struct BayerSample<uint8_t> { static constexpr uint32_t VEC_COLS = 16, ID_WORDS = 1, ID_ALIGN = 4; };
-template <> struct BayerSample<uint16_t> { static constexpr uint32_t VEC_COLS = 8, ID_WORDS = 2, ID_ALIGN = 8; };
+template <> struct BayerSample<uint8_t> {
+    static constexpr uint32_t VEC_COLS = 16, ID_WORDS = 1, ID_ALIGN = 4;
+    static constexpr int PACKED_BITS = 0;
+    using Word = uint8_t;
+};
+template <> struct BayerSample<uint16_t> {
+    static constexpr uint32_t VEC_COLS = 8, ID_WORDS = 2, ID_ALIGN = 8;
+    static constexpr int PACKED_BITS = 0;
+    using Word = uint16_t;
+};
+template <int BITS> struct BayerSample<BayerPacked<BITS>> {
+    static constexpr uint32_t VEC_COLS = 8, ID_WORDS = 2, ID_ALIGN = 16;
+    static constexpr int PACKED_BITS = BITS;
+    using Word = uint16_t;
+};
+
+// Sample x of a packed row at `row` (bits known at compile time in the fast kernels, at run time in the generic
+// preprocess): the high byte and the low field of its group, reading no byte outside the group.
+// Shifts, not divisions: with bits known only at run time a division by the group size is a long integer sequence.
+__device__ __forceinline__ int bayer_packed_sample(const uint8_t* __restrict__ row, int x, int bits) {
+    const int gs = bits == 12 ? 1 : 2, lo = bits - 8;   // log2 of the samples per group, low bits per sample
+    const int j = x & ((1 << gs) - 1);
+    const uint8_t* grp = row + (x >> gs) * ((bits << gs) >> 3);
+    const int at = lo * j, bi = at >> 3, sh = at & 7;
+    int field = __ldg(grp + (1 << gs) + bi);
+    if (sh + lo > 8) field |= (int)__ldg(grp + (1 << gs) + bi + 1) << 8;
+    return ((int)__ldg(grp + j) << lo) | ((field >> sh) & ((1 << lo) - 1));
+}
+
+// bayer_px on a packed frame: `pitch` in bytes.
+__device__ __forceinline__ void bayer_px_packed(const uint8_t* __restrict__ src, size_t pitch, int w, int h, int x, int y, int P, int bits,
+                                                int rgb[3]) {
+    const int cx = min(max(x, 1), w - 2), cy = min(max(y, 1), h - 2);
+    const uint8_t* up = src + (size_t)(cy - 1) * pitch;
+    const uint8_t* mid = up + pitch;
+    const uint8_t* dn = mid + pitch;
+    auto at = [&](const uint8_t* row, int c) { return bayer_packed_sample(row, c, bits); };
+    const int d = at(up, cx - 1) + at(up, cx + 1) + at(dn, cx - 1) + at(dn, cx + 1);
+    bayer_demosaic(P, cx & 1, cy & 1, at(mid, cx), at(up, cx), at(dn, cx), at(mid, cx - 1), at(mid, cx + 1), d, rgb[0], rgb[1], rgb[2]);
+}
+
+// Unpacks the N samples of whole groups held in `bytes` (little-endian, byte 0 the first byte of a group) into N / 2
+// words of 16-bit samples, sample 2m in the low half of word m: the layout bayer_row reads for uint16_t.
+template <int BITS, int N>
+__device__ __forceinline__ void bayer_unpack(const uint32_t* bytes, uint32_t words[N / 2]) {
+    constexpr int G = bayer_packed_group(BITS), GB = bayer_packed_group_bytes(BITS), LO = BITS - 8;
+    auto byte = [&](int k) { return (bytes[k >> 2] >> (8 * (k & 3))) & 0xFFu; };
+#pragma unroll
+    for (int s = 0; s < N; ++s) {
+        const int base = (s / G) * GB, j = s % G, at = LO * j;
+        uint32_t field = byte(base + G + (at >> 3));
+        if ((at & 7) + LO > 8) field |= byte(base + G + (at >> 3) + 1) << 8;
+        const uint32_t v = (byte(base + j) << LO) | ((field >> (at & 7)) & ((1u << LO) - 1u));
+        if (s & 1) words[s >> 1] |= v << 16; else words[s >> 1] = v;
+    }
+}
 
 // Samples of type T per 32-bit word of a row segment, and their width in bits.
 template <typename T> __host__ __device__ constexpr int bayer_per_word() { return 4 / (int)sizeof(T); }
@@ -109,6 +175,23 @@ __device__ __forceinline__ void bayer_load_rows(const T* __restrict__ frame, siz
         hr[k] = (int)(__shfl_down_sync(0xFFFFFFFFu, rows[k][0], 1) & M);
         if (lane == 0 && x > 0) hl[k] = __ldg(row + x - 1);
         if (lane == 31 && x + S * NW < w) hr[k] = __ldg(row + x + S * NW);
+    }
+}
+
+// bayer_load_rows on a packed frame of BITS-bit samples (`pitch` in bytes): LOAD(k, row, words) fills the NW words of
+// the lane's 2 * NW columns at x of row ya-1+k (clamped) in the uint16_t layout (bayer_unpack), and the edge lanes read
+// their halo sample from its group.
+template <int NW, int BITS, typename LOAD>
+__device__ __forceinline__ void bayer_load_rows_packed(const uint8_t* __restrict__ frame, size_t pitch, uint32_t w, uint32_t h, uint32_t x,
+                                                       uint32_t ya, uint32_t lane, LOAD load, uint32_t rows[4][NW], int hl[4], int hr[4]) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const uint8_t* row = frame + (size_t)min(ya - 1 + k, h - 1) * pitch;
+        load(k, row, rows[k]);
+        hl[k] = (int)(__shfl_up_sync(0xFFFFFFFFu, rows[k][NW - 1], 1) >> 16);
+        hr[k] = (int)(__shfl_down_sync(0xFFFFFFFFu, rows[k][0], 1) & 0xFFFFu);
+        if (lane == 0 && x > 0) hl[k] = bayer_packed_sample(row, (int)x - 1, BITS);
+        if (lane == 31 && x + 2 * NW < w) hr[k] = bayer_packed_sample(row, (int)(x + 2 * NW), BITS);
     }
 }
 

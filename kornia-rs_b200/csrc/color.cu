@@ -313,8 +313,14 @@ __device__ __forceinline__ void bayer_row48(const uint32_t n[4], const uint32_t 
 // and ya + 1 (bayer_row_pairs).  Loads the rows ya-1 .. ya+2 of its S columns as four lane-contiguous LDG.128 plus
 // shuffled halos (bayer_load_rows) and stores 48 B per row through store_rgb48_coalesced (three lane-contiguous STG.128
 // per warp and row).  Requires width % S == 0 and 16-B aligned bases, so every row of source and output starts 16-B aligned.
+// Packed samples (T = BayerPacked<BITS>): a warp's 32 * 8 columns are 32 * BITS contiguous bytes of a row (320, 384 or
+// 448), loaded as lane-contiguous LDG.128 into shared memory; each lane then unpacks its BITS bytes into the uint16_t
+// words of the 16-bit kernel.  Requires width * BITS % 128 == 0 (every row 16-B aligned) and 16-B aligned bases.
 template <typename T, int P>
-__global__ void __launch_bounds__(128) rgb_from_bayer_vec(const T* __restrict__ src, T* __restrict__ dst, uint32_t width, uint32_t height) {
+__global__ void __launch_bounds__(128) rgb_from_bayer_vec(const T* __restrict__ src, typename BayerSample<T>::Word* __restrict__ dst,
+                                                          uint32_t width, uint32_t height) {
+    using W = typename BayerSample<T>::Word;
+    constexpr int PB = BayerSample<T>::PACKED_BITS;
     constexpr uint32_t S = BayerSample<T>::VEC_COLS;
     __shared__ uint4 stage[4][96];
     const uint32_t gx = blockIdx.x * blockDim.x + threadIdx.x;  // S-column group
@@ -325,14 +331,37 @@ __global__ void __launch_bounds__(128) rgb_from_bayer_vec(const T* __restrict__ 
     const bool active = gx * S < width;
     const uint32_t x = gx * S;
     const uint32_t ya = 1 + 2 * blockIdx.y, yb = ya + 1;
-    const T* frame = src + (size_t)blockIdx.z * width * height;
-    T* out = dst + (size_t)blockIdx.z * width * height * 3;
     uint32_t rows[4][4];
     int hl[4], hr[4];
-    bayer_load_rows<4>(frame, width, width, height, x, ya, lane, [&](const T* p, uint32_t v[4]) {
-        const uint4 q = active ? ldg_stream_u4(reinterpret_cast<const uint4*>(p)) : make_uint4(0, 0, 0, 0);
-        v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
-    }, rows, hl, hr);
+    if constexpr (PB == 0) {
+        const T* frame = src + (size_t)blockIdx.z * width * height;
+        bayer_load_rows<4>(frame, width, width, height, x, ya, lane, [&](const T* p, uint32_t v[4]) {
+            const uint4 q = active ? ldg_stream_u4(reinterpret_cast<const uint4*>(p)) : make_uint4(0, 0, 0, 0);
+            v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
+        }, rows, hl, hr);
+    } else {
+        __shared__ uint4 packed[4][4][33];   // per warp and row: the warp's <= 448 bytes, and room for the last lane's over-read
+        const size_t pitch = (size_t)width * PB / 8;
+        const uint8_t* frame = reinterpret_cast<const uint8_t*>(src) + (size_t)blockIdx.z * pitch * height;
+        const uint32_t seg_bytes = (min(width - gx0 * S, 32u * S) * PB) / 8;   // this warp's bytes of a row
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint8_t* seg = frame + (size_t)min(ya - 1 + k, height - 1) * pitch + (size_t)gx0 * PB;
+            if (16u * lane < seg_bytes) packed[wid][k][lane] = ldg_stream_u4(reinterpret_cast<const uint4*>(seg) + lane);
+        }
+        __syncwarp();
+        bayer_load_rows_packed<4, PB>(frame, pitch, width, height, x, ya, lane, [&](int k, const uint8_t*, uint32_t v[4]) {
+            const uint32_t o = lane * PB;   // the lane's first byte in the warp's segment
+            const uint32_t* wds = reinterpret_cast<const uint32_t*>(packed[wid][k]) + (o >> 2);
+            const uint32_t sh = 8u * (o & 3u);
+            uint32_t bytes[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) bytes[i] = __funnelshift_r(wds[i], wds[i + 1], sh);
+            bayer_unpack<PB, 8>(bytes, v);
+            if (!active) { v[0] = 0; v[1] = 0; v[2] = 0; v[3] = 0; }
+        }, rows, hl, hr);
+    }
+    W* out = dst + (size_t)blockIdx.z * width * height * 3;
     const bool left_edge = x == 0, right_edge = x + S == width;
     auto store_row = [&](uint32_t y, const uint4 o[3]) {
         uint4* d = reinterpret_cast<uint4*>(out + ((size_t)y * width + (size_t)gx0 * S) * 3);   // this warp's run of row y
@@ -340,29 +369,38 @@ __global__ void __launch_bounds__(128) rgb_from_bayer_vec(const T* __restrict__ 
         else if (active) { stg_stream_u4(d + 3 * lane, o[0]); stg_stream_u4(d + 3 * lane + 1, o[1]); stg_stream_u4(d + 3 * lane + 2, o[2]); }
     };
     uint4 oa[3];
-    bayer_row48<T, P, 1>(rows[0], rows[1], rows[2], hl, hr, left_edge, right_edge, oa);   // ya is odd
+    bayer_row48<W, P, 1>(rows[0], rows[1], rows[2], hl, hr, left_edge, right_edge, oa);   // ya is odd
     store_row(ya, oa);
     if (ya == 1) store_row(0, oa);
     if (yb == height - 1) {
         store_row(yb, oa);
     } else {
         uint4 ob[3];
-        bayer_row48<T, P, 0>(rows[1], rows[2], rows[3], hl + 1, hr + 1, left_edge, right_edge, ob);
+        bayer_row48<W, P, 0>(rows[1], rows[2], rows[3], hl + 1, hr + 1, left_edge, right_edge, ob);
         store_row(yb, ob);
         if (yb == height - 2) store_row(height - 1, ob);
     }
 }
 
-// Generic fallback (any width, any base aligned to T): one thread per pixel, nine sample loads.
+// Generic fallback (any width, any base aligned to T; packed: any base): one thread per pixel, nine sample loads.
 template <typename T, int P>
-__global__ void rgb_from_bayer_generic(const T* __restrict__ src, T* __restrict__ dst, uint32_t width, uint32_t height) {
+__global__ void rgb_from_bayer_generic(const T* __restrict__ src, typename BayerSample<T>::Word* __restrict__ dst, uint32_t width,
+                                       uint32_t height) {
+    using W = typename BayerSample<T>::Word;
+    constexpr int PB = BayerSample<T>::PACKED_BITS;
     const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x >= width || y >= height) return;
     const size_t frame = (size_t)width * height;
     int rgb[3];
-    bayer_px(src + blockIdx.z * frame, width, (int)width, (int)height, (int)x, (int)y, P, rgb);
-    T* o = dst + (blockIdx.z * frame + (size_t)y * width + x) * 3;
-    o[0] = (T)rgb[0]; o[1] = (T)rgb[1]; o[2] = (T)rgb[2];
+    if constexpr (PB == 0) {
+        bayer_px(src + blockIdx.z * frame, width, (int)width, (int)height, (int)x, (int)y, P, rgb);
+    } else {
+        const size_t pitch = (size_t)width * PB / 8;
+        bayer_px_packed(reinterpret_cast<const uint8_t*>(src) + blockIdx.z * pitch * height, pitch, (int)width, (int)height, (int)x, (int)y, P,
+                        PB, rgb);
+    }
+    W* o = dst + (blockIdx.z * frame + (size_t)y * width + x) * 3;
+    o[0] = (W)rgb[0]; o[1] = (W)rgb[1]; o[2] = (W)rgb[2];
 }
 
 static inline unsigned stream_grid(size_t items, unsigned block, unsigned ctas_per_sm) {
@@ -400,8 +438,8 @@ static const Yuv422Kernels YUV422_KERNELS[3] = {
 static const char* const BAYER_PATTERNS[4] = {"RGGB", "BGGR", "GRBG", "GBRG"};
 template <typename T>
 struct BayerKernels {
-    void (*vec)(const T*, T*, uint32_t, uint32_t);
-    void (*generic)(const T*, T*, uint32_t, uint32_t);
+    void (*vec)(const T*, typename BayerSample<T>::Word*, uint32_t, uint32_t);
+    void (*generic)(const T*, typename BayerSample<T>::Word*, uint32_t, uint32_t);
     const char *vec_name, *generic_name;
 };
 static const BayerKernels<uint8_t> BAYER_KERNELS_U8[4] = {
@@ -440,6 +478,52 @@ static int launch_rgb_from_bayer(const BayerKernels<T> (&table)[4], kb200_stream
     }
     dim3 block(32, 8), grid(div_up(width, 32), div_up(height, 8), batch);
     k.generic<<<grid, block, 0, s>>>(src, dst, width, height);
+    return check_launch(k.generic_name);
+}
+
+// The packed decoders, by depth (10, 12, 14 bits) and pattern.
+#define KB200_BAYER_PACKED_KERNELS(B, p, P)                                                                            \
+    {rgb_from_bayer_vec<BayerPacked<B>, P>, rgb_from_bayer_generic<BayerPacked<B>, P>, "rgb_from_bayer" #B "p_" #p "_vec", \
+     "rgb_from_bayer" #B "p_" #p "_generic"}
+#define KB200_BAYER_PACKED_TABLE(B)                                                                                     \
+    static const BayerKernels<BayerPacked<B>> BAYER_KERNELS_##B##P[4] = {                                               \
+        KB200_BAYER_PACKED_KERNELS(B, rggb, KB200_BAYER_RGGB), KB200_BAYER_PACKED_KERNELS(B, bggr, KB200_BAYER_BGGR),   \
+        KB200_BAYER_PACKED_KERNELS(B, grbg, KB200_BAYER_GRBG), KB200_BAYER_PACKED_KERNELS(B, gbrg, KB200_BAYER_GBRG)};
+KB200_BAYER_PACKED_TABLE(10)
+KB200_BAYER_PACKED_TABLE(12)
+KB200_BAYER_PACKED_TABLE(14)
+#undef KB200_BAYER_PACKED_TABLE
+#undef KB200_BAYER_PACKED_KERNELS
+
+// The demosaic behind kb200_rgb_from_bayer_packed (pointers, pattern and bits already checked): `batch` tight frames of
+// h rows of width * BITS / 8 bytes.  The fast kernel when every row and both bases are 16-B aligned, the
+// one-thread-per-pixel kernel otherwise.  src_len in bytes, dst_len in elements.
+template <int BITS>
+static int launch_rgb_from_bayer_packed(const BayerKernels<BayerPacked<BITS>> (&table)[4], kb200_stream_t stream, const uint8_t* src,
+                                        size_t src_len, uint16_t* dst, size_t dst_len, uint32_t width, uint32_t height, uint32_t batch,
+                                        int pattern) {
+    const BayerKernels<BayerPacked<BITS>>& k = table[pattern];
+    KB200_TRY(check_geometry(width, height, width, height, batch));
+    if (width < 3 || height < 3)
+        return fail(KB200_ERR_INVALID_ARGUMENT, "Bayer %s%dP needs at least 3x3 pixels, got %ux%u", BAYER_PATTERNS[pattern], BITS, width, height);
+    constexpr uint32_t G = bayer_packed_group(BITS);
+    if (width % G)
+        return fail(KB200_ERR_INVALID_ARGUMENT, "Bayer %s%dP needs a width that is a multiple of %u (whole %d-byte groups), got %u",
+                    BAYER_PATTERNS[pattern], BITS, G, bayer_packed_group_bytes(BITS), width);
+    if (batch > 65535u) return fail(KB200_ERR_INVALID_ARGUMENT, "batch %u exceeds 65535", batch);
+    const size_t frame = (size_t)width * BITS / 8 * height;
+    KB200_TRY(check_slice("src", src_len, frame * batch)); KB200_TRY(check_slice("dst", dst_len, (size_t)width * height * 3 * batch));
+    cudaStream_t s = as_stream(stream);
+    const BayerPacked<BITS>* p = reinterpret_cast<const BayerPacked<BITS>*>(src);
+    if (((size_t)width * BITS) % 128 == 0 && aligned16(src) && aligned16(dst) && bayer_row_pairs(height) <= 65535u) {
+        const unsigned groups = width / 8;
+        const unsigned bx = groups >= 128 ? 128 : 32 * ((groups + 31) / 32);
+        dim3 grid(div_up(groups, bx), bayer_row_pairs(height), batch);
+        k.vec<<<grid, bx, 0, s>>>(p, dst, width, height);
+        return check_launch(k.vec_name);
+    }
+    dim3 block(32, 8), grid(div_up(width, 32), div_up(height, 8), batch);
+    k.generic<<<grid, block, 0, s>>>(p, dst, width, height);
     return check_launch(k.generic_name);
 }
 
@@ -611,6 +695,19 @@ KB200_API int kb200_rgb_from_bayer_u16(kb200_stream_t stream, const uint16_t* sr
     if (reinterpret_cast<uintptr_t>(src) & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "'src' is not 2-byte aligned (16-bit samples)");
     if (reinterpret_cast<uintptr_t>(dst) & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "'dst' is not 2-byte aligned (16-bit samples)");
     return launch_rgb_from_bayer(BAYER_KERNELS_U16, stream, src, src_len, dst, dst_len, width, height, batch, pattern);
+}
+
+KB200_API int kb200_rgb_from_bayer_packed(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint16_t* dst, size_t dst_len,
+                                          uint32_t width, uint32_t height, uint32_t batch, int pattern, int bits) {
+    KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
+    if (reinterpret_cast<uintptr_t>(dst) & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "'dst' is not 2-byte aligned (16-bit samples)");
+    if (pattern < KB200_BAYER_RGGB || pattern > KB200_BAYER_GBRG) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown Bayer pattern %d", pattern);
+    switch (bits) {
+        case 10: return launch_rgb_from_bayer_packed<10>(BAYER_KERNELS_10P, stream, src, src_len, dst, dst_len, width, height, batch, pattern);
+        case 12: return launch_rgb_from_bayer_packed<12>(BAYER_KERNELS_12P, stream, src, src_len, dst, dst_len, width, height, batch, pattern);
+        case 14: return launch_rgb_from_bayer_packed<14>(BAYER_KERNELS_14P, stream, src, src_len, dst, dst_len, width, height, batch, pattern);
+        default: return fail(KB200_ERR_INVALID_ARGUMENT, "packed Bayer samples are 10, 12 or 14 bits, got %d", bits);
+    }
 }
 
 

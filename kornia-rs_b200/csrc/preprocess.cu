@@ -99,14 +99,18 @@ __device__ __forceinline__ void fetch_px_yuv_ext(const uint8_t* __restrict__ src
 }
 
 // Which formats an instantiation of the generic kernel serves: the reference's (fmt 0-4), the YUV layouts beyond them
-// (fmt 5-9), the 8-bit Bayer mosaics (fmt 16-19) or the 16-bit ones (fmt 32-47).  Separate instantiations, so the
-// kernels of fmt 0-4 are unchanged by the others.
-static constexpr int SRC_BASE = 0, SRC_EXT_YUV = 1, SRC_BAYER = 2, SRC_BAYER16 = 3;
+// (fmt 5-9), the 8-bit Bayer mosaics (fmt 16-19), the 16-bit ones (fmt 32-47) or the packed ones (fmt 64-75).
+// Separate instantiations, so the kernels of fmt 0-4 are unchanged by the others.
+static constexpr int SRC_BASE = 0, SRC_EXT_YUV = 1, SRC_BAYER = 2, SRC_BAYER16 = 3, SRC_BAYER_PACKED = 4;
 
 // fmt 32-47 = 32 + 4*k + kb200_bayer_pattern, k = 0..3 for 10, 12, 14 and 16 bits per sample
 __host__ __device__ inline int bayer16_pattern(int fmt) { return (fmt - KB200_FMT_BAYER_RGGB10) & 3; }
 __host__ __device__ inline int bayer16_bits(int fmt) { return 10 + 2 * ((fmt - KB200_FMT_BAYER_RGGB10) >> 2); }
 __host__ __device__ inline float bayer16_white(int fmt) { return (float)((1u << bayer16_bits(fmt)) - 1u); }
+// fmt 64-75 = 64 + 4*k + kb200_bayer_pattern, k = 0..2 for 10, 12 and 14 bits per packed sample
+__host__ __device__ inline int bayer_packed_pattern(int fmt) { return (fmt - KB200_FMT_BAYER_RGGB10P) & 3; }
+__host__ __device__ inline int bayer_packed_bits(int fmt) { return 10 + 2 * ((fmt - KB200_FMT_BAYER_RGGB10P) >> 2); }
+__host__ __device__ inline float bayer_packed_white(int fmt) { return (float)((1u << bayer_packed_bits(fmt)) - 1u); }
 // kb200_bayer_pattern of a Bayer format: fmt 16-19 (8-bit samples) = 16 + pattern, fmt 32-47 (16-bit) as above
 __host__ __device__ inline int bayer_pattern(int fmt, bool bayer16) { return bayer16 ? bayer16_pattern(fmt) : fmt - KB200_FMT_BAYER_RGGB; }
 
@@ -117,6 +121,10 @@ __device__ __forceinline__ void fetch_px(const uint8_t* __restrict__ src, int x,
         using T = std::conditional_t<EXT == SRC_BAYER16, uint16_t, uint8_t>;
         int rgb[3];
         bayer_px(reinterpret_cast<const T*>(src), (size_t)d.src_pitch / sizeof(T), d.src_w, d.src_h, x, y, bayer_pattern(d.fmt, EXT == SRC_BAYER16), rgb);
+        px[0] = (float)rgb[0]; px[1] = (float)rgb[1]; px[2] = (float)rgb[2];
+    } else if (EXT == SRC_BAYER_PACKED) {
+        int rgb[3];
+        bayer_px_packed(src, (size_t)d.src_pitch, d.src_w, d.src_h, x, y, bayer_packed_pattern(d.fmt), bayer_packed_bits(d.fmt), rgb);
         px[0] = (float)rgb[0]; px[1] = (float)rgb[1]; px[2] = (float)rgb[2];
     } else if (EXT == SRC_EXT_YUV) {
         fetch_px_yuv_ext(src, x, y, d, px);
@@ -213,8 +221,8 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
         px[0] = d.pad_value; px[1] = d.pad_value; px[2] = d.pad_value;
     }
     float q0, q1, q2;
-    if (EXT == SRC_BAYER16 && inside) {   // px / W: taps up to 65535 and Lanczos overshoot, so the IEEE division
-        const float wl = bayer16_white(d.fmt);
+    if ((EXT == SRC_BAYER16 || EXT == SRC_BAYER_PACKED) && inside) {   // px / W: taps up to 65535 and Lanczos overshoot, so the IEEE division
+        const float wl = EXT == SRC_BAYER16 ? bayer16_white(d.fmt) : bayer_packed_white(d.fmt);
         q0 = __fdiv_rn(px[0], wl); q1 = __fdiv_rn(px[1], wl); q2 = __fdiv_rn(px[2], wl);
     } else if (inside && SAMP != KB200_INTERP_LANCZOS) { q0 = div255_exact(px[0]); q1 = div255_exact(px[1]); q2 = div255_exact(px[2]); }
     else if (inside) { q0 = __fdiv_rn(px[0], 255.0f); q1 = __fdiv_rn(px[1], 255.0f); q2 = __fdiv_rn(px[2], 255.0f); }  // Lanczos overshoots [0, 255]
@@ -326,11 +334,15 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const _
 // pairs of bayer_row_pairs): 4 lane-contiguous loads of the rows ya-1 .. ya+2 (LDG.32 of 8-bit samples, LDG.64 of 16-bit
 // ones: BayerSample<T>::ID_WORDS) plus shuffled halos (bayer_load_rows), 6 to 12 lane-contiguous 4-pixel stores per
 // thread (nv12_store4).  Requires w % 4 == 0 and rows aligned to BayerSample<T>::ID_ALIGN.
+// Packed samples (T = BayerPacked<BITS>): a thread's 4 columns are BITS / 2 bytes of a row, read as the aligned 8-byte
+// word that holds their first byte and, when they run past it, the next one (L1-allocating: the neighbouring lanes read
+// the same words), then unpacked into the words of the 16-bit kernel (bayer_unpack).  Rows and frames 16-B aligned.
 template <bool F16, bool PTRS, typename T, int P>
 __global__ void __launch_bounds__(128) preprocess_bayer_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                         const __grid_constant__ PreFrames fr, void* __restrict__ dst,
                                                                         uint32_t frame0, uint32_t groups_per_row, uint32_t items) {
     constexpr uint32_t NW = BayerSample<T>::ID_WORDS;
+    constexpr int PB = BayerSample<T>::PACKED_BITS;
     const uint32_t item = blockIdx.x * blockDim.x + threadIdx.x;
     const bool active = item < items;                         // the lanes past the end still take part in the shuffles
     const uint32_t it = active ? item : items - 1;
@@ -341,19 +353,34 @@ __global__ void __launch_bounds__(128) preprocess_bayer_identity_kernel(const __
     const uint32_t x = g * 4u, ya = 1u + 2u * rp, yb = ya + 1u;
     uint32_t rows[4][NW];
     int hl[4], hr[4];
-    bayer_load_rows<NW>(src, (size_t)d.src_pitch / sizeof(T), w, h, x, ya, threadIdx.x & 31u, [](const T* p, uint32_t v[NW]) {
-        if constexpr (NW == 1) {
-            v[0] = __ldg(reinterpret_cast<const uint32_t*>(p));
-        } else {
-            const uint2 q = __ldg(reinterpret_cast<const uint2*>(p));
-            v[0] = q.x; v[1] = q.y;
-        }
-    }, rows, hl, hr);
+    if constexpr (PB == 0) {
+        bayer_load_rows<NW>(src, (size_t)d.src_pitch / sizeof(T), w, h, x, ya, threadIdx.x & 31u, [](const T* p, uint32_t v[NW]) {
+            if constexpr (NW == 1) {
+                v[0] = __ldg(reinterpret_cast<const uint32_t*>(p));
+            } else {
+                const uint2 q = __ldg(reinterpret_cast<const uint2*>(p));
+                v[0] = q.x; v[1] = q.y;
+            }
+        }, rows, hl, hr);
+    } else {
+        const uint32_t off = x * PB / 8, s = off & 7u;   // the thread's first byte in its row, and its place in its 8-byte word
+        bayer_load_rows_packed<NW, PB>(reinterpret_cast<const uint8_t*>(src), (size_t)d.src_pitch, w, h, x, ya, threadIdx.x & 31u,
+                                       [&](int, const uint8_t* row, uint32_t v[NW]) {
+            const uint2* p = reinterpret_cast<const uint2*>(row + (off - s));
+            const uint2 a = __ldg(p);
+            const uint2 b = s + PB / 2 > 8u ? __ldg(p + 1) : make_uint2(0, 0);
+            const uint32_t t0 = s >= 4u ? a.y : a.x, t1 = s >= 4u ? b.x : a.y, t2 = s >= 4u ? b.y : b.x;
+            const uint32_t sh = 8u * (s & 3u);
+            const uint32_t bytes[2] = {__funnelshift_r(t0, t1, sh), __funnelshift_r(t1, t2, sh)};
+            bayer_unpack<PB, 4>(bytes, v);
+        }, rows, hl, hr);
+    }
     if (!active) return;
     const bool left_edge = x == 0, right_edge = x + 4u == w;
     const size_t plane = (size_t)w * h;
     const size_t base = (size_t)(frame0 + f) * 3 * plane + x;
-    [[maybe_unused]] const float wl = bayer16_white(d.fmt);   // the white level W of a 16-bit format
+    // the white level W of a 16-bit or packed format
+    [[maybe_unused]] const float wl = PB == 0 ? bayer16_white(d.fmt) : (float)((1u << PB) - 1u);
     const float m0 = d.mean[0], m1 = d.mean[1], m2 = d.mean[2], i0 = d.inv_std[0], i1 = d.inv_std[1], i2 = d.inv_std[2];
     float r4[4], g4[4], b4[4];
     auto store_row = [&](uint32_t y) {
@@ -362,11 +389,11 @@ __global__ void __launch_bounds__(128) preprocess_bayer_identity_kernel(const __
         nv12_store4<F16>(dst, o + plane, g4);
         nv12_store4<F16>(dst, o + 2 * plane, b4);
     };
-    // 8-bit: px / 255 by the exact 3-instruction form (norm_int_px); 16-bit: px / W, the IEEE division
+    // 8-bit: px / 255 by the exact 3-instruction form (norm_int_px); 16-bit and packed: px / W, the IEEE division
     auto norm = [&](const int r[4], const int gg[4], const int b[4]) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-            if constexpr (sizeof(T) == 1) {
+            if constexpr (std::is_same_v<T, uint8_t>) {
                 r4[i] = norm_int_px(r[i], m0, i0); g4[i] = norm_int_px(gg[i], m1, i1); b4[i] = norm_int_px(b[i], m2, i2);
             } else {
                 r4[i] = (__fdiv_rn((float)r[i], wl) - m0) * i0;
@@ -375,13 +402,14 @@ __global__ void __launch_bounds__(128) preprocess_bayer_identity_kernel(const __
             }
         }
     };
+    using W = typename BayerSample<T>::Word;
     int r[4], gg[4], b[4];
-    bayer_row<P, 1, NW, T>(rows[0], rows[1], rows[2], hl, hr, left_edge, right_edge, r, gg, b);   // ya is odd
+    bayer_row<P, 1, NW, W>(rows[0], rows[1], rows[2], hl, hr, left_edge, right_edge, r, gg, b);   // ya is odd
     norm(r, gg, b);
     store_row(ya);
     if (ya == 1u) store_row(0);
     if (yb == h - 1u) { store_row(yb); return; }
-    bayer_row<P, 0, NW, T>(rows[1], rows[2], rows[3], hl + 1, hr + 1, left_edge, right_edge, r, gg, b);
+    bayer_row<P, 0, NW, W>(rows[1], rows[2], rows[3], hl + 1, hr + 1, left_edge, right_edge, r, gg, b);
     norm(r, gg, b);
     store_row(yb);
     if (yb == h - 2u) store_row(h - 1u);
@@ -526,6 +554,7 @@ static int yuv420_layout(int fmt) {
 static bool is_yuv422(int fmt) { return fmt == KB200_FMT_YUYV || fmt == KB200_FMT_UYVY || fmt == KB200_FMT_YVYU; }
 static bool is_bayer(int fmt) { return fmt >= KB200_FMT_BAYER_RGGB && fmt <= KB200_FMT_BAYER_GBRG; }
 static bool is_bayer16(int fmt) { return fmt >= KB200_FMT_BAYER_RGGB10 && fmt <= KB200_FMT_BAYER_GBRG16; }
+static bool is_bayer_packed(int fmt) { return fmt >= KB200_FMT_BAYER_RGGB10P && fmt <= KB200_FMT_BAYER_GBRG14P; }
 // SourceFormat names, in the validation messages
 static const char* const FMT_NAMES[10] = {"Rgb8", "Bgr8", "Gray8", "Nv12", "Yuyv", "Nv21", "I420", "Yv12", "Uyvy", "Yvyu"};
 static const char* const BAYER_NAMES[4] = {"BayerRggb", "BayerBggr", "BayerGrbg", "BayerGbrg"};
@@ -542,7 +571,8 @@ static int validate_desc(const kb200_preprocess_desc* dp) {
     if (d.src_w <= 0 || d.src_h <= 0 || d.dst_w <= 0 || d.dst_h <= 0)
         return fail(KB200_ERR_INVALID_ARGUMENT, "image dimensions must be non-zero");
     if ((long long)d.dst_w * d.dst_h > 0x7FFFFFFFll) return fail(KB200_ERR_DIMS_TOO_LARGE, "dimensions exceed the 32-bit CUDA kernel index limit");  // :1336-1339
-    if (d.fmt < 0 || (d.fmt > KB200_FMT_YVYU && !is_bayer(d.fmt) && !is_bayer16(d.fmt))) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown source format code %d", d.fmt);
+    if (d.fmt < 0 || (d.fmt > KB200_FMT_YVYU && !is_bayer(d.fmt) && !is_bayer16(d.fmt) && !is_bayer_packed(d.fmt)))
+        return fail(KB200_ERR_INVALID_ARGUMENT, "unknown source format code %d", d.fmt);
     if (d.sampling != KB200_INTERP_NEAREST && d.sampling != KB200_INTERP_BILINEAR && d.sampling != KB200_INTERP_LANCZOS)
         return fail(KB200_ERR_UNSUPPORTED, "unsupported sampling mode %d (expected Nearest, Bilinear or Lanczos)", d.sampling);  // preprocess.rs:1044-1051
     if (d.fmt <= 1 && d.src_bpp != 3 && d.src_bpp != 4) return fail(KB200_ERR_UNSUPPORTED, "unsupported source channel count %d (expected 3 or 4)", d.src_bpp);
@@ -560,8 +590,21 @@ static int validate_desc(const kb200_preprocess_desc* dp) {
         if (d.src_pitch & 1)
             return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface for %s%d (pitch %d is odd: rows of 16-bit samples must start 2-byte aligned)", name, bits, d.src_pitch);
     }
+    if (is_bayer_packed(d.fmt)) {   // SourceFormat names: BayerRggb10p ... BayerGbrg14p
+        const char* name = BAYER_NAMES[bayer_packed_pattern(d.fmt)];
+        const int bits = bayer_packed_bits(d.fmt), g = bayer_packed_group(bits);
+        if (d.src_w < 3 || d.src_h < 3)
+            return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s%dp at %dx%d (at least 3x3 required)", name, bits, d.src_w, d.src_h);
+        if (d.src_w % g)
+            return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s%dp at %dx%d (the width must be a multiple of %d: whole %d-byte groups)", name,
+                        bits, d.src_w, d.src_h, g, bayer_packed_group_bytes(bits));
+        if ((long long)d.src_pitch < (long long)d.src_w * bits / 8)
+            return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface for %s%dp (pitch %d < %lld bytes of a packed row)", name, bits, d.src_pitch,
+                        (long long)d.src_w * bits / 8);
+    }
     const int bpp = d.fmt <= 1 ? d.src_bpp : (is_yuv422(d.fmt) || is_bayer16(d.fmt) ? 2 : 1);
-    if ((long long)d.src_pitch < (long long)d.src_w * bpp) return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface (need pitch >= width*channels and len >= pitch*height)");
+    if (!is_bayer_packed(d.fmt) && (long long)d.src_pitch < (long long)d.src_w * bpp)
+        return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface (need pitch >= width*channels and len >= pitch*height)");
     if (l420 >= 0 && d.src_pitch != d.src_w) return fail(KB200_ERR_INVALID_SOURCE, "%s frames must be tightly packed (pitch == width)", YUV420_UPPER[l420]);
     if (!(d.scale_x > 0.0f) || !(d.scale_y > 0.0f)) return fail(KB200_ERR_INVALID_ARGUMENT, "scale must be positive");
     return KB200_OK;
@@ -603,7 +646,8 @@ static void launch_generic(cudaStream_t s, dim3 grid, int sampling, const kb200_
 template <bool F16, bool PTRS>
 static void launch_generic_for(int ext, cudaStream_t s, dim3 grid, int sampling, const kb200_preprocess_desc& d, const PreFrames& fr, void* dst,
                                uint32_t f0) {
-    if (ext == SRC_BAYER16) launch_generic<F16, PTRS, SRC_BAYER16>(s, grid, sampling, d, fr, dst, f0);
+    if (ext == SRC_BAYER_PACKED) launch_generic<F16, PTRS, SRC_BAYER_PACKED>(s, grid, sampling, d, fr, dst, f0);
+    else if (ext == SRC_BAYER16) launch_generic<F16, PTRS, SRC_BAYER16>(s, grid, sampling, d, fr, dst, f0);
     else if (ext == SRC_BAYER) launch_generic<F16, PTRS, SRC_BAYER>(s, grid, sampling, d, fr, dst, f0);
     else if (ext == SRC_EXT_YUV) launch_generic<F16, PTRS, SRC_EXT_YUV>(s, grid, sampling, d, fr, dst, f0);
     else launch_generic<F16, PTRS, SRC_BASE>(s, grid, sampling, d, fr, dst, f0);
@@ -613,12 +657,13 @@ static void launch_generic_for(int ext, cudaStream_t s, dim3 grid, int sampling,
 static const char* const YUV420_IDENTITY_NAMES[4] = {"preprocess_nv12_identity_kernel", "preprocess_nv21_identity_kernel",
                                                      "preprocess_i420_identity_kernel", "preprocess_yv12_identity_kernel"};
 static const char* const YUV420_FAST_NAMES[4] = {"preprocess_nv12_kernel", "preprocess_nv21_kernel", "preprocess_i420_kernel", "preprocess_yv12_kernel"};
-// ... and of the Bayer identity kernels, by sample width (8-bit, 16-bit) and pattern
-static const char* const BAYER_IDENTITY_NAMES[2][4] = {
-    {"preprocess_bayer_rggb_identity_kernel", "preprocess_bayer_bggr_identity_kernel", "preprocess_bayer_grbg_identity_kernel",
-     "preprocess_bayer_gbrg_identity_kernel"},
-    {"preprocess_bayer16_rggb_identity_kernel", "preprocess_bayer16_bggr_identity_kernel", "preprocess_bayer16_grbg_identity_kernel",
-     "preprocess_bayer16_gbrg_identity_kernel"}};
+// ... and of the Bayer identity kernels, by sample type (8-bit, 16-bit, packed 10-, 12- and 14-bit) and pattern
+#define KB200_BAYER_IDENTITY_NAMES(s)                                                                                   \
+    {"preprocess_bayer" s "_rggb_identity_kernel", "preprocess_bayer" s "_bggr_identity_kernel", "preprocess_bayer" s "_grbg_identity_kernel", \
+     "preprocess_bayer" s "_gbrg_identity_kernel"}
+static const char* const BAYER_IDENTITY_NAMES[5][4] = {KB200_BAYER_IDENTITY_NAMES(""), KB200_BAYER_IDENTITY_NAMES("16"), KB200_BAYER_IDENTITY_NAMES("10p"),
+                                                       KB200_BAYER_IDENTITY_NAMES("12p"), KB200_BAYER_IDENTITY_NAMES("14p")};
+#undef KB200_BAYER_IDENTITY_NAMES
 
 template <bool F16>
 static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, const uint8_t* const* frames,
@@ -626,12 +671,14 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
     const int pixels = d.dst_w * d.dst_h;
     const bool bil = d.sampling == KB200_INTERP_BILINEAR, lanczos = d.sampling == KB200_INTERP_LANCZOS;
     const int l420 = yuv420_layout(d.fmt);
-    const bool bayer16 = is_bayer16(d.fmt), bayer = bayer16 || is_bayer(d.fmt);   // bayer: any Bayer mosaic
+    const bool bayer16 = is_bayer16(d.fmt), packed = is_bayer_packed(d.fmt);
+    const bool bayer = bayer16 || packed || is_bayer(d.fmt);   // bayer: any Bayer mosaic
     // identity fast path: a 4:2:0 or Bayer format, scale 1, no pad, same size, 8-column vectors possible
     // (Lanczos always takes the generic kernel: its off-centre weights at integer coordinates are sinf(k*pi) != 0 exactly).
     // A thread loads 4 samples per row, so rows and frames are aligned to that load: 4 B for 4:2:0 and 8-bit Bayer, 8 B
-    // for 16-bit Bayer.
-    const uint32_t row_align = bayer16 ? BayerSample<uint16_t>::ID_ALIGN : BayerSample<uint8_t>::ID_ALIGN;
+    // for 16-bit Bayer, 16 B for packed Bayer.
+    const uint32_t row_align = packed ? BayerSample<BayerPacked<12>>::ID_ALIGN
+                                      : bayer16 ? BayerSample<uint16_t>::ID_ALIGN : BayerSample<uint8_t>::ID_ALIGN;
     bool identity = !lanczos && (l420 >= 0 || bayer) && d.scale_x == 1.0f && d.scale_y == 1.0f && d.pad_x == 0.0f && d.pad_y == 0.0f &&
                     d.dst_w == d.src_w && d.dst_h == d.src_h && (d.src_w % 4) == 0 && (d.src_pitch % row_align) == 0 && aligned16(dst);
     if (identity) {
@@ -643,7 +690,7 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
     if (id_items > 0x7FFFFFFFull) identity = false;
     // 4:2:0 general fast path: vector stores need dst_w % 4 == 0 and a 16-B (f32) / 8-B (f16) aligned destination
     const bool yuv420_fast = !lanczos && l420 >= 0 && (d.dst_w % 4) == 0 && aligned16(dst) && d.dst_h <= 65535 * NV12_ROWS;
-    const int ext = bayer16 ? SRC_BAYER16 : bayer ? SRC_BAYER : d.fmt >= KB200_FMT_NV21 ? SRC_EXT_YUV : SRC_BASE;
+    const int ext = bayer16 ? SRC_BAYER16 : packed ? SRC_BAYER_PACKED : bayer ? SRC_BAYER : d.fmt >= KB200_FMT_NV21 ? SRC_EXT_YUV : SRC_BASE;
     Nv12Args nv{};
     nv.groups = (uint32_t)(d.dst_w + 3) / 4u;
     for (int c = 0; c < 3; ++c) nv.pad_norm[c] = (d.pad_value / 255.0f - d.mean[c]) * d.inv_std[c];  // BODY :610-612 on the host (f32, unfused)
@@ -654,7 +701,7 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
         if (frames) for (uint32_t k = 0; k < nb; ++k) fr.ptr[k] = frames[f0 + k];
         const bool p = frames != nullptr;
         if (identity && bayer) {
-            const int pattern = bayer_pattern(d.fmt, bayer16);
+            const int pattern = packed ? bayer_packed_pattern(d.fmt) : bayer_pattern(d.fmt, bayer16);
             auto launch = [&](auto sample) {   // the kernel of pattern `pattern` for samples of the type of `sample`
                 using T = decltype(sample);
                 switch (pattern) {
@@ -664,9 +711,13 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
                     default: launch_bayer_identity<F16, T, KB200_BAYER_GBRG>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
                 }
             };
-            if (bayer16) launch(uint16_t{});
+            const int bits = packed ? bayer_packed_bits(d.fmt) : 0;
+            if (bits == 10) launch(BayerPacked<10>{});
+            else if (bits == 12) launch(BayerPacked<12>{});
+            else if (bits == 14) launch(BayerPacked<14>{});
+            else if (bayer16) launch(uint16_t{});
             else launch(uint8_t{});
-            KB200_TRY(check_launch(BAYER_IDENTITY_NAMES[bayer16][pattern]));
+            KB200_TRY(check_launch(BAYER_IDENTITY_NAMES[packed ? 2 + (bits - 10) / 2 : bayer16][pattern]));
             continue;
         }
         if (identity || yuv420_fast) {

@@ -534,10 +534,11 @@ YUV422_YUYV, YUV422_UYVY, YUV422_YVYU = 0, 1, 2                   # kb200_yuv422
 
 
 def _rgb_from_yuv(src, dst: Image, what: str, bytes_num: int, bytes_den: int, fn_name: str, *layout,
-                  dtype: torch.dtype = torch.uint8) -> None:
-    """The video and Bayer decoders: `src` holds N tight frames of w*h*bytes_num/bytes_den samples of `dtype`, the dtype
-    of `dst` too; `layout` is the extra argument of the layout-generic entry points (none for the NV12 / YUYV ones)."""
-    t = _raw_frames(src, what, dtype)
+                  dtype: torch.dtype = torch.uint8, src_dtype: torch.dtype | None = None) -> None:
+    """The video and Bayer decoders: `src` holds N tight frames of w*h*bytes_num/bytes_den samples of `src_dtype`
+    (default: `dtype`, the dtype of `dst`); `layout` is the extra arguments of the layout-generic entry points (none for
+    the NV12 / YUYV ones)."""
+    t = _raw_frames(src, what, dtype if src_dtype is None else src_dtype)
     if not dst.is_device:
         raise ImageError.MixedResidency()
     if t.device != dst.device:
@@ -609,6 +610,20 @@ def rgb_from_bayer16(src, dst: Image, pattern: BayerPattern) -> None:
     samples, each an LSB-aligned little-endian word (V4L2's unpacked SRGGB10 ... SGBRG16); `dst`: a uint16 Image
     [N, h, w, 3].  The bit depth plays no part: the output is the same whatever it is."""
     _rgb_from_yuv(src, dst, "rgb_from_bayer16", 1, 1, "kb200_rgb_from_bayer_u16", int(BayerPattern(pattern)), dtype=torch.uint16)
+
+
+_PACKED_BYTES = {10: (5, 4), 12: (3, 2), 14: (7, 4)}   # bytes per pixel of a MIPI-packed sample, as a fraction
+
+
+def rgb_from_bayer_packed(src, dst: Image, pattern: BayerPattern, bits: int) -> None:
+    """MIPI CSI-2 packed 10-, 12- or 14-bit Bayer mosaic (V4L2's SRGGB10P ... SGBRG14P) -> RGB with 16-bit channels: the
+    same bits as rgb_from_bayer16 on the unpacked samples, read straight from the packed bytes.  `src`: uint8 device
+    tensor holding N tight frames of h rows of w*bits/8 bytes (w a whole number of groups: w % 4 == 0 for 10 and 14
+    bits, w % 2 == 0 for 12); `dst`: a uint16 Image [N, h, w, 3]."""
+    if bits not in _PACKED_BYTES:
+        raise ValueError(f"packed Bayer samples are 10, 12 or 14 bits, got {bits}")
+    _rgb_from_yuv(src, dst, "rgb_from_bayer_packed", *_PACKED_BYTES[bits], "kb200_rgb_from_bayer_packed", int(BayerPattern(pattern)), bits,
+                  dtype=torch.uint16, src_dtype=torch.uint8)
 
 
 def _encode(op: str, fn_name: str, src: Image, dst: torch.Tensor, bytes_per_px_num: int, bytes_per_px_den: int, need_even_h: bool) -> None:

@@ -2,7 +2,7 @@
 
 Built once via `Preprocessor.builder()…build_cuda()`, then applied to any number of frames of any
 resolution: the target H/W is read from the destination tensor each call.  Camera formats
-(NV12 / YUYV / Gray, the other YUV layouts and the 8- to 16-bit Bayer mosaics) go through `run_raw*`; colour decode is fused into the resample taps.  Unlike the
+(NV12 / YUYV / Gray, the other YUV layouts and the 8- to 16-bit Bayer mosaics, unpacked or MIPI-packed) go through `run_raw*`; colour decode is fused into the resample taps.  Unlike the
 reference (one launch per frame, preprocess.rs:1277-1280) a batch is ONE launch.
 
 Only the CUDA preprocessor exists here (`build()` = the reference's CPU preprocessor is out of scope:
@@ -81,22 +81,45 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
     BayerBggr16 = "bayer_bggr16"
     BayerGrbg16 = "bayer_grbg16"
     BayerGbrg16 = "bayer_gbrg16"
+    # The 10-, 12- and 14-bit mosaics MIPI CSI-2 packed (V4L2's SRGGB10P ... SGBRG14P): each row packed on its own in
+    # w*bits/8 bytes, groups of 4 samples in 5 bytes (RAW10), 2 in 3 (RAW12) or 4 in 7 (RAW14), the first bytes of a
+    # group holding the high 8 bits of each sample.  A tap is exactly the tap of the unpacked format of the same depth.
+    BayerRggb10p = "bayer_rggb10p"
+    BayerBggr10p = "bayer_bggr10p"
+    BayerGrbg10p = "bayer_grbg10p"
+    BayerGbrg10p = "bayer_gbrg10p"
+    BayerRggb12p = "bayer_rggb12p"
+    BayerBggr12p = "bayer_bggr12p"
+    BayerGrbg12p = "bayer_grbg12p"
+    BayerGbrg12p = "bayer_gbrg12p"
+    BayerRggb14p = "bayer_rggb14p"
+    BayerBggr14p = "bayer_bggr14p"
+    BayerGrbg14p = "bayer_grbg14p"
+    BayerGbrg14p = "bayer_gbrg14p"
 
     def fmt_code(self) -> int:  # :153-161
         if self.is_bayer16():   # 32 + 4*k + pattern, k = 0..3 for 10, 12, 14, 16 bits
             return 32 + 4 * ((self.bit_depth() - 10) // 2) + _BAYER_PATTERNS.index(self.value[6:10])
+        if self.is_bayer_packed():   # 64 + 4*k + pattern, k = 0..2 for 10, 12, 14 bits
+            return 64 + 4 * ((self.bit_depth() - 10) // 2) + _BAYER_PATTERNS.index(self.value[6:10])
         return {"rgb8": 0, "rgba8": 0, "bgr8": 1, "bgra8": 1, "gray8": 2, "nv12": 3, "yuyv": 4,
                 "nv21": 5, "i420": 6, "yv12": 7, "uyvy": 8, "yvyu": 9,
                 "bayer_rggb": 16, "bayer_bggr": 17, "bayer_grbg": 18, "bayer_gbrg": 19}[self.value]
 
     def bpp(self) -> int:  # :164-171
+        """Bytes per sample; 1 for the packed Bayer formats, whose rows pitch() counts."""
         if self.is_bayer16():
             return 2
+        if self.is_bayer_packed():
+            return 1
         return {"rgb8": 3, "bgr8": 3, "rgba8": 4, "bgra8": 4, "gray8": 1, "nv12": 1, "yuyv": 2,
                 "nv21": 1, "i420": 1, "yv12": 1, "uyvy": 2, "yvyu": 2,
                 "bayer_rggb": 1, "bayer_bggr": 1, "bayer_grbg": 1, "bayer_gbrg": 1}[self.value]
 
     def pitch(self, w: int) -> int:
+        """Bytes of a tight row of w pixels."""
+        if self.is_bayer_packed():
+            return w * self.bit_depth() // 8
         return w * self.bpp()
 
     def is_yuv420(self) -> bool:
@@ -110,12 +133,18 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
 
     def is_bayer16(self) -> bool:
         """A Bayer format of 16-bit samples (10 to 16 bits per pixel)."""
-        return self.is_bayer() and len(self.value) > 10
+        return self.is_bayer() and len(self.value) > 10 and not self.is_bayer_packed()
+
+    def is_bayer_packed(self) -> bool:
+        """A MIPI-packed Bayer format (10, 12 or 14 bits per pixel)."""
+        return self.is_bayer() and self.value.endswith("p")
 
     def bit_depth(self) -> int | None:
         """Bits per sample of a Bayer format (8 for the byte mosaics), None for the other formats."""
         if not self.is_bayer():
             return None
+        if self.is_bayer_packed():
+            return int(self.value[10:-1])
         return int(self.value[10:]) if self.is_bayer16() else 8
 
     def buffer_len(self, w: int, h: int) -> int:  # :177-186
@@ -127,6 +156,8 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
             return w % 2 == 0 and h % 2 == 0
         if self.is_yuv422():
             return w % 2 == 0
+        if self.is_bayer_packed():   # whole packed groups: 2 samples at 12 bits, 4 at 10 and 14
+            return w >= 3 and h >= 3 and w % (2 if self.bit_depth() == 12 else 4) == 0
         if self.is_bayer():
             return w >= 3 and h >= 3
         return True
@@ -141,6 +172,7 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
                  "nv21": "Nv21", "i420": "I420", "yv12": "Yv12", "uyvy": "Uyvy", "yvyu": "Yvyu",
                  "bayer_rggb": "BayerRggb", "bayer_bggr": "BayerBggr", "bayer_grbg": "BayerGrbg", "bayer_gbrg": "BayerGbrg"}
         table.update({f"bayer_{p}{b}": f"Bayer{p.capitalize()}{b}" for p in _BAYER_PATTERNS for b in (10, 12, 14, 16)})
+        table.update({f"bayer_{p}{b}p": f"Bayer{p.capitalize()}{b}p" for p in _BAYER_PATTERNS for b in (10, 12, 14)})
         key = table.get(name.lower())
         return None if key is None else SourceFormat[key]
 
