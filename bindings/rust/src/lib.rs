@@ -136,6 +136,8 @@ pub mod ffi {
         pub fn kb200_rgb_from_yuyv_u8(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, width: u32, height: u32, batch: u32) -> c_int;
         pub fn kb200_rgb_from_yuv420_u8(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, width: u32, height: u32, batch: u32, layout: c_int) -> c_int;
         pub fn kb200_rgb_from_yuv422_u8(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, width: u32, height: u32, batch: u32, layout: c_int) -> c_int;
+        pub fn kb200_rgb_from_yuv420_u8_matrix(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, width: u32, height: u32, batch: u32, layout: c_int, matrix: c_int) -> c_int;
+        pub fn kb200_rgb_from_yuv422_u8_matrix(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, width: u32, height: u32, batch: u32, layout: c_int, matrix: c_int) -> c_int;
         pub fn kb200_rgb_from_bayer_u8(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, width: u32, height: u32, batch: u32, pattern: c_int) -> c_int;
         pub fn kb200_rgb_from_bayer_u16(stream: *mut c_void, src: *const u16, src_len: usize, dst: *mut u16, dst_len: usize, width: u32, height: u32, batch: u32, pattern: c_int) -> c_int;
         pub fn kb200_rgb_from_bayer_packed(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u16, dst_len: usize, width: u32, height: u32, batch: u32, pattern: c_int, bits: c_int) -> c_int;
@@ -266,6 +268,19 @@ pub const YUV422_YUYV: c_int = 0;
 pub const YUV422_UYVY: c_int = 1;
 pub const YUV422_YVYU: c_int = 2;
 
+/// `matrix` of `kb200_rgb_from_yuv420_u8_matrix` / `_yuv422_u8_matrix` (kb200_yuv_matrix): the colour matrix and range a
+/// YUV frame decodes with.  BT.601 limited is the reference's decode.
+pub const YUV_BT601_LIMITED: c_int = 0;
+pub const YUV_BT601_FULL: c_int = 1;
+pub const YUV_BT709_LIMITED: c_int = 2;
+pub const YUV_BT709_FULL: c_int = 3;
+
+/// `KB200_FMT_YUV_MATRIX(m)`: OR it into a YUV format's `fmt` code of `kb200_preprocess_desc` to decode its frames with
+/// matrix `m`.  Any other format with a matrix is rejected.
+pub const fn fmt_yuv_matrix(matrix: c_int) -> i32 {
+    matrix << 8
+}
+
 /// `PixelMapping` of cuda/resize.rs:441.
 #[derive(Debug, Clone, Copy, PartialEq, Eq)]
 pub enum PixelMapping {
@@ -332,6 +347,38 @@ pub fn launch_separable_filter_f32(
     check(unsafe {
         ffi::kb200_separable_filter_f32(stream.cu_stream() as *mut c_void, sp as *const f32, src_len, dp as *mut f32, dst_len,
                                         std::ptr::null_mut(), kx.as_ptr(), kx.len() as u32, ky.as_ptr(), ky.len() as u32, cols, rows, channels, 1)
+    })
+}
+
+/// Replaces `launch_rgb_from_planar420` (cuda/color/video.rs:328) with a choice of colour matrix: `batch` tight 4:2:0
+/// frames of `layout` (`YUV420_*`) -> RGB8 HWC, decoded with `matrix` (`YUV_*`).
+#[allow(clippy::too_many_arguments)]
+pub fn launch_rgb_from_yuv420_matrix(
+    stream: &Arc<CudaStream>, src: &CudaSlice<u8>, dst: &mut CudaSlice<u8>, width: u32, height: u32, batch: u32, layout: c_int, matrix: c_int,
+) -> Result<(), Kb200Error> {
+    bind(stream.context())?;
+    let (sp, _g0) = src.device_ptr(stream);
+    let (src_len, dst_len) = (src.len(), dst.len());
+    let (dp, _g1) = dst.device_ptr_mut(stream);
+    check(unsafe {
+        ffi::kb200_rgb_from_yuv420_u8_matrix(stream.cu_stream() as *mut c_void, sp as *const u8, src_len, dp as *mut u8, dst_len, width, height,
+                                             batch, layout, matrix)
+    })
+}
+
+/// Replaces `launch_rgb_from_packed422` (cuda/color/video.rs:297) with a choice of colour matrix: `batch` tight 4:2:2
+/// frames of `layout` (`YUV422_*`) -> RGB8 HWC, decoded with `matrix` (`YUV_*`).
+#[allow(clippy::too_many_arguments)]
+pub fn launch_rgb_from_yuv422_matrix(
+    stream: &Arc<CudaStream>, src: &CudaSlice<u8>, dst: &mut CudaSlice<u8>, width: u32, height: u32, batch: u32, layout: c_int, matrix: c_int,
+) -> Result<(), Kb200Error> {
+    bind(stream.context())?;
+    let (sp, _g0) = src.device_ptr(stream);
+    let (src_len, dst_len) = (src.len(), dst.len());
+    let (dp, _g1) = dst.device_ptr_mut(stream);
+    check(unsafe {
+        ffi::kb200_rgb_from_yuv422_u8_matrix(stream.cu_stream() as *mut c_void, sp as *const u8, src_len, dp as *mut u8, dst_len, width, height,
+                                             batch, layout, matrix)
     })
 }
 

@@ -18,6 +18,7 @@ _lib.lib()  # fail loudly at import when libkornia_b200.so is absent
 
 from . import dist, fusion, imgproc  # noqa: E402
 from .image import Image, ImageError, ImageSize, InterpolationMode  # noqa: E402
+from .imgproc import YuvMatrix  # noqa: E402
 from .preprocess import (  # noqa: E402
     IMAGENET_MEAN,
     IMAGENET_STD,
@@ -49,6 +50,6 @@ def device_info() -> dict:
 
 __all__ = [
     "Image", "ImageError", "ImageSize", "InterpolationMode", "imgproc", "dist", "fusion", "Preprocessor", "PreprocessorBuilder",
-    "PreprocessError", "ResizeMode", "Normalize", "SourceFormat", "PitchedSurface", "IMAGENET_MEAN", "IMAGENET_STD",
+    "PreprocessError", "ResizeMode", "Normalize", "SourceFormat", "YuvMatrix", "PitchedSurface", "IMAGENET_MEAN", "IMAGENET_STD",
     "native_version", "device_info",
 ]

@@ -97,6 +97,8 @@ def _declare(l: C.CDLL) -> None:
         "kb200_rgb_from_yuyv_u8": ([vp, vp, sz, vp, sz, u32, u32, u32], i),
         "kb200_rgb_from_yuv420_u8": ([vp, vp, sz, vp, sz, u32, u32, u32, i], i),
         "kb200_rgb_from_yuv422_u8": ([vp, vp, sz, vp, sz, u32, u32, u32, i], i),
+        "kb200_rgb_from_yuv420_u8_matrix": ([vp, vp, sz, vp, sz, u32, u32, u32, i, i], i),
+        "kb200_rgb_from_yuv422_u8_matrix": ([vp, vp, sz, vp, sz, u32, u32, u32, i, i], i),
         "kb200_rgb_from_bayer_u8": ([vp, vp, sz, vp, sz, u32, u32, u32, i], i),
         "kb200_rgb_from_bayer_u16": ([vp, vp, sz, vp, sz, u32, u32, u32, i], i),
         "kb200_rgb_from_bayer_packed": ([vp, vp, sz, vp, sz, u32, u32, u32, i, i], i),

@@ -1,5 +1,5 @@
-// color.cu — gray_from_rgb (f32, u8), the BT.601-limited Q20 video decoders (4:2:0: NV12, NV21, I420, YV12;
-// 4:2:2: YUYV, UYVY, YVYU) and the bilinear Bayer demosaic (RGGB, BGGR, GRBG, GBRG; bayer.cuh).
+// color.cu — gray_from_rgb (f32, u8), the Q20 video decoders (4:2:0: NV12, NV21, I420, YV12; 4:2:2: YUYV, UYVY, YVYU;
+// BT.601 or BT.709, limited or full range: kb200_yuv_matrix) and the bilinear Bayer demosaic (RGGB, BGGR, GRBG, GBRG; bayer.cuh).
 //
 // Reference: color/gray/kernels.rs (CPU), cuda/color/gray.rs:17-68 (GPU twin, 1 px or 4 px per
 // thread, scalar 4-byte accesses); color/yuv/kernels.rs:707-1069 (CPU), cuda/color/video.rs:33-130
@@ -100,14 +100,14 @@ __device__ __forceinline__ uint32_t pack_sat2(int hi, int lo, uint32_t upper) {
 // four saturated bytes, b0 in the low byte
 __device__ __forceinline__ uint32_t pack_sat4(int b0, int b1, int b2, int b3) { return pack_sat2(b1, b0, pack_sat2(b3, b2, 0u)); }
 
-__device__ __forceinline__ void pack_rgb16(const uint32_t yw[4], const ChromaTerms ct[8], uint4 out[3]) {
+__device__ __forceinline__ void pack_rgb16(const uint32_t yw[4], const ChromaTerms ct[8], const YuvCoeffs& yc, uint4 out[3]) {
     uint32_t w[12];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {  // 4 px -> 12 bytes = 3 words: r0 g0 b0 r1 | g1 b1 r2 g2 | b2 r3 g3 b3
         int r[4], g[4], b[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-            const int yy = yy_term((int)((yw[k] >> (8 * j)) & 0xFFu));
+            const int yy = yy_term((int)((yw[k] >> (8 * j)) & 0xFFu), yc);
             const ChromaTerms& t = ct[2 * k + (j >> 1)];
             b[j] = (yy + t.b) >> 20; g[j] = (yy + t.g) >> 20; r[j] = (yy + t.r) >> 20;   // saturated by the pack below
         }
@@ -137,7 +137,7 @@ __device__ __forceinline__ void store_rgb48_coalesced(uint4* __restrict__ warp_d
 // width % 16 == 0 both planes and every thread's offset in them are 8-B aligned).
 template <int L>
 __global__ void __launch_bounds__(128) rgb_from_yuv420_vec16(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst,
-                                                             uint32_t width, uint32_t height, size_t frame_bytes) {
+                                                             uint32_t width, uint32_t height, size_t frame_bytes, const YuvCoeffs yc) {
     __shared__ uint4 stage[4][96];
     const uint32_t gx = blockIdx.x * blockDim.x + threadIdx.x;  // 16-column group
     const uint32_t cy = blockIdx.y;                             // chroma row
@@ -167,11 +167,11 @@ __global__ void __launch_bounds__(128) rgb_from_yuv420_vec16(const uint8_t* __re
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
         if (yuv420_planar(L)) {
-            ct[k] = chroma_terms((int)((uvw[k >> 2] >> (8 * (k & 3))) & 0xFFu), (int)((uvw[2 + (k >> 2)] >> (8 * (k & 3))) & 0xFFu));
+            ct[k] = chroma_terms((int)((uvw[k >> 2] >> (8 * (k & 3))) & 0xFFu), (int)((uvw[2 + (k >> 2)] >> (8 * (k & 3))) & 0xFFu), yc);
         } else {
             const uint32_t pair = (uvw[k >> 1] >> (16 * (k & 1))) & 0xFFFFu;
-            if (L == YUV420_NV21) ct[k] = chroma_terms((int)(pair >> 8), (int)(pair & 0xFFu));
-            else ct[k] = chroma_terms((int)(pair & 0xFFu), (int)(pair >> 8));
+            if (L == YUV420_NV21) ct[k] = chroma_terms((int)(pair >> 8), (int)(pair & 0xFFu), yc);
+            else ct[k] = chroma_terms((int)(pair & 0xFFu), (int)(pair >> 8), yc);
         }
     }
     uint4 o[3];
@@ -180,14 +180,14 @@ __global__ void __launch_bounds__(128) rgb_from_yuv420_vec16(const uint8_t* __re
     uint4* d0 = reinterpret_cast<uint4*>(out + ((size_t)(2 * cy) * width + (size_t)gx0 * 16) * 3);       // this warp's 1536-B run, top row
     uint4* d1 = reinterpret_cast<uint4*>(out + ((size_t)(2 * cy + 1) * width + (size_t)gx0 * 16) * 3);   // bottom row
     if (full_warp) {
-        pack_rgb16(ytw, ct, o);
+        pack_rgb16(ytw, ct, yc, o);
         store_rgb48_coalesced(d0, stage[wid], lane, o);
-        pack_rgb16(ybw, ct, o);
+        pack_rgb16(ybw, ct, yc, o);
         store_rgb48_coalesced(d1, stage[wid], lane, o);
     } else if (active) {   // ragged last warp of a row: direct 48-B stores
-        pack_rgb16(ytw, ct, o);
+        pack_rgb16(ytw, ct, yc, o);
         stg_stream_u4(d0 + 3 * lane, o[0]); stg_stream_u4(d0 + 3 * lane + 1, o[1]); stg_stream_u4(d0 + 3 * lane + 2, o[2]);
-        pack_rgb16(ybw, ct, o);
+        pack_rgb16(ybw, ct, yc, o);
         stg_stream_u4(d1 + 3 * lane, o[0]); stg_stream_u4(d1 + 3 * lane + 1, o[1]); stg_stream_u4(d1 + 3 * lane + 2, o[2]);
     }
 }
@@ -195,7 +195,7 @@ __global__ void __launch_bounds__(128) rgb_from_yuv420_vec16(const uint8_t* __re
 // Generic fallback (any even width / unaligned buffers): one thread per 2x2 block.
 template <int L>
 __global__ void rgb_from_yuv420_generic(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, uint32_t width,
-                                        uint32_t height, size_t frame_bytes) {
+                                        uint32_t height, size_t frame_bytes, const YuvCoeffs yc) {
     const uint32_t cx = blockIdx.x * blockDim.x + threadIdx.x, cy = blockIdx.y * blockDim.y + threadIdx.y;
     if (cx >= width / 2 || cy >= height / 2) return;
     const uint8_t* frame = src + (size_t)blockIdx.z * frame_bytes;
@@ -203,10 +203,10 @@ __global__ void rgb_from_yuv420_generic(const uint8_t* __restrict__ src, uint8_t
     ChromaTerms ct;
     if (yuv420_planar(L)) {
         const size_t c = (size_t)cy * (width / 2) + cx;
-        ct = chroma_terms(frame[yuv420_u_plane(L, width, height) + c], frame[yuv420_v_plane(L, width, height) + c]);
+        ct = chroma_terms(frame[yuv420_u_plane(L, width, height) + c], frame[yuv420_v_plane(L, width, height) + c], yc);
     } else {
         const uint8_t* uvp = frame + (size_t)width * height + (size_t)cy * width + 2 * cx;
-        ct = L == YUV420_NV21 ? chroma_terms(uvp[1], uvp[0]) : chroma_terms(uvp[0], uvp[1]);
+        ct = L == YUV420_NV21 ? chroma_terms(uvp[1], uvp[0], yc) : chroma_terms(uvp[0], uvp[1], yc);
     }
 #pragma unroll
     for (int dy = 0; dy < 2; ++dy)
@@ -214,7 +214,7 @@ __global__ void rgb_from_yuv420_generic(const uint8_t* __restrict__ src, uint8_t
         for (int dx = 0; dx < 2; ++dx) {
             const size_t p = (size_t)(2 * cy + dy) * width + 2 * cx + dx;
             int r, g, b;
-            decode_rgb(yy_term(frame[p]), ct, r, g, b);
+            decode_rgb(yy_term(frame[p], yc), ct, r, g, b);
             out[3 * p] = (uint8_t)r; out[3 * p + 1] = (uint8_t)g; out[3 * p + 2] = (uint8_t)b;
         }
 }
@@ -230,7 +230,7 @@ template <> struct Yuv422Bytes<YUV422_UYVY> { static constexpr int y0 = 1, y1 = 
 template <> struct Yuv422Bytes<YUV422_YVYU> { static constexpr int y0 = 0, y1 = 2, u = 3, v = 1; };
 
 template <int L>
-__device__ __forceinline__ void yuv422_decode16(const uint4& A, const uint4& B, uint4 o[3]) {
+__device__ __forceinline__ void yuv422_decode16(const uint4& A, const uint4& B, const YuvCoeffs& yc, uint4 o[3]) {
     using P = Yuv422Bytes<L>;
     const uint32_t g4[8] = {A.x, A.y, A.z, A.w, B.x, B.y, B.z, B.w};  // each word: one 2-px group
     uint32_t yw[4];
@@ -238,11 +238,11 @@ __device__ __forceinline__ void yuv422_decode16(const uint4& A, const uint4& B, 
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
         const uint32_t w = g4[k];
-        ct[k] = chroma_terms((int)((w >> (8 * P::u)) & 0xFFu), (int)((w >> (8 * P::v)) & 0xFFu));
+        ct[k] = chroma_terms((int)((w >> (8 * P::u)) & 0xFFu), (int)((w >> (8 * P::v)) & 0xFFu), yc);
         const uint32_t ypair = __byte_perm(w, 0, 0x4400 | (P::y1 << 4) | P::y0);   // {Y0, Y1, 0, 0}
         if (k & 1) yw[k >> 1] |= ypair << 16; else yw[k >> 1] = ypair;
     }
-    pack_rgb16(yw, ct, o);
+    pack_rgb16(yw, ct, yc, o);
 }
 
 // A warp owns 32 consecutive 16-px groups = 1024 B in, 1536 B out, both contiguous: the loads are issued
@@ -250,7 +250,7 @@ __device__ __forceinline__ void yuv422_decode16(const uint4& A, const uint4& B, 
 // stores go back through it (store_rgb48_coalesced) — every global access instruction covers whole 128-B lines.
 template <int L>
 __global__ void __launch_bounds__(256) rgb_from_yuv422_vec16(const uint4* __restrict__ src, uint4* __restrict__ dst,
-                                                             size_t ngroups) {
+                                                             size_t ngroups, const YuvCoeffs yc) {
     __shared__ uint4 stage[8][96];
     const uint32_t lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
     const size_t stride = (size_t)gridDim.x * blockDim.x;
@@ -263,11 +263,11 @@ __global__ void __launch_bounds__(256) rgb_from_yuv422_vec16(const uint4* __rest
             __syncwarp();
             const uint4 A = st[2 * lane], B = st[2 * lane + 1];
             __syncwarp();
-            yuv422_decode16<L>(A, B, o);
+            yuv422_decode16<L>(A, B, yc, o);
             store_rgb48_coalesced(dst + 3 * q0, st, lane, o);
         } else if (q0 + lane < ngroups) {   // ragged tail warp
             const size_t q = q0 + lane;
-            yuv422_decode16<L>(ldg_stream_u4(src + 2 * q), ldg_stream_u4(src + 2 * q + 1), o);
+            yuv422_decode16<L>(ldg_stream_u4(src + 2 * q), ldg_stream_u4(src + 2 * q + 1), yc, o);
             stg_stream_u4(dst + 3 * q, o[0]); stg_stream_u4(dst + 3 * q + 1, o[1]); stg_stream_u4(dst + 3 * q + 2, o[2]);
         }
     }
@@ -275,16 +275,16 @@ __global__ void __launch_bounds__(256) rgb_from_yuv422_vec16(const uint4* __rest
 
 template <int L>
 __global__ void rgb_from_yuv422_generic(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, size_t first_group,
-                                        size_t ngroups) {
+                                        size_t ngroups, const YuvCoeffs yc) {
     using P = Yuv422Bytes<L>;
     const size_t g = first_group + (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= ngroups) return;
     const uint8_t* s = src + 4 * g;
-    const ChromaTerms ct = chroma_terms(s[P::u], s[P::v]);
+    const ChromaTerms ct = chroma_terms(s[P::u], s[P::v], yc);
     int r, gg, b;
-    decode_rgb(yy_term(s[P::y0]), ct, r, gg, b);
+    decode_rgb(yy_term(s[P::y0], yc), ct, r, gg, b);
     dst[6 * g] = (uint8_t)r; dst[6 * g + 1] = (uint8_t)gg; dst[6 * g + 2] = (uint8_t)b;
-    decode_rgb(yy_term(s[P::y1]), ct, r, gg, b);
+    decode_rgb(yy_term(s[P::y1], yc), ct, r, gg, b);
     dst[6 * g + 3] = (uint8_t)r; dst[6 * g + 4] = (uint8_t)gg; dst[6 * g + 5] = (uint8_t)b;
 }
 
@@ -413,8 +413,8 @@ static inline unsigned stream_grid(size_t items, unsigned block, unsigned ctas_p
 // kb200_last_kernel().
 struct Yuv420Kernels {
     const char* layout;
-    void (*vec16)(const uint8_t*, uint8_t*, uint32_t, uint32_t, size_t);
-    void (*generic)(const uint8_t*, uint8_t*, uint32_t, uint32_t, size_t);
+    void (*vec16)(const uint8_t*, uint8_t*, uint32_t, uint32_t, size_t, YuvCoeffs);
+    void (*generic)(const uint8_t*, uint8_t*, uint32_t, uint32_t, size_t, YuvCoeffs);
     const char *vec16_name, *generic_name;
 };
 static const Yuv420Kernels YUV420_KERNELS[4] = {
@@ -425,8 +425,8 @@ static const Yuv420Kernels YUV420_KERNELS[4] = {
 };
 struct Yuv422Kernels {
     const char* layout;
-    void (*vec16)(const uint4*, uint4*, size_t);
-    void (*generic)(const uint8_t*, uint8_t*, size_t, size_t);
+    void (*vec16)(const uint4*, uint4*, size_t, YuvCoeffs);
+    void (*generic)(const uint8_t*, uint8_t*, size_t, size_t, YuvCoeffs);
     const char *vec16_name, *generic_name;
 };
 static const Yuv422Kernels YUV422_KERNELS[3] = {
@@ -623,10 +623,12 @@ KB200_API int kb200_gray_from_rgb_u8(kb200_stream_t stream, const uint8_t* src, 
     return KB200_OK;
 }
 
-KB200_API int kb200_rgb_from_yuv420_u8(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst,
-                                       size_t dst_len, uint32_t width, uint32_t height, uint32_t batch, int layout) {
+KB200_API int kb200_rgb_from_yuv420_u8_matrix(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst,
+                                              size_t dst_len, uint32_t width, uint32_t height, uint32_t batch, int layout, int matrix) {
     KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
     if (layout < KB200_YUV420_NV12 || layout > KB200_YUV420_YV12) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown 4:2:0 layout %d", layout);
+    if (matrix < KB200_YUV_BT601_LIMITED || matrix > KB200_YUV_BT709_FULL) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown YUV matrix %d", matrix);
+    const YuvCoeffs& yc = YUV_COEFFS[matrix];
     const Yuv420Kernels& k = YUV420_KERNELS[layout];
     KB200_TRY(check_geometry(width, height, width, height, batch));
     if ((width & 1u) || (height & 1u)) return fail(KB200_ERR_INVALID_ARGUMENT, "%s needs even dimensions, got %ux%u", k.layout, width, height);
@@ -638,18 +640,20 @@ KB200_API int kb200_rgb_from_yuv420_u8(kb200_stream_t stream, const uint8_t* src
         const unsigned groups = width / 16;
         const unsigned bx = groups >= 128 ? 128 : 32 * ((groups + 31) / 32);
         dim3 grid(div_up(groups, bx), height / 2, batch);
-        k.vec16<<<grid, bx, 0, s>>>(src, dst, width, height, frame);
+        k.vec16<<<grid, bx, 0, s>>>(src, dst, width, height, frame, yc);
         return check_launch(k.vec16_name);
     }
     dim3 block(32, 8), grid(div_up(width / 2, 32), div_up(height / 2, 8), batch);
-    k.generic<<<grid, block, 0, s>>>(src, dst, width, height, frame);
+    k.generic<<<grid, block, 0, s>>>(src, dst, width, height, frame, yc);
     return check_launch(k.generic_name);
 }
 
-KB200_API int kb200_rgb_from_yuv422_u8(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst,
-                                       size_t dst_len, uint32_t width, uint32_t height, uint32_t batch, int layout) {
+KB200_API int kb200_rgb_from_yuv422_u8_matrix(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst,
+                                              size_t dst_len, uint32_t width, uint32_t height, uint32_t batch, int layout, int matrix) {
     KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
     if (layout < KB200_YUV422_YUYV || layout > KB200_YUV422_YVYU) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown 4:2:2 layout %d", layout);
+    if (matrix < KB200_YUV_BT601_LIMITED || matrix > KB200_YUV_BT709_FULL) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown YUV matrix %d", matrix);
+    const YuvCoeffs& yc = YUV_COEFFS[matrix];
     const Yuv422Kernels& k = YUV422_KERNELS[layout];
     KB200_TRY(check_geometry(width, height, width, height, batch));
     if (width & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "%s needs an even width, got %u", k.layout, width);
@@ -661,16 +665,26 @@ KB200_API int kb200_rgb_from_yuv422_u8(kb200_stream_t stream, const uint8_t* src
     if (aligned16(src) && aligned16(dst)) {
         const size_t n16 = npx / 16;
         if (n16) {
-            k.vec16<<<stream_grid(n16, 256, 8), 256, 0, s>>>(reinterpret_cast<const uint4*>(src), reinterpret_cast<uint4*>(dst), n16);
+            k.vec16<<<stream_grid(n16, 256, 8), 256, 0, s>>>(reinterpret_cast<const uint4*>(src), reinterpret_cast<uint4*>(dst), n16, yc);
             KB200_TRY(check_launch(k.vec16_name));
         }
         done = n16 * 8;
     }
     if (done < ngroups2) {
-        k.generic<<<div_up(ngroups2 - done, 256), 256, 0, s>>>(src, dst, done, ngroups2);
+        k.generic<<<div_up(ngroups2 - done, 256), 256, 0, s>>>(src, dst, done, ngroups2, yc);
         KB200_TRY(check_launch(k.generic_name));
     }
     return KB200_OK;
+}
+
+KB200_API int kb200_rgb_from_yuv420_u8(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst,
+                                       size_t dst_len, uint32_t width, uint32_t height, uint32_t batch, int layout) {
+    return kb200_rgb_from_yuv420_u8_matrix(stream, src, src_len, dst, dst_len, width, height, batch, layout, KB200_YUV_BT601_LIMITED);
+}
+
+KB200_API int kb200_rgb_from_yuv422_u8(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst,
+                                       size_t dst_len, uint32_t width, uint32_t height, uint32_t batch, int layout) {
+    return kb200_rgb_from_yuv422_u8_matrix(stream, src, src_len, dst, dst_len, width, height, batch, layout, KB200_YUV_BT601_LIMITED);
 }
 
 KB200_API int kb200_rgb_from_nv12_u8(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst,

@@ -141,20 +141,37 @@ __device__ __forceinline__ float byte_to_float(uint32_t w, int i) {
     return __uint_as_float(bits) - 8388608.0f;
 }
 
-// BT.601 limited-range Q20 decode — color/yuv/kernels.rs:707-737 / preprocess.rs:501-508.
-struct ChromaTerms {
-    int b, g, r;  // CUB*u + half, CUG*u + CVG*v + half, CVR*v + half   (u, v already -128)
+// Q20 YUV -> RGB decode, one coefficient set per kb200_yuv_matrix — color/yuv/kernels.rs:707-737 / preprocess.rs:501-508:
+//   yy = max(Y - y_off, 0) * cy,  u = U - 128,  v = V - 128
+//   R = sat((yy + cvr*v + 2^19) >> 20),  G = sat((yy + cug*u + cvg*v + 2^19) >> 20),  B = sat((yy + cub*u + 2^19) >> 20)
+// The kernels take the set as a launch argument (the same kernels serve every matrix).  Every term is below 5.8e8 in
+// magnitude, so the i32 sums cannot overflow.
+struct YuvCoeffs {
+    int y_off, cy, cvr, cub, cug, cvg;
 };
-__device__ __forceinline__ ChromaTerms chroma_terms(int u, int v) {
+// Indexed by kb200_yuv_matrix.  BT.601 limited keeps the reference's literal constants; the others are round(c * 2^20)
+// of the exact coefficients from (Kr, Kb) = (0.299, 0.114) for BT.601 and (0.2126, 0.0722) for BT.709: cvr = 2(1-Kr),
+// cub = 2(1-Kb), cug = -2Kb(1-Kb)/Kg, cvg = -2Kr(1-Kr)/Kg, with Kg = 1-Kr-Kb; limited range scales luma by 255/219
+// and chroma by 255/224 (y_off 16), full range uses them as they are (y_off 0).
+static constexpr YuvCoeffs YUV_COEFFS[4] = {
+    {16, 1220542, 1673527, 2116026, -409993, -852492},   // KB200_YUV_BT601_LIMITED
+    {0, 1048576, 1470104, 1858077, -360853, -748826},    // KB200_YUV_BT601_FULL
+    {16, 1220945, 1879825, 2215014, -223607, -558796},   // KB200_YUV_BT709_LIMITED
+    {0, 1048576, 1651297, 1945738, -196424, -490864},    // KB200_YUV_BT709_FULL
+};
+struct ChromaTerms {
+    int b, g, r;  // cub*u + half, cug*u + cvg*v + half, cvr*v + half   (u, v already -128)
+};
+__device__ __forceinline__ ChromaTerms chroma_terms(int u, int v, const YuvCoeffs& c) {
     u -= 128;
     v -= 128;
     ChromaTerms t;
-    t.b = 2116026 * u + (1 << 19);
-    t.g = (-409993) * u + (-852492) * v + (1 << 19);
-    t.r = 1673527 * v + (1 << 19);
+    t.b = c.cub * u + (1 << 19);
+    t.g = c.cug * u + c.cvg * v + (1 << 19);
+    t.r = c.cvr * v + (1 << 19);
     return t;
 }
-__device__ __forceinline__ int yy_term(int y) { return max(y - 16, 0) * 1220542; }
+__device__ __forceinline__ int yy_term(int y, const YuvCoeffs& c) { return max(y - c.y_off, 0) * c.cy; }
 __device__ __forceinline__ int sat_u8(int v) { return min(max(v, 0), 255); }
 // integer adds are associative (two's complement, no overflow here: |terms| < 2^30), so
 // (yy + CUB*u + half) == yy + (CUB*u + half) bit-for-bit.

@@ -6,6 +6,8 @@
 // A Bayer tap is the demosaiced pixel at the tap's coordinate (bayer.cuh); Bayer frames take the generic kernel, except
 // the identity geometry, which has its own fast kernel.  A 16-bit Bayer tap is normalised against the white level
 // W = 2^bits - 1 of its format: (px / W - mean) * inv_std, px / W the IEEE quotient.
+// A YUV tap decodes with the colour matrix the fmt code carries in bits 8-9 (KB200_FMT_YUV_MATRIX): the entry points
+// strip those bits from the descriptor and hand every kernel the matrix's coefficient set (YuvCoeffs) as an argument.
 //
 // Reference: preprocess.rs:430-647 (the CUDA source string — the specification of this path; there
 // is no CPU implementation for the camera formats), launch seam :1324-1372, batch loop :1277-1280
@@ -71,30 +73,30 @@ __device__ __forceinline__ float div255_exact(float p) {
     return fmaf(e, c, q);
 }
 
-__device__ __forceinline__ void yuv_to_rgbf(int yv, int u, int v, float px[3]) {  // :501-508
-    const ChromaTerms t = chroma_terms(u, v);
+__device__ __forceinline__ void yuv_to_rgbf(int yv, int u, int v, const YuvCoeffs& yc, float px[3]) {  // :501-508
+    const ChromaTerms t = chroma_terms(u, v, yc);
     int r, g, b;
-    decode_rgb(yy_term(yv), t, r, g, b);
+    decode_rgb(yy_term(yv, yc), t, r, g, b);
     px[0] = (float)r; px[1] = (float)g; px[2] = (float)b;
 }
 
 // fmt 5-9, the YUV layouts beyond the reference's SourceFormat: the chroma addressing of the standalone decoders (color.cu)
 __device__ __forceinline__ void fetch_px_yuv_ext(const uint8_t* __restrict__ src, int x, int y, const kb200_preprocess_desc& d,
-                                                 float px[3]) {
+                                                 const YuvCoeffs& yc, float px[3]) {
     if (d.fmt == KB200_FMT_UYVY || d.fmt == KB200_FMT_YVYU) {
         const uint8_t* grp = src + (long long)y * d.src_pitch + (x >> 1) * 4;
-        if (d.fmt == KB200_FMT_UYVY) yuv_to_rgbf(grp[(x & 1) ? 3 : 1], grp[0], grp[2], px);   // U Y0 V Y1
-        else yuv_to_rgbf(grp[(x & 1) ? 2 : 0], grp[3], grp[1], px);                           // Y0 V Y1 U
+        if (d.fmt == KB200_FMT_UYVY) yuv_to_rgbf(grp[(x & 1) ? 3 : 1], grp[0], grp[2], yc, px);   // U Y0 V Y1
+        else yuv_to_rgbf(grp[(x & 1) ? 2 : 0], grp[3], grp[1], yc, px);                           // Y0 V Y1 U
         return;
     }
     const int yv = src[(long long)y * d.src_w + x];
     if (d.fmt == KB200_FMT_NV21) {
         const uint8_t* vu = src + (long long)d.src_w * d.src_h + (long long)(y >> 1) * d.src_w + (x >> 1) * 2;
-        yuv_to_rgbf(yv, vu[1], vu[0], px);
+        yuv_to_rgbf(yv, vu[1], vu[0], yc, px);
     } else {
         const int L = d.fmt == KB200_FMT_I420 ? YUV420_I420 : YUV420_YV12;
         const size_t c = (size_t)(y >> 1) * (d.src_w >> 1) + (x >> 1);
-        yuv_to_rgbf(yv, src[yuv420_u_plane(L, d.src_w, d.src_h) + c], src[yuv420_v_plane(L, d.src_w, d.src_h) + c], px);
+        yuv_to_rgbf(yv, src[yuv420_u_plane(L, d.src_w, d.src_h) + c], src[yuv420_v_plane(L, d.src_w, d.src_h) + c], yc, px);
     }
 }
 
@@ -116,7 +118,7 @@ __host__ __device__ inline int bayer_pattern(int fmt, bool bayer16) { return bay
 
 template <int EXT>
 __device__ __forceinline__ void fetch_px(const uint8_t* __restrict__ src, int x, int y, const kb200_preprocess_desc& d,
-                                         float px[3]) {  // :510-530
+                                         const YuvCoeffs& yc, float px[3]) {  // :510-530
     if (EXT == SRC_BAYER || EXT == SRC_BAYER16) {   // src_pitch is in bytes (even for 16-bit samples)
         using T = std::conditional_t<EXT == SRC_BAYER16, uint16_t, uint8_t>;
         int rgb[3];
@@ -127,7 +129,7 @@ __device__ __forceinline__ void fetch_px(const uint8_t* __restrict__ src, int x,
         bayer_px_packed(src, (size_t)d.src_pitch, d.src_w, d.src_h, x, y, bayer_packed_pattern(d.fmt), bayer_packed_bits(d.fmt), rgb);
         px[0] = (float)rgb[0]; px[1] = (float)rgb[1]; px[2] = (float)rgb[2];
     } else if (EXT == SRC_EXT_YUV) {
-        fetch_px_yuv_ext(src, x, y, d, px);
+        fetch_px_yuv_ext(src, x, y, d, yc, px);
     } else if (d.fmt <= 1) {
         const uint8_t* p = src + (long long)y * d.src_pitch + x * d.src_bpp;
         if (d.fmt == 0) { px[0] = (float)p[0]; px[1] = (float)p[1]; px[2] = (float)p[2]; }
@@ -138,11 +140,11 @@ __device__ __forceinline__ void fetch_px(const uint8_t* __restrict__ src, int x,
     } else if (d.fmt == 3) {
         const int yv = src[(long long)y * d.src_w + x];
         const uint8_t* uv = src + (long long)d.src_w * d.src_h + (long long)(y >> 1) * d.src_w + (x >> 1) * 2;
-        yuv_to_rgbf(yv, uv[0], uv[1], px);
+        yuv_to_rgbf(yv, uv[0], uv[1], yc, px);
     } else {
         const uint8_t* grp = src + (long long)y * d.src_pitch + (x >> 1) * 4;
         const int yv = grp[(x & 1) ? 2 : 0];
-        yuv_to_rgbf(yv, grp[1], grp[3], px);
+        yuv_to_rgbf(yv, grp[1], grp[3], yc, px);
     }
 }
 
@@ -159,7 +161,7 @@ __device__ __forceinline__ float pre_lanczos_w(float dd) {
 template <bool F16, int SAMP, bool PTRS, int EXT>
 __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                  const __grid_constant__ PreFrames fr, void* __restrict__ dst,
-                                                                 uint32_t frame0) {
+                                                                 uint32_t frame0, const YuvCoeffs yc) {
     const int pixels = d.dst_w * d.dst_h;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= pixels) return;
@@ -177,13 +179,13 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
             for (int j = -2; j <= 3; ++j) {
                 const int yj = y0 + j;
                 const float wy = pre_lanczos_w(sy - (float)yj);
-                const int yc = min(max(yj, 0), d.src_h - 1);
+                const int ycl = min(max(yj, 0), d.src_h - 1);
                 for (int ii = -2; ii <= 3; ++ii) {
                     const int xi = x0 + ii;
                     const float w = wy * pre_lanczos_w(sx - (float)xi);
                     const int xc = min(max(xi, 0), d.src_w - 1);
                     float t[3];
-                    fetch_px<EXT>(src, xc, yc, d, t);
+                    fetch_px<EXT>(src, xc, ycl, d, yc, t);
                     acc0 += w * t[0]; acc1 += w * t[1]; acc2 += w * t[2];
                     wsum += w;
                 }
@@ -195,12 +197,12 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
             const int x1 = min(x0 + 1, d.src_w - 1), y1 = min(y0 + 1, d.src_h - 1);
             x0 = max(x0, 0); y0 = max(y0, 0);
             float t00[3], t10[3], t01[3], t11[3];
-            fetch_px<EXT>(src, x0, y0, d, t00);
+            fetch_px<EXT>(src, x0, y0, d, yc, t00);
             const bool need_x = ax != 0.0f, need_y = ay != 0.0f;
-            if (need_x) fetch_px<EXT>(src, x1, y0, d, t10);
+            if (need_x) fetch_px<EXT>(src, x1, y0, d, yc, t10);
             if (need_y) {
-                fetch_px<EXT>(src, x0, y1, d, t01);
-                if (need_x) fetch_px<EXT>(src, x1, y1, d, t11);
+                fetch_px<EXT>(src, x0, y1, d, yc, t01);
+                if (need_x) fetch_px<EXT>(src, x1, y1, d, yc, t11);
             }
 #pragma unroll
             for (int c = 0; c < 3; ++c) {
@@ -215,7 +217,7 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
         } else {
             const int xn = min(max((int)roundf(sx), 0), d.src_w - 1);
             const int yn = min(max((int)roundf(sy), 0), d.src_h - 1);
-            fetch_px<EXT>(src, xn, yn, d, px);
+            fetch_px<EXT>(src, xn, yn, d, yc, px);
         }
     } else {
         px[0] = d.pad_value; px[1] = d.pad_value; px[2] = d.pad_value;
@@ -279,7 +281,8 @@ __device__ __forceinline__ float norm_int_px(int r, float m, float is) { return 
 template <bool F16, bool PTRS, int L>
 __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                          const __grid_constant__ PreFrames fr, void* __restrict__ dst,
-                                                                         uint32_t frame0, uint32_t groups_per_row, uint32_t items) {
+                                                                         uint32_t frame0, uint32_t groups_per_row, uint32_t items,
+                                                                         const YuvCoeffs yc) {
     const uint32_t item = blockIdx.x * blockDim.x + threadIdx.x;
     if (item >= items) return;
     const uint32_t rp = item / groups_per_row, g = item - rp * groups_per_row;
@@ -294,16 +297,16 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const _
         const size_t c = (size_t)rp * (w / 2u) + x / 2u;
         const uint32_t u2 = __ldg(reinterpret_cast<const unsigned short*>(src + yuv420_u_plane(L, w, h) + c));
         const uint32_t v2 = __ldg(reinterpret_cast<const unsigned short*>(src + yuv420_v_plane(L, w, h) + c));
-        ct[0] = chroma_terms((int)(u2 & 0xFFu), (int)(v2 & 0xFFu));
-        ct[1] = chroma_terms((int)(u2 >> 8), (int)(v2 >> 8));
+        ct[0] = chroma_terms((int)(u2 & 0xFFu), (int)(v2 & 0xFFu), yc);
+        ct[1] = chroma_terms((int)(u2 >> 8), (int)(v2 >> 8), yc);
     } else {
         const uint32_t uvw = __ldg(reinterpret_cast<const uint32_t*>(src + (size_t)w * h + (size_t)rp * w + x));
         if (L == YUV420_NV21) {
-            ct[0] = chroma_terms((int)((uvw >> 8) & 0xFFu), (int)(uvw & 0xFFu));
-            ct[1] = chroma_terms((int)(uvw >> 24), (int)((uvw >> 16) & 0xFFu));
+            ct[0] = chroma_terms((int)((uvw >> 8) & 0xFFu), (int)(uvw & 0xFFu), yc);
+            ct[1] = chroma_terms((int)(uvw >> 24), (int)((uvw >> 16) & 0xFFu), yc);
         } else {
-            ct[0] = chroma_terms((int)(uvw & 0xFFu), (int)((uvw >> 8) & 0xFFu));
-            ct[1] = chroma_terms((int)((uvw >> 16) & 0xFFu), (int)(uvw >> 24));
+            ct[0] = chroma_terms((int)(uvw & 0xFFu), (int)((uvw >> 8) & 0xFFu), yc);
+            ct[1] = chroma_terms((int)((uvw >> 16) & 0xFFu), (int)(uvw >> 24), yc);
         }
     }
     const size_t plane = (size_t)w * h;
@@ -317,7 +320,7 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const _
         for (int i = 0; i < 4; ++i) {
             const int yv = (int)((yw >> (8 * i)) & 0xFFu);
             int r, gg, b;
-            decode_rgb(yy_term(yv), ct[i >> 1], r, gg, b);
+            decode_rgb(yy_term(yv, yc), ct[i >> 1], r, gg, b);
             r4[i] = norm_int_px(r, m0, i0);
             g4[i] = norm_int_px(gg, m1, i1);
             b4[i] = norm_int_px(b, m2, i2);
@@ -431,17 +434,17 @@ struct Nv12Args {
 
 // One decoded tap of a 4:2:0 frame in layout L (kb200_yuv420_layout): the kernel below serves all four layouts.
 template <int L>
-__device__ __forceinline__ void yuv420_tap(const uint8_t* __restrict__ src, int x, int y, int w, int h, int rgb[3]) {
+__device__ __forceinline__ void yuv420_tap(const uint8_t* __restrict__ src, int x, int y, int w, int h, const YuvCoeffs& yc, int rgb[3]) {
     const int yv = __ldg(src + (size_t)y * w + x);
     ChromaTerms t;
     if (yuv420_planar(L)) {
         const size_t c = (size_t)(y >> 1) * (w >> 1) + (x >> 1);
-        t = chroma_terms(__ldg(src + yuv420_u_plane(L, w, h) + c), __ldg(src + yuv420_v_plane(L, w, h) + c));
+        t = chroma_terms(__ldg(src + yuv420_u_plane(L, w, h) + c), __ldg(src + yuv420_v_plane(L, w, h) + c), yc);
     } else {
         const uint32_t uv = __ldg(reinterpret_cast<const unsigned short*>(src + (size_t)w * h + (size_t)(y >> 1) * w + (x >> 1) * 2));
-        t = L == YUV420_NV21 ? chroma_terms((int)(uv >> 8), (int)(uv & 0xFFu)) : chroma_terms((int)(uv & 0xFFu), (int)(uv >> 8));
+        t = L == YUV420_NV21 ? chroma_terms((int)(uv >> 8), (int)(uv & 0xFFu), yc) : chroma_terms((int)(uv & 0xFFu), (int)(uv >> 8), yc);
     }
-    decode_rgb(yy_term(yv), t, rgb[0], rgb[1], rgb[2]);
+    decode_rgb(yy_term(yv, yc), t, rgb[0], rgb[1], rgb[2]);
 }
 
 static constexpr int NV12_ROWS = 8;  // destination rows per thread: the x-side of the sampler is computed once for all of them
@@ -449,7 +452,7 @@ static constexpr int NV12_ROWS = 8;  // destination rows per thread: the x-side 
 template <bool F16, bool BILINEAR, bool PTRS, int L>
 __global__ void __launch_bounds__(128) preprocess_yuv420_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                 const __grid_constant__ PreFrames fr, const __grid_constant__ Nv12Args na,
-                                                                void* __restrict__ dst, uint32_t frame0) {
+                                                                void* __restrict__ dst, uint32_t frame0, const YuvCoeffs yc) {
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= na.groups) return;
     const uint32_t f = blockIdx.z;
@@ -505,17 +508,17 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_kernel(const __grid_con
             for (int j = 0; j < 4; ++j) {
                 if (!xin[j]) { o[0][j] = na.pad_norm[0]; o[1][j] = na.pad_norm[1]; o[2][j] = na.pad_norm[2]; continue; }
                 int t00[3];
-                yuv420_tap<L>(src, xa[j], y0, w, h, t00);
+                yuv420_tap<L>(src, xa[j], y0, w, h, yc, t00);
                 const bool need_x = BILINEAR && ax[j] != 0.0f;
                 float px[3];
                 if (!need_x && !need_y) {  // the sample IS the decoded tap (exact, see header)
                     px[0] = (float)t00[0]; px[1] = (float)t00[1]; px[2] = (float)t00[2];
                 } else {
                     int t10[3] = {0, 0, 0}, t01[3] = {0, 0, 0}, t11[3] = {0, 0, 0};
-                    if (need_x) yuv420_tap<L>(src, xb[j], y0, w, h, t10);
+                    if (need_x) yuv420_tap<L>(src, xb[j], y0, w, h, yc, t10);
                     if (need_y) {
-                        yuv420_tap<L>(src, xa[j], y1, w, h, t01);
-                        if (need_x) yuv420_tap<L>(src, xb[j], y1, w, h, t11);
+                        yuv420_tap<L>(src, xa[j], y1, w, h, yc, t01);
+                        if (need_x) yuv420_tap<L>(src, xb[j], y1, w, h, yc, t11);
                     }
 #pragma unroll
                     for (int c = 0; c < 3; ++c) {
@@ -560,6 +563,17 @@ static const char* const FMT_NAMES[10] = {"Rgb8", "Bgr8", "Gray8", "Nv12", "Yuyv
 static const char* const BAYER_NAMES[4] = {"BayerRggb", "BayerBggr", "BayerGrbg", "BayerGbrg"};
 static const char* const YUV420_UPPER[4] = {"NV12", "NV21", "I420", "YV12"};
 
+static bool is_yuv(int fmt) { return yuv420_layout(fmt) >= 0 || is_yuv422(fmt); }
+
+// kb200_preprocess_desc::fmt = format code (bits 0-7) | KB200_FMT_YUV_MATRIX(m) (bits 8-9).  The entry points strip the
+// matrix once, here: every other function sees the plain code and takes the coefficient set apart.
+static kb200_preprocess_desc plain_desc(const kb200_preprocess_desc& d) {
+    kb200_preprocess_desc p = d;
+    p.fmt = d.fmt & 0xFF;
+    return p;
+}
+static const YuvCoeffs& yuv_coeffs(const kb200_preprocess_desc& d) { return YUV_COEFFS[(d.fmt >> 8) & 3]; }
+
 static size_t src_bytes(const kb200_preprocess_desc& d) {
     const size_t chroma = yuv420_layout(d.fmt) >= 0 ? (size_t)d.src_w * d.src_h / 2 : 0;
     return (size_t)d.src_pitch * d.src_h + chroma;
@@ -567,12 +581,17 @@ static size_t src_bytes(const kb200_preprocess_desc& d) {
 
 static int validate_desc(const kb200_preprocess_desc* dp) {
     if (!dp) return fail(KB200_ERR_INVALID_ARGUMENT, "null preprocess descriptor");
-    const kb200_preprocess_desc& d = *dp;
-    if (d.src_w <= 0 || d.src_h <= 0 || d.dst_w <= 0 || d.dst_h <= 0)
+    if (dp->src_w <= 0 || dp->src_h <= 0 || dp->dst_w <= 0 || dp->dst_h <= 0)
         return fail(KB200_ERR_INVALID_ARGUMENT, "image dimensions must be non-zero");
-    if ((long long)d.dst_w * d.dst_h > 0x7FFFFFFFll) return fail(KB200_ERR_DIMS_TOO_LARGE, "dimensions exceed the 32-bit CUDA kernel index limit");  // :1336-1339
-    if (d.fmt < 0 || (d.fmt > KB200_FMT_YVYU && !is_bayer(d.fmt) && !is_bayer16(d.fmt) && !is_bayer_packed(d.fmt)))
-        return fail(KB200_ERR_INVALID_ARGUMENT, "unknown source format code %d", d.fmt);
+    if ((long long)dp->dst_w * dp->dst_h > 0x7FFFFFFFll) return fail(KB200_ERR_DIMS_TOO_LARGE, "dimensions exceed the 32-bit CUDA kernel index limit");  // :1336-1339
+    const kb200_preprocess_desc d = plain_desc(*dp);
+    if (dp->fmt < 0 || (d.fmt > KB200_FMT_YVYU && !is_bayer(d.fmt) && !is_bayer16(d.fmt) && !is_bayer_packed(d.fmt)))
+        return fail(KB200_ERR_INVALID_ARGUMENT, "unknown source format code %d", dp->fmt);
+    if (dp->fmt >> 10)
+        return fail(KB200_ERR_INVALID_ARGUMENT, "source format code %d has bits set above bit 9 (bits 8-9 are the YUV matrix, 0-3)", dp->fmt);
+    if ((dp->fmt >> 8) && !is_yuv(d.fmt))
+        return fail(KB200_ERR_INVALID_ARGUMENT, "source format code %d: a YUV matrix (%d) applies only to the YUV formats, not format code %d", dp->fmt,
+                    dp->fmt >> 8, d.fmt);
     if (d.sampling != KB200_INTERP_NEAREST && d.sampling != KB200_INTERP_BILINEAR && d.sampling != KB200_INTERP_LANCZOS)
         return fail(KB200_ERR_UNSUPPORTED, "unsupported sampling mode %d (expected Nearest, Bilinear or Lanczos)", d.sampling);  // preprocess.rs:1044-1051
     if (d.fmt <= 1 && d.src_bpp != 3 && d.src_bpp != 4) return fail(KB200_ERR_UNSUPPORTED, "unsupported source channel count %d (expected 3 or 4)", d.src_bpp);
@@ -612,16 +631,16 @@ static int validate_desc(const kb200_preprocess_desc* dp) {
 
 // The 4:2:0 fast kernels of layout L, for one launch of <= 256 frames.
 template <bool F16, int L>
-static void launch_yuv420_fast(cudaStream_t s, bool identity, bool bil, const kb200_preprocess_desc& d, const PreFrames& fr, bool ptrs,
-                               const Nv12Args& nv, void* dst, uint32_t f0, uint32_t nb, uint32_t id_groups, size_t id_items) {
+static void launch_yuv420_fast(cudaStream_t s, bool identity, bool bil, const kb200_preprocess_desc& d, const YuvCoeffs& yc, const PreFrames& fr,
+                               bool ptrs, const Nv12Args& nv, void* dst, uint32_t f0, uint32_t nb, uint32_t id_groups, size_t id_items) {
     if (identity) {
         dim3 grid(div_up(id_items, 128), nb);
-        if (ptrs) preprocess_yuv420_identity_kernel<F16, true, L><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
-        else preprocess_yuv420_identity_kernel<F16, false, L><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
+        if (ptrs) preprocess_yuv420_identity_kernel<F16, true, L><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
+        else preprocess_yuv420_identity_kernel<F16, false, L><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
         return;
     }
     dim3 grid(div_up(nv.groups, 128), div_up((size_t)d.dst_h, NV12_ROWS), nb);
-#define KB200_YUV420_LAUNCH(BIL, PT) preprocess_yuv420_kernel<F16, BIL, PT, L><<<grid, 128, 0, s>>>(d, fr, nv, dst, f0)
+#define KB200_YUV420_LAUNCH(BIL, PT) preprocess_yuv420_kernel<F16, BIL, PT, L><<<grid, 128, 0, s>>>(d, fr, nv, dst, f0, yc)
     if (bil) { if (ptrs) KB200_YUV420_LAUNCH(true, true); else KB200_YUV420_LAUNCH(true, false); }
     else     { if (ptrs) KB200_YUV420_LAUNCH(false, true); else KB200_YUV420_LAUNCH(false, false); }
 #undef KB200_YUV420_LAUNCH
@@ -637,20 +656,21 @@ static void launch_bayer_identity(cudaStream_t s, const kb200_preprocess_desc& d
 }
 
 template <bool F16, bool PTRS, int EXT>
-static void launch_generic(cudaStream_t s, dim3 grid, int sampling, const kb200_preprocess_desc& d, const PreFrames& fr, void* dst, uint32_t f0) {
-    if (sampling == KB200_INTERP_LANCZOS) preprocess_generic_kernel<F16, KB200_INTERP_LANCZOS, PTRS, EXT><<<grid, 256, 0, s>>>(d, fr, dst, f0);
-    else if (sampling == KB200_INTERP_BILINEAR) preprocess_generic_kernel<F16, KB200_INTERP_BILINEAR, PTRS, EXT><<<grid, 256, 0, s>>>(d, fr, dst, f0);
-    else preprocess_generic_kernel<F16, KB200_INTERP_NEAREST, PTRS, EXT><<<grid, 256, 0, s>>>(d, fr, dst, f0);
+static void launch_generic(cudaStream_t s, dim3 grid, int sampling, const kb200_preprocess_desc& d, const YuvCoeffs& yc, const PreFrames& fr, void* dst,
+                           uint32_t f0) {
+    if (sampling == KB200_INTERP_LANCZOS) preprocess_generic_kernel<F16, KB200_INTERP_LANCZOS, PTRS, EXT><<<grid, 256, 0, s>>>(d, fr, dst, f0, yc);
+    else if (sampling == KB200_INTERP_BILINEAR) preprocess_generic_kernel<F16, KB200_INTERP_BILINEAR, PTRS, EXT><<<grid, 256, 0, s>>>(d, fr, dst, f0, yc);
+    else preprocess_generic_kernel<F16, KB200_INTERP_NEAREST, PTRS, EXT><<<grid, 256, 0, s>>>(d, fr, dst, f0, yc);
 }
 
 template <bool F16, bool PTRS>
-static void launch_generic_for(int ext, cudaStream_t s, dim3 grid, int sampling, const kb200_preprocess_desc& d, const PreFrames& fr, void* dst,
-                               uint32_t f0) {
-    if (ext == SRC_BAYER_PACKED) launch_generic<F16, PTRS, SRC_BAYER_PACKED>(s, grid, sampling, d, fr, dst, f0);
-    else if (ext == SRC_BAYER16) launch_generic<F16, PTRS, SRC_BAYER16>(s, grid, sampling, d, fr, dst, f0);
-    else if (ext == SRC_BAYER) launch_generic<F16, PTRS, SRC_BAYER>(s, grid, sampling, d, fr, dst, f0);
-    else if (ext == SRC_EXT_YUV) launch_generic<F16, PTRS, SRC_EXT_YUV>(s, grid, sampling, d, fr, dst, f0);
-    else launch_generic<F16, PTRS, SRC_BASE>(s, grid, sampling, d, fr, dst, f0);
+static void launch_generic_for(int ext, cudaStream_t s, dim3 grid, int sampling, const kb200_preprocess_desc& d, const YuvCoeffs& yc,
+                               const PreFrames& fr, void* dst, uint32_t f0) {
+    if (ext == SRC_BAYER_PACKED) launch_generic<F16, PTRS, SRC_BAYER_PACKED>(s, grid, sampling, d, yc, fr, dst, f0);
+    else if (ext == SRC_BAYER16) launch_generic<F16, PTRS, SRC_BAYER16>(s, grid, sampling, d, yc, fr, dst, f0);
+    else if (ext == SRC_BAYER) launch_generic<F16, PTRS, SRC_BAYER>(s, grid, sampling, d, yc, fr, dst, f0);
+    else if (ext == SRC_EXT_YUV) launch_generic<F16, PTRS, SRC_EXT_YUV>(s, grid, sampling, d, yc, fr, dst, f0);
+    else launch_generic<F16, PTRS, SRC_BASE>(s, grid, sampling, d, yc, fr, dst, f0);
 }
 
 // kb200_last_kernel() names of the 4:2:0 fast kernels, by layout
@@ -666,7 +686,7 @@ static const char* const BAYER_IDENTITY_NAMES[5][4] = {KB200_BAYER_IDENTITY_NAME
 #undef KB200_BAYER_IDENTITY_NAMES
 
 template <bool F16>
-static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, const uint8_t* const* frames,
+static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, const YuvCoeffs& yc, const uint8_t* const* frames,
                              const uint8_t* base, size_t stride, uint32_t batch, void* dst) {
     const int pixels = d.dst_w * d.dst_h;
     const bool bil = d.sampling == KB200_INTERP_BILINEAR, lanczos = d.sampling == KB200_INTERP_LANCZOS;
@@ -722,17 +742,17 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
         }
         if (identity || yuv420_fast) {
             switch (l420) {
-                case YUV420_NV12: launch_yuv420_fast<F16, YUV420_NV12>(s, identity, bil, d, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
-                case YUV420_NV21: launch_yuv420_fast<F16, YUV420_NV21>(s, identity, bil, d, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
-                case YUV420_I420: launch_yuv420_fast<F16, YUV420_I420>(s, identity, bil, d, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
-                default: launch_yuv420_fast<F16, YUV420_YV12>(s, identity, bil, d, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                case YUV420_NV12: launch_yuv420_fast<F16, YUV420_NV12>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                case YUV420_NV21: launch_yuv420_fast<F16, YUV420_NV21>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                case YUV420_I420: launch_yuv420_fast<F16, YUV420_I420>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                default: launch_yuv420_fast<F16, YUV420_YV12>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
             }
             KB200_TRY(check_launch(identity ? YUV420_IDENTITY_NAMES[l420] : YUV420_FAST_NAMES[l420]));
             continue;
         }
         dim3 grid(div_up(pixels, 256), nb);
-        if (p) launch_generic_for<F16, true>(ext, s, grid, d.sampling, d, fr, dst, f0);
-        else launch_generic_for<F16, false>(ext, s, grid, d.sampling, d, fr, dst, f0);
+        if (p) launch_generic_for<F16, true>(ext, s, grid, d.sampling, d, yc, fr, dst, f0);
+        else launch_generic_for<F16, false>(ext, s, grid, d.sampling, d, yc, fr, dst, f0);
         KB200_TRY(check_launch("preprocess_generic_kernel"));
     }
     return KB200_OK;
@@ -740,16 +760,20 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
 
 // used by the host-buffer pipeline (host_pipeline.cu): frames already staged at base + i*stride on the device
 int preprocess_validate(const kb200_preprocess_desc* desc) { return validate_desc(desc); }
-size_t preprocess_frame_bytes(const kb200_preprocess_desc& d) { return src_bytes(d); }
-int preprocess_launch_strided(cudaStream_t s, const kb200_preprocess_desc& d, const uint8_t* base, size_t stride, uint32_t batch, void* dst, bool f16) {
-    return f16 ? launch_preprocess<true>(s, d, nullptr, base, stride, batch, dst) : launch_preprocess<false>(s, d, nullptr, base, stride, batch, dst);
+size_t preprocess_frame_bytes(const kb200_preprocess_desc& d) { return src_bytes(plain_desc(d)); }
+int preprocess_launch_strided(cudaStream_t s, const kb200_preprocess_desc& desc, const uint8_t* base, size_t stride, uint32_t batch, void* dst, bool f16) {
+    const kb200_preprocess_desc d = plain_desc(desc);
+    const YuvCoeffs& yc = yuv_coeffs(desc);
+    return f16 ? launch_preprocess<true>(s, d, yc, nullptr, base, stride, batch, dst) : launch_preprocess<false>(s, d, yc, nullptr, base, stride, batch, dst);
 }
 
 template <bool F16>
-static int preprocess_entry(kb200_stream_t stream, const kb200_preprocess_desc* desc, const uint8_t* const* frames,
+static int preprocess_entry(kb200_stream_t stream, const kb200_preprocess_desc* raw_desc, const uint8_t* const* frames,
                             const size_t* frame_len, const uint8_t* base, size_t base_len, size_t stride,
                             uint32_t batch, void* dst, size_t dst_len) {
-    KB200_TRY(validate_desc(desc));
+    KB200_TRY(validate_desc(raw_desc));
+    const kb200_preprocess_desc plain = plain_desc(*raw_desc);
+    const kb200_preprocess_desc* desc = &plain;
     KB200_TRY(check_ptr("dst", dst));
     if (batch == 0) return fail(KB200_ERR_INVALID_ARGUMENT, "batch must be non-zero");
     const size_t need = src_bytes(*desc);
@@ -773,7 +797,7 @@ static int preprocess_entry(kb200_stream_t stream, const kb200_preprocess_desc* 
     }
     // BatchMismatch / BadOutputShape: dst must hold [batch,3,H,W]
     KB200_TRY(check_slice("dst", dst_len, (size_t)batch * 3 * desc->dst_w * desc->dst_h));
-    return launch_preprocess<F16>(as_stream(stream), *desc, frames, base, stride, batch, dst);
+    return launch_preprocess<F16>(as_stream(stream), *desc, yuv_coeffs(*raw_desc), frames, base, stride, batch, dst);
 }
 
 __global__ void selftest_div255_kernel(unsigned long long* mismatches) {
@@ -807,7 +831,7 @@ KB200_API int kb200_selftest_div255(kb200_stream_t stream, uint64_t* mismatches_
     return check_launch("selftest_div255_kernel");
 }
 
-KB200_API size_t kb200_preprocess_src_bytes(const kb200_preprocess_desc* desc) { return desc ? src_bytes(*desc) : 0; }
+KB200_API size_t kb200_preprocess_src_bytes(const kb200_preprocess_desc* desc) { return desc ? src_bytes(plain_desc(*desc)) : 0; }
 
 KB200_API int kb200_preprocess_f32(kb200_stream_t stream, const kb200_preprocess_desc* desc, const uint8_t* const* frames,
                                    const size_t* frame_len, uint32_t batch, float* dst, size_t dst_len) {

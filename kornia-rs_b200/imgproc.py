@@ -533,11 +533,22 @@ YUV420_NV12, YUV420_NV21, YUV420_I420, YUV420_YV12 = 0, 1, 2, 3   # kb200_yuv420
 YUV422_YUYV, YUV422_UYVY, YUV422_YVYU = 0, 1, 2                   # kb200_yuv422_layout
 
 
+class YuvMatrix(enum.IntEnum):
+    """kb200_yuv_matrix: the colour matrix and range a YUV frame is decoded with.  Bt601Limited is the reference's decode
+    (SD video, cv2's COLOR_YUV2RGB_*); Bt601Full is JPEG / JFIF (MJPEG webcams, cv2's COLOR_YCrCb2RGB); Bt709Limited is
+    HD video (H.264 / HEVC at 720p and above, most NVDEC output); Bt709Full its full-range form.  All four are the same
+    Q20 integer arithmetic with another coefficient set (include/kornia_b200.h lists them)."""
+    Bt601Limited = 0
+    Bt601Full = 1
+    Bt709Limited = 2
+    Bt709Full = 3
+
+
 def _rgb_from_yuv(src, dst: Image, what: str, bytes_num: int, bytes_den: int, fn_name: str, *layout,
                   dtype: torch.dtype = torch.uint8, src_dtype: torch.dtype | None = None) -> None:
     """The video and Bayer decoders: `src` holds N tight frames of w*h*bytes_num/bytes_den samples of `src_dtype`
-    (default: `dtype`, the dtype of `dst`); `layout` is the extra arguments of the layout-generic entry points (none for
-    the NV12 / YUYV ones)."""
+    (default: `dtype`, the dtype of `dst`); `layout` is the extra arguments of the entry point (layout and matrix of the
+    YUV decoders, pattern and bits of the Bayer ones)."""
     t = _raw_frames(src, what, dtype if src_dtype is None else src_dtype)
     if not dst.is_device:
         raise ImageError.MixedResidency()
@@ -552,40 +563,41 @@ def _rgb_from_yuv(src, dst: Image, what: str, bytes_num: int, bytes_den: int, fn
     _check(getattr(_lib.lib(), fn_name)(_stream(t.device), t.data_ptr(), t.numel(), dst.data.data_ptr(), dst.numel(), w, h, n, *layout))
 
 
-def rgb_from_nv12(src, dst: Image) -> None:
+def rgb_from_nv12(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -> None:
     """color/yuv/mod.rs:235 — `src`: u8 tensor holding, per frame, w*h Y bytes then w*h/2 interleaved UV
-    bytes ([len] or [N,len]); BT.601 limited, Q20, bit-exact."""
-    _rgb_from_yuv(src, dst, "rgb_from_nv12", 3, 2, "kb200_rgb_from_nv12_u8")
+    bytes ([len] or [N,len]); Q20, bit-exact.  `matrix`: the colour matrix and range (default BT.601 limited, the
+    reference's decode)."""
+    _rgb_from_yuv(src, dst, "rgb_from_nv12", 3, 2, "kb200_rgb_from_yuv420_u8_matrix", YUV420_NV12, int(YuvMatrix(matrix)))
 
 
-def rgb_from_nv21(src, dst: Image) -> None:
+def rgb_from_nv21(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -> None:
     """Like rgb_from_nv12, with the chroma pairs stored V U (the Android camera default)."""
-    _rgb_from_yuv(src, dst, "rgb_from_nv21", 3, 2, "kb200_rgb_from_yuv420_u8", YUV420_NV21)
+    _rgb_from_yuv(src, dst, "rgb_from_nv21", 3, 2, "kb200_rgb_from_yuv420_u8_matrix", YUV420_NV21, int(YuvMatrix(matrix)))
 
 
-def rgb_from_i420(src, dst: Image) -> None:
+def rgb_from_i420(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -> None:
     """Like rgb_from_nv12, with the chroma in two (w/2 x h/2) planes after the Y plane: U, then V (yuv420p)."""
-    _rgb_from_yuv(src, dst, "rgb_from_i420", 3, 2, "kb200_rgb_from_yuv420_u8", YUV420_I420)
+    _rgb_from_yuv(src, dst, "rgb_from_i420", 3, 2, "kb200_rgb_from_yuv420_u8_matrix", YUV420_I420, int(YuvMatrix(matrix)))
 
 
-def rgb_from_yv12(src, dst: Image) -> None:
+def rgb_from_yv12(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -> None:
     """Like rgb_from_i420, with the V plane before the U plane."""
-    _rgb_from_yuv(src, dst, "rgb_from_yv12", 3, 2, "kb200_rgb_from_yuv420_u8", YUV420_YV12)
+    _rgb_from_yuv(src, dst, "rgb_from_yv12", 3, 2, "kb200_rgb_from_yuv420_u8_matrix", YUV420_YV12, int(YuvMatrix(matrix)))
 
 
-def rgb_from_yuyv(src, dst: Image) -> None:
-    """color/yuv/mod.rs:209 (impl_packed422!, Yuyv)."""
-    _rgb_from_yuv(src, dst, "rgb_from_yuyv", 2, 1, "kb200_rgb_from_yuyv_u8")
+def rgb_from_yuyv(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -> None:
+    """color/yuv/mod.rs:209 (impl_packed422!, Yuyv).  `matrix`: as for rgb_from_nv12."""
+    _rgb_from_yuv(src, dst, "rgb_from_yuyv", 2, 1, "kb200_rgb_from_yuv422_u8_matrix", YUV422_YUYV, int(YuvMatrix(matrix)))
 
 
-def rgb_from_uyvy(src, dst: Image) -> None:
+def rgb_from_uyvy(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -> None:
     """Like rgb_from_yuyv, with each pixel pair stored `U Y0 V Y1`."""
-    _rgb_from_yuv(src, dst, "rgb_from_uyvy", 2, 1, "kb200_rgb_from_yuv422_u8", YUV422_UYVY)
+    _rgb_from_yuv(src, dst, "rgb_from_uyvy", 2, 1, "kb200_rgb_from_yuv422_u8_matrix", YUV422_UYVY, int(YuvMatrix(matrix)))
 
 
-def rgb_from_yvyu(src, dst: Image) -> None:
+def rgb_from_yvyu(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -> None:
     """Like rgb_from_yuyv, with each pixel pair stored `Y0 V Y1 U`."""
-    _rgb_from_yuv(src, dst, "rgb_from_yvyu", 2, 1, "kb200_rgb_from_yuv422_u8", YUV422_YVYU)
+    _rgb_from_yuv(src, dst, "rgb_from_yvyu", 2, 1, "kb200_rgb_from_yuv422_u8_matrix", YUV422_YVYU, int(YuvMatrix(matrix)))
 
 
 class BayerPattern(enum.IntEnum):

@@ -19,6 +19,7 @@ import torch
 
 from . import _lib
 from .image import Image, InterpolationMode
+from .imgproc import YuvMatrix
 
 IMAGENET_MEAN = (0.485, 0.456, 0.406)  # preprocess.rs:93
 IMAGENET_STD = (0.229, 0.224, 0.225)   # preprocess.rs:95
@@ -128,6 +129,10 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
     def is_yuv422(self) -> bool:
         return self in (SourceFormat.Yuyv, SourceFormat.Uyvy, SourceFormat.Yvyu)
 
+    def is_yuv(self) -> bool:
+        """A YUV format: one a YuvMatrix applies to."""
+        return self.is_yuv420() or self.is_yuv422()
+
     def is_bayer(self) -> bool:
         return self.value.startswith("bayer_")
 
@@ -231,6 +236,7 @@ class PreprocessorBuilder:  # preprocess.rs:654-779
         self._pad_value = 114
         self._sampling = InterpolationMode.Bilinear
         self._source_format = SourceFormat.Rgb8
+        self._yuv_matrix = YuvMatrix.Bt601Limited
 
     def source_format(self, fmt: SourceFormat):
         self._source_format = fmt
@@ -252,9 +258,18 @@ class PreprocessorBuilder:  # preprocess.rs:654-779
         self._sampling = sampling
         return self
 
+    def yuv_matrix(self, matrix: YuvMatrix):
+        """The colour matrix and range YUV frames decode with (default Bt601Limited, the reference's decode).  Only the YUV
+        source formats take one: build_cuda() rejects any other matrix on an RGB, Gray or Bayer format."""
+        self._yuv_matrix = YuvMatrix(matrix)
+        return self
+
     def _validated(self):
         if self._sampling not in (InterpolationMode.Nearest, InterpolationMode.Bilinear, InterpolationMode.Lanczos):
             raise PreprocessError("UnsupportedSampling", f"unsupported sampling mode {self._sampling!r} (expected Nearest, Bilinear, or Lanczos)")
+        if self._yuv_matrix != YuvMatrix.Bt601Limited and not self._source_format.is_yuv():
+            raise PreprocessError("YuvMatrixNeedsYuvSource", f"YUV matrix {self._yuv_matrix!r} given for source format {self._source_format!r}, "
+                                  "which is not a YUV format", matrix=self._yuv_matrix, format=self._source_format)
         return self._normalize.mean_inv_std()
 
     def build(self):
@@ -266,14 +281,15 @@ class PreprocessorBuilder:  # preprocess.rs:654-779
         mean, inv_std = self._validated()
         _lib.lib()  # fail loudly if the native library is missing
         return Preprocessor(self._mode, self._sampling, self._source_format, mean, inv_std, float(self._pad_value),
-                            torch.device(device) if device is not None else None)
+                            torch.device(device) if device is not None else None, self._yuv_matrix)
 
 
 class Preprocessor:
-    def __init__(self, mode, sampling, source_format, mean, inv_std, pad_value, device):
+    def __init__(self, mode, sampling, source_format, mean, inv_std, pad_value, device, yuv_matrix=YuvMatrix.Bt601Limited):
         self._mode, self._sampling, self._fmt = mode, sampling, source_format
         self._mean, self._inv_std, self._pad = mean, inv_std, pad_value
         self._device = device
+        self._yuv_matrix = YuvMatrix(yuv_matrix)
 
     @staticmethod
     def builder() -> PreprocessorBuilder:
@@ -294,6 +310,9 @@ class Preprocessor:
     def mode(self) -> ResizeMode:
         return self._mode
 
+    def yuv_matrix(self) -> YuvMatrix:
+        return self._yuv_matrix
+
     # ── helpers ─────────────────────────────────────────────────────────────
     def _desc(self, sw, sh, pitch, bpp, fmt_code, dw, dh) -> _lib.PreprocessDesc:
         lim = 2 ** 31 - 1
@@ -303,7 +322,8 @@ class Preprocessor:
         _lib.lib().kb200_preprocess_affine(self._mode.value, sw, sh, dw, dh, a)
         d = _lib.PreprocessDesc()
         d.scale_x, d.scale_y, d.pad_x, d.pad_y = a[0], a[1], a[2], a[3]
-        d.src_w, d.src_h, d.src_pitch, d.src_bpp, d.fmt = sw, sh, pitch, bpp, fmt_code
+        d.src_w, d.src_h, d.src_pitch, d.src_bpp = sw, sh, pitch, bpp
+        d.fmt = fmt_code | (int(self._yuv_matrix) << 8)   # KB200_FMT_YUV_MATRIX: 0 unless the format is a YUV one (build_cuda)
         d.dst_w, d.dst_h = dw, dh
         d.mean = (C.c_float * 3)(*self._mean)
         d.inv_std = (C.c_float * 3)(*self._inv_std)
