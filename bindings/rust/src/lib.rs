@@ -141,6 +141,7 @@ pub mod ffi {
         pub fn kb200_rgb_from_bayer_u8(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, width: u32, height: u32, batch: u32, pattern: c_int) -> c_int;
         pub fn kb200_rgb_from_bayer_u16(stream: *mut c_void, src: *const u16, src_len: usize, dst: *mut u16, dst_len: usize, width: u32, height: u32, batch: u32, pattern: c_int) -> c_int;
         pub fn kb200_rgb_from_bayer_packed(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u16, dst_len: usize, width: u32, height: u32, batch: u32, pattern: c_int, bits: c_int) -> c_int;
+        pub fn kb200_rgb_from_yuv420_u16(stream: *mut c_void, src: *const u16, src_len: usize, dst: *mut u16, dst_len: usize, width: u32, height: u32, batch: u32, layout: c_int, bits: c_int, matrix: c_int) -> c_int;
         pub fn kb200_normalize_mean_std_f32(stream: *mut c_void, src: *const f32, dst: *mut f32, npixels: usize, channels: u32, mean: *const f32, std: *const f32) -> c_int;
         pub fn kb200_normalize_rgb_u8_f32(stream: *mut c_void, src: *const u8, dst: *mut f32, npixels: usize, scale: *const f32, offset: *const f32, leaf: c_int) -> c_int;
         pub fn kb200_find_min_max_f32(stream: *mut c_void, src: *const f32, n: usize, minmax_dev: *mut f32) -> c_int;
@@ -250,6 +251,12 @@ pub const FMT_BAYER_PACKED_BASE: i32 = 64;
 pub const FMT_BAYER_RGGB10P: i32 = 64;
 pub const FMT_BAYER_RGGB12P: i32 = 68;
 pub const FMT_BAYER_RGGB14P: i32 = 72;
+/// 10- and 12-bit 4:2:0 video, tight frames of w * h * 3 / 2 little-endian u16 words: P010 / P012 (NV12's layout, the
+/// code in the high bits) and I010 / I012 (I420's layout, the code in the low bits).  They take `fmt_yuv_matrix`.
+pub const FMT_P010: i32 = 80;
+pub const FMT_P012: i32 = 81;
+pub const FMT_I010: i32 = 82;
+pub const FMT_I012: i32 = 83;
 
 /// `pattern` of `kb200_rgb_from_bayer_u8` (kb200_bayer_pattern): the mosaic's 2x2 quad read row-major.
 pub const BAYER_RGGB: c_int = 0;
@@ -267,6 +274,11 @@ pub const YUV420_YV12: c_int = 3;
 pub const YUV422_YUYV: c_int = 0;
 pub const YUV422_UYVY: c_int = 1;
 pub const YUV422_YVYU: c_int = 2;
+
+/// `layout` of `kb200_rgb_from_yuv420_u16` (kb200_yuv420_u16_layout): P010 / P012 (interleaved chroma, codes in the
+/// high bits of each word) or I010 / I012 (U and V planes, codes in the low bits).
+pub const YUV420_P01X: c_int = 0;
+pub const YUV420_I01X: c_int = 1;
 
 /// `matrix` of `kb200_rgb_from_yuv420_u8_matrix` / `_yuv422_u8_matrix` (kb200_yuv_matrix): the colour matrix and range a
 /// YUV frame decodes with.  BT.601 limited is the reference's decode.

@@ -219,6 +219,101 @@ __global__ void rgb_from_yuv420_generic(const uint8_t* __restrict__ src, uint8_t
         }
 }
 
+// ── 10- and 12-bit 4:2:0 (P010, P012, I010, I012) → RGB16 ─────────────────────────────────────────────
+// L = kb200_yuv420_u16_layout; the depth and matrix arrive in Yuv16Coeffs (code extraction and Q16 set), so one kernel
+// serves both depths of a layout.  One thread: 8 luma columns x 2 rows (one chroma row) — 16 B of Y words per row, and
+// the 4 chroma pairs: one 16-B load of the interleaved row (P01x), or 8 B of the U plane and 8 B of the V plane (I01x;
+// with width % 8 == 0 both planes and every thread's offset in them are 8-B aligned).  8 pixels of 16-bit RGB are 48 B
+// per row, stored through store_rgb48_coalesced like the 8-bit kernels' 16 pixels.
+template <int L>
+__global__ void __launch_bounds__(128) rgb_from_yuv420_u16_vec(const uint16_t* __restrict__ src, uint16_t* __restrict__ dst,
+                                                               uint32_t width, uint32_t height, const Yuv16Coeffs k) {
+    __shared__ uint4 stage[4][96];
+    const uint32_t gx = blockIdx.x * blockDim.x + threadIdx.x;  // 8-column group
+    const uint32_t cy = blockIdx.y;                             // chroma row
+    const uint32_t lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
+    const uint32_t gx0 = gx - lane;                             // first group of this warp
+    if (gx0 * 8 >= width) return;                               // whole warp out of the row
+    const bool full_warp = (gx0 + 32) * 8 <= width;
+    const bool active = gx * 8 < width;
+    const size_t plane = (size_t)width * height;
+    const uint16_t* frame = src + (size_t)blockIdx.z * (plane * 3 / 2);
+    uint16_t* out = dst + (size_t)blockIdx.z * plane * 3;
+    const size_t x = (size_t)gx * 8;
+    uint4 yt = make_uint4(0, 0, 0, 0), yb = yt, uv = yt;   // I01x: uv = {U words 0-3, V words 0-3}; P01x: 4 (U, V) word pairs
+    if (active) {
+        yt = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + (size_t)(2 * cy) * width + x));
+        yb = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + (size_t)(2 * cy + 1) * width + x));
+        if (L == KB200_YUV420_I01X) {
+            const size_t c = (size_t)cy * (width / 2) + x / 2;
+            const uint2 u = ldg_stream_u2(reinterpret_cast<const uint2*>(frame + plane + c));
+            const uint2 v = ldg_stream_u2(reinterpret_cast<const uint2*>(frame + plane + plane / 4 + c));
+            uv = make_uint4(u.x, u.y, v.x, v.y);
+        } else {
+            uv = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + plane + (size_t)cy * width + x));
+        }
+    }
+    const uint32_t uvw[4] = {uv.x, uv.y, uv.z, uv.w};
+    ChromaTerms ct[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {   // yuv16_code keeps the n code bits of the low half-word it is shifted to
+        if (L == KB200_YUV420_I01X)
+            ct[j] = chroma_terms16(yuv16_code(uvw[j >> 1] >> (16 * (j & 1)), k), yuv16_code(uvw[2 + (j >> 1)] >> (16 * (j & 1)), k), k);
+        else
+            ct[j] = chroma_terms16(yuv16_code(uvw[j], k), yuv16_code(uvw[j] >> 16, k), k);
+    }
+    auto pack = [&](const uint4& yv, uint4 o[3]) {   // 8 pixels -> 24 samples r0 g0 b0 r1 ..., two per 32-bit word
+        const uint32_t yw[4] = {yv.x, yv.y, yv.z, yv.w};
+        int rgb[3][8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+            decode_rgb16(yy_term16(yuv16_code(yw[j >> 1] >> (16 * (j & 1)), k), k), ct[j >> 1], k.white, rgb[0][j], rgb[1][j], rgb[2][j]);
+        uint32_t w[12];
+#pragma unroll
+        for (int m = 0; m < 12; ++m) w[m] = (uint32_t)rgb[(2 * m) % 3][(2 * m) / 3] | ((uint32_t)rgb[(2 * m + 1) % 3][(2 * m + 1) / 3] << 16);
+        o[0] = make_uint4(w[0], w[1], w[2], w[3]);
+        o[1] = make_uint4(w[4], w[5], w[6], w[7]);
+        o[2] = make_uint4(w[8], w[9], w[10], w[11]);
+    };
+    uint4 o[3];
+    uint4* d0 = reinterpret_cast<uint4*>(out + ((size_t)(2 * cy) * width + (size_t)gx0 * 8) * 3);       // this warp's 1536-B run, top row
+    uint4* d1 = reinterpret_cast<uint4*>(out + ((size_t)(2 * cy + 1) * width + (size_t)gx0 * 8) * 3);   // bottom row
+    if (full_warp) {
+        pack(yt, o);
+        store_rgb48_coalesced(d0, stage[wid], lane, o);
+        pack(yb, o);
+        store_rgb48_coalesced(d1, stage[wid], lane, o);
+    } else if (active) {   // ragged last warp of a row: direct 48-B stores
+        pack(yt, o);
+        stg_stream_u4(d0 + 3 * lane, o[0]); stg_stream_u4(d0 + 3 * lane + 1, o[1]); stg_stream_u4(d0 + 3 * lane + 2, o[2]);
+        pack(yb, o);
+        stg_stream_u4(d1 + 3 * lane, o[0]); stg_stream_u4(d1 + 3 * lane + 1, o[1]); stg_stream_u4(d1 + 3 * lane + 2, o[2]);
+    }
+}
+
+// Generic fallback (any even width, 2-B aligned buffers): one thread per pixel.
+template <int L>
+__global__ void rgb_from_yuv420_u16_generic(const uint16_t* __restrict__ src, uint16_t* __restrict__ dst, uint32_t width,
+                                            uint32_t height, const Yuv16Coeffs k) {
+    const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= width || y >= height) return;
+    const size_t plane = (size_t)width * height;
+    const uint16_t* frame = src + (size_t)blockIdx.z * (plane * 3 / 2);
+    size_t cu, cv;
+    if (L == KB200_YUV420_I01X) {
+        cu = plane + (size_t)(y >> 1) * (width / 2) + (x >> 1);
+        cv = cu + plane / 4;
+    } else {
+        cu = plane + (size_t)(y >> 1) * width + (x & ~1u);
+        cv = cu + 1;
+    }
+    const ChromaTerms ct = chroma_terms16(yuv16_code(frame[cu], k), yuv16_code(frame[cv], k), k);
+    int r, g, b;
+    decode_rgb16(yy_term16(yuv16_code(frame[(size_t)y * width + x], k), k), ct, k.white, r, g, b);
+    uint16_t* o = dst + ((size_t)blockIdx.z * plane + (size_t)y * width + x) * 3;
+    o[0] = (uint16_t)r; o[1] = (uint16_t)g; o[2] = (uint16_t)b;
+}
+
 // ── YUYV → RGB8 ─────────────────────────────────────────────────────────────────────────────
 // One thread: 16 px = 32 B in (2 x LDG.128), 48 B out (3 x STG.128).  Flat over the whole batch
 // (rows are independent and tight), requires total px % 16 == 0 and aligned bases.
@@ -646,6 +741,38 @@ KB200_API int kb200_rgb_from_yuv420_u8_matrix(kb200_stream_t stream, const uint8
     dim3 block(32, 8), grid(div_up(width / 2, 32), div_up(height / 2, 8), batch);
     k.generic<<<grid, block, 0, s>>>(src, dst, width, height, frame, yc);
     return check_launch(k.generic_name);
+}
+
+KB200_API int kb200_rgb_from_yuv420_u16(kb200_stream_t stream, const uint16_t* src, size_t src_len, uint16_t* dst, size_t dst_len,
+                                        uint32_t width, uint32_t height, uint32_t batch, int layout, int bits, int matrix) {
+    KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
+    if (reinterpret_cast<uintptr_t>(src) & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "'src' is not 2-byte aligned (16-bit samples)");
+    if (reinterpret_cast<uintptr_t>(dst) & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "'dst' is not 2-byte aligned (16-bit samples)");
+    if (layout != KB200_YUV420_P01X && layout != KB200_YUV420_I01X) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown 16-bit 4:2:0 layout %d", layout);
+    if (bits != 10 && bits != 12) return fail(KB200_ERR_INVALID_ARGUMENT, "16-bit 4:2:0 samples are 10 or 12 bits, got %d", bits);
+    if (matrix < KB200_YUV_BT601_LIMITED || matrix > KB200_YUV_BT709_FULL) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown YUV matrix %d", matrix);
+    const bool planar = layout == KB200_YUV420_I01X;
+    const Yuv16Coeffs k = yuv16_coeffs(matrix, bits, !planar);
+    char name[8];
+    snprintf(name, sizeof name, "%c01%d", planar ? 'I' : 'P', bits - 10);
+    KB200_TRY(check_geometry(width, height, width, height, batch));
+    if ((width & 1u) || (height & 1u)) return fail(KB200_ERR_INVALID_ARGUMENT, "%s needs even dimensions, got %ux%u", name, width, height);
+    if (batch > 65535u) return fail(KB200_ERR_INVALID_ARGUMENT, "batch %u exceeds 65535", batch);
+    const size_t plane = (size_t)width * height;
+    KB200_TRY(check_slice("src", src_len, plane * 3 / 2 * batch)); KB200_TRY(check_slice("dst", dst_len, plane * 3 * batch));
+    cudaStream_t s = as_stream(stream);
+    if ((width % 8u) == 0 && aligned16(src) && aligned16(dst) && height / 2 <= 65535u) {   // w % 8 == 0, h even: every frame 16-B aligned
+        const unsigned groups = width / 8;
+        const unsigned bx = groups >= 128 ? 128 : 32 * ((groups + 31) / 32);
+        dim3 grid(div_up(groups, bx), height / 2, batch);
+        if (planar) rgb_from_yuv420_u16_vec<KB200_YUV420_I01X><<<grid, bx, 0, s>>>(src, dst, width, height, k);
+        else rgb_from_yuv420_u16_vec<KB200_YUV420_P01X><<<grid, bx, 0, s>>>(src, dst, width, height, k);
+        return check_launch(planar ? "rgb_from_i01x_vec" : "rgb_from_p01x_vec");
+    }
+    dim3 block(32, 8), grid(div_up(width, 32), div_up(height, 8), batch);
+    if (planar) rgb_from_yuv420_u16_generic<KB200_YUV420_I01X><<<grid, block, 0, s>>>(src, dst, width, height, k);
+    else rgb_from_yuv420_u16_generic<KB200_YUV420_P01X><<<grid, block, 0, s>>>(src, dst, width, height, k);
+    return check_launch(planar ? "rgb_from_i01x_generic" : "rgb_from_p01x_generic");
 }
 
 KB200_API int kb200_rgb_from_yuv422_u8_matrix(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst,

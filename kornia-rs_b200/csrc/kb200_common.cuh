@@ -181,6 +181,52 @@ __device__ __forceinline__ void decode_rgb(int yy, const ChromaTerms& t, int& r,
     r = sat_u8((yy + t.r) >> 20);
 }
 
+// Q16 decode of n-bit codes (n = 10, 12: the 16-bit-word 4:2:0 formats P010, P012, I010, I012), the Q20 decode above
+// rescaled.  With s = 2^(n-8) and W = 2^n - 1:
+//   yy = max(Y - y_off, 0) * cy,  u = U - 128*s,  v = V - 128*s
+//   R = clamp((yy + cvr*v + 2^15) >> 16, 0, W),  G = clamp((yy + cug*u + cvg*v + 2^15) >> 16, 0, W),  B = ... cub*u ...
+// y_off = 16*s for limited range, 0 for full range.  The constants are round(c * 2^16) of the exact coefficients of the
+// Q20 table's derivation, with the limited-range scales W/(219*s) for luma and W/(224*s) for chroma (1 for full range).
+// At 12 bits every term is below 5.8e8 in magnitude, so the i32 sums cannot overflow.
+// A 16-bit word holds its code in the high bits (P01x: code = word >> (16 - n)) or the low bits (I01x: word & W); the
+// other bits are ignored, which also bounds every code by W.
+static constexpr YuvCoeffs YUV16_COEFFS[2][4] = {   // [n == 12][kb200_yuv_matrix]
+    {{64, 76533, 104905, 132590, -25750, -53435},    // 10 bits: KB200_YUV_BT601_LIMITED
+     {0, 65536, 91881, 116130, -22553, -46802},      //          KB200_YUV_BT601_FULL
+     {64, 76533, 117835, 138846, -14017, -35027},    //          KB200_YUV_BT709_LIMITED
+     {0, 65536, 103206, 121609, -12276, -30679}},    //          KB200_YUV_BT709_FULL
+    {{256, 76590, 104982, 132687, -25769, -53475},   // 12 bits
+     {0, 65536, 91881, 116130, -22553, -46802},
+     {256, 76590, 117921, 138947, -14027, -35053},
+     {0, 65536, 103206, 121609, -12276, -30679}},
+};
+// One coefficient set of YUV16_COEFFS with the depth's code extraction: code = (word >> shift) & white.
+struct Yuv16Coeffs {
+    YuvCoeffs c;
+    int shift;   // 16 - n for the MSB-aligned (P01x) layout, 0 for the LSB-aligned (I01x) one
+    int white;   // W = 2^n - 1
+};
+inline Yuv16Coeffs yuv16_coeffs(int matrix, int bits, bool msb_aligned) {
+    return {YUV16_COEFFS[bits == 12][matrix], msb_aligned ? 16 - bits : 0, (1 << bits) - 1};
+}
+__device__ __forceinline__ int yuv16_code(uint32_t word, const Yuv16Coeffs& k) { return (int)((word >> k.shift) & (uint32_t)k.white); }
+__device__ __forceinline__ ChromaTerms chroma_terms16(int u, int v, const Yuv16Coeffs& k) {
+    const int half = (k.white + 1) >> 1;   // 128 * s
+    u -= half;
+    v -= half;
+    ChromaTerms t;
+    t.b = k.c.cub * u + (1 << 15);
+    t.g = k.c.cug * u + k.c.cvg * v + (1 << 15);
+    t.r = k.c.cvr * v + (1 << 15);
+    return t;
+}
+__device__ __forceinline__ int yy_term16(int y, const Yuv16Coeffs& k) { return max(y - k.c.y_off, 0) * k.c.cy; }
+__device__ __forceinline__ void decode_rgb16(int yy, const ChromaTerms& t, int white, int& r, int& g, int& b) {
+    b = min(max((yy + t.b) >> 16, 0), white);
+    g = min(max((yy + t.g) >> 16, 0), white);
+    r = min(max((yy + t.r) >> 16, 0), white);
+}
+
 #endif  // __CUDACC__
 
 }  // namespace kb200

@@ -1,6 +1,6 @@
 // preprocess.cu — the fused camera preprocess (a12; BASELINE config 3): raw frame (RGB/BGR/RGBA/
-// Gray/NV12/YUYV, tight or pitched; beyond the reference also NV21/I420/YV12/UYVY/YVYU and the 8- and 16-bit Bayer
-// mosaics) →
+// Gray/NV12/YUYV, tight or pitched; beyond the reference also NV21/I420/YV12/UYVY/YVYU, the 8- and 16-bit Bayer
+// mosaics and the 10- and 12-bit 4:2:0 video P010/P012/I010/I012) →
 // letterbox/stretch resample → (v/255 - mean) * inv_std → planar CHW f32 or f16, for a whole batch in ONE launch.
 // The 4:2:0 formats share the NV12 kernels (templated on the chroma layout); the 4:2:2 formats take the generic kernel.
 // A Bayer tap is the demosaiced pixel at the tap's coordinate (bayer.cuh); Bayer frames take the generic kernel, except
@@ -8,6 +8,9 @@
 // W = 2^bits - 1 of its format: (px / W - mean) * inv_std, px / W the IEEE quotient.
 // A YUV tap decodes with the colour matrix the fmt code carries in bits 8-9 (KB200_FMT_YUV_MATRIX): the entry points
 // strip those bits from the descriptor and hand every kernel the matrix's coefficient set (YuvCoeffs) as an argument.
+// The 10- and 12-bit 4:2:0 formats (fmt 80-83: P010, P012 in NV12's layout, I010, I012 in I420's, one 16-bit word per
+// sample) take the 4:2:0 fast kernels instantiated for 16-bit words, with the Q16 set of their matrix and depth; a tap is
+// the decoded n-bit code, normalised like a 16-bit Bayer tap by W = 2^n - 1.
 //
 // Reference: preprocess.rs:430-647 (the CUDA source string — the specification of this path; there
 // is no CPU implementation for the camera formats), launch seam :1324-1372, batch loop :1277-1280
@@ -101,9 +104,46 @@ __device__ __forceinline__ void fetch_px_yuv_ext(const uint8_t* __restrict__ src
 }
 
 // Which formats an instantiation of the generic kernel serves: the reference's (fmt 0-4), the YUV layouts beyond them
-// (fmt 5-9), the 8-bit Bayer mosaics (fmt 16-19), the 16-bit ones (fmt 32-47) or the packed ones (fmt 64-75).
-// Separate instantiations, so the kernels of fmt 0-4 are unchanged by the others.
-static constexpr int SRC_BASE = 0, SRC_EXT_YUV = 1, SRC_BAYER = 2, SRC_BAYER16 = 3, SRC_BAYER_PACKED = 4;
+// (fmt 5-9), the 8-bit Bayer mosaics (fmt 16-19), the 16-bit ones (fmt 32-47), the packed ones (fmt 64-75) or the 10- and
+// 12-bit 4:2:0 video (fmt 80-83).  Separate instantiations, so the kernels of fmt 0-4 are unchanged by the others.
+static constexpr int SRC_BASE = 0, SRC_EXT_YUV = 1, SRC_BAYER = 2, SRC_BAYER16 = 3, SRC_BAYER_PACKED = 4, SRC_YUV16 = 5;
+
+// fmt 80-83 = P010, P012 (NV12's layout, codes in the high bits of each word), I010, I012 (I420's, codes in the low bits)
+__host__ __device__ inline bool yuv16_planar(int fmt) { return fmt >= KB200_FMT_I010; }
+__host__ __device__ inline int yuv16_bits(int fmt) { return ((fmt - KB200_FMT_P010) & 1) ? 12 : 10; }
+// The generic kernel gets the matrix's Q16 set as its YuvCoeffs argument and the code extraction from the format
+__host__ __device__ inline Yuv16Coeffs yuv16_of(int fmt, const YuvCoeffs& c) {
+    return {c, yuv16_planar(fmt) ? 0 : 16 - yuv16_bits(fmt), (1 << yuv16_bits(fmt)) - 1};
+}
+
+// p / W of a 16-bit YUV tap, bit for bit the IEEE quotient __fdiv_rn(p, W) (W = 1023 or 4095), but the division never sees
+// a zero dividend: 0 / W is p itself (+0 or -0, since W > 0), so a zero p is returned as it is and 1 is divided in its
+// place.  A zero operand fails the fast-path check (FCHK) of __fdiv_rn and enters its slow-path subroutine, and decoded
+// video is full of codes clamped to 0 (blacks, out-of-gamut chroma), so without this most warps took the subroutine on
+// some lane.
+__device__ __forceinline__ float div_white(float p, float w) {
+    const bool zero = p == 0.0f;
+    const float q = __fdiv_rn(zero ? 1.0f : p, w);
+    return zero ? p : q;
+}
+
+// One decoded pixel of a P01x / I01x frame (tight, 16-bit words)
+__device__ __forceinline__ void fetch_px_yuv16(const uint16_t* __restrict__ s, int x, int y, const kb200_preprocess_desc& d,
+                                               const Yuv16Coeffs& k, float px[3]) {
+    const size_t plane = (size_t)d.src_w * d.src_h;
+    size_t cu, cv;
+    if (yuv16_planar(d.fmt)) {
+        cu = plane + (size_t)(y >> 1) * (d.src_w >> 1) + (x >> 1);
+        cv = cu + plane / 4;
+    } else {
+        cu = plane + (size_t)(y >> 1) * d.src_w + (x & ~1);
+        cv = cu + 1;
+    }
+    const ChromaTerms t = chroma_terms16(yuv16_code(s[cu], k), yuv16_code(s[cv], k), k);
+    int r, g, b;
+    decode_rgb16(yy_term16(yuv16_code(s[(size_t)y * d.src_w + x], k), k), t, k.white, r, g, b);
+    px[0] = (float)r; px[1] = (float)g; px[2] = (float)b;
+}
 
 // fmt 32-47 = 32 + 4*k + kb200_bayer_pattern, k = 0..3 for 10, 12, 14 and 16 bits per sample
 __host__ __device__ inline int bayer16_pattern(int fmt) { return (fmt - KB200_FMT_BAYER_RGGB10) & 3; }
@@ -130,6 +170,8 @@ __device__ __forceinline__ void fetch_px(const uint8_t* __restrict__ src, int x,
         px[0] = (float)rgb[0]; px[1] = (float)rgb[1]; px[2] = (float)rgb[2];
     } else if (EXT == SRC_EXT_YUV) {
         fetch_px_yuv_ext(src, x, y, d, yc, px);
+    } else if (EXT == SRC_YUV16) {
+        fetch_px_yuv16(reinterpret_cast<const uint16_t*>(src), x, y, d, yuv16_of(d.fmt, yc), px);
     } else if (d.fmt <= 1) {
         const uint8_t* p = src + (long long)y * d.src_pitch + x * d.src_bpp;
         if (d.fmt == 0) { px[0] = (float)p[0]; px[1] = (float)p[1]; px[2] = (float)p[2]; }
@@ -223,7 +265,10 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
         px[0] = d.pad_value; px[1] = d.pad_value; px[2] = d.pad_value;
     }
     float q0, q1, q2;
-    if ((EXT == SRC_BAYER16 || EXT == SRC_BAYER_PACKED) && inside) {   // px / W: taps up to 65535 and Lanczos overshoot, so the IEEE division
+    if (EXT == SRC_YUV16 && inside) {   // px / W, the IEEE quotient (div_white: no zero dividend reaches the division)
+        const float wl = (float)yuv16_of(d.fmt, yc).white;
+        q0 = div_white(px[0], wl); q1 = div_white(px[1], wl); q2 = div_white(px[2], wl);
+    } else if ((EXT == SRC_BAYER16 || EXT == SRC_BAYER_PACKED) && inside) {   // px / W: taps up to 65535 and Lanczos overshoot, so the IEEE division
         const float wl = EXT == SRC_BAYER16 ? bayer16_white(d.fmt) : bayer_packed_white(d.fmt);
         q0 = __fdiv_rn(px[0], wl); q1 = __fdiv_rn(px[1], wl); q2 = __fdiv_rn(px[2], wl);
     } else if (inside && SAMP != KB200_INTERP_LANCZOS) { q0 = div255_exact(px[0]); q1 = div255_exact(px[1]); q2 = div255_exact(px[2]); }
@@ -272,17 +317,26 @@ __device__ __forceinline__ void nv12_store4(void* __restrict__ dst, size_t idx, 
 
 __device__ __forceinline__ float norm_int_px(int r, float m, float is) { return (div255_exact((float)r) - m) * is; }
 
+// The sample type T of a 4:2:0 frame: bytes (NV12, NV21, I420, YV12), or 16-bit words holding n-bit codes — P01x in the
+// NV12 layout, I01x in the I420 layout.  Coeffs is the fast kernels' coefficient argument: the Q20 set for bytes, the Q16
+// set with its code extraction (Yuv16Coeffs) for words.
+template <typename T> struct Yuv420Sample { using Coeffs = YuvCoeffs; };
+template <> struct Yuv420Sample<uint16_t> { using Coeffs = Yuv16Coeffs; };
+
 // One thread = 4 luma columns x 2 rows.  Every warp-level access is lane-contiguous: 3 x LDG.32 (128 B per
 // warp), 6 x STG.128 (512 contiguous bytes per warp per plane row).  [The first version gave each thread 8
 // columns = two STG.128 per plane row; each store instruction then wrote only half of every 32-B sector and
 // ncu showed 2x the write sectors at L2 (lts__t_sectors_srcunit_tex_op_write).]
 // The other 4:2:0 layouts (L, kb200_yuv420_layout) take this kernel too: NV21 loads the same 4 chroma bytes and swaps
 // each pair; I420 / YV12 load 2 U bytes and 2 V bytes (LDG.16 each; w % 4 == 0 keeps them 2-B aligned).
-template <bool F16, bool PTRS, int L>
+// 16-bit words (T = uint16_t): LDG.64 of 4 Y words per row; P01x one LDG.64 of the 2 chroma pairs, I01x 2 U words and
+// 2 V words (LDG.32 each; w % 4 == 0 and even h keep them 4-B aligned in an 8-B aligned frame).  A pixel is normalised
+// as (px / W - mean) * inv_std with the IEEE division, like a 16-bit Bayer tap.
+template <bool F16, bool PTRS, int L, typename T>
 __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                          const __grid_constant__ PreFrames fr, void* __restrict__ dst,
                                                                          uint32_t frame0, uint32_t groups_per_row, uint32_t items,
-                                                                         const YuvCoeffs yc) {
+                                                                         const typename Yuv420Sample<T>::Coeffs yc) {
     const uint32_t item = blockIdx.x * blockDim.x + threadIdx.x;
     if (item >= items) return;
     const uint32_t rp = item / groups_per_row, g = item - rp * groups_per_row;
@@ -290,45 +344,85 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const _
     const uint32_t f = blockIdx.y;
     const uint8_t* src = PTRS ? fr.ptr[f] : fr.base + (size_t)(frame0 + f) * fr.stride;
     const uint32_t x = g * 4u;
-    const uint32_t y0w = __ldg(reinterpret_cast<const uint32_t*>(src + (size_t)(2u * rp) * w + x));
-    const uint32_t y1w = __ldg(reinterpret_cast<const uint32_t*>(src + (size_t)(2u * rp + 1u) * w + x));
-    ChromaTerms ct[2];
-    if (yuv420_planar(L)) {
-        const size_t c = (size_t)rp * (w / 2u) + x / 2u;
-        const uint32_t u2 = __ldg(reinterpret_cast<const unsigned short*>(src + yuv420_u_plane(L, w, h) + c));
-        const uint32_t v2 = __ldg(reinterpret_cast<const unsigned short*>(src + yuv420_v_plane(L, w, h) + c));
-        ct[0] = chroma_terms((int)(u2 & 0xFFu), (int)(v2 & 0xFFu), yc);
-        ct[1] = chroma_terms((int)(u2 >> 8), (int)(v2 >> 8), yc);
-    } else {
-        const uint32_t uvw = __ldg(reinterpret_cast<const uint32_t*>(src + (size_t)w * h + (size_t)rp * w + x));
-        if (L == YUV420_NV21) {
-            ct[0] = chroma_terms((int)((uvw >> 8) & 0xFFu), (int)(uvw & 0xFFu), yc);
-            ct[1] = chroma_terms((int)(uvw >> 24), (int)((uvw >> 16) & 0xFFu), yc);
+    if constexpr (sizeof(T) == 2) {
+        const uint16_t* s = reinterpret_cast<const uint16_t*>(src);
+        const size_t plane = (size_t)w * h;
+        const uint2 y0 = __ldg(reinterpret_cast<const uint2*>(s + (size_t)(2u * rp) * w + x));
+        const uint2 y1 = __ldg(reinterpret_cast<const uint2*>(s + (size_t)(2u * rp + 1u) * w + x));
+        ChromaTerms ct[2];
+        if (yuv420_planar(L)) {
+            const size_t c = (size_t)rp * (w / 2u) + x / 2u;
+            const uint32_t u2 = __ldg(reinterpret_cast<const uint32_t*>(s + plane + c));
+            const uint32_t v2 = __ldg(reinterpret_cast<const uint32_t*>(s + plane + plane / 4 + c));
+            ct[0] = chroma_terms16(yuv16_code(u2, yc), yuv16_code(v2, yc), yc);
+            ct[1] = chroma_terms16(yuv16_code(u2 >> 16, yc), yuv16_code(v2 >> 16, yc), yc);
         } else {
-            ct[0] = chroma_terms((int)(uvw & 0xFFu), (int)((uvw >> 8) & 0xFFu), yc);
-            ct[1] = chroma_terms((int)((uvw >> 16) & 0xFFu), (int)(uvw >> 24), yc);
+            const uint2 uv = __ldg(reinterpret_cast<const uint2*>(s + plane + (size_t)rp * w + x));
+            ct[0] = chroma_terms16(yuv16_code(uv.x, yc), yuv16_code(uv.x >> 16, yc), yc);
+            ct[1] = chroma_terms16(yuv16_code(uv.y, yc), yuv16_code(uv.y >> 16, yc), yc);
         }
-    }
-    const size_t plane = (size_t)w * h;
-    const size_t base = (size_t)(frame0 + f) * 3 * plane + (size_t)(2u * rp) * w + x;
-    const float m0 = d.mean[0], m1 = d.mean[1], m2 = d.mean[2], i0 = d.inv_std[0], i1 = d.inv_std[1], i2 = d.inv_std[2];
+        const size_t base = (size_t)(frame0 + f) * 3 * plane + (size_t)(2u * rp) * w + x;
+        const float m0 = d.mean[0], m1 = d.mean[1], m2 = d.mean[2], i0 = d.inv_std[0], i1 = d.inv_std[1], i2 = d.inv_std[2];
+        const float wl = (float)yc.white;
 #pragma unroll
-    for (int row = 0; row < 2; ++row) {
-        const uint32_t yw = row == 0 ? y0w : y1w;
-        float r4[4], g4[4], b4[4];
+        for (int row = 0; row < 2; ++row) {
+            const uint2 yw = row == 0 ? y0 : y1;
+            float r4[4], g4[4], b4[4];
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int yv = (int)((yw >> (8 * i)) & 0xFFu);
-            int r, gg, b;
-            decode_rgb(yy_term(yv, yc), ct[i >> 1], r, gg, b);
-            r4[i] = norm_int_px(r, m0, i0);
-            g4[i] = norm_int_px(gg, m1, i1);
-            b4[i] = norm_int_px(b, m2, i2);
+            for (int i = 0; i < 4; ++i) {
+                const int yv = yuv16_code((i < 2 ? yw.x : yw.y) >> (16 * (i & 1)), yc);
+                int r, gg, b;
+                decode_rgb16(yy_term16(yv, yc), ct[i >> 1], yc.white, r, gg, b);
+                r4[i] = (div_white((float)r, wl) - m0) * i0;
+                g4[i] = (div_white((float)gg, wl) - m1) * i1;
+                b4[i] = (div_white((float)b, wl) - m2) * i2;
+            }
+            const size_t o = base + (size_t)row * w;
+            nv12_store4<F16>(dst, o, r4);
+            nv12_store4<F16>(dst, o + plane, g4);
+            nv12_store4<F16>(dst, o + 2 * plane, b4);
         }
-        const size_t o = base + (size_t)row * w;
-        nv12_store4<F16>(dst, o, r4);
-        nv12_store4<F16>(dst, o + plane, g4);
-        nv12_store4<F16>(dst, o + 2 * plane, b4);
+    } else {
+        const uint32_t y0w = __ldg(reinterpret_cast<const uint32_t*>(src + (size_t)(2u * rp) * w + x));
+        const uint32_t y1w = __ldg(reinterpret_cast<const uint32_t*>(src + (size_t)(2u * rp + 1u) * w + x));
+        ChromaTerms ct[2];
+        if (yuv420_planar(L)) {
+            const size_t c = (size_t)rp * (w / 2u) + x / 2u;
+            const uint32_t u2 = __ldg(reinterpret_cast<const unsigned short*>(src + yuv420_u_plane(L, w, h) + c));
+            const uint32_t v2 = __ldg(reinterpret_cast<const unsigned short*>(src + yuv420_v_plane(L, w, h) + c));
+            ct[0] = chroma_terms((int)(u2 & 0xFFu), (int)(v2 & 0xFFu), yc);
+            ct[1] = chroma_terms((int)(u2 >> 8), (int)(v2 >> 8), yc);
+        } else {
+            const uint32_t uvw = __ldg(reinterpret_cast<const uint32_t*>(src + (size_t)w * h + (size_t)rp * w + x));
+            if (L == YUV420_NV21) {
+                ct[0] = chroma_terms((int)((uvw >> 8) & 0xFFu), (int)(uvw & 0xFFu), yc);
+                ct[1] = chroma_terms((int)(uvw >> 24), (int)((uvw >> 16) & 0xFFu), yc);
+            } else {
+                ct[0] = chroma_terms((int)(uvw & 0xFFu), (int)((uvw >> 8) & 0xFFu), yc);
+                ct[1] = chroma_terms((int)((uvw >> 16) & 0xFFu), (int)(uvw >> 24), yc);
+            }
+        }
+        const size_t plane = (size_t)w * h;
+        const size_t base = (size_t)(frame0 + f) * 3 * plane + (size_t)(2u * rp) * w + x;
+        const float m0 = d.mean[0], m1 = d.mean[1], m2 = d.mean[2], i0 = d.inv_std[0], i1 = d.inv_std[1], i2 = d.inv_std[2];
+#pragma unroll
+        for (int row = 0; row < 2; ++row) {
+            const uint32_t yw = row == 0 ? y0w : y1w;
+            float r4[4], g4[4], b4[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int yv = (int)((yw >> (8 * i)) & 0xFFu);
+                int r, gg, b;
+                decode_rgb(yy_term(yv, yc), ct[i >> 1], r, gg, b);
+                r4[i] = norm_int_px(r, m0, i0);
+                g4[i] = norm_int_px(gg, m1, i1);
+                b4[i] = norm_int_px(b, m2, i2);
+            }
+            const size_t o = base + (size_t)row * w;
+            nv12_store4<F16>(dst, o, r4);
+            nv12_store4<F16>(dst, o + plane, g4);
+            nv12_store4<F16>(dst, o + 2 * plane, b4);
+        }
     }
 }
 
@@ -446,13 +540,32 @@ __device__ __forceinline__ void yuv420_tap(const uint8_t* __restrict__ src, int 
     }
     decode_rgb(yy_term(yv, yc), t, rgb[0], rgb[1], rgb[2]);
 }
+// ... and of a frame of 16-bit words (the coefficient type selects it): P01x in the NV12 layout, I01x in the I420 layout.
+// A P01x tap reads its chroma pair as two 16-bit words, since frames are only 2-B aligned on this path.
+template <int L>
+__device__ __forceinline__ void yuv420_tap(const uint8_t* __restrict__ src, int x, int y, int w, int h, const Yuv16Coeffs& k, int rgb[3]) {
+    const uint16_t* s = reinterpret_cast<const uint16_t*>(src);
+    const size_t plane = (size_t)w * h;
+    size_t cu, cv;
+    if (yuv420_planar(L)) {
+        cu = plane + (size_t)(y >> 1) * (w >> 1) + (x >> 1);
+        cv = cu + plane / 4;
+    } else {
+        cu = plane + (size_t)(y >> 1) * w + (x & ~1);
+        cv = cu + 1;
+    }
+    const ChromaTerms t = chroma_terms16(yuv16_code(__ldg(s + cu), k), yuv16_code(__ldg(s + cv), k), k);
+    decode_rgb16(yy_term16(yuv16_code(__ldg(s + (size_t)y * w + x), k), k), t, k.white, rgb[0], rgb[1], rgb[2]);
+}
 
 static constexpr int NV12_ROWS = 8;  // destination rows per thread: the x-side of the sampler is computed once for all of them
 
-template <bool F16, bool BILINEAR, bool PTRS, int L>
+// T: the sample type (Yuv420Sample).  A pixel of 16-bit words is normalised as (px / W - mean) * inv_std with the IEEE
+// division, interpolated or not.
+template <bool F16, bool BILINEAR, bool PTRS, int L, typename T>
 __global__ void __launch_bounds__(128) preprocess_yuv420_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                 const __grid_constant__ PreFrames fr, const __grid_constant__ Nv12Args na,
-                                                                void* __restrict__ dst, uint32_t frame0, const YuvCoeffs yc) {
+                                                                void* __restrict__ dst, uint32_t frame0, const typename Yuv420Sample<T>::Coeffs yc) {
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= na.groups) return;
     const uint32_t f = blockIdx.z;
@@ -465,9 +578,16 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_kernel(const __grid_con
     float ax[4];
     bool xin[4];
     bool any_in = false;
+    // 16-bit samples: the four divisions first, so that only their quotients are live across the slow-path calls they may
+    // make (the interleaved form spilled in the f16 bilinear instantiation); the 8-bit kernels keep the interleaved form
+    [[maybe_unused]] float sx16[4];
+    if constexpr (sizeof(T) == 2) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) sx16[j] = __fdiv_rn((float)(ox0 + j) - d.pad_x, d.scale_x);
+    }
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-        const float sx = __fdiv_rn((float)(ox0 + j) - d.pad_x, d.scale_x);
+        const float sx = sizeof(T) == 2 ? sx16[j] : __fdiv_rn((float)(ox0 + j) - d.pad_x, d.scale_x);
         xin[j] = !(sx < 0.0f || sx >= (float)w);
         any_in = any_in || xin[j];
         if (BILINEAR) {
@@ -533,9 +653,16 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_kernel(const __grid_con
                         }
                     }
                 }
-                o[0][j] = (div255_exact(px[0]) - d.mean[0]) * d.inv_std[0];
-                o[1][j] = (div255_exact(px[1]) - d.mean[1]) * d.inv_std[1];
-                o[2][j] = (div255_exact(px[2]) - d.mean[2]) * d.inv_std[2];
+                if constexpr (sizeof(T) == 2) {
+                    const float wl = (float)yc.white;
+                    o[0][j] = (div_white(px[0], wl) - d.mean[0]) * d.inv_std[0];
+                    o[1][j] = (div_white(px[1], wl) - d.mean[1]) * d.inv_std[1];
+                    o[2][j] = (div_white(px[2], wl) - d.mean[2]) * d.inv_std[2];
+                } else {
+                    o[0][j] = (div255_exact(px[0]) - d.mean[0]) * d.inv_std[0];
+                    o[1][j] = (div255_exact(px[1]) - d.mean[1]) * d.inv_std[1];
+                    o[2][j] = (div255_exact(px[2]) - d.mean[2]) * d.inv_std[2];
+                }
             }
         }
         nv12_store4<F16>(dst, obase, o[0]);
@@ -558,12 +685,14 @@ static bool is_yuv422(int fmt) { return fmt == KB200_FMT_YUYV || fmt == KB200_FM
 static bool is_bayer(int fmt) { return fmt >= KB200_FMT_BAYER_RGGB && fmt <= KB200_FMT_BAYER_GBRG; }
 static bool is_bayer16(int fmt) { return fmt >= KB200_FMT_BAYER_RGGB10 && fmt <= KB200_FMT_BAYER_GBRG16; }
 static bool is_bayer_packed(int fmt) { return fmt >= KB200_FMT_BAYER_RGGB10P && fmt <= KB200_FMT_BAYER_GBRG14P; }
+static bool is_yuv16(int fmt) { return fmt >= KB200_FMT_P010 && fmt <= KB200_FMT_I012; }
 // SourceFormat names, in the validation messages
 static const char* const FMT_NAMES[10] = {"Rgb8", "Bgr8", "Gray8", "Nv12", "Yuyv", "Nv21", "I420", "Yv12", "Uyvy", "Yvyu"};
 static const char* const BAYER_NAMES[4] = {"BayerRggb", "BayerBggr", "BayerGrbg", "BayerGbrg"};
 static const char* const YUV420_UPPER[4] = {"NV12", "NV21", "I420", "YV12"};
+static const char* const YUV16_NAMES[4] = {"P010", "P012", "I010", "I012"};   // fmt 80-83
 
-static bool is_yuv(int fmt) { return yuv420_layout(fmt) >= 0 || is_yuv422(fmt); }
+static bool is_yuv(int fmt) { return yuv420_layout(fmt) >= 0 || is_yuv422(fmt) || is_yuv16(fmt); }
 
 // kb200_preprocess_desc::fmt = format code (bits 0-7) | KB200_FMT_YUV_MATRIX(m) (bits 8-9).  The entry points strip the
 // matrix once, here: every other function sees the plain code and takes the coefficient set apart.
@@ -572,10 +701,15 @@ static kb200_preprocess_desc plain_desc(const kb200_preprocess_desc& d) {
     p.fmt = d.fmt & 0xFF;
     return p;
 }
-static const YuvCoeffs& yuv_coeffs(const kb200_preprocess_desc& d) { return YUV_COEFFS[(d.fmt >> 8) & 3]; }
+// The coefficient set of a raw descriptor: the Q20 set of its matrix, or for fmt 80-83 the Q16 set of its matrix and depth
+static const YuvCoeffs& yuv_coeffs(const kb200_preprocess_desc& d) {
+    const int fmt = d.fmt & 0xFF;
+    return is_yuv16(fmt) ? YUV16_COEFFS[yuv16_bits(fmt) == 12][(d.fmt >> 8) & 3] : YUV_COEFFS[(d.fmt >> 8) & 3];
+}
 
 static size_t src_bytes(const kb200_preprocess_desc& d) {
-    const size_t chroma = yuv420_layout(d.fmt) >= 0 ? (size_t)d.src_w * d.src_h / 2 : 0;
+    // 4:2:0 chroma after the pitch * h luma bytes: w*h/2 samples, of 1 byte (fmt 3, 5-7) or 2 bytes (fmt 80-83)
+    const size_t chroma = yuv420_layout(d.fmt) >= 0 ? (size_t)d.src_w * d.src_h / 2 : is_yuv16(d.fmt) ? (size_t)d.src_w * d.src_h : 0;
     return (size_t)d.src_pitch * d.src_h + chroma;
 }
 
@@ -585,7 +719,7 @@ static int validate_desc(const kb200_preprocess_desc* dp) {
         return fail(KB200_ERR_INVALID_ARGUMENT, "image dimensions must be non-zero");
     if ((long long)dp->dst_w * dp->dst_h > 0x7FFFFFFFll) return fail(KB200_ERR_DIMS_TOO_LARGE, "dimensions exceed the 32-bit CUDA kernel index limit");  // :1336-1339
     const kb200_preprocess_desc d = plain_desc(*dp);
-    if (dp->fmt < 0 || (d.fmt > KB200_FMT_YVYU && !is_bayer(d.fmt) && !is_bayer16(d.fmt) && !is_bayer_packed(d.fmt)))
+    if (dp->fmt < 0 || (d.fmt > KB200_FMT_YVYU && !is_bayer(d.fmt) && !is_bayer16(d.fmt) && !is_bayer_packed(d.fmt) && !is_yuv16(d.fmt)))
         return fail(KB200_ERR_INVALID_ARGUMENT, "unknown source format code %d", dp->fmt);
     if (dp->fmt >> 10)
         return fail(KB200_ERR_INVALID_ARGUMENT, "source format code %d has bits set above bit 9 (bits 8-9 are the YUV matrix, 0-3)", dp->fmt);
@@ -621,7 +755,15 @@ static int validate_desc(const kb200_preprocess_desc* dp) {
             return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface for %s%dp (pitch %d < %lld bytes of a packed row)", name, bits, d.src_pitch,
                         (long long)d.src_w * bits / 8);
     }
-    const int bpp = d.fmt <= 1 ? d.src_bpp : (is_yuv422(d.fmt) || is_bayer16(d.fmt) ? 2 : 1);
+    if (is_yuv16(d.fmt)) {   // SourceFormat names: P010, P012, I010, I012
+        const char* name = YUV16_NAMES[d.fmt - KB200_FMT_P010];
+        if ((d.src_w | d.src_h) & 1)
+            return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s at %dx%d (even dimensions required)", name, d.src_w, d.src_h);
+        if ((long long)d.src_pitch != 2ll * d.src_w)
+            return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface for %s (pitch %d bytes at width %d: frames must be tightly packed, pitch == 2*width)",
+                        name, d.src_pitch, d.src_w);
+    }
+    const int bpp = d.fmt <= 1 ? d.src_bpp : (is_yuv422(d.fmt) || is_bayer16(d.fmt) || is_yuv16(d.fmt) ? 2 : 1);
     if (!is_bayer_packed(d.fmt) && (long long)d.src_pitch < (long long)d.src_w * bpp)
         return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface (need pitch >= width*channels and len >= pitch*height)");
     if (l420 >= 0 && d.src_pitch != d.src_w) return fail(KB200_ERR_INVALID_SOURCE, "%s frames must be tightly packed (pitch == width)", YUV420_UPPER[l420]);
@@ -629,18 +771,19 @@ static int validate_desc(const kb200_preprocess_desc* dp) {
     return KB200_OK;
 }
 
-// The 4:2:0 fast kernels of layout L, for one launch of <= 256 frames.
-template <bool F16, int L>
-static void launch_yuv420_fast(cudaStream_t s, bool identity, bool bil, const kb200_preprocess_desc& d, const YuvCoeffs& yc, const PreFrames& fr,
-                               bool ptrs, const Nv12Args& nv, void* dst, uint32_t f0, uint32_t nb, uint32_t id_groups, size_t id_items) {
+// The 4:2:0 fast kernels of layout L and sample type T, for one launch of <= 256 frames.
+template <bool F16, int L, typename T = uint8_t>
+static void launch_yuv420_fast(cudaStream_t s, bool identity, bool bil, const kb200_preprocess_desc& d, const typename Yuv420Sample<T>::Coeffs& yc,
+                               const PreFrames& fr, bool ptrs, const Nv12Args& nv, void* dst, uint32_t f0, uint32_t nb, uint32_t id_groups,
+                               size_t id_items) {
     if (identity) {
         dim3 grid(div_up(id_items, 128), nb);
-        if (ptrs) preprocess_yuv420_identity_kernel<F16, true, L><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
-        else preprocess_yuv420_identity_kernel<F16, false, L><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
+        if (ptrs) preprocess_yuv420_identity_kernel<F16, true, L, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
+        else preprocess_yuv420_identity_kernel<F16, false, L, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
         return;
     }
     dim3 grid(div_up(nv.groups, 128), div_up((size_t)d.dst_h, NV12_ROWS), nb);
-#define KB200_YUV420_LAUNCH(BIL, PT) preprocess_yuv420_kernel<F16, BIL, PT, L><<<grid, 128, 0, s>>>(d, fr, nv, dst, f0, yc)
+#define KB200_YUV420_LAUNCH(BIL, PT) preprocess_yuv420_kernel<F16, BIL, PT, L, T><<<grid, 128, 0, s>>>(d, fr, nv, dst, f0, yc)
     if (bil) { if (ptrs) KB200_YUV420_LAUNCH(true, true); else KB200_YUV420_LAUNCH(true, false); }
     else     { if (ptrs) KB200_YUV420_LAUNCH(false, true); else KB200_YUV420_LAUNCH(false, false); }
 #undef KB200_YUV420_LAUNCH
@@ -666,7 +809,8 @@ static void launch_generic(cudaStream_t s, dim3 grid, int sampling, const kb200_
 template <bool F16, bool PTRS>
 static void launch_generic_for(int ext, cudaStream_t s, dim3 grid, int sampling, const kb200_preprocess_desc& d, const YuvCoeffs& yc,
                                const PreFrames& fr, void* dst, uint32_t f0) {
-    if (ext == SRC_BAYER_PACKED) launch_generic<F16, PTRS, SRC_BAYER_PACKED>(s, grid, sampling, d, yc, fr, dst, f0);
+    if (ext == SRC_YUV16) launch_generic<F16, PTRS, SRC_YUV16>(s, grid, sampling, d, yc, fr, dst, f0);
+    else if (ext == SRC_BAYER_PACKED) launch_generic<F16, PTRS, SRC_BAYER_PACKED>(s, grid, sampling, d, yc, fr, dst, f0);
     else if (ext == SRC_BAYER16) launch_generic<F16, PTRS, SRC_BAYER16>(s, grid, sampling, d, yc, fr, dst, f0);
     else if (ext == SRC_BAYER) launch_generic<F16, PTRS, SRC_BAYER>(s, grid, sampling, d, yc, fr, dst, f0);
     else if (ext == SRC_EXT_YUV) launch_generic<F16, PTRS, SRC_EXT_YUV>(s, grid, sampling, d, yc, fr, dst, f0);
@@ -677,6 +821,9 @@ static void launch_generic_for(int ext, cudaStream_t s, dim3 grid, int sampling,
 static const char* const YUV420_IDENTITY_NAMES[4] = {"preprocess_nv12_identity_kernel", "preprocess_nv21_identity_kernel",
                                                      "preprocess_i420_identity_kernel", "preprocess_yv12_identity_kernel"};
 static const char* const YUV420_FAST_NAMES[4] = {"preprocess_nv12_kernel", "preprocess_nv21_kernel", "preprocess_i420_kernel", "preprocess_yv12_kernel"};
+// ... and of their 16-bit instantiations, by layout (P01x, I01x: each serves both depths)
+static const char* const YUV16_IDENTITY_NAMES[2] = {"preprocess_p01x_identity_kernel", "preprocess_i01x_identity_kernel"};
+static const char* const YUV16_FAST_NAMES[2] = {"preprocess_p01x_kernel", "preprocess_i01x_kernel"};
 // ... and of the Bayer identity kernels, by sample type (8-bit, 16-bit, packed 10-, 12- and 14-bit) and pattern
 #define KB200_BAYER_IDENTITY_NAMES(s)                                                                                   \
     {"preprocess_bayer" s "_rggb_identity_kernel", "preprocess_bayer" s "_bggr_identity_kernel", "preprocess_bayer" s "_grbg_identity_kernel", \
@@ -690,15 +837,17 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
                              const uint8_t* base, size_t stride, uint32_t batch, void* dst) {
     const int pixels = d.dst_w * d.dst_h;
     const bool bil = d.sampling == KB200_INTERP_BILINEAR, lanczos = d.sampling == KB200_INTERP_LANCZOS;
-    const int l420 = yuv420_layout(d.fmt);
+    // fmt 80-83 take the 4:2:0 fast kernels of their layout (P01x: NV12's, I01x: I420's) instantiated for 16-bit words
+    const bool yuv16 = is_yuv16(d.fmt);
+    const int l420 = yuv16 ? (yuv16_planar(d.fmt) ? YUV420_I420 : YUV420_NV12) : yuv420_layout(d.fmt);
     const bool bayer16 = is_bayer16(d.fmt), packed = is_bayer_packed(d.fmt);
     const bool bayer = bayer16 || packed || is_bayer(d.fmt);   // bayer: any Bayer mosaic
     // identity fast path: a 4:2:0 or Bayer format, scale 1, no pad, same size, 8-column vectors possible
     // (Lanczos always takes the generic kernel: its off-centre weights at integer coordinates are sinf(k*pi) != 0 exactly).
-    // A thread loads 4 samples per row, so rows and frames are aligned to that load: 4 B for 4:2:0 and 8-bit Bayer, 8 B
-    // for 16-bit Bayer, 16 B for packed Bayer.
+    // A thread loads 4 samples per row, so rows and frames are aligned to that load: 4 B for 8-bit 4:2:0 and 8-bit Bayer,
+    // 8 B for 16-bit 4:2:0 and 16-bit Bayer, 16 B for packed Bayer.
     const uint32_t row_align = packed ? BayerSample<BayerPacked<12>>::ID_ALIGN
-                                      : bayer16 ? BayerSample<uint16_t>::ID_ALIGN : BayerSample<uint8_t>::ID_ALIGN;
+                                      : (bayer16 || yuv16) ? BayerSample<uint16_t>::ID_ALIGN : BayerSample<uint8_t>::ID_ALIGN;
     bool identity = !lanczos && (l420 >= 0 || bayer) && d.scale_x == 1.0f && d.scale_y == 1.0f && d.pad_x == 0.0f && d.pad_y == 0.0f &&
                     d.dst_w == d.src_w && d.dst_h == d.src_h && (d.src_w % 4) == 0 && (d.src_pitch % row_align) == 0 && aligned16(dst);
     if (identity) {
@@ -710,7 +859,8 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
     if (id_items > 0x7FFFFFFFull) identity = false;
     // 4:2:0 general fast path: vector stores need dst_w % 4 == 0 and a 16-B (f32) / 8-B (f16) aligned destination
     const bool yuv420_fast = !lanczos && l420 >= 0 && (d.dst_w % 4) == 0 && aligned16(dst) && d.dst_h <= 65535 * NV12_ROWS;
-    const int ext = bayer16 ? SRC_BAYER16 : packed ? SRC_BAYER_PACKED : bayer ? SRC_BAYER : d.fmt >= KB200_FMT_NV21 ? SRC_EXT_YUV : SRC_BASE;
+    const int ext = yuv16 ? SRC_YUV16 : bayer16 ? SRC_BAYER16 : packed ? SRC_BAYER_PACKED : bayer ? SRC_BAYER : d.fmt >= KB200_FMT_NV21 ? SRC_EXT_YUV : SRC_BASE;
+    const Yuv16Coeffs yc16 = yuv16_of(d.fmt, yc);   // used by fmt 80-83 only
     Nv12Args nv{};
     nv.groups = (uint32_t)(d.dst_w + 3) / 4u;
     for (int c = 0; c < 3; ++c) nv.pad_norm[c] = (d.pad_value / 255.0f - d.mean[c]) * d.inv_std[c];  // BODY :610-612 on the host (f32, unfused)
@@ -738,6 +888,13 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
             else if (bayer16) launch(uint16_t{});
             else launch(uint8_t{});
             KB200_TRY(check_launch(BAYER_IDENTITY_NAMES[packed ? 2 + (bits - 10) / 2 : bayer16][pattern]));
+            continue;
+        }
+        if ((identity || yuv420_fast) && yuv16) {
+            if (l420 == YUV420_I420) launch_yuv420_fast<F16, YUV420_I420, uint16_t>(s, identity, bil, d, yc16, fr, p, nv, dst, f0, nb, id_groups, id_items);
+            else launch_yuv420_fast<F16, YUV420_NV12, uint16_t>(s, identity, bil, d, yc16, fr, p, nv, dst, f0, nb, id_groups, id_items);
+            const int k = l420 == YUV420_I420;
+            KB200_TRY(check_launch(identity ? YUV16_IDENTITY_NAMES[k] : YUV16_FAST_NAMES[k]));
             continue;
         }
         if (identity || yuv420_fast) {
@@ -777,15 +934,17 @@ static int preprocess_entry(kb200_stream_t stream, const kb200_preprocess_desc* 
     KB200_TRY(check_ptr("dst", dst));
     if (batch == 0) return fail(KB200_ERR_INVALID_ARGUMENT, "batch must be non-zero");
     const size_t need = src_bytes(*desc);
-    const bool bayer16 = is_bayer16(desc->fmt);   // 16-bit samples: every frame must start 2-byte aligned
-    if (bayer16 && !frames && ((reinterpret_cast<uintptr_t>(base) & 1u) || (batch > 1 && (stride & 1u))))
-        return fail(KB200_ERR_INVALID_SOURCE, "%s%d frames must start 2-byte aligned (base %p, stride %zu)", BAYER_NAMES[bayer16_pattern(desc->fmt)],
-                    bayer16_bits(desc->fmt), (const void*)base, stride);
+    // 16-bit samples (fmt 32-47, 80-83): every frame must start 2-byte aligned.  `words` names the format in the messages.
+    char words[16] = "";
+    if (is_bayer16(desc->fmt)) snprintf(words, sizeof words, "%s%d", BAYER_NAMES[bayer16_pattern(desc->fmt)], bayer16_bits(desc->fmt));
+    else if (is_yuv16(desc->fmt)) snprintf(words, sizeof words, "%s", YUV16_NAMES[desc->fmt - KB200_FMT_P010]);
+    if (words[0] && !frames && ((reinterpret_cast<uintptr_t>(base) & 1u) || (batch > 1 && (stride & 1u))))
+        return fail(KB200_ERR_INVALID_SOURCE, "%s frames must start 2-byte aligned (base %p, stride %zu)", words, (const void*)base, stride);
     if (frames) {
         for (uint32_t i = 0; i < batch; ++i) {
             if (!frames[i]) return fail(KB200_ERR_INVALID_ARGUMENT, "null frame pointer at index %u", i);
-            if (bayer16 && (reinterpret_cast<uintptr_t>(frames[i]) & 1u))
-                return fail(KB200_ERR_INVALID_SOURCE, "%s%d frame %u is not 2-byte aligned", BAYER_NAMES[bayer16_pattern(desc->fmt)], bayer16_bits(desc->fmt), i);
+            if (words[0] && (reinterpret_cast<uintptr_t>(frames[i]) & 1u))
+                return fail(KB200_ERR_INVALID_SOURCE, "%s frame %u is not 2-byte aligned", words, i);
             if (frame_len && frame_len[i] < need)  // InvalidRawSource{got,need}, preprocess.rs:1287-1300
                 return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source at %dx%d (got %zu bytes, need %zu)", desc->src_w, desc->src_h, frame_len[i], need);
         }

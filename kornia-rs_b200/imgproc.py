@@ -600,6 +600,38 @@ def rgb_from_yvyu(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -
     _rgb_from_yuv(src, dst, "rgb_from_yvyu", 2, 1, "kb200_rgb_from_yuv422_u8_matrix", YUV422_YVYU, int(YuvMatrix(matrix)))
 
 
+YUV420_P01X, YUV420_I01X = 0, 1   # kb200_yuv420_u16_layout
+
+
+def _rgb_from_yuv16(src, dst: Image, what: str, layout: int, bits: int, matrix: YuvMatrix) -> None:
+    _rgb_from_yuv(src, dst, what, 3, 2, "kb200_rgb_from_yuv420_u16", layout, bits, int(YuvMatrix(matrix)), dtype=torch.uint16)
+
+
+def rgb_from_p010(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -> None:
+    """10-bit 4:2:0 video in P010 (HEVC Main10 / AV1 10-bit from NVDEC, VA-API, V4L2) -> RGB with 16-bit channels holding
+    10-bit codes 0..1023.  `src`: uint16 device tensor holding N tight frames of w*h*3/2 little-endian words: the Y plane,
+    then h/2 rows of w/2 interleaved (U, V) pairs, each code in the high 10 bits of its word (the low 6 bits are ignored);
+    `dst`: a uint16 Image [N, h, w, 3].  `matrix`: as for rgb_from_nv12, decoded by the Q16 arithmetic of
+    include/kornia_b200.h."""
+    _rgb_from_yuv16(src, dst, "rgb_from_p010", YUV420_P01X, 10, matrix)
+
+
+def rgb_from_p012(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -> None:
+    """Like rgb_from_p010 for 12-bit content (P012, the code in the high 12 bits of each word): codes 0..4095."""
+    _rgb_from_yuv16(src, dst, "rgb_from_p012", YUV420_P01X, 12, matrix)
+
+
+def rgb_from_i010(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -> None:
+    """Like rgb_from_p010 for I010 (libavcodec's yuv420p10le): after the Y plane a (w/2 x h/2) U plane, then a V plane, each
+    code in the low 10 bits of its word (the high 6 bits are ignored)."""
+    _rgb_from_yuv16(src, dst, "rgb_from_i010", YUV420_I01X, 10, matrix)
+
+
+def rgb_from_i012(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -> None:
+    """Like rgb_from_i010 for I012 (yuv420p12le, codes in the low 12 bits): codes 0..4095."""
+    _rgb_from_yuv16(src, dst, "rgb_from_i012", YUV420_I01X, 12, matrix)
+
+
 class BayerPattern(enum.IntEnum):
     """kb200_bayer_pattern: the 2x2 quad of a Bayer mosaic read row-major (RGGB: the top-left pixel is R).  OpenCV names
     the same patterns by another pair of the quad: RGGB = COLOR_BayerBG2RGB, BGGR = COLOR_BayerRG2RGB,

@@ -2,7 +2,8 @@
 
 Built once via `Preprocessor.builder()…build_cuda()`, then applied to any number of frames of any
 resolution: the target H/W is read from the destination tensor each call.  Camera formats
-(NV12 / YUYV / Gray, the other YUV layouts and the 8- to 16-bit Bayer mosaics, unpacked or MIPI-packed) go through `run_raw*`; colour decode is fused into the resample taps.  Unlike the
+(NV12 / YUYV / Gray, the other YUV layouts, the 10- and 12-bit 4:2:0 video P010 / P012 / I010 / I012 and the 8- to
+16-bit Bayer mosaics, unpacked or MIPI-packed) go through `run_raw*`; colour decode is fused into the resample taps.  Unlike the
 reference (one launch per frame, preprocess.rs:1277-1280) a batch is ONE launch.
 
 Only the CUDA preprocessor exists here (`build()` = the reference's CPU preprocessor is out of scope:
@@ -97,6 +98,14 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
     BayerBggr14p = "bayer_bggr14p"
     BayerGrbg14p = "bayer_grbg14p"
     BayerGbrg14p = "bayer_gbrg14p"
+    # 10- and 12-bit 4:2:0 video: tight frames of w*h*3/2 little-endian 16-bit words (3*w*h bytes), w and h even.  P010 /
+    # P012 (NVDEC, VA-API and V4L2 output of HEVC Main10, AV1 10-bit) are Nv12's layout with each code in the high bits of
+    # its word; I010 / I012 (libavcodec's yuv420p10le / yuv420p12le) are I420's with each code in the low bits.  A tap is
+    # the decoded n-bit RGB code normalised by W = 2^n - 1, (px / W - mean) * inv_std; pad_value stays 0..255.
+    P010 = "p010"
+    P012 = "p012"
+    I010 = "i010"
+    I012 = "i012"
 
     def fmt_code(self) -> int:  # :153-161
         if self.is_bayer16():   # 32 + 4*k + pattern, k = 0..3 for 10, 12, 14, 16 bits
@@ -105,11 +114,12 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
             return 64 + 4 * ((self.bit_depth() - 10) // 2) + _BAYER_PATTERNS.index(self.value[6:10])
         return {"rgb8": 0, "rgba8": 0, "bgr8": 1, "bgra8": 1, "gray8": 2, "nv12": 3, "yuyv": 4,
                 "nv21": 5, "i420": 6, "yv12": 7, "uyvy": 8, "yvyu": 9,
-                "bayer_rggb": 16, "bayer_bggr": 17, "bayer_grbg": 18, "bayer_gbrg": 19}[self.value]
+                "bayer_rggb": 16, "bayer_bggr": 17, "bayer_grbg": 18, "bayer_gbrg": 19,
+                "p010": 80, "p012": 81, "i010": 82, "i012": 83}[self.value]
 
     def bpp(self) -> int:  # :164-171
         """Bytes per sample; 1 for the packed Bayer formats, whose rows pitch() counts."""
-        if self.is_bayer16():
+        if self.is_bayer16() or self.is_yuv16():
             return 2
         if self.is_bayer_packed():
             return 1
@@ -124,14 +134,19 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
         return w * self.bpp()
 
     def is_yuv420(self) -> bool:
+        """An 8-bit 4:2:0 format (one byte per sample); is_yuv16() names the 16-bit-word ones."""
         return self in (SourceFormat.Nv12, SourceFormat.Nv21, SourceFormat.I420, SourceFormat.Yv12)
+
+    def is_yuv16(self) -> bool:
+        """A 10- or 12-bit 4:2:0 format of 16-bit words: P010, P012, I010, I012."""
+        return self in (SourceFormat.P010, SourceFormat.P012, SourceFormat.I010, SourceFormat.I012)
 
     def is_yuv422(self) -> bool:
         return self in (SourceFormat.Yuyv, SourceFormat.Uyvy, SourceFormat.Yvyu)
 
     def is_yuv(self) -> bool:
         """A YUV format: one a YuvMatrix applies to."""
-        return self.is_yuv420() or self.is_yuv422()
+        return self.is_yuv420() or self.is_yuv422() or self.is_yuv16()
 
     def is_bayer(self) -> bool:
         return self.value.startswith("bayer_")
@@ -145,7 +160,10 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
         return self.is_bayer() and self.value.endswith("p")
 
     def bit_depth(self) -> int | None:
-        """Bits per sample of a Bayer format (8 for the byte mosaics), None for the other formats."""
+        """Bits per sample of a Bayer format (8 for the byte mosaics) or of a 16-bit-word 4:2:0 format (10, 12), None for
+        the other formats."""
+        if self.is_yuv16():
+            return int(self.value[2:])
         if not self.is_bayer():
             return None
         if self.is_bayer_packed():
@@ -153,11 +171,12 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
         return int(self.value[10:]) if self.is_bayer16() else 8
 
     def buffer_len(self, w: int, h: int) -> int:  # :177-186
-        chroma = w * h // 2 if self.is_yuv420() else 0
+        # 4:2:0 chroma after the luma rows: w*h/2 samples, of 1 byte (is_yuv420) or 2 bytes (is_yuv16)
+        chroma = w * h // 2 if self.is_yuv420() else w * h if self.is_yuv16() else 0
         return self.pitch(w) * h + chroma
 
     def dims_ok(self, w: int, h: int) -> bool:  # :188-195
-        if self.is_yuv420():
+        if self.is_yuv420() or self.is_yuv16():
             return w % 2 == 0 and h % 2 == 0
         if self.is_yuv422():
             return w % 2 == 0
@@ -178,6 +197,8 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
                  "bayer_rggb": "BayerRggb", "bayer_bggr": "BayerBggr", "bayer_grbg": "BayerGrbg", "bayer_gbrg": "BayerGbrg"}
         table.update({f"bayer_{p}{b}": f"Bayer{p.capitalize()}{b}" for p in _BAYER_PATTERNS for b in (10, 12, 14, 16)})
         table.update({f"bayer_{p}{b}p": f"Bayer{p.capitalize()}{b}p" for p in _BAYER_PATTERNS for b in (10, 12, 14)})
+        table.update({"p010": "P010", "p012": "P012", "i010": "I010", "i012": "I012", "p010le": "P010", "p012le": "P012",
+                      "yuv420p10le": "I010", "yuv420p12le": "I012"})
         key = table.get(name.lower())
         return None if key is None else SourceFormat[key]
 
@@ -450,7 +471,8 @@ class Preprocessor:
                      f16: bool = False, pipeline=None) -> torch.Tensor:
         """HOST camera frames in, HOST tensor out — what the reference's Python `Preprocessor` does around its kernel (pinned
         staging, upload, launch: kornia-py/src/cuda_ext/mod.rs:700-760), as one call: `host_frames` is a [N, frame_bytes] uint8
-        host tensor, or [N, w*h] uint16 for the 16-bit Bayer formats (page-locked for overlap), the result a [N,3,H,W] f32 / f16 host tensor (pinned when allocated here).
+        host tensor, or [N, w*h] uint16 for the 16-bit Bayer formats and [N, w*h*3/2] uint16 for P010 / P012 / I010 / I012 (page-locked
+        for overlap), the result a [N,3,H,W] f32 / f16 host tensor (pinned when allocated here).
         Chunks ride a `HostPipeline` ring: upload -> ONE fused launch per chunk -> download.  Enqueue-only: synchronise the
         current stream of the pipeline's device before reading the result."""
         from . import imgproc
@@ -482,7 +504,7 @@ class Preprocessor:
     def run_raw_strided(self, base: torch.Tensor, frame_stride: int, batch: int, src_w: int, src_h: int,
                         dst: torch.Tensor, f16: bool = False) -> None:
         """Frames at `base + i*frame_stride` bytes (a capture ring buffer): no pointer table.  `base` may be uint8 or, for
-        the 16-bit Bayer formats, uint16: its length is counted in bytes."""
+        the formats of 16-bit samples (16-bit Bayer, P010 / P012 / I010 / I012), uint16: its length is counted in bytes."""
         self._validate_dst(dst, batch, f16)
         fmt = self._fmt
         nbytes = base.numel() * base.element_size()
