@@ -316,13 +316,8 @@ __global__ void rgb_from_yuv420_u16_generic(const uint16_t* __restrict__ src, ui
 
 // ── YUYV → RGB8 ─────────────────────────────────────────────────────────────────────────────
 // One thread: 16 px = 32 B in (2 x LDG.128), 48 B out (3 x STG.128).  Flat over the whole batch
-// (rows are independent and tight), requires total px % 16 == 0 and aligned bases.
-// 4:2:2 layouts (kb200_yuv422_layout): each 2-px group is one 32-bit word; Yuv422Bytes<L> gives the byte of Y0, Y1,
-// U and V in it.  YUYV = Y0 U Y1 V, UYVY = U Y0 V Y1, YVYU = Y0 V Y1 U.
-static constexpr int YUV422_YUYV = KB200_YUV422_YUYV, YUV422_UYVY = KB200_YUV422_UYVY, YUV422_YVYU = KB200_YUV422_YVYU;
-template <int L> struct Yuv422Bytes { static constexpr int y0 = 0, y1 = 2, u = 1, v = 3; };
-template <> struct Yuv422Bytes<YUV422_UYVY> { static constexpr int y0 = 1, y1 = 3, u = 0, v = 2; };
-template <> struct Yuv422Bytes<YUV422_YVYU> { static constexpr int y0 = 0, y1 = 2, u = 3, v = 1; };
+// (rows are independent and tight), requires total px % 16 == 0 and aligned bases.  The byte places of the 4:2:2
+// layouts are Yuv422Bytes<L> (kb200_common.cuh).
 
 template <int L>
 __device__ __forceinline__ void yuv422_decode16(const uint4& A, const uint4& B, const YuvCoeffs& yc, uint4 o[3]) {

@@ -94,6 +94,13 @@ __host__ __device__ constexpr bool yuv420_planar(int L) { return L == YUV420_I42
 __host__ __device__ inline size_t yuv420_u_plane(int L, size_t w, size_t h) { return L == YUV420_I420 ? w * h : w * h + w * h / 4; }
 __host__ __device__ inline size_t yuv420_v_plane(int L, size_t w, size_t h) { return L == YUV420_I420 ? w * h + w * h / 4 : w * h; }
 
+// 4:2:2 layouts (kb200_yuv422_layout): each 2-px group is one 32-bit word; Yuv422Bytes<L> gives the byte of Y0, Y1,
+// U and V in it.  YUYV = Y0 U Y1 V, UYVY = U Y0 V Y1, YVYU = Y0 V Y1 U.
+static constexpr int YUV422_YUYV = KB200_YUV422_YUYV, YUV422_UYVY = KB200_YUV422_UYVY, YUV422_YVYU = KB200_YUV422_YVYU;
+template <int L> struct Yuv422Bytes { static constexpr int y0 = 0, y1 = 2, u = 1, v = 3; };
+template <> struct Yuv422Bytes<YUV422_UYVY> { static constexpr int y0 = 1, y1 = 3, u = 0, v = 2; };
+template <> struct Yuv422Bytes<YUV422_YVYU> { static constexpr int y0 = 0, y1 = 2, u = 3, v = 1; };
+
 // Streaming (read-once / write-once) vector accesses: keep L1 for the gather taps.
 __device__ __forceinline__ float4 ldg_stream_f4(const float4* p) {
     float4 v;

@@ -26,6 +26,7 @@
 // integer scales (1080p NV12 → 1080p CHW, config 3a) that removes 3 of the 4 decodes per pixel.
 #include <cuda_fp16.h>
 
+#include <cctype>
 #include <type_traits>
 
 #include "bayer.cuh"
@@ -76,45 +77,22 @@ __device__ __forceinline__ float div255_exact(float p) {
     return fmaf(e, c, q);
 }
 
-__device__ __forceinline__ void yuv_to_rgbf(int yv, int u, int v, const YuvCoeffs& yc, float px[3]) {  // :501-508
-    const ChromaTerms t = chroma_terms(u, v, yc);
-    int r, g, b;
-    decode_rgb(yy_term(yv, yc), t, r, g, b);
-    px[0] = (float)r; px[1] = (float)g; px[2] = (float)b;
-}
-
-// fmt 5-9, the YUV layouts beyond the reference's SourceFormat: the chroma addressing of the standalone decoders (color.cu)
-__device__ __forceinline__ void fetch_px_yuv_ext(const uint8_t* __restrict__ src, int x, int y, const kb200_preprocess_desc& d,
-                                                 const YuvCoeffs& yc, float px[3]) {
-    if (d.fmt == KB200_FMT_UYVY || d.fmt == KB200_FMT_YVYU) {
-        const uint8_t* grp = src + (long long)y * d.src_pitch + (x >> 1) * 4;
-        if (d.fmt == KB200_FMT_UYVY) yuv_to_rgbf(grp[(x & 1) ? 3 : 1], grp[0], grp[2], yc, px);   // U Y0 V Y1
-        else yuv_to_rgbf(grp[(x & 1) ? 2 : 0], grp[3], grp[1], yc, px);                           // Y0 V Y1 U
-        return;
-    }
-    const int yv = src[(long long)y * d.src_w + x];
-    if (d.fmt == KB200_FMT_NV21) {
-        const uint8_t* vu = src + (long long)d.src_w * d.src_h + (long long)(y >> 1) * d.src_w + (x >> 1) * 2;
-        yuv_to_rgbf(yv, vu[1], vu[0], yc, px);
-    } else {
-        const int L = d.fmt == KB200_FMT_I420 ? YUV420_I420 : YUV420_YV12;
-        const size_t c = (size_t)(y >> 1) * (d.src_w >> 1) + (x >> 1);
-        yuv_to_rgbf(yv, src[yuv420_u_plane(L, d.src_w, d.src_h) + c], src[yuv420_v_plane(L, d.src_w, d.src_h) + c], yc, px);
-    }
-}
-
-// Which formats an instantiation of the generic kernel serves: the reference's (fmt 0-4), the YUV layouts beyond them
-// (fmt 5-9), the 8-bit Bayer mosaics (fmt 16-19), the 16-bit ones (fmt 32-47), the packed ones (fmt 64-75) or the 10- and
-// 12-bit 4:2:0 video (fmt 80-83).  Separate instantiations, so the kernels of fmt 0-4 are unchanged by the others.
-static constexpr int SRC_BASE = 0, SRC_EXT_YUV = 1, SRC_BAYER = 2, SRC_BAYER16 = 3, SRC_BAYER_PACKED = 4, SRC_YUV16 = 5;
-
-// fmt 80-83 = P010, P012 (NV12's layout, codes in the high bits of each word), I010, I012 (I420's, codes in the low bits)
-__host__ __device__ inline bool yuv16_planar(int fmt) { return fmt >= KB200_FMT_I010; }
-__host__ __device__ inline int yuv16_bits(int fmt) { return ((fmt - KB200_FMT_P010) & 1) ? 12 : 10; }
-// The generic kernel gets the matrix's Q16 set as its YuvCoeffs argument and the code extraction from the format
-__host__ __device__ inline Yuv16Coeffs yuv16_of(int fmt, const YuvCoeffs& c) {
-    return {c, yuv16_planar(fmt) ? 0 : 16 - yuv16_bits(fmt), (1 << yuv16_bits(fmt)) - 1};
-}
+// The facts of one source format code (kb200_src_fmt without the matrix bits), from SRC_FORMATS below.  Every host
+// function reads them from here; the generic kernel takes its format's as an argument.
+enum SrcFamily { SRC_NONE, SRC_RGB, SRC_GRAY, SRC_YUV420, SRC_YUV422, SRC_BAYER };
+struct SrcFormat {
+    int code = -1;
+    const char* name = nullptr;   // the SourceFormat name in messages; nullptr: the code is not a format
+    SrcFamily family = SRC_NONE;
+    int layout = 0;    // SRC_RGB: 0 RGB, 1 BGR order; SRC_YUV420: kb200_yuv420_layout (P01x NV12's, I01x I420's); SRC_YUV422: kb200_yuv422_layout
+    int pattern = 0;   // SRC_BAYER: kb200_bayer_pattern
+    int bits = 8;      // bits per sample
+    bool words = false;    // one little-endian 16-bit word per sample
+    bool packed = false;   // MIPI CSI-2 packed samples (bits / 8 bytes each)
+    const char* identity_kernel = nullptr;   // kb200_last_kernel() names of the format's fast kernels, nullptr: none
+    const char* fast_kernel = nullptr;
+    __host__ __device__ float white() const { return (float)((1u << bits) - 1u); }   // the white level W = 2^bits - 1
+};
 
 // p / W of a 16-bit YUV tap, bit for bit the IEEE quotient __fdiv_rn(p, W) (W = 1023 or 4095), but the division never sees
 // a zero dividend: 0 / W is p itself (+0 or -0, since W > 0), so a zero p is returned as it is and 1 is divided in its
@@ -127,67 +105,93 @@ __device__ __forceinline__ float div_white(float p, float w) {
     return zero ? p : q;
 }
 
-// One decoded pixel of a P01x / I01x frame (tight, 16-bit words)
-__device__ __forceinline__ void fetch_px_yuv16(const uint16_t* __restrict__ s, int x, int y, const kb200_preprocess_desc& d,
-                                               const Yuv16Coeffs& k, float px[3]) {
-    const size_t plane = (size_t)d.src_w * d.src_h;
+// One decoded tap of a 4:2:0 frame in layout L (kb200_yuv420_layout): the generic kernel and preprocess_yuv420_kernel
+// serve all four layouts through it.  PAIR: an interleaved chroma pair is read as one 16-bit word, which needs a 2-B
+// aligned frame (the fast kernel's); the generic kernel reads its two bytes, so it takes frames at any address.
+template <int L, bool PAIR = true>
+__device__ __forceinline__ void yuv420_tap(const uint8_t* __restrict__ src, int x, int y, int w, int h, const YuvCoeffs& yc, int rgb[3]) {
+    const int yv = __ldg(src + (size_t)y * w + x);
+    ChromaTerms t;
+    if (yuv420_planar(L)) {
+        const size_t c = (size_t)(y >> 1) * (w >> 1) + (x >> 1);
+        t = chroma_terms(__ldg(src + yuv420_u_plane(L, w, h) + c), __ldg(src + yuv420_v_plane(L, w, h) + c), yc);
+    } else {
+        const uint8_t* p = src + (size_t)w * h + (size_t)(y >> 1) * w + (x >> 1) * 2;
+        uint32_t uv;
+        if constexpr (PAIR) uv = __ldg(reinterpret_cast<const unsigned short*>(p));
+        else uv = __ldg(p) | (uint32_t)__ldg(p + 1) << 8;
+        t = L == YUV420_NV21 ? chroma_terms((int)(uv >> 8), (int)(uv & 0xFFu), yc) : chroma_terms((int)(uv & 0xFFu), (int)(uv >> 8), yc);
+    }
+    decode_rgb(yy_term(yv, yc), t, rgb[0], rgb[1], rgb[2]);
+}
+// ... and of a frame of 16-bit words (the coefficient type selects it): P01x in the NV12 layout, I01x in the I420 layout.
+// A P01x tap reads its chroma pair as two 16-bit words, since frames are only 2-B aligned.
+template <int L>
+__device__ __forceinline__ void yuv420_tap(const uint8_t* __restrict__ src, int x, int y, int w, int h, const Yuv16Coeffs& k, int rgb[3]) {
+    const uint16_t* s = reinterpret_cast<const uint16_t*>(src);
+    const size_t plane = (size_t)w * h;
     size_t cu, cv;
-    if (yuv16_planar(d.fmt)) {
-        cu = plane + (size_t)(y >> 1) * (d.src_w >> 1) + (x >> 1);
+    if (yuv420_planar(L)) {
+        cu = plane + (size_t)(y >> 1) * (w >> 1) + (x >> 1);
         cv = cu + plane / 4;
     } else {
-        cu = plane + (size_t)(y >> 1) * d.src_w + (x & ~1);
+        cu = plane + (size_t)(y >> 1) * w + (x & ~1);
         cv = cu + 1;
     }
-    const ChromaTerms t = chroma_terms16(yuv16_code(s[cu], k), yuv16_code(s[cv], k), k);
-    int r, g, b;
-    decode_rgb16(yy_term16(yuv16_code(s[(size_t)y * d.src_w + x], k), k), t, k.white, r, g, b);
-    px[0] = (float)r; px[1] = (float)g; px[2] = (float)b;
+    const ChromaTerms t = chroma_terms16(yuv16_code(__ldg(s + cu), k), yuv16_code(__ldg(s + cv), k), k);
+    decode_rgb16(yy_term16(yuv16_code(__ldg(s + (size_t)y * w + x), k), k), t, k.white, rgb[0], rgb[1], rgb[2]);
 }
 
-// fmt 32-47 = 32 + 4*k + kb200_bayer_pattern, k = 0..3 for 10, 12, 14 and 16 bits per sample
-__host__ __device__ inline int bayer16_pattern(int fmt) { return (fmt - KB200_FMT_BAYER_RGGB10) & 3; }
-__host__ __device__ inline int bayer16_bits(int fmt) { return 10 + 2 * ((fmt - KB200_FMT_BAYER_RGGB10) >> 2); }
-__host__ __device__ inline float bayer16_white(int fmt) { return (float)((1u << bayer16_bits(fmt)) - 1u); }
-// fmt 64-75 = 64 + 4*k + kb200_bayer_pattern, k = 0..2 for 10, 12 and 14 bits per packed sample
-__host__ __device__ inline int bayer_packed_pattern(int fmt) { return (fmt - KB200_FMT_BAYER_RGGB10P) & 3; }
-__host__ __device__ inline int bayer_packed_bits(int fmt) { return 10 + 2 * ((fmt - KB200_FMT_BAYER_RGGB10P) >> 2); }
-__host__ __device__ inline float bayer_packed_white(int fmt) { return (float)((1u << bayer_packed_bits(fmt)) - 1u); }
-// kb200_bayer_pattern of a Bayer format: fmt 16-19 (8-bit samples) = 16 + pattern, fmt 32-47 (16-bit) as above
-__host__ __device__ inline int bayer_pattern(int fmt, bool bayer16) { return bayer16 ? bayer16_pattern(fmt) : fmt - KB200_FMT_BAYER_RGGB; }
+// One decoded tap of a 4:2:2 frame in layout L (kb200_yuv422_layout): the pixel's 2-px group at its byte places.
+template <int L>
+__device__ __forceinline__ void yuv422_tap(const uint8_t* __restrict__ src, int x, int y, int pitch, const YuvCoeffs& yc, int rgb[3]) {
+    using P = Yuv422Bytes<L>;
+    const uint8_t* grp = src + (long long)y * pitch + (x >> 1) * 4;
+    const ChromaTerms t = chroma_terms(grp[P::u], grp[P::v], yc);
+    decode_rgb(yy_term(grp[(x & 1) ? P::y1 : P::y0], yc), t, rgb[0], rgb[1], rgb[2]);
+}
 
-template <int EXT>
-__device__ __forceinline__ void fetch_px(const uint8_t* __restrict__ src, int x, int y, const kb200_preprocess_desc& d,
-                                         const YuvCoeffs& yc, float px[3]) {  // :510-530
-    if (EXT == SRC_BAYER || EXT == SRC_BAYER16) {   // src_pitch is in bytes (even for 16-bit samples)
-        using T = std::conditional_t<EXT == SRC_BAYER16, uint16_t, uint8_t>;
-        int rgb[3];
-        bayer_px(reinterpret_cast<const T*>(src), (size_t)d.src_pitch / sizeof(T), d.src_w, d.src_h, x, y, bayer_pattern(d.fmt, EXT == SRC_BAYER16), rgb);
-        px[0] = (float)rgb[0]; px[1] = (float)rgb[1]; px[2] = (float)rgb[2];
-    } else if (EXT == SRC_BAYER_PACKED) {
-        int rgb[3];
-        bayer_px_packed(src, (size_t)d.src_pitch, d.src_w, d.src_h, x, y, bayer_packed_pattern(d.fmt), bayer_packed_bits(d.fmt), rgb);
-        px[0] = (float)rgb[0]; px[1] = (float)rgb[1]; px[2] = (float)rgb[2];
-    } else if (EXT == SRC_EXT_YUV) {
-        fetch_px_yuv_ext(src, x, y, d, yc, px);
-    } else if (EXT == SRC_YUV16) {
-        fetch_px_yuv16(reinterpret_cast<const uint16_t*>(src), x, y, d, yuv16_of(d.fmt, yc), px);
-    } else if (d.fmt <= 1) {
+// The taps an instantiation of the generic kernel reads: interleaved RGB / BGR or gray bytes, 4:2:2, the 16-bit words of
+// P01x / I01x, a Bayer mosaic of bytes, 16-bit words or packed samples, or 8-bit 4:2:0 in one layout (TAP_YUV420 +
+// kb200_yuv420_layout).  Within a kind the format's layout is a uniform branch.  The 4:2:0 layouts get an instantiation
+// each: with the four taps in one kernel, its Lanczos loop no longer unrolls and spills.  TapCoeffs: the coefficient
+// argument, the Q16 set with its code extraction for the 16-bit words (as in the fast kernels), the Q20 set otherwise.
+static constexpr int TAP_RGB = 0, TAP_YUV422 = 1, TAP_YUV16 = 2, TAP_BAYER = 3, TAP_BAYER16 = 4, TAP_BAYER_PACKED = 5, TAP_YUV420 = 6;
+template <int TAP> using TapCoeffs = std::conditional_t<TAP == TAP_YUV16, Yuv16Coeffs, YuvCoeffs>;
+
+template <int TAP>
+__device__ __forceinline__ void fetch_px(const uint8_t* __restrict__ src, int x, int y, const kb200_preprocess_desc& d, const SrcFormat& f,
+                                         const TapCoeffs<TAP>& yc, float px[3]) {  // :510-530
+    if constexpr (TAP == TAP_RGB) {
+        if (f.family == SRC_GRAY) {
+            const float v = (float)src[(long long)y * d.src_pitch + x];
+            px[0] = v; px[1] = v; px[2] = v;
+            return;
+        }
         const uint8_t* p = src + (long long)y * d.src_pitch + x * d.src_bpp;
-        if (d.fmt == 0) { px[0] = (float)p[0]; px[1] = (float)p[1]; px[2] = (float)p[2]; }
+        if (f.layout == 0) { px[0] = (float)p[0]; px[1] = (float)p[1]; px[2] = (float)p[2]; }
         else { px[0] = (float)p[2]; px[1] = (float)p[1]; px[2] = (float)p[0]; }
-    } else if (d.fmt == 2) {
-        const float v = (float)src[(long long)y * d.src_pitch + x];
-        px[0] = v; px[1] = v; px[2] = v;
-    } else if (d.fmt == 3) {
-        const int yv = src[(long long)y * d.src_w + x];
-        const uint8_t* uv = src + (long long)d.src_w * d.src_h + (long long)(y >> 1) * d.src_w + (x >> 1) * 2;
-        yuv_to_rgbf(yv, uv[0], uv[1], yc, px);
-    } else {
-        const uint8_t* grp = src + (long long)y * d.src_pitch + (x >> 1) * 4;
-        const int yv = grp[(x & 1) ? 2 : 0];
-        yuv_to_rgbf(yv, grp[1], grp[3], yc, px);
+        return;
     }
+    int rgb[3];
+    if constexpr (TAP == TAP_BAYER || TAP == TAP_BAYER16) {   // src_pitch is in bytes (even for 16-bit samples)
+        using T = std::conditional_t<TAP == TAP_BAYER16, uint16_t, uint8_t>;
+        bayer_px(reinterpret_cast<const T*>(src), (size_t)d.src_pitch / sizeof(T), d.src_w, d.src_h, x, y, f.pattern, rgb);
+    } else if constexpr (TAP == TAP_BAYER_PACKED) {
+        bayer_px_packed(src, (size_t)d.src_pitch, d.src_w, d.src_h, x, y, f.pattern, f.bits, rgb);
+    } else if constexpr (TAP == TAP_YUV16) {
+        if (f.layout == YUV420_I420) yuv420_tap<YUV420_I420>(src, x, y, d.src_w, d.src_h, yc, rgb);
+        else yuv420_tap<YUV420_NV12>(src, x, y, d.src_w, d.src_h, yc, rgb);
+    } else if constexpr (TAP >= TAP_YUV420) {
+        yuv420_tap<TAP - TAP_YUV420, false>(src, x, y, d.src_w, d.src_h, yc, rgb);
+    } else {
+        switch (f.layout) {
+            case YUV422_YUYV: yuv422_tap<YUV422_YUYV>(src, x, y, d.src_pitch, yc, rgb); break;
+            case YUV422_UYVY: yuv422_tap<YUV422_UYVY>(src, x, y, d.src_pitch, yc, rgb); break;
+            default: yuv422_tap<YUV422_YVYU>(src, x, y, d.src_pitch, yc, rgb); break;
+        }
+    }
+    px[0] = (float)rgb[0]; px[1] = (float)rgb[1]; px[2] = (float)rgb[2];
 }
 
 // preprocess.rs:481-488 (kernel source): 1-D Lanczos-3 weight — the CUDA math library's sinf, like the reference kernel
@@ -200,10 +204,10 @@ __device__ __forceinline__ float pre_lanczos_w(float dd) {
 }
 
 // SAMP: kb200_interp — 0 nearest, 1 bilinear, 3 Lanczos-3 (6x6 taps, clamp-to-edge, weights renormalised by their sum)
-template <bool F16, int SAMP, bool PTRS, int EXT>
+template <bool F16, int SAMP, bool PTRS, int TAP>
 __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                  const __grid_constant__ PreFrames fr, void* __restrict__ dst,
-                                                                 uint32_t frame0, const YuvCoeffs yc) {
+                                                                 uint32_t frame0, const SrcFormat sf, const TapCoeffs<TAP> yc) {
     const int pixels = d.dst_w * d.dst_h;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= pixels) return;
@@ -227,7 +231,7 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
                     const float w = wy * pre_lanczos_w(sx - (float)xi);
                     const int xc = min(max(xi, 0), d.src_w - 1);
                     float t[3];
-                    fetch_px<EXT>(src, xc, ycl, d, yc, t);
+                    fetch_px<TAP>(src, xc, ycl, d, sf, yc, t);
                     acc0 += w * t[0]; acc1 += w * t[1]; acc2 += w * t[2];
                     wsum += w;
                 }
@@ -239,12 +243,12 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
             const int x1 = min(x0 + 1, d.src_w - 1), y1 = min(y0 + 1, d.src_h - 1);
             x0 = max(x0, 0); y0 = max(y0, 0);
             float t00[3], t10[3], t01[3], t11[3];
-            fetch_px<EXT>(src, x0, y0, d, yc, t00);
+            fetch_px<TAP>(src, x0, y0, d, sf, yc, t00);
             const bool need_x = ax != 0.0f, need_y = ay != 0.0f;
-            if (need_x) fetch_px<EXT>(src, x1, y0, d, yc, t10);
+            if (need_x) fetch_px<TAP>(src, x1, y0, d, sf, yc, t10);
             if (need_y) {
-                fetch_px<EXT>(src, x0, y1, d, yc, t01);
-                if (need_x) fetch_px<EXT>(src, x1, y1, d, yc, t11);
+                fetch_px<TAP>(src, x0, y1, d, sf, yc, t01);
+                if (need_x) fetch_px<TAP>(src, x1, y1, d, sf, yc, t11);
             }
 #pragma unroll
             for (int c = 0; c < 3; ++c) {
@@ -259,17 +263,17 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
         } else {
             const int xn = min(max((int)roundf(sx), 0), d.src_w - 1);
             const int yn = min(max((int)roundf(sy), 0), d.src_h - 1);
-            fetch_px<EXT>(src, xn, yn, d, yc, px);
+            fetch_px<TAP>(src, xn, yn, d, sf, yc, px);
         }
     } else {
         px[0] = d.pad_value; px[1] = d.pad_value; px[2] = d.pad_value;
     }
     float q0, q1, q2;
-    if (EXT == SRC_YUV16 && inside) {   // px / W, the IEEE quotient (div_white: no zero dividend reaches the division)
-        const float wl = (float)yuv16_of(d.fmt, yc).white;
+    if (TAP == TAP_YUV16 && inside) {   // px / W, the IEEE quotient (div_white: no zero dividend reaches the division)
+        const float wl = sf.white();
         q0 = div_white(px[0], wl); q1 = div_white(px[1], wl); q2 = div_white(px[2], wl);
-    } else if ((EXT == SRC_BAYER16 || EXT == SRC_BAYER_PACKED) && inside) {   // px / W: taps up to 65535 and Lanczos overshoot, so the IEEE division
-        const float wl = EXT == SRC_BAYER16 ? bayer16_white(d.fmt) : bayer_packed_white(d.fmt);
+    } else if ((TAP == TAP_BAYER16 || TAP == TAP_BAYER_PACKED) && inside) {   // px / W: taps up to 65535 and Lanczos overshoot, so the IEEE division
+        const float wl = sf.white();
         q0 = __fdiv_rn(px[0], wl); q1 = __fdiv_rn(px[1], wl); q2 = __fdiv_rn(px[2], wl);
     } else if (inside && SAMP != KB200_INTERP_LANCZOS) { q0 = div255_exact(px[0]); q1 = div255_exact(px[1]); q2 = div255_exact(px[2]); }
     else if (inside) { q0 = __fdiv_rn(px[0], 255.0f); q1 = __fdiv_rn(px[1], 255.0f); q2 = __fdiv_rn(px[2], 255.0f); }  // Lanczos overshoots [0, 255]
@@ -437,7 +441,7 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const _
 template <bool F16, bool PTRS, typename T, int P>
 __global__ void __launch_bounds__(128) preprocess_bayer_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                         const __grid_constant__ PreFrames fr, void* __restrict__ dst,
-                                                                        uint32_t frame0, uint32_t groups_per_row, uint32_t items) {
+                                                                        uint32_t frame0, uint32_t groups_per_row, uint32_t items, uint32_t bits) {
     constexpr uint32_t NW = BayerSample<T>::ID_WORDS;
     constexpr int PB = BayerSample<T>::PACKED_BITS;
     const uint32_t item = blockIdx.x * blockDim.x + threadIdx.x;
@@ -476,8 +480,8 @@ __global__ void __launch_bounds__(128) preprocess_bayer_identity_kernel(const __
     const bool left_edge = x == 0, right_edge = x + 4u == w;
     const size_t plane = (size_t)w * h;
     const size_t base = (size_t)(frame0 + f) * 3 * plane + x;
-    // the white level W of a 16-bit or packed format
-    [[maybe_unused]] const float wl = PB == 0 ? bayer16_white(d.fmt) : (float)((1u << PB) - 1u);
+    // the white level W of a 16-bit (`bits` from the host's SrcFormat) or packed format
+    [[maybe_unused]] const float wl = PB == 0 ? (float)((1u << bits) - 1u) : (float)((1u << PB) - 1u);
     const float m0 = d.mean[0], m1 = d.mean[1], m2 = d.mean[2], i0 = d.inv_std[0], i1 = d.inv_std[1], i2 = d.inv_std[2];
     float r4[4], g4[4], b4[4];
     auto store_row = [&](uint32_t y) {
@@ -525,38 +529,6 @@ struct Nv12Args {
     float pad_norm[3];  // ((pad_value / 255) - mean) * inv_std, evaluated on the host in f32
     uint32_t groups;    // ceil(dst_w / 4)
 };
-
-// One decoded tap of a 4:2:0 frame in layout L (kb200_yuv420_layout): the kernel below serves all four layouts.
-template <int L>
-__device__ __forceinline__ void yuv420_tap(const uint8_t* __restrict__ src, int x, int y, int w, int h, const YuvCoeffs& yc, int rgb[3]) {
-    const int yv = __ldg(src + (size_t)y * w + x);
-    ChromaTerms t;
-    if (yuv420_planar(L)) {
-        const size_t c = (size_t)(y >> 1) * (w >> 1) + (x >> 1);
-        t = chroma_terms(__ldg(src + yuv420_u_plane(L, w, h) + c), __ldg(src + yuv420_v_plane(L, w, h) + c), yc);
-    } else {
-        const uint32_t uv = __ldg(reinterpret_cast<const unsigned short*>(src + (size_t)w * h + (size_t)(y >> 1) * w + (x >> 1) * 2));
-        t = L == YUV420_NV21 ? chroma_terms((int)(uv >> 8), (int)(uv & 0xFFu), yc) : chroma_terms((int)(uv & 0xFFu), (int)(uv >> 8), yc);
-    }
-    decode_rgb(yy_term(yv, yc), t, rgb[0], rgb[1], rgb[2]);
-}
-// ... and of a frame of 16-bit words (the coefficient type selects it): P01x in the NV12 layout, I01x in the I420 layout.
-// A P01x tap reads its chroma pair as two 16-bit words, since frames are only 2-B aligned on this path.
-template <int L>
-__device__ __forceinline__ void yuv420_tap(const uint8_t* __restrict__ src, int x, int y, int w, int h, const Yuv16Coeffs& k, int rgb[3]) {
-    const uint16_t* s = reinterpret_cast<const uint16_t*>(src);
-    const size_t plane = (size_t)w * h;
-    size_t cu, cv;
-    if (yuv420_planar(L)) {
-        cu = plane + (size_t)(y >> 1) * (w >> 1) + (x >> 1);
-        cv = cu + plane / 4;
-    } else {
-        cu = plane + (size_t)(y >> 1) * w + (x & ~1);
-        cv = cu + 1;
-    }
-    const ChromaTerms t = chroma_terms16(yuv16_code(__ldg(s + cu), k), yuv16_code(__ldg(s + cv), k), k);
-    decode_rgb16(yy_term16(yuv16_code(__ldg(s + (size_t)y * w + x), k), k), t, k.white, rgb[0], rgb[1], rgb[2]);
-}
 
 static constexpr int NV12_ROWS = 8;  // destination rows per thread: the x-side of the sampler is computed once for all of them
 
@@ -671,45 +643,61 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_kernel(const __grid_con
     }
 }
 
-// fmt -> kb200_yuv420_layout, or -1 for the formats that are not 4:2:0
-static int yuv420_layout(int fmt) {
-    switch (fmt) {
-        case KB200_FMT_NV12: return YUV420_NV12;
-        case KB200_FMT_NV21: return YUV420_NV21;
-        case KB200_FMT_I420: return YUV420_I420;
-        case KB200_FMT_YV12: return YUV420_YV12;
-        default: return -1;
-    }
-}
-static bool is_yuv422(int fmt) { return fmt == KB200_FMT_YUYV || fmt == KB200_FMT_UYVY || fmt == KB200_FMT_YVYU; }
-static bool is_bayer(int fmt) { return fmt >= KB200_FMT_BAYER_RGGB && fmt <= KB200_FMT_BAYER_GBRG; }
-static bool is_bayer16(int fmt) { return fmt >= KB200_FMT_BAYER_RGGB10 && fmt <= KB200_FMT_BAYER_GBRG16; }
-static bool is_bayer_packed(int fmt) { return fmt >= KB200_FMT_BAYER_RGGB10P && fmt <= KB200_FMT_BAYER_GBRG14P; }
-static bool is_yuv16(int fmt) { return fmt >= KB200_FMT_P010 && fmt <= KB200_FMT_I012; }
-// SourceFormat names, in the validation messages
-static const char* const FMT_NAMES[10] = {"Rgb8", "Bgr8", "Gray8", "Nv12", "Yuyv", "Nv21", "I420", "Yv12", "Uyvy", "Yvyu"};
-static const char* const BAYER_NAMES[4] = {"BayerRggb", "BayerBggr", "BayerGrbg", "BayerGbrg"};
-static const char* const YUV420_UPPER[4] = {"NV12", "NV21", "I420", "YV12"};
-static const char* const YUV16_NAMES[4] = {"P010", "P012", "I010", "I012"};   // fmt 80-83
+// One row per format code.  A Bayer code is 16 + pattern (8-bit samples), 32 + 4*k + pattern (16-bit words, k = 0..3 for
+// 10, 12, 14 and 16 bits) or 64 + 4*k + pattern (packed, k = 0..2 for 10, 12 and 14 bits); each sample type has its own
+// identity kernel, and the 16-bit one serves every depth.
+#define KB200_BAYER_FORMATS(code, suffix, bits, words, packed, kernel)                                                            \
+    {code, "BayerRggb" suffix, SRC_BAYER, 0, KB200_BAYER_RGGB, bits, words, packed, "preprocess_" kernel "_rggb_identity_kernel"},     \
+    {code + 1, "BayerBggr" suffix, SRC_BAYER, 0, KB200_BAYER_BGGR, bits, words, packed, "preprocess_" kernel "_bggr_identity_kernel"}, \
+    {code + 2, "BayerGrbg" suffix, SRC_BAYER, 0, KB200_BAYER_GRBG, bits, words, packed, "preprocess_" kernel "_grbg_identity_kernel"}, \
+    {code + 3, "BayerGbrg" suffix, SRC_BAYER, 0, KB200_BAYER_GBRG, bits, words, packed, "preprocess_" kernel "_gbrg_identity_kernel"}
+static const SrcFormat SRC_FORMATS[] = {
+    {KB200_FMT_RGB, "Rgb8", SRC_RGB, 0},
+    {KB200_FMT_BGR, "Bgr8", SRC_RGB, 1},
+    {KB200_FMT_GRAY, "Gray8", SRC_GRAY},
+    {KB200_FMT_NV12, "Nv12", SRC_YUV420, YUV420_NV12, 0, 8, false, false, "preprocess_nv12_identity_kernel", "preprocess_nv12_kernel"},
+    {KB200_FMT_YUYV, "Yuyv", SRC_YUV422, YUV422_YUYV},
+    {KB200_FMT_NV21, "Nv21", SRC_YUV420, YUV420_NV21, 0, 8, false, false, "preprocess_nv21_identity_kernel", "preprocess_nv21_kernel"},
+    {KB200_FMT_I420, "I420", SRC_YUV420, YUV420_I420, 0, 8, false, false, "preprocess_i420_identity_kernel", "preprocess_i420_kernel"},
+    {KB200_FMT_YV12, "Yv12", SRC_YUV420, YUV420_YV12, 0, 8, false, false, "preprocess_yv12_identity_kernel", "preprocess_yv12_kernel"},
+    {KB200_FMT_UYVY, "Uyvy", SRC_YUV422, YUV422_UYVY},
+    {KB200_FMT_YVYU, "Yvyu", SRC_YUV422, YUV422_YVYU},
+    KB200_BAYER_FORMATS(KB200_FMT_BAYER_RGGB, "", 8, false, false, "bayer"),
+    KB200_BAYER_FORMATS(KB200_FMT_BAYER_RGGB10, "10", 10, true, false, "bayer16"),
+    KB200_BAYER_FORMATS(KB200_FMT_BAYER_RGGB12, "12", 12, true, false, "bayer16"),
+    KB200_BAYER_FORMATS(KB200_FMT_BAYER_RGGB14, "14", 14, true, false, "bayer16"),
+    KB200_BAYER_FORMATS(KB200_FMT_BAYER_RGGB16, "16", 16, true, false, "bayer16"),
+    KB200_BAYER_FORMATS(KB200_FMT_BAYER_RGGB10P, "10p", 10, false, true, "bayer10p"),
+    KB200_BAYER_FORMATS(KB200_FMT_BAYER_RGGB12P, "12p", 12, false, true, "bayer12p"),
+    KB200_BAYER_FORMATS(KB200_FMT_BAYER_RGGB14P, "14p", 14, false, true, "bayer14p"),
+    // 10- and 12-bit 4:2:0 video: P01x in NV12's layout with each code in the high bits of its word, I01x in I420's with it
+    // in the low bits; the 16-bit instantiations of the 4:2:0 fast kernels serve both depths
+    {KB200_FMT_P010, "P010", SRC_YUV420, YUV420_NV12, 0, 10, true, false, "preprocess_p01x_identity_kernel", "preprocess_p01x_kernel"},
+    {KB200_FMT_P012, "P012", SRC_YUV420, YUV420_NV12, 0, 12, true, false, "preprocess_p01x_identity_kernel", "preprocess_p01x_kernel"},
+    {KB200_FMT_I010, "I010", SRC_YUV420, YUV420_I420, 0, 10, true, false, "preprocess_i01x_identity_kernel", "preprocess_i01x_kernel"},
+    {KB200_FMT_I012, "I012", SRC_YUV420, YUV420_I420, 0, 12, true, false, "preprocess_i01x_identity_kernel", "preprocess_i01x_kernel"},
+};
+#undef KB200_BAYER_FORMATS
 
-static bool is_yuv(int fmt) { return yuv420_layout(fmt) >= 0 || is_yuv422(fmt) || is_yuv16(fmt); }
+static SrcFormat src_format(int fmt) {
+    for (const SrcFormat& f : SRC_FORMATS)
+        if (f.code == fmt) return f;
+    return {};
+}
 
 // kb200_preprocess_desc::fmt = format code (bits 0-7) | KB200_FMT_YUV_MATRIX(m) (bits 8-9).  The entry points strip the
-// matrix once, here: every other function sees the plain code and takes the coefficient set apart.
+// matrix once, here: every other function sees the plain code and gets the matrix (kb200_yuv_matrix) on its own.
 static kb200_preprocess_desc plain_desc(const kb200_preprocess_desc& d) {
     kb200_preprocess_desc p = d;
     p.fmt = d.fmt & 0xFF;
     return p;
 }
-// The coefficient set of a raw descriptor: the Q20 set of its matrix, or for fmt 80-83 the Q16 set of its matrix and depth
-static const YuvCoeffs& yuv_coeffs(const kb200_preprocess_desc& d) {
-    const int fmt = d.fmt & 0xFF;
-    return is_yuv16(fmt) ? YUV16_COEFFS[yuv16_bits(fmt) == 12][(d.fmt >> 8) & 3] : YUV_COEFFS[(d.fmt >> 8) & 3];
-}
+static int yuv_matrix(const kb200_preprocess_desc& raw) { return (raw.fmt >> 8) & 3; }
 
 static size_t src_bytes(const kb200_preprocess_desc& d) {
-    // 4:2:0 chroma after the pitch * h luma bytes: w*h/2 samples, of 1 byte (fmt 3, 5-7) or 2 bytes (fmt 80-83)
-    const size_t chroma = yuv420_layout(d.fmt) >= 0 ? (size_t)d.src_w * d.src_h / 2 : is_yuv16(d.fmt) ? (size_t)d.src_w * d.src_h : 0;
+    // 4:2:0 chroma after the pitch * h luma bytes: w*h/2 samples, of 1 byte or of 2 (16-bit words)
+    const SrcFormat f = src_format(d.fmt);
+    const size_t chroma = f.family != SRC_YUV420 ? 0 : f.words ? (size_t)d.src_w * d.src_h : (size_t)d.src_w * d.src_h / 2;
     return (size_t)d.src_pitch * d.src_h + chroma;
 }
 
@@ -719,54 +707,43 @@ static int validate_desc(const kb200_preprocess_desc* dp) {
         return fail(KB200_ERR_INVALID_ARGUMENT, "image dimensions must be non-zero");
     if ((long long)dp->dst_w * dp->dst_h > 0x7FFFFFFFll) return fail(KB200_ERR_DIMS_TOO_LARGE, "dimensions exceed the 32-bit CUDA kernel index limit");  // :1336-1339
     const kb200_preprocess_desc d = plain_desc(*dp);
-    if (dp->fmt < 0 || (d.fmt > KB200_FMT_YVYU && !is_bayer(d.fmt) && !is_bayer16(d.fmt) && !is_bayer_packed(d.fmt) && !is_yuv16(d.fmt)))
-        return fail(KB200_ERR_INVALID_ARGUMENT, "unknown source format code %d", dp->fmt);
+    const SrcFormat f = src_format(d.fmt);
+    if (dp->fmt < 0 || !f.name) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown source format code %d", dp->fmt);
     if (dp->fmt >> 10)
         return fail(KB200_ERR_INVALID_ARGUMENT, "source format code %d has bits set above bit 9 (bits 8-9 are the YUV matrix, 0-3)", dp->fmt);
-    if ((dp->fmt >> 8) && !is_yuv(d.fmt))
+    if ((dp->fmt >> 8) && f.family != SRC_YUV420 && f.family != SRC_YUV422)
         return fail(KB200_ERR_INVALID_ARGUMENT, "source format code %d: a YUV matrix (%d) applies only to the YUV formats, not format code %d", dp->fmt,
                     dp->fmt >> 8, d.fmt);
     if (d.sampling != KB200_INTERP_NEAREST && d.sampling != KB200_INTERP_BILINEAR && d.sampling != KB200_INTERP_LANCZOS)
         return fail(KB200_ERR_UNSUPPORTED, "unsupported sampling mode %d (expected Nearest, Bilinear or Lanczos)", d.sampling);  // preprocess.rs:1044-1051
-    if (d.fmt <= 1 && d.src_bpp != 3 && d.src_bpp != 4) return fail(KB200_ERR_UNSUPPORTED, "unsupported source channel count %d (expected 3 or 4)", d.src_bpp);
+    if (f.family == SRC_RGB && d.src_bpp != 3 && d.src_bpp != 4) return fail(KB200_ERR_UNSUPPORTED, "unsupported source channel count %d (expected 3 or 4)", d.src_bpp);
     // SourceFormat::dims_ok :188-195 ; pitch covers a row (PitchedSurface::validate :829-842)
-    const int l420 = yuv420_layout(d.fmt);
-    if (l420 >= 0 && ((d.src_w | d.src_h) & 1)) return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s at %dx%d (even dimensions required)", FMT_NAMES[d.fmt], d.src_w, d.src_h);
-    if (is_yuv422(d.fmt) && (d.src_w & 1)) return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s at %dx%d (even width required)", FMT_NAMES[d.fmt], d.src_w, d.src_h);
-    if (is_bayer(d.fmt) && (d.src_w < 3 || d.src_h < 3))
-        return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s at %dx%d (at least 3x3 required)", BAYER_NAMES[d.fmt - KB200_FMT_BAYER_RGGB], d.src_w, d.src_h);
-    if (is_bayer16(d.fmt)) {   // SourceFormat names: BayerRggb10 ... BayerGbrg16
-        const char* name = BAYER_NAMES[bayer16_pattern(d.fmt)];
-        const int bits = bayer16_bits(d.fmt);
-        if (d.src_w < 3 || d.src_h < 3)
-            return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s%d at %dx%d (at least 3x3 required)", name, bits, d.src_w, d.src_h);
-        if (d.src_pitch & 1)
-            return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface for %s%d (pitch %d is odd: rows of 16-bit samples must start 2-byte aligned)", name, bits, d.src_pitch);
-    }
-    if (is_bayer_packed(d.fmt)) {   // SourceFormat names: BayerRggb10p ... BayerGbrg14p
-        const char* name = BAYER_NAMES[bayer_packed_pattern(d.fmt)];
-        const int bits = bayer_packed_bits(d.fmt), g = bayer_packed_group(bits);
-        if (d.src_w < 3 || d.src_h < 3)
-            return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s%dp at %dx%d (at least 3x3 required)", name, bits, d.src_w, d.src_h);
+    if (f.family == SRC_YUV420 && ((d.src_w | d.src_h) & 1)) return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s at %dx%d (even dimensions required)", f.name, d.src_w, d.src_h);
+    if (f.family == SRC_YUV422 && (d.src_w & 1)) return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s at %dx%d (even width required)", f.name, d.src_w, d.src_h);
+    if (f.family == SRC_BAYER && (d.src_w < 3 || d.src_h < 3))
+        return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s at %dx%d (at least 3x3 required)", f.name, d.src_w, d.src_h);
+    if (f.family == SRC_BAYER && f.words && (d.src_pitch & 1))
+        return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface for %s (pitch %d is odd: rows of 16-bit samples must start 2-byte aligned)", f.name, d.src_pitch);
+    if (f.packed) {
+        const int g = bayer_packed_group(f.bits);
         if (d.src_w % g)
-            return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s%dp at %dx%d (the width must be a multiple of %d: whole %d-byte groups)", name,
-                        bits, d.src_w, d.src_h, g, bayer_packed_group_bytes(bits));
-        if ((long long)d.src_pitch < (long long)d.src_w * bits / 8)
-            return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface for %s%dp (pitch %d < %lld bytes of a packed row)", name, bits, d.src_pitch,
-                        (long long)d.src_w * bits / 8);
+            return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s at %dx%d (the width must be a multiple of %d: whole %d-byte groups)", f.name,
+                        d.src_w, d.src_h, g, bayer_packed_group_bytes(f.bits));
+        if ((long long)d.src_pitch < (long long)d.src_w * f.bits / 8)
+            return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface for %s (pitch %d < %lld bytes of a packed row)", f.name, d.src_pitch,
+                        (long long)d.src_w * f.bits / 8);
     }
-    if (is_yuv16(d.fmt)) {   // SourceFormat names: P010, P012, I010, I012
-        const char* name = YUV16_NAMES[d.fmt - KB200_FMT_P010];
-        if ((d.src_w | d.src_h) & 1)
-            return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source for %s at %dx%d (even dimensions required)", name, d.src_w, d.src_h);
-        if ((long long)d.src_pitch != 2ll * d.src_w)
-            return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface for %s (pitch %d bytes at width %d: frames must be tightly packed, pitch == 2*width)",
-                        name, d.src_pitch, d.src_w);
-    }
-    const int bpp = d.fmt <= 1 ? d.src_bpp : (is_yuv422(d.fmt) || is_bayer16(d.fmt) || is_yuv16(d.fmt) ? 2 : 1);
-    if (!is_bayer_packed(d.fmt) && (long long)d.src_pitch < (long long)d.src_w * bpp)
+    if (f.family == SRC_YUV420 && f.words && (long long)d.src_pitch != 2ll * d.src_w)
+        return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface for %s (pitch %d bytes at width %d: frames must be tightly packed, pitch == 2*width)",
+                    f.name, d.src_pitch, d.src_w);
+    const int bpp = f.family == SRC_RGB ? d.src_bpp : f.family == SRC_YUV422 || f.words ? 2 : 1;
+    if (!f.packed && (long long)d.src_pitch < (long long)d.src_w * bpp)
         return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface (need pitch >= width*channels and len >= pitch*height)");
-    if (l420 >= 0 && d.src_pitch != d.src_w) return fail(KB200_ERR_INVALID_SOURCE, "%s frames must be tightly packed (pitch == width)", YUV420_UPPER[l420]);
+    if (f.family == SRC_YUV420 && !f.words && d.src_pitch != d.src_w) {
+        char upper[8] = "";   // the layout's own spelling: NV12, NV21, I420, YV12
+        for (int i = 0; f.name[i] && i < 7; ++i) upper[i] = (char)toupper((unsigned char)f.name[i]);
+        return fail(KB200_ERR_INVALID_SOURCE, "%s frames must be tightly packed (pitch == width)", upper);
+    }
     if (!(d.scale_x > 0.0f) || !(d.scale_y > 0.0f)) return fail(KB200_ERR_INVALID_ARGUMENT, "scale must be positive");
     return KB200_OK;
 }
@@ -792,63 +769,58 @@ static void launch_yuv420_fast(cudaStream_t s, bool identity, bool bil, const kb
 // The Bayer identity kernel of sample type T and pattern P, for one launch of <= 256 frames.
 template <bool F16, typename T, int P>
 static void launch_bayer_identity(cudaStream_t s, const kb200_preprocess_desc& d, const PreFrames& fr, bool ptrs, void* dst, uint32_t f0,
-                                  uint32_t nb, uint32_t id_groups, size_t id_items) {
+                                  uint32_t nb, uint32_t id_groups, size_t id_items, uint32_t bits) {
     dim3 grid(div_up(id_items, 128), nb);
-    if (ptrs) preprocess_bayer_identity_kernel<F16, true, T, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
-    else preprocess_bayer_identity_kernel<F16, false, T, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items);
+    if (ptrs) preprocess_bayer_identity_kernel<F16, true, T, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, bits);
+    else preprocess_bayer_identity_kernel<F16, false, T, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, bits);
 }
 
-template <bool F16, bool PTRS, int EXT>
-static void launch_generic(cudaStream_t s, dim3 grid, int sampling, const kb200_preprocess_desc& d, const YuvCoeffs& yc, const PreFrames& fr, void* dst,
-                           uint32_t f0) {
-    if (sampling == KB200_INTERP_LANCZOS) preprocess_generic_kernel<F16, KB200_INTERP_LANCZOS, PTRS, EXT><<<grid, 256, 0, s>>>(d, fr, dst, f0, yc);
-    else if (sampling == KB200_INTERP_BILINEAR) preprocess_generic_kernel<F16, KB200_INTERP_BILINEAR, PTRS, EXT><<<grid, 256, 0, s>>>(d, fr, dst, f0, yc);
-    else preprocess_generic_kernel<F16, KB200_INTERP_NEAREST, PTRS, EXT><<<grid, 256, 0, s>>>(d, fr, dst, f0, yc);
+template <bool F16, bool PTRS, int TAP>
+static void launch_generic(cudaStream_t s, dim3 grid, const kb200_preprocess_desc& d, const SrcFormat& f, const TapCoeffs<TAP>& yc,
+                           const PreFrames& fr, void* dst, uint32_t f0) {
+    if (d.sampling == KB200_INTERP_LANCZOS) preprocess_generic_kernel<F16, KB200_INTERP_LANCZOS, PTRS, TAP><<<grid, 256, 0, s>>>(d, fr, dst, f0, f, yc);
+    else if (d.sampling == KB200_INTERP_BILINEAR) preprocess_generic_kernel<F16, KB200_INTERP_BILINEAR, PTRS, TAP><<<grid, 256, 0, s>>>(d, fr, dst, f0, f, yc);
+    else preprocess_generic_kernel<F16, KB200_INTERP_NEAREST, PTRS, TAP><<<grid, 256, 0, s>>>(d, fr, dst, f0, f, yc);
 }
 
 template <bool F16, bool PTRS>
-static void launch_generic_for(int ext, cudaStream_t s, dim3 grid, int sampling, const kb200_preprocess_desc& d, const YuvCoeffs& yc,
-                               const PreFrames& fr, void* dst, uint32_t f0) {
-    if (ext == SRC_YUV16) launch_generic<F16, PTRS, SRC_YUV16>(s, grid, sampling, d, yc, fr, dst, f0);
-    else if (ext == SRC_BAYER_PACKED) launch_generic<F16, PTRS, SRC_BAYER_PACKED>(s, grid, sampling, d, yc, fr, dst, f0);
-    else if (ext == SRC_BAYER16) launch_generic<F16, PTRS, SRC_BAYER16>(s, grid, sampling, d, yc, fr, dst, f0);
-    else if (ext == SRC_BAYER) launch_generic<F16, PTRS, SRC_BAYER>(s, grid, sampling, d, yc, fr, dst, f0);
-    else if (ext == SRC_EXT_YUV) launch_generic<F16, PTRS, SRC_EXT_YUV>(s, grid, sampling, d, yc, fr, dst, f0);
-    else launch_generic<F16, PTRS, SRC_BASE>(s, grid, sampling, d, yc, fr, dst, f0);
+static void launch_generic_for(cudaStream_t s, dim3 grid, const kb200_preprocess_desc& d, const SrcFormat& f, const YuvCoeffs& yc,
+                               const Yuv16Coeffs& yc16, const PreFrames& fr, void* dst, uint32_t f0) {
+    if (f.family == SRC_BAYER) {
+        if (f.packed) launch_generic<F16, PTRS, TAP_BAYER_PACKED>(s, grid, d, f, yc, fr, dst, f0);
+        else if (f.words) launch_generic<F16, PTRS, TAP_BAYER16>(s, grid, d, f, yc, fr, dst, f0);
+        else launch_generic<F16, PTRS, TAP_BAYER>(s, grid, d, f, yc, fr, dst, f0);
+    } else if (f.words) {
+        launch_generic<F16, PTRS, TAP_YUV16>(s, grid, d, f, yc16, fr, dst, f0);
+    } else if (f.family == SRC_YUV420) {
+        switch (f.layout) {
+            case YUV420_NV12: launch_generic<F16, PTRS, TAP_YUV420 + YUV420_NV12>(s, grid, d, f, yc, fr, dst, f0); break;
+            case YUV420_NV21: launch_generic<F16, PTRS, TAP_YUV420 + YUV420_NV21>(s, grid, d, f, yc, fr, dst, f0); break;
+            case YUV420_I420: launch_generic<F16, PTRS, TAP_YUV420 + YUV420_I420>(s, grid, d, f, yc, fr, dst, f0); break;
+            default: launch_generic<F16, PTRS, TAP_YUV420 + YUV420_YV12>(s, grid, d, f, yc, fr, dst, f0); break;
+        }
+    } else if (f.family == SRC_YUV422) {
+        launch_generic<F16, PTRS, TAP_YUV422>(s, grid, d, f, yc, fr, dst, f0);
+    } else {
+        launch_generic<F16, PTRS, TAP_RGB>(s, grid, d, f, yc, fr, dst, f0);
+    }
 }
 
-// kb200_last_kernel() names of the 4:2:0 fast kernels, by layout
-static const char* const YUV420_IDENTITY_NAMES[4] = {"preprocess_nv12_identity_kernel", "preprocess_nv21_identity_kernel",
-                                                     "preprocess_i420_identity_kernel", "preprocess_yv12_identity_kernel"};
-static const char* const YUV420_FAST_NAMES[4] = {"preprocess_nv12_kernel", "preprocess_nv21_kernel", "preprocess_i420_kernel", "preprocess_yv12_kernel"};
-// ... and of their 16-bit instantiations, by layout (P01x, I01x: each serves both depths)
-static const char* const YUV16_IDENTITY_NAMES[2] = {"preprocess_p01x_identity_kernel", "preprocess_i01x_identity_kernel"};
-static const char* const YUV16_FAST_NAMES[2] = {"preprocess_p01x_kernel", "preprocess_i01x_kernel"};
-// ... and of the Bayer identity kernels, by sample type (8-bit, 16-bit, packed 10-, 12- and 14-bit) and pattern
-#define KB200_BAYER_IDENTITY_NAMES(s)                                                                                   \
-    {"preprocess_bayer" s "_rggb_identity_kernel", "preprocess_bayer" s "_bggr_identity_kernel", "preprocess_bayer" s "_grbg_identity_kernel", \
-     "preprocess_bayer" s "_gbrg_identity_kernel"}
-static const char* const BAYER_IDENTITY_NAMES[5][4] = {KB200_BAYER_IDENTITY_NAMES(""), KB200_BAYER_IDENTITY_NAMES("16"), KB200_BAYER_IDENTITY_NAMES("10p"),
-                                                       KB200_BAYER_IDENTITY_NAMES("12p"), KB200_BAYER_IDENTITY_NAMES("14p")};
-#undef KB200_BAYER_IDENTITY_NAMES
-
+// d: a validated descriptor with the plain format code; matrix: its kb200_yuv_matrix
 template <bool F16>
-static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, const YuvCoeffs& yc, const uint8_t* const* frames,
-                             const uint8_t* base, size_t stride, uint32_t batch, void* dst) {
+static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, int matrix, const uint8_t* const* frames, const uint8_t* base,
+                             size_t stride, uint32_t batch, void* dst) {
+    const SrcFormat f = src_format(d.fmt);
     const int pixels = d.dst_w * d.dst_h;
     const bool bil = d.sampling == KB200_INTERP_BILINEAR, lanczos = d.sampling == KB200_INTERP_LANCZOS;
-    // fmt 80-83 take the 4:2:0 fast kernels of their layout (P01x: NV12's, I01x: I420's) instantiated for 16-bit words
-    const bool yuv16 = is_yuv16(d.fmt);
-    const int l420 = yuv16 ? (yuv16_planar(d.fmt) ? YUV420_I420 : YUV420_NV12) : yuv420_layout(d.fmt);
-    const bool bayer16 = is_bayer16(d.fmt), packed = is_bayer_packed(d.fmt);
-    const bool bayer = bayer16 || packed || is_bayer(d.fmt);   // bayer: any Bayer mosaic
-    // identity fast path: a 4:2:0 or Bayer format, scale 1, no pad, same size, 8-column vectors possible
-    // (Lanczos always takes the generic kernel: its off-centre weights at integer coordinates are sinf(k*pi) != 0 exactly).
-    // A thread loads 4 samples per row, so rows and frames are aligned to that load: 4 B for 8-bit 4:2:0 and 8-bit Bayer,
-    // 8 B for 16-bit 4:2:0 and 16-bit Bayer, 16 B for packed Bayer.
-    const uint32_t row_align = packed ? BayerSample<BayerPacked<12>>::ID_ALIGN
-                                      : (bayer16 || yuv16) ? BayerSample<uint16_t>::ID_ALIGN : BayerSample<uint8_t>::ID_ALIGN;
-    bool identity = !lanczos && (l420 >= 0 || bayer) && d.scale_x == 1.0f && d.scale_y == 1.0f && d.pad_x == 0.0f && d.pad_y == 0.0f &&
+    const bool bayer = f.family == SRC_BAYER;
+    // identity fast path: a format with an identity kernel (4:2:0 or Bayer), scale 1, no pad, same size, 8-column vectors
+    // possible (Lanczos always takes the generic kernel: its off-centre weights at integer coordinates are sinf(k*pi) != 0
+    // exactly).  A thread loads 4 samples per row, so rows and frames are aligned to that load: 4 B for bytes, 8 B for
+    // 16-bit words, 16 B for packed Bayer.
+    const uint32_t row_align = f.packed ? BayerSample<BayerPacked<12>>::ID_ALIGN
+                                        : f.words ? BayerSample<uint16_t>::ID_ALIGN : BayerSample<uint8_t>::ID_ALIGN;
+    bool identity = !lanczos && f.identity_kernel && d.scale_x == 1.0f && d.scale_y == 1.0f && d.pad_x == 0.0f && d.pad_y == 0.0f &&
                     d.dst_w == d.src_w && d.dst_h == d.src_h && (d.src_w % 4) == 0 && (d.src_pitch % row_align) == 0 && aligned16(dst);
     if (identity) {
         if (frames) { for (uint32_t k = 0; k < batch; ++k) identity = identity && ((reinterpret_cast<uintptr_t>(frames[k]) & (row_align - 1)) == 0); }
@@ -858,9 +830,9 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
     const size_t id_items = (size_t)id_groups * (bayer ? bayer_row_pairs((uint32_t)d.src_h) : (size_t)d.src_h / 2);
     if (id_items > 0x7FFFFFFFull) identity = false;
     // 4:2:0 general fast path: vector stores need dst_w % 4 == 0 and a 16-B (f32) / 8-B (f16) aligned destination
-    const bool yuv420_fast = !lanczos && l420 >= 0 && (d.dst_w % 4) == 0 && aligned16(dst) && d.dst_h <= 65535 * NV12_ROWS;
-    const int ext = yuv16 ? SRC_YUV16 : bayer16 ? SRC_BAYER16 : packed ? SRC_BAYER_PACKED : bayer ? SRC_BAYER : d.fmt >= KB200_FMT_NV21 ? SRC_EXT_YUV : SRC_BASE;
-    const Yuv16Coeffs yc16 = yuv16_of(d.fmt, yc);   // used by fmt 80-83 only
+    const bool yuv420_fast = !lanczos && f.fast_kernel && (d.dst_w % 4) == 0 && aligned16(dst) && d.dst_h <= 65535 * NV12_ROWS;
+    const YuvCoeffs& yc = YUV_COEFFS[matrix];
+    const Yuv16Coeffs yc16 = yuv16_coeffs(matrix, f.bits, f.layout == YUV420_NV12);   // used by the 16-bit 4:2:0 formats only
     Nv12Args nv{};
     nv.groups = (uint32_t)(d.dst_w + 3) / 4u;
     for (int c = 0; c < 3; ++c) nv.pad_norm[c] = (d.pad_value / 255.0f - d.mean[c]) * d.inv_std[c];  // BODY :610-612 on the host (f32, unfused)
@@ -871,45 +843,41 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, con
         if (frames) for (uint32_t k = 0; k < nb; ++k) fr.ptr[k] = frames[f0 + k];
         const bool p = frames != nullptr;
         if (identity && bayer) {
-            const int pattern = packed ? bayer_packed_pattern(d.fmt) : bayer_pattern(d.fmt, bayer16);
-            auto launch = [&](auto sample) {   // the kernel of pattern `pattern` for samples of the type of `sample`
+            auto launch = [&](auto sample) {   // the kernel of the format's pattern for samples of the type of `sample`
                 using T = decltype(sample);
-                switch (pattern) {
-                    case KB200_BAYER_RGGB: launch_bayer_identity<F16, T, KB200_BAYER_RGGB>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
-                    case KB200_BAYER_BGGR: launch_bayer_identity<F16, T, KB200_BAYER_BGGR>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
-                    case KB200_BAYER_GRBG: launch_bayer_identity<F16, T, KB200_BAYER_GRBG>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
-                    default: launch_bayer_identity<F16, T, KB200_BAYER_GBRG>(s, d, fr, p, dst, f0, nb, id_groups, id_items); break;
+                switch (f.pattern) {
+                    case KB200_BAYER_RGGB: launch_bayer_identity<F16, T, KB200_BAYER_RGGB>(s, d, fr, p, dst, f0, nb, id_groups, id_items, f.bits); break;
+                    case KB200_BAYER_BGGR: launch_bayer_identity<F16, T, KB200_BAYER_BGGR>(s, d, fr, p, dst, f0, nb, id_groups, id_items, f.bits); break;
+                    case KB200_BAYER_GRBG: launch_bayer_identity<F16, T, KB200_BAYER_GRBG>(s, d, fr, p, dst, f0, nb, id_groups, id_items, f.bits); break;
+                    default: launch_bayer_identity<F16, T, KB200_BAYER_GBRG>(s, d, fr, p, dst, f0, nb, id_groups, id_items, f.bits); break;
                 }
             };
-            const int bits = packed ? bayer_packed_bits(d.fmt) : 0;
-            if (bits == 10) launch(BayerPacked<10>{});
-            else if (bits == 12) launch(BayerPacked<12>{});
-            else if (bits == 14) launch(BayerPacked<14>{});
-            else if (bayer16) launch(uint16_t{});
-            else launch(uint8_t{});
-            KB200_TRY(check_launch(BAYER_IDENTITY_NAMES[packed ? 2 + (bits - 10) / 2 : bayer16][pattern]));
-            continue;
-        }
-        if ((identity || yuv420_fast) && yuv16) {
-            if (l420 == YUV420_I420) launch_yuv420_fast<F16, YUV420_I420, uint16_t>(s, identity, bil, d, yc16, fr, p, nv, dst, f0, nb, id_groups, id_items);
-            else launch_yuv420_fast<F16, YUV420_NV12, uint16_t>(s, identity, bil, d, yc16, fr, p, nv, dst, f0, nb, id_groups, id_items);
-            const int k = l420 == YUV420_I420;
-            KB200_TRY(check_launch(identity ? YUV16_IDENTITY_NAMES[k] : YUV16_FAST_NAMES[k]));
+            if (!f.packed && f.words) launch(uint16_t{});
+            else if (!f.packed) launch(uint8_t{});
+            else if (f.bits == 10) launch(BayerPacked<10>{});
+            else if (f.bits == 12) launch(BayerPacked<12>{});
+            else launch(BayerPacked<14>{});
+            KB200_TRY(check_launch(f.identity_kernel));
             continue;
         }
         if (identity || yuv420_fast) {
-            switch (l420) {
-                case YUV420_NV12: launch_yuv420_fast<F16, YUV420_NV12>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
-                case YUV420_NV21: launch_yuv420_fast<F16, YUV420_NV21>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
-                case YUV420_I420: launch_yuv420_fast<F16, YUV420_I420>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
-                default: launch_yuv420_fast<F16, YUV420_YV12>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+            if (f.words) {
+                if (f.layout == YUV420_I420) launch_yuv420_fast<F16, YUV420_I420, uint16_t>(s, identity, bil, d, yc16, fr, p, nv, dst, f0, nb, id_groups, id_items);
+                else launch_yuv420_fast<F16, YUV420_NV12, uint16_t>(s, identity, bil, d, yc16, fr, p, nv, dst, f0, nb, id_groups, id_items);
+            } else {
+                switch (f.layout) {
+                    case YUV420_NV12: launch_yuv420_fast<F16, YUV420_NV12>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                    case YUV420_NV21: launch_yuv420_fast<F16, YUV420_NV21>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                    case YUV420_I420: launch_yuv420_fast<F16, YUV420_I420>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                    default: launch_yuv420_fast<F16, YUV420_YV12>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                }
             }
-            KB200_TRY(check_launch(identity ? YUV420_IDENTITY_NAMES[l420] : YUV420_FAST_NAMES[l420]));
+            KB200_TRY(check_launch(identity ? f.identity_kernel : f.fast_kernel));
             continue;
         }
         dim3 grid(div_up(pixels, 256), nb);
-        if (p) launch_generic_for<F16, true>(ext, s, grid, d.sampling, d, yc, fr, dst, f0);
-        else launch_generic_for<F16, false>(ext, s, grid, d.sampling, d, yc, fr, dst, f0);
+        if (p) launch_generic_for<F16, true>(s, grid, d, f, yc, yc16, fr, dst, f0);
+        else launch_generic_for<F16, false>(s, grid, d, f, yc, yc16, fr, dst, f0);
         KB200_TRY(check_launch("preprocess_generic_kernel"));
     }
     return KB200_OK;
@@ -920,8 +888,8 @@ int preprocess_validate(const kb200_preprocess_desc* desc) { return validate_des
 size_t preprocess_frame_bytes(const kb200_preprocess_desc& d) { return src_bytes(plain_desc(d)); }
 int preprocess_launch_strided(cudaStream_t s, const kb200_preprocess_desc& desc, const uint8_t* base, size_t stride, uint32_t batch, void* dst, bool f16) {
     const kb200_preprocess_desc d = plain_desc(desc);
-    const YuvCoeffs& yc = yuv_coeffs(desc);
-    return f16 ? launch_preprocess<true>(s, d, yc, nullptr, base, stride, batch, dst) : launch_preprocess<false>(s, d, yc, nullptr, base, stride, batch, dst);
+    const int m = yuv_matrix(desc);
+    return f16 ? launch_preprocess<true>(s, d, m, nullptr, base, stride, batch, dst) : launch_preprocess<false>(s, d, m, nullptr, base, stride, batch, dst);
 }
 
 template <bool F16>
@@ -931,20 +899,18 @@ static int preprocess_entry(kb200_stream_t stream, const kb200_preprocess_desc* 
     KB200_TRY(validate_desc(raw_desc));
     const kb200_preprocess_desc plain = plain_desc(*raw_desc);
     const kb200_preprocess_desc* desc = &plain;
+    const SrcFormat f = src_format(desc->fmt);
     KB200_TRY(check_ptr("dst", dst));
     if (batch == 0) return fail(KB200_ERR_INVALID_ARGUMENT, "batch must be non-zero");
     const size_t need = src_bytes(*desc);
-    // 16-bit samples (fmt 32-47, 80-83): every frame must start 2-byte aligned.  `words` names the format in the messages.
-    char words[16] = "";
-    if (is_bayer16(desc->fmt)) snprintf(words, sizeof words, "%s%d", BAYER_NAMES[bayer16_pattern(desc->fmt)], bayer16_bits(desc->fmt));
-    else if (is_yuv16(desc->fmt)) snprintf(words, sizeof words, "%s", YUV16_NAMES[desc->fmt - KB200_FMT_P010]);
-    if (words[0] && !frames && ((reinterpret_cast<uintptr_t>(base) & 1u) || (batch > 1 && (stride & 1u))))
-        return fail(KB200_ERR_INVALID_SOURCE, "%s frames must start 2-byte aligned (base %p, stride %zu)", words, (const void*)base, stride);
+    // 16-bit samples: every frame must start 2-byte aligned
+    if (f.words && !frames && ((reinterpret_cast<uintptr_t>(base) & 1u) || (batch > 1 && (stride & 1u))))
+        return fail(KB200_ERR_INVALID_SOURCE, "%s frames must start 2-byte aligned (base %p, stride %zu)", f.name, (const void*)base, stride);
     if (frames) {
         for (uint32_t i = 0; i < batch; ++i) {
             if (!frames[i]) return fail(KB200_ERR_INVALID_ARGUMENT, "null frame pointer at index %u", i);
-            if (words[0] && (reinterpret_cast<uintptr_t>(frames[i]) & 1u))
-                return fail(KB200_ERR_INVALID_SOURCE, "%s frame %u is not 2-byte aligned", words, i);
+            if (f.words && (reinterpret_cast<uintptr_t>(frames[i]) & 1u))
+                return fail(KB200_ERR_INVALID_SOURCE, "%s frame %u is not 2-byte aligned", f.name, i);
             if (frame_len && frame_len[i] < need)  // InvalidRawSource{got,need}, preprocess.rs:1287-1300
                 return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source at %dx%d (got %zu bytes, need %zu)", desc->src_w, desc->src_h, frame_len[i], need);
         }
@@ -956,7 +922,7 @@ static int preprocess_entry(kb200_stream_t stream, const kb200_preprocess_desc* 
     }
     // BatchMismatch / BadOutputShape: dst must hold [batch,3,H,W]
     KB200_TRY(check_slice("dst", dst_len, (size_t)batch * 3 * desc->dst_w * desc->dst_h));
-    return launch_preprocess<F16>(as_stream(stream), *desc, yuv_coeffs(*raw_desc), frames, base, stride, batch, dst);
+    return launch_preprocess<F16>(as_stream(stream), *desc, yuv_matrix(*raw_desc), frames, base, stride, batch, dst);
 }
 
 __global__ void selftest_div255_kernel(unsigned long long* mismatches) {

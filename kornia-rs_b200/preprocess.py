@@ -14,7 +14,7 @@ from __future__ import annotations
 import ctypes as C
 import enum
 from dataclasses import dataclass
-from typing import Sequence
+from typing import NamedTuple, Sequence
 
 import torch
 
@@ -38,9 +38,6 @@ class PreprocessError(Exception):
 class ResizeMode(enum.Enum):  # preprocess.rs:67
     Letterbox = 0
     Stretch = 1
-
-
-_BAYER_PATTERNS = ("rggb", "bggr", "grbg", "gbrg")   # kb200_bayer_pattern order
 
 
 class SourceFormat(enum.Enum):  # preprocess.rs:130
@@ -107,68 +104,51 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
     I010 = "i010"
     I012 = "i012"
 
+    def _rec(self) -> "_Rec":
+        return _RECORDS[self.name]
+
     def fmt_code(self) -> int:  # :153-161
-        if self.is_bayer16():   # 32 + 4*k + pattern, k = 0..3 for 10, 12, 14, 16 bits
-            return 32 + 4 * ((self.bit_depth() - 10) // 2) + _BAYER_PATTERNS.index(self.value[6:10])
-        if self.is_bayer_packed():   # 64 + 4*k + pattern, k = 0..2 for 10, 12, 14 bits
-            return 64 + 4 * ((self.bit_depth() - 10) // 2) + _BAYER_PATTERNS.index(self.value[6:10])
-        return {"rgb8": 0, "rgba8": 0, "bgr8": 1, "bgra8": 1, "gray8": 2, "nv12": 3, "yuyv": 4,
-                "nv21": 5, "i420": 6, "yv12": 7, "uyvy": 8, "yvyu": 9,
-                "bayer_rggb": 16, "bayer_bggr": 17, "bayer_grbg": 18, "bayer_gbrg": 19,
-                "p010": 80, "p012": 81, "i010": 82, "i012": 83}[self.value]
+        return self._rec().code
 
     def bpp(self) -> int:  # :164-171
         """Bytes per sample; 1 for the packed Bayer formats, whose rows pitch() counts."""
-        if self.is_bayer16() or self.is_yuv16():
-            return 2
-        if self.is_bayer_packed():
-            return 1
-        return {"rgb8": 3, "bgr8": 3, "rgba8": 4, "bgra8": 4, "gray8": 1, "nv12": 1, "yuyv": 2,
-                "nv21": 1, "i420": 1, "yv12": 1, "uyvy": 2, "yvyu": 2,
-                "bayer_rggb": 1, "bayer_bggr": 1, "bayer_grbg": 1, "bayer_gbrg": 1}[self.value]
+        return self._rec().bpp or 1
 
     def pitch(self, w: int) -> int:
         """Bytes of a tight row of w pixels."""
-        if self.is_bayer_packed():
-            return w * self.bit_depth() // 8
-        return w * self.bpp()
+        r = self._rec()
+        return w * r.bits // 8 if r.bpp == 0 else w * r.bpp
 
     def is_yuv420(self) -> bool:
         """An 8-bit 4:2:0 format (one byte per sample); is_yuv16() names the 16-bit-word ones."""
-        return self in (SourceFormat.Nv12, SourceFormat.Nv21, SourceFormat.I420, SourceFormat.Yv12)
+        return self._rec().family == "yuv420" and self._rec().bpp == 1
 
     def is_yuv16(self) -> bool:
         """A 10- or 12-bit 4:2:0 format of 16-bit words: P010, P012, I010, I012."""
-        return self in (SourceFormat.P010, SourceFormat.P012, SourceFormat.I010, SourceFormat.I012)
+        return self._rec().family == "yuv420" and self._rec().bpp == 2
 
     def is_yuv422(self) -> bool:
-        return self in (SourceFormat.Yuyv, SourceFormat.Uyvy, SourceFormat.Yvyu)
+        return self._rec().family == "yuv422"
 
     def is_yuv(self) -> bool:
         """A YUV format: one a YuvMatrix applies to."""
-        return self.is_yuv420() or self.is_yuv422() or self.is_yuv16()
+        return self._rec().family in ("yuv420", "yuv422")
 
     def is_bayer(self) -> bool:
-        return self.value.startswith("bayer_")
+        return self._rec().family == "bayer"
 
     def is_bayer16(self) -> bool:
         """A Bayer format of 16-bit samples (10 to 16 bits per pixel)."""
-        return self.is_bayer() and len(self.value) > 10 and not self.is_bayer_packed()
+        return self.is_bayer() and self._rec().bpp == 2
 
     def is_bayer_packed(self) -> bool:
         """A MIPI-packed Bayer format (10, 12 or 14 bits per pixel)."""
-        return self.is_bayer() and self.value.endswith("p")
+        return self.is_bayer() and self._rec().bpp == 0
 
     def bit_depth(self) -> int | None:
         """Bits per sample of a Bayer format (8 for the byte mosaics) or of a 16-bit-word 4:2:0 format (10, 12), None for
         the other formats."""
-        if self.is_yuv16():
-            return int(self.value[2:])
-        if not self.is_bayer():
-            return None
-        if self.is_bayer_packed():
-            return int(self.value[10:-1])
-        return int(self.value[10:]) if self.is_bayer16() else 8
+        return self._rec().bits
 
     def buffer_len(self, w: int, h: int) -> int:  # :177-186
         # 4:2:0 chroma after the luma rows: w*h/2 samples, of 1 byte (is_yuv420) or 2 bytes (is_yuv16)
@@ -187,20 +167,37 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
         return True
 
     def interleaved(self) -> bool:  # :211-216
-        return self in (SourceFormat.Rgb8, SourceFormat.Bgr8, SourceFormat.Rgba8, SourceFormat.Bgra8)
+        return self._rec().family == "rgb"
 
     @staticmethod
     def from_name(name: str):  # :221-233
-        table = {"rgb": "Rgb8", "rgb8": "Rgb8", "bgr": "Bgr8", "bgr8": "Bgr8", "rgba": "Rgba8", "rgba8": "Rgba8",
-                 "bgra": "Bgra8", "bgra8": "Bgra8", "gray": "Gray8", "gray8": "Gray8", "nv12": "Nv12", "yuyv": "Yuyv",
-                 "nv21": "Nv21", "i420": "I420", "yv12": "Yv12", "uyvy": "Uyvy", "yvyu": "Yvyu",
-                 "bayer_rggb": "BayerRggb", "bayer_bggr": "BayerBggr", "bayer_grbg": "BayerGrbg", "bayer_gbrg": "BayerGbrg"}
-        table.update({f"bayer_{p}{b}": f"Bayer{p.capitalize()}{b}" for p in _BAYER_PATTERNS for b in (10, 12, 14, 16)})
-        table.update({f"bayer_{p}{b}p": f"Bayer{p.capitalize()}{b}p" for p in _BAYER_PATTERNS for b in (10, 12, 14)})
-        table.update({"p010": "P010", "p012": "P012", "i010": "I010", "i012": "I012", "p010le": "P010", "p012le": "P012",
-                      "yuv420p10le": "I010", "yuv420p12le": "I012"})
-        key = table.get(name.lower())
-        return None if key is None else SourceFormat[key]
+        name = name.lower()
+        return next((m for m in SourceFormat if name == m.value or name in m._rec().aliases), None)
+
+
+class _Rec(NamedTuple):   # one SourceFormat's facts
+    code: int                 # kb200_src_fmt
+    family: str               # "rgb" (interleaved RGB / BGR, with or without alpha), "gray", "yuv420", "yuv422" or "bayer"
+    bits: int | None = None   # bits per sample of a Bayer or 16-bit-word 4:2:0 format
+    bpp: int = 1              # bytes per sample (per pixel for "rgb" and "yuv422"); 0: MIPI-packed, bits / 8 per sample
+    aliases: tuple = ()       # from_name spellings besides the value
+
+
+_RECORDS = {
+    "Rgb8": _Rec(0, "rgb", bpp=3, aliases=("rgb",)), "Bgr8": _Rec(1, "rgb", bpp=3, aliases=("bgr",)),
+    "Rgba8": _Rec(0, "rgb", bpp=4, aliases=("rgba",)), "Bgra8": _Rec(1, "rgb", bpp=4, aliases=("bgra",)),
+    "Gray8": _Rec(2, "gray", aliases=("gray",)), "Nv12": _Rec(3, "yuv420"), "Yuyv": _Rec(4, "yuv422", bpp=2),
+    "Nv21": _Rec(5, "yuv420"), "I420": _Rec(6, "yuv420"), "Yv12": _Rec(7, "yuv420"),
+    "Uyvy": _Rec(8, "yuv422", bpp=2), "Yvyu": _Rec(9, "yuv422", bpp=2),
+    "P010": _Rec(80, "yuv420", 10, 2, ("p010le",)), "P012": _Rec(81, "yuv420", 12, 2, ("p012le",)),
+    "I010": _Rec(82, "yuv420", 10, 2, ("yuv420p10le",)), "I012": _Rec(83, "yuv420", 12, 2, ("yuv420p12le",)),
+}
+for _k, _p in enumerate(("rggb", "bggr", "grbg", "gbrg")):   # kb200_bayer_pattern order; codes 16 + pattern; 32 + 4*d + pattern, d = 0..3; 64 + 4*d + pattern, d = 0..2
+    _RECORDS[f"Bayer{_p.capitalize()}"] = _Rec(16 + _k, "bayer", 8)
+    for _d, _b in enumerate((10, 12, 14, 16)):
+        _RECORDS[f"Bayer{_p.capitalize()}{_b}"] = _Rec(32 + 4 * _d + _k, "bayer", _b, 2)
+    for _d, _b in enumerate((10, 12, 14)):
+        _RECORDS[f"Bayer{_p.capitalize()}{_b}p"] = _Rec(64 + 4 * _d + _k, "bayer", _b, 0)
 
 
 @dataclass(frozen=True)
