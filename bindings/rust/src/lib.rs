@@ -142,6 +142,8 @@ pub mod ffi {
         pub fn kb200_rgb_from_bayer_u16(stream: *mut c_void, src: *const u16, src_len: usize, dst: *mut u16, dst_len: usize, width: u32, height: u32, batch: u32, pattern: c_int) -> c_int;
         pub fn kb200_rgb_from_bayer_packed(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u16, dst_len: usize, width: u32, height: u32, batch: u32, pattern: c_int, bits: c_int) -> c_int;
         pub fn kb200_rgb_from_yuv420_u16(stream: *mut c_void, src: *const u16, src_len: usize, dst: *mut u16, dst_len: usize, width: u32, height: u32, batch: u32, layout: c_int, bits: c_int, matrix: c_int) -> c_int;
+        pub fn kb200_rgb_from_yuv444_u8(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut u8, dst_len: usize, width: u32, height: u32, batch: u32, matrix: c_int) -> c_int;
+        pub fn kb200_rgb_from_yuv444_u16(stream: *mut c_void, src: *const u16, src_len: usize, dst: *mut u16, dst_len: usize, width: u32, height: u32, batch: u32, layout: c_int, bits: c_int, matrix: c_int) -> c_int;
         pub fn kb200_normalize_mean_std_f32(stream: *mut c_void, src: *const f32, dst: *mut f32, npixels: usize, channels: u32, mean: *const f32, std: *const f32) -> c_int;
         pub fn kb200_normalize_rgb_u8_f32(stream: *mut c_void, src: *const u8, dst: *mut f32, npixels: usize, scale: *const f32, offset: *const f32, leaf: c_int) -> c_int;
         pub fn kb200_find_min_max_f32(stream: *mut c_void, src: *const f32, n: usize, minmax_dev: *mut f32) -> c_int;
@@ -257,6 +259,14 @@ pub const FMT_P010: i32 = 80;
 pub const FMT_P012: i32 = 81;
 pub const FMT_I010: i32 = 82;
 pub const FMT_I012: i32 = 83;
+/// 4:4:4 video, three full-resolution planes Y, U, V per tight frame: I444 (bytes, 3 * w * h), and I410 / I412 (16-bit
+/// little-endian words, 6 * w * h bytes, the code in the low bits) and I410 / I412 MSB (the code in the high bits:
+/// NVDEC's YUV444_16Bit surface).  Any w, h >= 1.  They take `fmt_yuv_matrix`.
+pub const FMT_I444: i32 = 11;
+pub const FMT_I410: i32 = 85;
+pub const FMT_I412: i32 = 86;
+pub const FMT_I410_MSB: i32 = 87;
+pub const FMT_I412_MSB: i32 = 88;
 
 /// `pattern` of `kb200_rgb_from_bayer_u8` (kb200_bayer_pattern): the mosaic's 2x2 quad read row-major.
 pub const BAYER_RGGB: c_int = 0;
@@ -279,6 +289,11 @@ pub const YUV422_YVYU: c_int = 2;
 /// high bits of each word) or I010 / I012 (U and V planes, codes in the low bits).
 pub const YUV420_P01X: c_int = 0;
 pub const YUV420_I01X: c_int = 1;
+
+/// `layout` of `kb200_rgb_from_yuv444_u16` (kb200_yuv444_u16_layout): I410 / I412 (codes in the low bits of each word)
+/// or their MSB-aligned form (codes in the high bits).
+pub const YUV444_I41X: c_int = 0;
+pub const YUV444_I41X_MSB: c_int = 1;
 
 /// `matrix` of `kb200_rgb_from_yuv420_u8_matrix` / `_yuv422_u8_matrix` (kb200_yuv_matrix): the colour matrix and range a
 /// YUV frame decodes with.  BT.601 limited is the reference's decode.
@@ -391,6 +406,37 @@ pub fn launch_rgb_from_yuv422_matrix(
     check(unsafe {
         ffi::kb200_rgb_from_yuv422_u8_matrix(stream.cu_stream() as *mut c_void, sp as *const u8, src_len, dp as *mut u8, dst_len, width, height,
                                              batch, layout, matrix)
+    })
+}
+
+/// An extension with no reference launcher: `batch` tight 8-bit 4:4:4 frames (I444: three w * h byte planes Y, U, V)
+/// -> RGB8 HWC, decoded with `matrix` (`YUV_*`).
+pub fn launch_rgb_from_yuv444_u8(
+    stream: &Arc<CudaStream>, src: &CudaSlice<u8>, dst: &mut CudaSlice<u8>, width: u32, height: u32, batch: u32, matrix: c_int,
+) -> Result<(), Kb200Error> {
+    bind(stream.context())?;
+    let (sp, _g0) = src.device_ptr(stream);
+    let (src_len, dst_len) = (src.len(), dst.len());
+    let (dp, _g1) = dst.device_ptr_mut(stream);
+    check(unsafe {
+        ffi::kb200_rgb_from_yuv444_u8(stream.cu_stream() as *mut c_void, sp as *const u8, src_len, dp as *mut u8, dst_len, width, height, batch, matrix)
+    })
+}
+
+/// An extension with no reference launcher: `batch` tight 10- or 12-bit (`bits`) 4:4:4 frames of 16-bit words in
+/// `layout` (`YUV444_*`) -> RGB16 HWC holding the n-bit codes, decoded with `matrix` (`YUV_*`).  Lengths in elements.
+#[allow(clippy::too_many_arguments)]
+pub fn launch_rgb_from_yuv444_u16(
+    stream: &Arc<CudaStream>, src: &CudaSlice<u16>, dst: &mut CudaSlice<u16>, width: u32, height: u32, batch: u32, layout: c_int, bits: c_int,
+    matrix: c_int,
+) -> Result<(), Kb200Error> {
+    bind(stream.context())?;
+    let (sp, _g0) = src.device_ptr(stream);
+    let (src_len, dst_len) = (src.len(), dst.len());
+    let (dp, _g1) = dst.device_ptr_mut(stream);
+    check(unsafe {
+        ffi::kb200_rgb_from_yuv444_u16(stream.cu_stream() as *mut c_void, sp as *const u16, src_len, dp as *mut u16, dst_len, width, height,
+                                       batch, layout, bits, matrix)
     })
 }
 

@@ -103,6 +103,8 @@ def _declare(l: C.CDLL) -> None:
         "kb200_rgb_from_bayer_u16": ([vp, vp, sz, vp, sz, u32, u32, u32, i], i),
         "kb200_rgb_from_bayer_packed": ([vp, vp, sz, vp, sz, u32, u32, u32, i, i], i),
         "kb200_rgb_from_yuv420_u16": ([vp, vp, sz, vp, sz, u32, u32, u32, i, i, i], i),
+        "kb200_rgb_from_yuv444_u8": ([vp, vp, sz, vp, sz, u32, u32, u32, i], i),
+        "kb200_rgb_from_yuv444_u16": ([vp, vp, sz, vp, sz, u32, u32, u32, i, i, i], i),
         "kb200_normalize_mean_std_f32": ([vp, vp, vp, sz, u32, fp, fp], i),
         "kb200_normalize_rgb_u8_f32": ([vp, vp, vp, sz, fp, fp, i], i),
         "kb200_find_min_max_f32": ([vp, vp, sz, vp], i),

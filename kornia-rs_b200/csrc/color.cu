@@ -1,5 +1,6 @@
 // color.cu — gray_from_rgb (f32, u8), the Q20 video decoders (4:2:0: NV12, NV21, I420, YV12; 4:2:2: YUYV, UYVY, YVYU;
-// BT.601 or BT.709, limited or full range: kb200_yuv_matrix) and the bilinear Bayer demosaic (RGGB, BGGR, GRBG, GBRG; bayer.cuh).
+// 4:4:4: I444; BT.601 or BT.709, limited or full range: kb200_yuv_matrix), their Q16 forms for 10- and 12-bit codes
+// (P010, P012, I010, I012; I410, I412 and their MSB-aligned forms) and the bilinear Bayer demosaic (RGGB, BGGR, GRBG, GBRG; bayer.cuh).
 //
 // Reference: color/gray/kernels.rs (CPU), cuda/color/gray.rs:17-68 (GPU twin, 1 px or 4 px per
 // thread, scalar 4-byte accesses); color/yuv/kernels.rs:707-1069 (CPU), cuda/color/video.rs:33-130
@@ -311,6 +312,114 @@ __global__ void rgb_from_yuv420_u16_generic(const uint16_t* __restrict__ src, ui
     int r, g, b;
     decode_rgb16(yy_term16(yuv16_code(frame[(size_t)y * width + x], k), k), ct, k.white, r, g, b);
     uint16_t* o = dst + ((size_t)blockIdx.z * plane + (size_t)y * width + x) * 3;
+    o[0] = (uint16_t)r; o[1] = (uint16_t)g; o[2] = (uint16_t)b;
+}
+
+// ── 4:4:4 (I444 bytes; I410, I412 and their MSB-aligned forms in 16-bit words) → RGB8 / RGB16 ──────────────────────
+// Three full-resolution planes Y, U, V: every pixel decodes from its own chroma.  One thread: one row's 16 pixels of bytes
+// or 8 pixels of words, i.e. one 16-B load from each plane (lane-contiguous over the warp), and 48 B of RGB stored through
+// store_rgb48_coalesced.  Requires width % 16 == 0 (bytes) / width % 8 == 0 (words) and 16-B aligned bases: then every
+// row of every plane starts 16-B aligned.  grid = (groups of a row, rows, frames).
+__global__ void __launch_bounds__(128) rgb_from_i444_vec16(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, uint32_t width,
+                                                           uint32_t height, const YuvCoeffs yc) {
+    __shared__ uint4 stage[4][96];
+    const uint32_t gx = blockIdx.x * blockDim.x + threadIdx.x;  // 16-column group
+    const uint32_t lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
+    const uint32_t gx0 = gx - lane;                             // first group of this warp
+    if (gx0 * 16 >= width) return;                              // whole warp out of the row
+    const bool full_warp = (gx0 + 32) * 16 <= width;
+    const bool active = gx * 16 < width;
+    const size_t plane = (size_t)width * height;
+    const uint8_t* frame = src + (size_t)blockIdx.z * plane * 3;
+    const size_t row = (size_t)blockIdx.y * width;
+    uint4 yv = make_uint4(0, 0, 0, 0), uv = yv, vv = yv;
+    if (active) {
+        const size_t p = row + (size_t)gx * 16;
+        yv = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + p));
+        uv = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + plane + p));
+        vv = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + 2 * plane + p));
+    }
+    const uint32_t yw[4] = {yv.x, yv.y, yv.z, yv.w}, uw[4] = {uv.x, uv.y, uv.z, uv.w}, vw[4] = {vv.x, vv.y, vv.z, vv.w};
+    uint32_t w[12];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {  // 4 px -> 12 bytes = 3 words: r0 g0 b0 r1 | g1 b1 r2 g2 | b2 r3 g3 b3
+        int r[4], g[4], b[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const ChromaTerms t = chroma_terms((int)byte_of(uw[k], j), (int)byte_of(vw[k], j), yc);
+            const int yy = yy_term((int)byte_of(yw[k], j), yc);
+            b[j] = (yy + t.b) >> 20; g[j] = (yy + t.g) >> 20; r[j] = (yy + t.r) >> 20;   // saturated by the pack below
+        }
+        w[3 * k] = pack_sat4(r[0], g[0], b[0], r[1]);
+        w[3 * k + 1] = pack_sat4(g[1], b[1], r[2], g[2]);
+        w[3 * k + 2] = pack_sat4(b[2], r[3], g[3], b[3]);
+    }
+    const uint4 o[3] = {make_uint4(w[0], w[1], w[2], w[3]), make_uint4(w[4], w[5], w[6], w[7]), make_uint4(w[8], w[9], w[10], w[11])};
+    uint4* d = reinterpret_cast<uint4*>(dst + (size_t)blockIdx.z * plane * 3 + (row + (size_t)gx0 * 16) * 3);   // this warp's 1536-B run
+    if (full_warp) store_rgb48_coalesced(d, stage[wid], lane, o);
+    else if (active) { stg_stream_u4(d + 3 * lane, o[0]); stg_stream_u4(d + 3 * lane + 1, o[1]); stg_stream_u4(d + 3 * lane + 2, o[2]); }
+}
+
+// The depth, code position and matrix arrive in Yuv16Coeffs, so one kernel serves I410, I412, I410Msb and I412Msb.
+__global__ void __launch_bounds__(128) rgb_from_i41x_vec(const uint16_t* __restrict__ src, uint16_t* __restrict__ dst, uint32_t width,
+                                                         uint32_t height, const Yuv16Coeffs k) {
+    __shared__ uint4 stage[4][96];
+    const uint32_t gx = blockIdx.x * blockDim.x + threadIdx.x;  // 8-column group
+    const uint32_t lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
+    const uint32_t gx0 = gx - lane;                             // first group of this warp
+    if (gx0 * 8 >= width) return;                               // whole warp out of the row
+    const bool full_warp = (gx0 + 32) * 8 <= width;
+    const bool active = gx * 8 < width;
+    const size_t plane = (size_t)width * height;
+    const uint16_t* frame = src + (size_t)blockIdx.z * plane * 3;
+    const size_t row = (size_t)blockIdx.y * width;
+    uint4 yv = make_uint4(0, 0, 0, 0), uv = yv, vv = yv;
+    if (active) {
+        const size_t p = row + (size_t)gx * 8;
+        yv = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + p));
+        uv = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + plane + p));
+        vv = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + 2 * plane + p));
+    }
+    const uint32_t yw[4] = {yv.x, yv.y, yv.z, yv.w}, uw[4] = {uv.x, uv.y, uv.z, uv.w}, vw[4] = {vv.x, vv.y, vv.z, vv.w};
+    int rgb[3][8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {   // yuv16_code keeps the n code bits of the low half-word it is shifted to
+        const int sh = 16 * (j & 1);
+        const ChromaTerms t = chroma_terms16(yuv16_code(uw[j >> 1] >> sh, k), yuv16_code(vw[j >> 1] >> sh, k), k);
+        decode_rgb16(yy_term16(yuv16_code(yw[j >> 1] >> sh, k), k), t, k.white, rgb[0][j], rgb[1][j], rgb[2][j]);
+    }
+    uint32_t w[12];   // 8 pixels -> 24 samples r0 g0 b0 r1 ..., two per 32-bit word
+#pragma unroll
+    for (int m = 0; m < 12; ++m) w[m] = (uint32_t)rgb[(2 * m) % 3][(2 * m) / 3] | ((uint32_t)rgb[(2 * m + 1) % 3][(2 * m + 1) / 3] << 16);
+    const uint4 o[3] = {make_uint4(w[0], w[1], w[2], w[3]), make_uint4(w[4], w[5], w[6], w[7]), make_uint4(w[8], w[9], w[10], w[11])};
+    uint4* d = reinterpret_cast<uint4*>(dst + (size_t)blockIdx.z * plane * 3 + (row + (size_t)gx0 * 8) * 3);   // this warp's 1536-B run
+    if (full_warp) store_rgb48_coalesced(d, stage[wid], lane, o);
+    else if (active) { stg_stream_u4(d + 3 * lane, o[0]); stg_stream_u4(d + 3 * lane + 1, o[1]); stg_stream_u4(d + 3 * lane + 2, o[2]); }
+}
+
+// Generic fallbacks (any width, unaligned bases; words 2-B aligned): one thread per pixel.
+__global__ void rgb_from_i444_generic(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, uint32_t width, uint32_t height,
+                                      const YuvCoeffs yc) {
+    const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= width || y >= height) return;
+    const size_t plane = (size_t)width * height, p = (size_t)y * width + x;
+    const uint8_t* frame = src + (size_t)blockIdx.z * plane * 3;
+    int r, g, b;
+    decode_rgb(yy_term(frame[p], yc), chroma_terms(frame[plane + p], frame[2 * plane + p], yc), r, g, b);
+    uint8_t* o = dst + ((size_t)blockIdx.z * plane + p) * 3;
+    o[0] = (uint8_t)r; o[1] = (uint8_t)g; o[2] = (uint8_t)b;
+}
+
+__global__ void rgb_from_i41x_generic(const uint16_t* __restrict__ src, uint16_t* __restrict__ dst, uint32_t width, uint32_t height,
+                                      const Yuv16Coeffs k) {
+    const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= width || y >= height) return;
+    const size_t plane = (size_t)width * height, p = (size_t)y * width + x;
+    const uint16_t* frame = src + (size_t)blockIdx.z * plane * 3;
+    int r, g, b;
+    decode_rgb16(yy_term16(yuv16_code(frame[p], k), k), chroma_terms16(yuv16_code(frame[plane + p], k), yuv16_code(frame[2 * plane + p], k), k),
+                 k.white, r, g, b);
+    uint16_t* o = dst + ((size_t)blockIdx.z * plane + p) * 3;
     o[0] = (uint16_t)r; o[1] = (uint16_t)g; o[2] = (uint16_t)b;
 }
 
@@ -768,6 +877,54 @@ KB200_API int kb200_rgb_from_yuv420_u16(kb200_stream_t stream, const uint16_t* s
     if (planar) rgb_from_yuv420_u16_generic<KB200_YUV420_I01X><<<grid, block, 0, s>>>(src, dst, width, height, k);
     else rgb_from_yuv420_u16_generic<KB200_YUV420_P01X><<<grid, block, 0, s>>>(src, dst, width, height, k);
     return check_launch(planar ? "rgb_from_i01x_generic" : "rgb_from_p01x_generic");
+}
+
+KB200_API int kb200_rgb_from_yuv444_u8(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst, size_t dst_len,
+                                       uint32_t width, uint32_t height, uint32_t batch, int matrix) {
+    KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
+    if (matrix < KB200_YUV_BT601_LIMITED || matrix > KB200_YUV_BT709_FULL) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown YUV matrix %d", matrix);
+    const YuvCoeffs& yc = YUV_COEFFS[matrix];
+    KB200_TRY(check_geometry(width, height, width, height, batch));
+    if (batch > 65535u) return fail(KB200_ERR_INVALID_ARGUMENT, "batch %u exceeds 65535", batch);
+    const size_t plane = (size_t)width * height;
+    KB200_TRY(check_slice("src", src_len, plane * 3 * batch)); KB200_TRY(check_slice("dst", dst_len, plane * 3 * batch));
+    cudaStream_t s = as_stream(stream);
+    if ((width % 16u) == 0 && aligned16(src) && aligned16(dst) && height <= 65535u) {
+        const unsigned groups = width / 16;
+        const unsigned bx = groups >= 128 ? 128 : 32 * ((groups + 31) / 32);
+        dim3 grid(div_up(groups, bx), height, batch);
+        rgb_from_i444_vec16<<<grid, bx, 0, s>>>(src, dst, width, height, yc);
+        return check_launch("rgb_from_i444_vec16");
+    }
+    dim3 block(32, 8), grid(div_up(width, 32), div_up(height, 8), batch);
+    rgb_from_i444_generic<<<grid, block, 0, s>>>(src, dst, width, height, yc);
+    return check_launch("rgb_from_i444_generic");
+}
+
+KB200_API int kb200_rgb_from_yuv444_u16(kb200_stream_t stream, const uint16_t* src, size_t src_len, uint16_t* dst, size_t dst_len,
+                                        uint32_t width, uint32_t height, uint32_t batch, int layout, int bits, int matrix) {
+    KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
+    if (reinterpret_cast<uintptr_t>(src) & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "'src' is not 2-byte aligned (16-bit samples)");
+    if (reinterpret_cast<uintptr_t>(dst) & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "'dst' is not 2-byte aligned (16-bit samples)");
+    if (layout != KB200_YUV444_I41X && layout != KB200_YUV444_I41X_MSB) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown 16-bit 4:4:4 layout %d", layout);
+    if (bits != 10 && bits != 12) return fail(KB200_ERR_INVALID_ARGUMENT, "16-bit 4:4:4 samples are 10 or 12 bits, got %d", bits);
+    if (matrix < KB200_YUV_BT601_LIMITED || matrix > KB200_YUV_BT709_FULL) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown YUV matrix %d", matrix);
+    const Yuv16Coeffs k = yuv16_coeffs(matrix, bits, layout == KB200_YUV444_I41X_MSB);
+    KB200_TRY(check_geometry(width, height, width, height, batch));
+    if (batch > 65535u) return fail(KB200_ERR_INVALID_ARGUMENT, "batch %u exceeds 65535", batch);
+    const size_t plane = (size_t)width * height;
+    KB200_TRY(check_slice("src", src_len, plane * 3 * batch)); KB200_TRY(check_slice("dst", dst_len, plane * 3 * batch));
+    cudaStream_t s = as_stream(stream);
+    if ((width % 8u) == 0 && aligned16(src) && aligned16(dst) && height <= 65535u) {
+        const unsigned groups = width / 8;
+        const unsigned bx = groups >= 128 ? 128 : 32 * ((groups + 31) / 32);
+        dim3 grid(div_up(groups, bx), height, batch);
+        rgb_from_i41x_vec<<<grid, bx, 0, s>>>(src, dst, width, height, k);
+        return check_launch("rgb_from_i41x_vec");
+    }
+    dim3 block(32, 8), grid(div_up(width, 32), div_up(height, 8), batch);
+    rgb_from_i41x_generic<<<grid, block, 0, s>>>(src, dst, width, height, k);
+    return check_launch("rgb_from_i41x_generic");
 }
 
 KB200_API int kb200_rgb_from_yuv422_u8_matrix(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst,

@@ -93,6 +93,8 @@ __host__ __device__ constexpr bool yuv420_planar(int L) { return L == YUV420_I42
 // byte offsets of the U and V planes of a planar frame (w, h even)
 __host__ __device__ inline size_t yuv420_u_plane(int L, size_t w, size_t h) { return L == YUV420_I420 ? w * h : w * h + w * h / 4; }
 __host__ __device__ inline size_t yuv420_v_plane(int L, size_t w, size_t h) { return L == YUV420_I420 ? w * h + w * h / 4 : w * h; }
+// 4:4:4 as a layout beside the 4:2:0 ones, for the preprocess taps: three full-resolution planes Y, U, V (I444, I41x).
+static constexpr int YUV444 = 4;
 
 // 4:2:2 layouts (kb200_yuv422_layout): each 2-px group is one 32-bit word; Yuv422Bytes<L> gives the byte of Y0, Y1,
 // U and V in it.  YUYV = Y0 U Y1 V, UYVY = U Y0 V Y1, YVYU = Y0 V Y1 U.

@@ -1,6 +1,6 @@
 // preprocess.cu — the fused camera preprocess (a12; BASELINE config 3): raw frame (RGB/BGR/RGBA/
 // Gray/NV12/YUYV, tight or pitched; beyond the reference also NV21/I420/YV12/UYVY/YVYU, the 8- and 16-bit Bayer
-// mosaics and the 10- and 12-bit 4:2:0 video P010/P012/I010/I012) →
+// mosaics, the 10- and 12-bit 4:2:0 video P010/P012/I010/I012 and the 4:4:4 video I444/I410/I412/I410Msb/I412Msb) →
 // letterbox/stretch resample → (v/255 - mean) * inv_std → planar CHW f32 or f16, for a whole batch in ONE launch.
 // The 4:2:0 formats share the NV12 kernels (templated on the chroma layout); the 4:2:2 formats take the generic kernel.
 // A Bayer tap is the demosaiced pixel at the tap's coordinate (bayer.cuh); Bayer frames take the generic kernel, except
@@ -11,6 +11,8 @@
 // The 10- and 12-bit 4:2:0 formats (fmt 80-83: P010, P012 in NV12's layout, I010, I012 in I420's, one 16-bit word per
 // sample) take the 4:2:0 fast kernels instantiated for 16-bit words, with the Q16 set of their matrix and depth; a tap is
 // the decoded n-bit code, normalised like a 16-bit Bayer tap by W = 2^n - 1.
+// The 4:4:4 formats (fmt 11: I444 bytes; 85-88: I410, I412, I410Msb, I412Msb words) take their own identity kernel and
+// preprocess_yuv_kernel in the YUV444 layout, the 4:2:0 layouts' resampler with a tap that reads the pixel's own chroma.
 //
 // Reference: preprocess.rs:430-647 (the CUDA source string — the specification of this path; there
 // is no CPU implementation for the camera formats), launch seam :1324-1372, batch loop :1277-1280
@@ -79,12 +81,13 @@ __device__ __forceinline__ float div255_exact(float p) {
 
 // The facts of one source format code (kb200_src_fmt without the matrix bits), from SRC_FORMATS below.  Every host
 // function reads them from here; the generic kernel takes its format's as an argument.
-enum SrcFamily { SRC_NONE, SRC_RGB, SRC_GRAY, SRC_YUV420, SRC_YUV422, SRC_BAYER };
+enum SrcFamily { SRC_NONE, SRC_RGB, SRC_GRAY, SRC_YUV420, SRC_YUV422, SRC_BAYER, SRC_YUV444 };
 struct SrcFormat {
     int code = -1;
     const char* name = nullptr;   // the SourceFormat name in messages; nullptr: the code is not a format
     SrcFamily family = SRC_NONE;
-    int layout = 0;    // SRC_RGB: 0 RGB, 1 BGR order; SRC_YUV420: kb200_yuv420_layout (P01x NV12's, I01x I420's); SRC_YUV422: kb200_yuv422_layout
+    int layout = 0;    // SRC_RGB: 0 RGB, 1 BGR order; SRC_YUV420: kb200_yuv420_layout (P01x NV12's, I01x I420's); SRC_YUV422: kb200_yuv422_layout;
+                       // SRC_YUV444: kb200_yuv444_u16_layout (I41x's code position; 0 for I444)
     int pattern = 0;   // SRC_BAYER: kb200_bayer_pattern
     int bits = 8;      // bits per sample
     bool words = false;    // one little-endian 16-bit word per sample
@@ -105,11 +108,26 @@ __device__ __forceinline__ float div_white(float p, float w) {
     return zero ? p : q;
 }
 
-// One decoded tap of a 4:2:0 frame in layout L (kb200_yuv420_layout): the generic kernel and preprocess_yuv420_kernel
-// serve all four layouts through it.  PAIR: an interleaved chroma pair is read as one 16-bit word, which needs a 2-B
-// aligned frame (the fast kernel's); the generic kernel reads its two bytes, so it takes frames at any address.
+// One decoded tap of a 4:2:0 frame in layout L (kb200_yuv420_layout), or of a 4:4:4 frame (L = YUV444: the pixel's own
+// U and V from the full-resolution planes): the generic kernel and preprocess_yuv_kernel serve all five layouts through
+// it.  PAIR: an interleaved chroma pair is read as one 16-bit word, which needs a 2-B aligned frame (the fast kernel's);
+// the generic kernel reads its two bytes, so it takes frames at any address.
 template <int L, bool PAIR = true>
-__device__ __forceinline__ void yuv420_tap(const uint8_t* __restrict__ src, int x, int y, int w, int h, const YuvCoeffs& yc, int rgb[3]) {
+__device__ __forceinline__ void yuv_tap(const uint8_t* __restrict__ src, int x, int y, int w, int h, const YuvCoeffs& yc, int rgb[3]) {
+    if constexpr (L == YUV444) {
+        // The same three bytes either way; each kernel gets the addressing with which ptxas allocates it without spills:
+        // the fast kernel's f16 bilinear instantiations spill with the row form, the generic Lanczos loop with the other.
+        int yv, u, v;
+        if constexpr (PAIR) {
+            const uint8_t* p = src + (size_t)y * w + x;
+            const size_t plane = (size_t)w * h;
+            yv = __ldg(p); u = __ldg(p + plane); v = __ldg(p + 2 * plane);
+        } else {   // the frame as 3h rows: Y rows, then U rows, then V rows
+            yv = __ldg(src + (size_t)y * w + x); u = __ldg(src + (size_t)(y + h) * w + x); v = __ldg(src + (size_t)(y + 2 * h) * w + x);
+        }
+        decode_rgb(yy_term(yv, yc), chroma_terms(u, v, yc), rgb[0], rgb[1], rgb[2]);
+        return;
+    }
     const int yv = __ldg(src + (size_t)y * w + x);
     ChromaTerms t;
     if (yuv420_planar(L)) {
@@ -124,14 +142,17 @@ __device__ __forceinline__ void yuv420_tap(const uint8_t* __restrict__ src, int 
     }
     decode_rgb(yy_term(yv, yc), t, rgb[0], rgb[1], rgb[2]);
 }
-// ... and of a frame of 16-bit words (the coefficient type selects it): P01x in the NV12 layout, I01x in the I420 layout.
-// A P01x tap reads its chroma pair as two 16-bit words, since frames are only 2-B aligned.
+// ... and of a frame of 16-bit words (the coefficient type selects it): P01x in the NV12 layout, I01x in the I420 layout,
+// I41x in the 4:4:4 one.  A P01x tap reads its chroma pair as two 16-bit words, since frames are only 2-B aligned.
 template <int L>
-__device__ __forceinline__ void yuv420_tap(const uint8_t* __restrict__ src, int x, int y, int w, int h, const Yuv16Coeffs& k, int rgb[3]) {
+__device__ __forceinline__ void yuv_tap(const uint8_t* __restrict__ src, int x, int y, int w, int h, const Yuv16Coeffs& k, int rgb[3]) {
     const uint16_t* s = reinterpret_cast<const uint16_t*>(src);
     const size_t plane = (size_t)w * h;
     size_t cu, cv;
-    if (yuv420_planar(L)) {
+    if constexpr (L == YUV444) {
+        cu = plane + (size_t)y * w + x;
+        cv = cu + plane;
+    } else if (yuv420_planar(L)) {
         cu = plane + (size_t)(y >> 1) * (w >> 1) + (x >> 1);
         cv = cu + plane / 4;
     } else {
@@ -152,12 +173,16 @@ __device__ __forceinline__ void yuv422_tap(const uint8_t* __restrict__ src, int 
 }
 
 // The taps an instantiation of the generic kernel reads: interleaved RGB / BGR or gray bytes, 4:2:2, the 16-bit words of
-// P01x / I01x, a Bayer mosaic of bytes, 16-bit words or packed samples, or 8-bit 4:2:0 in one layout (TAP_YUV420 +
-// kb200_yuv420_layout).  Within a kind the format's layout is a uniform branch.  The 4:2:0 layouts get an instantiation
-// each: with the four taps in one kernel, its Lanczos loop no longer unrolls and spills.  TapCoeffs: the coefficient
-// argument, the Q16 set with its code extraction for the 16-bit words (as in the fast kernels), the Q20 set otherwise.
+// P01x / I01x, a Bayer mosaic of bytes, 16-bit words or packed samples, 8-bit 4:2:0 in one layout (TAP_YUV420 +
+// kb200_yuv420_layout), 8-bit 4:4:4 (TAP_YUV444, the same tap in the YUV444 layout) or the 16-bit words of I41x
+// (TAP_YUV444_16).  Within a kind the format's layout is a uniform branch.  The 4:2:0 layouts get an instantiation
+// each: with the four taps in one kernel, its Lanczos loop no longer unrolls and spills; for the same reason 4:4:4 is not
+// a branch of TAP_YUV16.  TapCoeffs: the coefficient argument, the Q16 set with its code extraction for the 16-bit words
+// (as in the fast kernels), the Q20 set otherwise.
 static constexpr int TAP_RGB = 0, TAP_YUV422 = 1, TAP_YUV16 = 2, TAP_BAYER = 3, TAP_BAYER16 = 4, TAP_BAYER_PACKED = 5, TAP_YUV420 = 6;
-template <int TAP> using TapCoeffs = std::conditional_t<TAP == TAP_YUV16, Yuv16Coeffs, YuvCoeffs>;
+static constexpr int TAP_YUV444 = TAP_YUV420 + YUV444, TAP_YUV444_16 = TAP_YUV444 + 1;
+template <int TAP> constexpr bool tap_words = TAP == TAP_YUV16 || TAP == TAP_YUV444_16;   // YUV taps of 16-bit words
+template <int TAP> using TapCoeffs = std::conditional_t<tap_words<TAP>, Yuv16Coeffs, YuvCoeffs>;
 
 template <int TAP>
 __device__ __forceinline__ void fetch_px(const uint8_t* __restrict__ src, int x, int y, const kb200_preprocess_desc& d, const SrcFormat& f,
@@ -180,10 +205,12 @@ __device__ __forceinline__ void fetch_px(const uint8_t* __restrict__ src, int x,
     } else if constexpr (TAP == TAP_BAYER_PACKED) {
         bayer_px_packed(src, (size_t)d.src_pitch, d.src_w, d.src_h, x, y, f.pattern, f.bits, rgb);
     } else if constexpr (TAP == TAP_YUV16) {
-        if (f.layout == YUV420_I420) yuv420_tap<YUV420_I420>(src, x, y, d.src_w, d.src_h, yc, rgb);
-        else yuv420_tap<YUV420_NV12>(src, x, y, d.src_w, d.src_h, yc, rgb);
+        if (f.layout == YUV420_I420) yuv_tap<YUV420_I420>(src, x, y, d.src_w, d.src_h, yc, rgb);
+        else yuv_tap<YUV420_NV12>(src, x, y, d.src_w, d.src_h, yc, rgb);
+    } else if constexpr (TAP == TAP_YUV444_16) {
+        yuv_tap<YUV444>(src, x, y, d.src_w, d.src_h, yc, rgb);
     } else if constexpr (TAP >= TAP_YUV420) {
-        yuv420_tap<TAP - TAP_YUV420, false>(src, x, y, d.src_w, d.src_h, yc, rgb);
+        yuv_tap<TAP - TAP_YUV420, false>(src, x, y, d.src_w, d.src_h, yc, rgb);
     } else {
         switch (f.layout) {
             case YUV422_YUYV: yuv422_tap<YUV422_YUYV>(src, x, y, d.src_pitch, yc, rgb); break;
@@ -269,7 +296,7 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
         px[0] = d.pad_value; px[1] = d.pad_value; px[2] = d.pad_value;
     }
     float q0, q1, q2;
-    if (TAP == TAP_YUV16 && inside) {   // px / W, the IEEE quotient (div_white: no zero dividend reaches the division)
+    if (tap_words<TAP> && inside) {   // px / W, the IEEE quotient (div_white: no zero dividend reaches the division)
         const float wl = sf.white();
         q0 = div_white(px[0], wl); q1 = div_white(px[1], wl); q2 = div_white(px[2], wl);
     } else if ((TAP == TAP_BAYER16 || TAP == TAP_BAYER_PACKED) && inside) {   // px / W: taps up to 65535 and Lanczos overshoot, so the IEEE division
@@ -321,11 +348,11 @@ __device__ __forceinline__ void nv12_store4(void* __restrict__ dst, size_t idx, 
 
 __device__ __forceinline__ float norm_int_px(int r, float m, float is) { return (div255_exact((float)r) - m) * is; }
 
-// The sample type T of a 4:2:0 frame: bytes (NV12, NV21, I420, YV12), or 16-bit words holding n-bit codes — P01x in the
-// NV12 layout, I01x in the I420 layout.  Coeffs is the fast kernels' coefficient argument: the Q20 set for bytes, the Q16
+// The sample type T of a 4:2:0 or 4:4:4 frame: bytes (NV12, NV21, I420, YV12, I444), or 16-bit words holding n-bit codes
+// — P01x in the NV12 layout, I01x in the I420 layout, I41x in the 4:4:4 one.  Coeffs is the fast kernels' coefficient argument: the Q20 set for bytes, the Q16
 // set with its code extraction (Yuv16Coeffs) for words.
-template <typename T> struct Yuv420Sample { using Coeffs = YuvCoeffs; };
-template <> struct Yuv420Sample<uint16_t> { using Coeffs = Yuv16Coeffs; };
+template <typename T> struct YuvSample { using Coeffs = YuvCoeffs; };
+template <> struct YuvSample<uint16_t> { using Coeffs = Yuv16Coeffs; };
 
 // One thread = 4 luma columns x 2 rows.  Every warp-level access is lane-contiguous: 3 x LDG.32 (128 B per
 // warp), 6 x STG.128 (512 contiguous bytes per warp per plane row).  [The first version gave each thread 8
@@ -340,7 +367,7 @@ template <bool F16, bool PTRS, int L, typename T>
 __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                          const __grid_constant__ PreFrames fr, void* __restrict__ dst,
                                                                          uint32_t frame0, uint32_t groups_per_row, uint32_t items,
-                                                                         const typename Yuv420Sample<T>::Coeffs yc) {
+                                                                         const typename YuvSample<T>::Coeffs yc) {
     const uint32_t item = blockIdx.x * blockDim.x + threadIdx.x;
     if (item >= items) return;
     const uint32_t rp = item / groups_per_row, g = item - rp * groups_per_row;
@@ -428,6 +455,61 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const _
             nv12_store4<F16>(dst, o + 2 * plane, b4);
         }
     }
+}
+
+// ── 4:4:4 identity fast path (the config-3a shape from I444 / I41x frames: scale 1, no pad, same size) ──────────────
+// Every pixel has its own chroma, so one thread = 4 columns of one row: one lane-contiguous load from each of the Y, U
+// and V planes (LDG.32 of 4 bytes, LDG.64 of 4 words: w % 4 == 0 and a frame aligned to that load align every plane's
+// rows), 3 x nv12_store4.  Bytes are normalised as in the 4:2:0 kernel (norm_int_px), words by W through div_white.
+template <bool F16, bool PTRS, typename T>
+__global__ void __launch_bounds__(128) preprocess_yuv444_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
+                                                                         const __grid_constant__ PreFrames fr, void* __restrict__ dst,
+                                                                         uint32_t frame0, uint32_t groups_per_row, uint32_t items,
+                                                                         const typename YuvSample<T>::Coeffs yc) {
+    const uint32_t item = blockIdx.x * blockDim.x + threadIdx.x;
+    if (item >= items) return;
+    const uint32_t y = item / groups_per_row, g = item - y * groups_per_row;
+    const uint32_t w = (uint32_t)d.src_w, h = (uint32_t)d.src_h;
+    const uint32_t f = blockIdx.y;
+    const uint8_t* src = PTRS ? fr.ptr[f] : fr.base + (size_t)(frame0 + f) * fr.stride;
+    const size_t plane = (size_t)w * h, p = (size_t)y * w + g * 4u;
+    const float m0 = d.mean[0], m1 = d.mean[1], m2 = d.mean[2], i0 = d.inv_std[0], i1 = d.inv_std[1], i2 = d.inv_std[2];
+    float r4[4], g4[4], b4[4];
+    if constexpr (sizeof(T) == 2) {
+        const uint16_t* s = reinterpret_cast<const uint16_t*>(src);
+        const uint2 yv = __ldg(reinterpret_cast<const uint2*>(s + p));
+        const uint2 uv = __ldg(reinterpret_cast<const uint2*>(s + plane + p));
+        const uint2 vv = __ldg(reinterpret_cast<const uint2*>(s + 2 * plane + p));
+        const float wl = (float)yc.white;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int sh = 16 * (i & 1);
+            const uint32_t yw = i < 2 ? yv.x : yv.y, uw = i < 2 ? uv.x : uv.y, vw = i < 2 ? vv.x : vv.y;
+            int r, gg, b;
+            decode_rgb16(yy_term16(yuv16_code(yw >> sh, yc), yc), chroma_terms16(yuv16_code(uw >> sh, yc), yuv16_code(vw >> sh, yc), yc),
+                         yc.white, r, gg, b);
+            r4[i] = (div_white((float)r, wl) - m0) * i0;
+            g4[i] = (div_white((float)gg, wl) - m1) * i1;
+            b4[i] = (div_white((float)b, wl) - m2) * i2;
+        }
+    } else {
+        const uint32_t yw = __ldg(reinterpret_cast<const uint32_t*>(src + p));
+        const uint32_t uw = __ldg(reinterpret_cast<const uint32_t*>(src + plane + p));
+        const uint32_t vw = __ldg(reinterpret_cast<const uint32_t*>(src + 2 * plane + p));
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            int r, gg, b;
+            decode_rgb(yy_term((int)((yw >> (8 * i)) & 0xFFu), yc), chroma_terms((int)((uw >> (8 * i)) & 0xFFu), (int)((vw >> (8 * i)) & 0xFFu), yc),
+                       r, gg, b);
+            r4[i] = norm_int_px(r, m0, i0);
+            g4[i] = norm_int_px(gg, m1, i1);
+            b4[i] = norm_int_px(b, m2, i2);
+        }
+    }
+    const size_t o = (size_t)(frame0 + f) * 3 * plane + p;
+    nv12_store4<F16>(dst, o, r4);
+    nv12_store4<F16>(dst, o + plane, g4);
+    nv12_store4<F16>(dst, o + 2 * plane, b4);
 }
 
 // ── Bayer identity fast path (the config-3a shape from a Bayer mosaic: scale 1, no pad, same size) ──────────────
@@ -532,12 +614,12 @@ struct Nv12Args {
 
 static constexpr int NV12_ROWS = 8;  // destination rows per thread: the x-side of the sampler is computed once for all of them
 
-// T: the sample type (Yuv420Sample).  A pixel of 16-bit words is normalised as (px / W - mean) * inv_std with the IEEE
-// division, interpolated or not.
+// L: a 4:2:0 layout or YUV444 (yuv_tap); T: the sample type (YuvSample).  A pixel of 16-bit words is normalised as
+// (px / W - mean) * inv_std with the IEEE division, interpolated or not.
 template <bool F16, bool BILINEAR, bool PTRS, int L, typename T>
-__global__ void __launch_bounds__(128) preprocess_yuv420_kernel(const __grid_constant__ kb200_preprocess_desc d,
-                                                                const __grid_constant__ PreFrames fr, const __grid_constant__ Nv12Args na,
-                                                                void* __restrict__ dst, uint32_t frame0, const typename Yuv420Sample<T>::Coeffs yc) {
+__global__ void __launch_bounds__(128) preprocess_yuv_kernel(const __grid_constant__ kb200_preprocess_desc d,
+                                                             const __grid_constant__ PreFrames fr, const __grid_constant__ Nv12Args na,
+                                                             void* __restrict__ dst, uint32_t frame0, const typename YuvSample<T>::Coeffs yc) {
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= na.groups) return;
     const uint32_t f = blockIdx.z;
@@ -550,16 +632,18 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_kernel(const __grid_con
     float ax[4];
     bool xin[4];
     bool any_in = false;
-    // 16-bit samples: the four divisions first, so that only their quotients are live across the slow-path calls they may
-    // make (the interleaved form spilled in the f16 bilinear instantiation); the 8-bit kernels keep the interleaved form
+    // 16-bit samples and 4:4:4: the four divisions first, so that only their quotients are live across the slow-path calls
+    // they may make (the interleaved form spilled in the f16 bilinear instantiations); the 8-bit 4:2:0 kernels keep the
+    // interleaved form
+    constexpr bool SX_FIRST = sizeof(T) == 2 || L == YUV444;
     [[maybe_unused]] float sx16[4];
-    if constexpr (sizeof(T) == 2) {
+    if constexpr (SX_FIRST) {
 #pragma unroll
         for (int j = 0; j < 4; ++j) sx16[j] = __fdiv_rn((float)(ox0 + j) - d.pad_x, d.scale_x);
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-        const float sx = sizeof(T) == 2 ? sx16[j] : __fdiv_rn((float)(ox0 + j) - d.pad_x, d.scale_x);
+        const float sx = SX_FIRST ? sx16[j] : __fdiv_rn((float)(ox0 + j) - d.pad_x, d.scale_x);
         xin[j] = !(sx < 0.0f || sx >= (float)w);
         any_in = any_in || xin[j];
         if (BILINEAR) {
@@ -600,17 +684,17 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_kernel(const __grid_con
             for (int j = 0; j < 4; ++j) {
                 if (!xin[j]) { o[0][j] = na.pad_norm[0]; o[1][j] = na.pad_norm[1]; o[2][j] = na.pad_norm[2]; continue; }
                 int t00[3];
-                yuv420_tap<L>(src, xa[j], y0, w, h, yc, t00);
+                yuv_tap<L>(src, xa[j], y0, w, h, yc, t00);
                 const bool need_x = BILINEAR && ax[j] != 0.0f;
                 float px[3];
                 if (!need_x && !need_y) {  // the sample IS the decoded tap (exact, see header)
                     px[0] = (float)t00[0]; px[1] = (float)t00[1]; px[2] = (float)t00[2];
                 } else {
                     int t10[3] = {0, 0, 0}, t01[3] = {0, 0, 0}, t11[3] = {0, 0, 0};
-                    if (need_x) yuv420_tap<L>(src, xb[j], y0, w, h, yc, t10);
+                    if (need_x) yuv_tap<L>(src, xb[j], y0, w, h, yc, t10);
                     if (need_y) {
-                        yuv420_tap<L>(src, xa[j], y1, w, h, yc, t01);
-                        if (need_x) yuv420_tap<L>(src, xb[j], y1, w, h, yc, t11);
+                        yuv_tap<L>(src, xa[j], y1, w, h, yc, t01);
+                        if (need_x) yuv_tap<L>(src, xb[j], y1, w, h, yc, t11);
                     }
 #pragma unroll
                     for (int c = 0; c < 3; ++c) {
@@ -676,6 +760,13 @@ static const SrcFormat SRC_FORMATS[] = {
     {KB200_FMT_P012, "P012", SRC_YUV420, YUV420_NV12, 0, 12, true, false, "preprocess_p01x_identity_kernel", "preprocess_p01x_kernel"},
     {KB200_FMT_I010, "I010", SRC_YUV420, YUV420_I420, 0, 10, true, false, "preprocess_i01x_identity_kernel", "preprocess_i01x_kernel"},
     {KB200_FMT_I012, "I012", SRC_YUV420, YUV420_I420, 0, 12, true, false, "preprocess_i01x_identity_kernel", "preprocess_i01x_kernel"},
+    // 4:4:4 video: three full-resolution planes, of bytes (I444) or of 16-bit words with each code in the low (I41x) or the
+    // high bits (I41xMsb); the 4:4:4 identity kernel and the YUV444 instantiations of preprocess_yuv_kernel serve them
+    {KB200_FMT_I444, "I444", SRC_YUV444, 0, 0, 8, false, false, "preprocess_i444_identity_kernel", "preprocess_i444_kernel"},
+    {KB200_FMT_I410, "I410", SRC_YUV444, KB200_YUV444_I41X, 0, 10, true, false, "preprocess_i41x_identity_kernel", "preprocess_i41x_kernel"},
+    {KB200_FMT_I412, "I412", SRC_YUV444, KB200_YUV444_I41X, 0, 12, true, false, "preprocess_i41x_identity_kernel", "preprocess_i41x_kernel"},
+    {KB200_FMT_I410_MSB, "I410Msb", SRC_YUV444, KB200_YUV444_I41X_MSB, 0, 10, true, false, "preprocess_i41x_identity_kernel", "preprocess_i41x_kernel"},
+    {KB200_FMT_I412_MSB, "I412Msb", SRC_YUV444, KB200_YUV444_I41X_MSB, 0, 12, true, false, "preprocess_i41x_identity_kernel", "preprocess_i41x_kernel"},
 };
 #undef KB200_BAYER_FORMATS
 
@@ -695,8 +786,9 @@ static kb200_preprocess_desc plain_desc(const kb200_preprocess_desc& d) {
 static int yuv_matrix(const kb200_preprocess_desc& raw) { return (raw.fmt >> 8) & 3; }
 
 static size_t src_bytes(const kb200_preprocess_desc& d) {
-    // 4:2:0 chroma after the pitch * h luma bytes: w*h/2 samples, of 1 byte or of 2 (16-bit words)
+    // 4:2:0 chroma after the pitch * h luma bytes: w*h/2 samples, of 1 byte or of 2 (16-bit words); 4:4:4: two more planes
     const SrcFormat f = src_format(d.fmt);
+    if (f.family == SRC_YUV444) return (size_t)d.src_pitch * d.src_h * 3;
     const size_t chroma = f.family != SRC_YUV420 ? 0 : f.words ? (size_t)d.src_w * d.src_h : (size_t)d.src_w * d.src_h / 2;
     return (size_t)d.src_pitch * d.src_h + chroma;
 }
@@ -711,7 +803,7 @@ static int validate_desc(const kb200_preprocess_desc* dp) {
     if (dp->fmt < 0 || !f.name) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown source format code %d", dp->fmt);
     if (dp->fmt >> 10)
         return fail(KB200_ERR_INVALID_ARGUMENT, "source format code %d has bits set above bit 9 (bits 8-9 are the YUV matrix, 0-3)", dp->fmt);
-    if ((dp->fmt >> 8) && f.family != SRC_YUV420 && f.family != SRC_YUV422)
+    if ((dp->fmt >> 8) && f.family != SRC_YUV420 && f.family != SRC_YUV422 && f.family != SRC_YUV444)
         return fail(KB200_ERR_INVALID_ARGUMENT, "source format code %d: a YUV matrix (%d) applies only to the YUV formats, not format code %d", dp->fmt,
                     dp->fmt >> 8, d.fmt);
     if (d.sampling != KB200_INTERP_NEAREST && d.sampling != KB200_INTERP_BILINEAR && d.sampling != KB200_INTERP_LANCZOS)
@@ -733,14 +825,14 @@ static int validate_desc(const kb200_preprocess_desc* dp) {
             return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface for %s (pitch %d < %lld bytes of a packed row)", f.name, d.src_pitch,
                         (long long)d.src_w * f.bits / 8);
     }
-    if (f.family == SRC_YUV420 && f.words && (long long)d.src_pitch != 2ll * d.src_w)
+    if ((f.family == SRC_YUV420 || f.family == SRC_YUV444) && f.words && (long long)d.src_pitch != 2ll * d.src_w)
         return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface for %s (pitch %d bytes at width %d: frames must be tightly packed, pitch == 2*width)",
                     f.name, d.src_pitch, d.src_w);
     const int bpp = f.family == SRC_RGB ? d.src_bpp : f.family == SRC_YUV422 || f.words ? 2 : 1;
     if (!f.packed && (long long)d.src_pitch < (long long)d.src_w * bpp)
         return fail(KB200_ERR_INVALID_SOURCE, "invalid pitched surface (need pitch >= width*channels and len >= pitch*height)");
-    if (f.family == SRC_YUV420 && !f.words && d.src_pitch != d.src_w) {
-        char upper[8] = "";   // the layout's own spelling: NV12, NV21, I420, YV12
+    if ((f.family == SRC_YUV420 || f.family == SRC_YUV444) && !f.words && d.src_pitch != d.src_w) {
+        char upper[8] = "";   // the layout's own spelling: NV12, NV21, I420, YV12, I444
         for (int i = 0; f.name[i] && i < 7; ++i) upper[i] = (char)toupper((unsigned char)f.name[i]);
         return fail(KB200_ERR_INVALID_SOURCE, "%s frames must be tightly packed (pitch == width)", upper);
     }
@@ -748,22 +840,27 @@ static int validate_desc(const kb200_preprocess_desc* dp) {
     return KB200_OK;
 }
 
-// The 4:2:0 fast kernels of layout L and sample type T, for one launch of <= 256 frames.
+// The fast kernels of layout L (4:2:0, or YUV444) and sample type T, for one launch of <= 256 frames.
 template <bool F16, int L, typename T = uint8_t>
-static void launch_yuv420_fast(cudaStream_t s, bool identity, bool bil, const kb200_preprocess_desc& d, const typename Yuv420Sample<T>::Coeffs& yc,
-                               const PreFrames& fr, bool ptrs, const Nv12Args& nv, void* dst, uint32_t f0, uint32_t nb, uint32_t id_groups,
-                               size_t id_items) {
+static void launch_yuv_fast(cudaStream_t s, bool identity, bool bil, const kb200_preprocess_desc& d, const typename YuvSample<T>::Coeffs& yc,
+                            const PreFrames& fr, bool ptrs, const Nv12Args& nv, void* dst, uint32_t f0, uint32_t nb, uint32_t id_groups,
+                            size_t id_items) {
     if (identity) {
         dim3 grid(div_up(id_items, 128), nb);
-        if (ptrs) preprocess_yuv420_identity_kernel<F16, true, L, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
-        else preprocess_yuv420_identity_kernel<F16, false, L, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
+        if constexpr (L == YUV444) {
+            if (ptrs) preprocess_yuv444_identity_kernel<F16, true, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
+            else preprocess_yuv444_identity_kernel<F16, false, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
+        } else {
+            if (ptrs) preprocess_yuv420_identity_kernel<F16, true, L, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
+            else preprocess_yuv420_identity_kernel<F16, false, L, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
+        }
         return;
     }
     dim3 grid(div_up(nv.groups, 128), div_up((size_t)d.dst_h, NV12_ROWS), nb);
-#define KB200_YUV420_LAUNCH(BIL, PT) preprocess_yuv420_kernel<F16, BIL, PT, L, T><<<grid, 128, 0, s>>>(d, fr, nv, dst, f0, yc)
-    if (bil) { if (ptrs) KB200_YUV420_LAUNCH(true, true); else KB200_YUV420_LAUNCH(true, false); }
-    else     { if (ptrs) KB200_YUV420_LAUNCH(false, true); else KB200_YUV420_LAUNCH(false, false); }
-#undef KB200_YUV420_LAUNCH
+#define KB200_YUV_LAUNCH(BIL, PT) preprocess_yuv_kernel<F16, BIL, PT, L, T><<<grid, 128, 0, s>>>(d, fr, nv, dst, f0, yc)
+    if (bil) { if (ptrs) KB200_YUV_LAUNCH(true, true); else KB200_YUV_LAUNCH(true, false); }
+    else     { if (ptrs) KB200_YUV_LAUNCH(false, true); else KB200_YUV_LAUNCH(false, false); }
+#undef KB200_YUV_LAUNCH
 }
 
 // The Bayer identity kernel of sample type T and pattern P, for one launch of <= 256 frames.
@@ -790,6 +887,9 @@ static void launch_generic_for(cudaStream_t s, dim3 grid, const kb200_preprocess
         if (f.packed) launch_generic<F16, PTRS, TAP_BAYER_PACKED>(s, grid, d, f, yc, fr, dst, f0);
         else if (f.words) launch_generic<F16, PTRS, TAP_BAYER16>(s, grid, d, f, yc, fr, dst, f0);
         else launch_generic<F16, PTRS, TAP_BAYER>(s, grid, d, f, yc, fr, dst, f0);
+    } else if (f.family == SRC_YUV444) {
+        if (f.words) launch_generic<F16, PTRS, TAP_YUV444_16>(s, grid, d, f, yc16, fr, dst, f0);
+        else launch_generic<F16, PTRS, TAP_YUV444>(s, grid, d, f, yc, fr, dst, f0);
     } else if (f.words) {
         launch_generic<F16, PTRS, TAP_YUV16>(s, grid, d, f, yc16, fr, dst, f0);
     } else if (f.family == SRC_YUV420) {
@@ -814,7 +914,7 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, int
     const int pixels = d.dst_w * d.dst_h;
     const bool bil = d.sampling == KB200_INTERP_BILINEAR, lanczos = d.sampling == KB200_INTERP_LANCZOS;
     const bool bayer = f.family == SRC_BAYER;
-    // identity fast path: a format with an identity kernel (4:2:0 or Bayer), scale 1, no pad, same size, 8-column vectors
+    // identity fast path: a format with an identity kernel (4:2:0, 4:4:4 or Bayer), scale 1, no pad, same size, 8-column vectors
     // possible (Lanczos always takes the generic kernel: its off-centre weights at integer coordinates are sinf(k*pi) != 0
     // exactly).  A thread loads 4 samples per row, so rows and frames are aligned to that load: 4 B for bytes, 8 B for
     // 16-bit words, 16 B for packed Bayer.
@@ -827,12 +927,14 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, int
         else identity = ((reinterpret_cast<uintptr_t>(base) & (row_align - 1)) == 0) && (stride % row_align == 0);
     }
     const uint32_t id_groups = (uint32_t)d.src_w / 4u;
-    const size_t id_items = (size_t)id_groups * (bayer ? bayer_row_pairs((uint32_t)d.src_h) : (size_t)d.src_h / 2);
+    const size_t id_rows = bayer ? bayer_row_pairs((uint32_t)d.src_h) : f.family == SRC_YUV444 ? (size_t)d.src_h : (size_t)d.src_h / 2;
+    const size_t id_items = (size_t)id_groups * id_rows;   // threads of 4 columns x (2 rows, or 1 row of 4:4:4)
     if (id_items > 0x7FFFFFFFull) identity = false;
     // 4:2:0 general fast path: vector stores need dst_w % 4 == 0 and a 16-B (f32) / 8-B (f16) aligned destination
     const bool yuv420_fast = !lanczos && f.fast_kernel && (d.dst_w % 4) == 0 && aligned16(dst) && d.dst_h <= 65535 * NV12_ROWS;
     const YuvCoeffs& yc = YUV_COEFFS[matrix];
-    const Yuv16Coeffs yc16 = yuv16_coeffs(matrix, f.bits, f.layout == YUV420_NV12);   // used by the 16-bit 4:2:0 formats only
+    const bool msb = f.family == SRC_YUV444 ? f.layout == KB200_YUV444_I41X_MSB : f.layout == YUV420_NV12;   // P01x, I41xMsb
+    const Yuv16Coeffs yc16 = yuv16_coeffs(matrix, f.bits, msb);   // used by the 16-bit 4:2:0 and 4:4:4 formats only
     Nv12Args nv{};
     nv.groups = (uint32_t)(d.dst_w + 3) / 4u;
     for (int c = 0; c < 3; ++c) nv.pad_norm[c] = (d.pad_value / 255.0f - d.mean[c]) * d.inv_std[c];  // BODY :610-612 on the host (f32, unfused)
@@ -861,15 +963,18 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, int
             continue;
         }
         if (identity || yuv420_fast) {
-            if (f.words) {
-                if (f.layout == YUV420_I420) launch_yuv420_fast<F16, YUV420_I420, uint16_t>(s, identity, bil, d, yc16, fr, p, nv, dst, f0, nb, id_groups, id_items);
-                else launch_yuv420_fast<F16, YUV420_NV12, uint16_t>(s, identity, bil, d, yc16, fr, p, nv, dst, f0, nb, id_groups, id_items);
+            if (f.family == SRC_YUV444) {
+                if (f.words) launch_yuv_fast<F16, YUV444, uint16_t>(s, identity, bil, d, yc16, fr, p, nv, dst, f0, nb, id_groups, id_items);
+                else launch_yuv_fast<F16, YUV444>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items);
+            } else if (f.words) {
+                if (f.layout == YUV420_I420) launch_yuv_fast<F16, YUV420_I420, uint16_t>(s, identity, bil, d, yc16, fr, p, nv, dst, f0, nb, id_groups, id_items);
+                else launch_yuv_fast<F16, YUV420_NV12, uint16_t>(s, identity, bil, d, yc16, fr, p, nv, dst, f0, nb, id_groups, id_items);
             } else {
                 switch (f.layout) {
-                    case YUV420_NV12: launch_yuv420_fast<F16, YUV420_NV12>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
-                    case YUV420_NV21: launch_yuv420_fast<F16, YUV420_NV21>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
-                    case YUV420_I420: launch_yuv420_fast<F16, YUV420_I420>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
-                    default: launch_yuv420_fast<F16, YUV420_YV12>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                    case YUV420_NV12: launch_yuv_fast<F16, YUV420_NV12>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                    case YUV420_NV21: launch_yuv_fast<F16, YUV420_NV21>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                    case YUV420_I420: launch_yuv_fast<F16, YUV420_I420>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                    default: launch_yuv_fast<F16, YUV420_YV12>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
                 }
             }
             KB200_TRY(check_launch(identity ? f.identity_kernel : f.fast_kernel));

@@ -632,6 +632,43 @@ def rgb_from_i012(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -
     _rgb_from_yuv16(src, dst, "rgb_from_i012", YUV420_I01X, 12, matrix)
 
 
+def rgb_from_i444(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -> None:
+    """8-bit 4:4:4 video (libavcodec's yuv444p, nvJPEG's planar 4:4:4, NVDEC's YUV444 surface) -> RGB8.  `src`: uint8
+    device tensor holding N tight frames of three w*h planes Y, U, V; every pixel decodes from its own U and V.  `dst`: a
+    uint8 Image [N, h, w, 3], any w and h.  `matrix`: as for rgb_from_nv12 (JPEG is Bt601Full)."""
+    _rgb_from_yuv(src, dst, "rgb_from_i444", 3, 1, "kb200_rgb_from_yuv444_u8", int(YuvMatrix(matrix)))
+
+
+YUV444_I41X, YUV444_I41X_MSB = 0, 1   # kb200_yuv444_u16_layout
+
+
+def _rgb_from_yuv444_16(src, dst: Image, what: str, layout: int, bits: int, matrix: YuvMatrix) -> None:
+    _rgb_from_yuv(src, dst, what, 3, 1, "kb200_rgb_from_yuv444_u16", layout, bits, int(YuvMatrix(matrix)), dtype=torch.uint16)
+
+
+def rgb_from_i410(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -> None:
+    """10-bit 4:4:4 video in I410 (libavcodec's yuv444p10le) -> RGB with 16-bit channels holding 10-bit codes 0..1023.
+    `src`: uint16 device tensor holding N tight frames of three w*h planes Y, U, V of little-endian words, each code in the
+    low 10 bits (the high 6 bits are ignored); `dst`: a uint16 Image [N, h, w, 3].  `matrix`: as for rgb_from_p010."""
+    _rgb_from_yuv444_16(src, dst, "rgb_from_i410", YUV444_I41X, 10, matrix)
+
+
+def rgb_from_i412(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -> None:
+    """Like rgb_from_i410 for I412 (yuv444p12le, codes in the low 12 bits): codes 0..4095."""
+    _rgb_from_yuv444_16(src, dst, "rgb_from_i412", YUV444_I41X, 12, matrix)
+
+
+def rgb_from_i410msb(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -> None:
+    """Like rgb_from_i410 with each code in the high 10 bits of its word (NVDEC's YUV444_16Bit surface of 10-bit content;
+    the low 6 bits are ignored)."""
+    _rgb_from_yuv444_16(src, dst, "rgb_from_i410msb", YUV444_I41X_MSB, 10, matrix)
+
+
+def rgb_from_i412msb(src, dst: Image, matrix: YuvMatrix = YuvMatrix.Bt601Limited) -> None:
+    """Like rgb_from_i410msb for 12-bit content (the code in the high 12 bits): codes 0..4095."""
+    _rgb_from_yuv444_16(src, dst, "rgb_from_i412msb", YUV444_I41X_MSB, 12, matrix)
+
+
 class BayerPattern(enum.IntEnum):
     """kb200_bayer_pattern: the 2x2 quad of a Bayer mosaic read row-major (RGGB: the top-left pixel is R).  OpenCV names
     the same patterns by another pair of the quad: RGGB = COLOR_BayerBG2RGB, BGGR = COLOR_BayerRG2RGB,

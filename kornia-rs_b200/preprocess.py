@@ -2,7 +2,8 @@
 
 Built once via `Preprocessor.builder()…build_cuda()`, then applied to any number of frames of any
 resolution: the target H/W is read from the destination tensor each call.  Camera formats
-(NV12 / YUYV / Gray, the other YUV layouts, the 10- and 12-bit 4:2:0 video P010 / P012 / I010 / I012 and the 8- to
+(NV12 / YUYV / Gray, the other YUV layouts, the 10- and 12-bit 4:2:0 video P010 / P012 / I010 / I012, the 4:4:4 video
+I444 / I410 / I412 / I410Msb / I412Msb and the 8- to
 16-bit Bayer mosaics, unpacked or MIPI-packed) go through `run_raw*`; colour decode is fused into the resample taps.  Unlike the
 reference (one launch per frame, preprocess.rs:1277-1280) a batch is ONE launch.
 
@@ -103,6 +104,16 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
     P012 = "p012"
     I010 = "i010"
     I012 = "i012"
+    # 4:4:4 video: three full-resolution planes Y, U, V, every pixel with its own chroma; any w and h.  I444: w*h bytes each
+    # (libavcodec's yuv444p, nvJPEG's planar 4:4:4, NVDEC's YUV444 surface), decoded like I420.  I410 / I412: w*h
+    # little-endian 16-bit words each (6*w*h bytes), the code in the low bits (yuv444p10le / yuv444p12le); I410Msb /
+    # I412Msb: the code in the high bits (NVDEC's YUV444_16Bit surface of 10- and 12-bit content).  A 16-bit tap is
+    # normalised like a P010 tap by W = 2^n - 1; pad_value stays 0..255.
+    I444 = "i444"
+    I410 = "i410"
+    I412 = "i412"
+    I410Msb = "i410msb"
+    I412Msb = "i412msb"
 
     def _rec(self) -> "_Rec":
         return _RECORDS[self.name]
@@ -130,9 +141,13 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
     def is_yuv422(self) -> bool:
         return self._rec().family == "yuv422"
 
+    def is_yuv444(self) -> bool:
+        """A 4:4:4 format: I444 (bytes) or I410, I412, I410Msb, I412Msb (16-bit words)."""
+        return self._rec().family == "yuv444"
+
     def is_yuv(self) -> bool:
         """A YUV format: one a YuvMatrix applies to."""
-        return self._rec().family in ("yuv420", "yuv422")
+        return self._rec().family in ("yuv420", "yuv422", "yuv444")
 
     def is_bayer(self) -> bool:
         return self._rec().family == "bayer"
@@ -146,13 +161,15 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
         return self.is_bayer() and self._rec().bpp == 0
 
     def bit_depth(self) -> int | None:
-        """Bits per sample of a Bayer format (8 for the byte mosaics) or of a 16-bit-word 4:2:0 format (10, 12), None for
-        the other formats."""
+        """Bits per sample of a Bayer format (8 for the byte mosaics), of a 16-bit-word 4:2:0 format (10, 12) or of a 4:4:4
+        format (8, 10, 12), None for the other formats."""
         return self._rec().bits
 
     def buffer_len(self, w: int, h: int) -> int:  # :177-186
         # 4:2:0 chroma after the luma rows: w*h/2 samples, of 1 byte (is_yuv420) or 2 bytes (is_yuv16)
         chroma = w * h // 2 if self.is_yuv420() else w * h if self.is_yuv16() else 0
+        if self.is_yuv444():   # two more full planes
+            return self.pitch(w) * h * 3
         return self.pitch(w) * h + chroma
 
     def dims_ok(self, w: int, h: int) -> bool:  # :188-195
@@ -177,8 +194,8 @@ class SourceFormat(enum.Enum):  # preprocess.rs:130
 
 class _Rec(NamedTuple):   # one SourceFormat's facts
     code: int                 # kb200_src_fmt
-    family: str               # "rgb" (interleaved RGB / BGR, with or without alpha), "gray", "yuv420", "yuv422" or "bayer"
-    bits: int | None = None   # bits per sample of a Bayer or 16-bit-word 4:2:0 format
+    family: str               # "rgb" (interleaved RGB / BGR, with or without alpha), "gray", "yuv420", "yuv422", "yuv444" or "bayer"
+    bits: int | None = None   # bits per sample of a Bayer, 16-bit-word 4:2:0 or 4:4:4 format
     bpp: int = 1              # bytes per sample (per pixel for "rgb" and "yuv422"); 0: MIPI-packed, bits / 8 per sample
     aliases: tuple = ()       # from_name spellings besides the value
 
@@ -191,6 +208,9 @@ _RECORDS = {
     "Uyvy": _Rec(8, "yuv422", bpp=2), "Yvyu": _Rec(9, "yuv422", bpp=2),
     "P010": _Rec(80, "yuv420", 10, 2, ("p010le",)), "P012": _Rec(81, "yuv420", 12, 2, ("p012le",)),
     "I010": _Rec(82, "yuv420", 10, 2, ("yuv420p10le",)), "I012": _Rec(83, "yuv420", 12, 2, ("yuv420p12le",)),
+    "I444": _Rec(11, "yuv444", 8, 1, ("yuv444p",)),
+    "I410": _Rec(85, "yuv444", 10, 2, ("yuv444p10le",)), "I412": _Rec(86, "yuv444", 12, 2, ("yuv444p12le",)),
+    "I410Msb": _Rec(87, "yuv444", 10, 2), "I412Msb": _Rec(88, "yuv444", 12, 2),
 }
 for _k, _p in enumerate(("rggb", "bggr", "grbg", "gbrg")):   # kb200_bayer_pattern order; codes 16 + pattern; 32 + 4*d + pattern, d = 0..3; 64 + 4*d + pattern, d = 0..2
     _RECORDS[f"Bayer{_p.capitalize()}"] = _Rec(16 + _k, "bayer", 8)
@@ -468,7 +488,8 @@ class Preprocessor:
                      f16: bool = False, pipeline=None) -> torch.Tensor:
         """HOST camera frames in, HOST tensor out — what the reference's Python `Preprocessor` does around its kernel (pinned
         staging, upload, launch: kornia-py/src/cuda_ext/mod.rs:700-760), as one call: `host_frames` is a [N, frame_bytes] uint8
-        host tensor, or [N, w*h] uint16 for the 16-bit Bayer formats and [N, w*h*3/2] uint16 for P010 / P012 / I010 / I012 (page-locked
+        host tensor, or [N, w*h] uint16 for the 16-bit Bayer formats, [N, w*h*3/2] uint16 for P010 / P012 / I010 / I012 and
+        [N, 3*w*h] uint16 for I410 / I412 / I410Msb / I412Msb (page-locked
         for overlap), the result a [N,3,H,W] f32 / f16 host tensor (pinned when allocated here).
         Chunks ride a `HostPipeline` ring: upload -> ONE fused launch per chunk -> download.  Enqueue-only: synchronise the
         current stream of the pipeline's device before reading the result."""
@@ -501,7 +522,8 @@ class Preprocessor:
     def run_raw_strided(self, base: torch.Tensor, frame_stride: int, batch: int, src_w: int, src_h: int,
                         dst: torch.Tensor, f16: bool = False) -> None:
         """Frames at `base + i*frame_stride` bytes (a capture ring buffer): no pointer table.  `base` may be uint8 or, for
-        the formats of 16-bit samples (16-bit Bayer, P010 / P012 / I010 / I012), uint16: its length is counted in bytes."""
+        the formats of 16-bit samples (16-bit Bayer, P010 / P012 / I010 / I012, I410 / I412 / I410Msb / I412Msb), uint16: its
+        length is counted in bytes."""
         self._validate_dst(dst, batch, f16)
         fmt = self._fmt
         nbytes = base.numel() * base.element_size()
