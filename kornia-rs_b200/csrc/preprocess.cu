@@ -920,18 +920,25 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, int
     // 16-bit words, 16 B for packed Bayer.
     const uint32_t row_align = f.packed ? BayerSample<BayerPacked<12>>::ID_ALIGN
                                         : f.words ? BayerSample<uint16_t>::ID_ALIGN : BayerSample<uint8_t>::ID_ALIGN;
+    auto frames_aligned = [&](uint32_t a) {   // every frame of the call starts a-byte aligned
+        if (!frames) return ((reinterpret_cast<uintptr_t>(base) & (a - 1)) == 0) && (stride % a == 0);
+        for (uint32_t k = 0; k < batch; ++k)
+            if (reinterpret_cast<uintptr_t>(frames[k]) & (a - 1)) return false;
+        return true;
+    };
     bool identity = !lanczos && f.identity_kernel && d.scale_x == 1.0f && d.scale_y == 1.0f && d.pad_x == 0.0f && d.pad_y == 0.0f &&
-                    d.dst_w == d.src_w && d.dst_h == d.src_h && (d.src_w % 4) == 0 && (d.src_pitch % row_align) == 0 && aligned16(dst);
-    if (identity) {
-        if (frames) { for (uint32_t k = 0; k < batch; ++k) identity = identity && ((reinterpret_cast<uintptr_t>(frames[k]) & (row_align - 1)) == 0); }
-        else identity = ((reinterpret_cast<uintptr_t>(base) & (row_align - 1)) == 0) && (stride % row_align == 0);
-    }
+                    d.dst_w == d.src_w && d.dst_h == d.src_h && (d.src_w % 4) == 0 && (d.src_pitch % row_align) == 0 && aligned16(dst) &&
+                    frames_aligned(row_align);
     const uint32_t id_groups = (uint32_t)d.src_w / 4u;
     const size_t id_rows = bayer ? bayer_row_pairs((uint32_t)d.src_h) : f.family == SRC_YUV444 ? (size_t)d.src_h : (size_t)d.src_h / 2;
     const size_t id_items = (size_t)id_groups * id_rows;   // threads of 4 columns x (2 rows, or 1 row of 4:4:4)
     if (id_items > 0x7FFFFFFFull) identity = false;
-    // 4:2:0 general fast path: vector stores need dst_w % 4 == 0 and a 16-B (f32) / 8-B (f16) aligned destination
-    const bool yuv420_fast = !lanczos && f.fast_kernel && (d.dst_w % 4) == 0 && aligned16(dst) && d.dst_h <= 65535 * NV12_ROWS;
+    // 4:2:0 general fast path: vector stores need dst_w % 4 == 0 and a 16-B (f32) / 8-B (f16) aligned destination.  Its
+    // NV12 / NV21 tap reads a chroma pair as one 16-bit word (yuv_tap), so those frames must start 2-B aligned; frames at
+    // odd addresses take the generic kernel, which reads the pair's two bytes.
+    const bool pair_loads = f.family == SRC_YUV420 && !f.words && (f.layout == YUV420_NV12 || f.layout == YUV420_NV21);
+    const bool yuv420_fast = !lanczos && f.fast_kernel && (d.dst_w % 4) == 0 && aligned16(dst) && d.dst_h <= 65535 * NV12_ROWS &&
+                             (!pair_loads || frames_aligned(2));
     const YuvCoeffs& yc = YUV_COEFFS[matrix];
     const bool msb = f.family == SRC_YUV444 ? f.layout == KB200_YUV444_I41X_MSB : f.layout == YUV420_NV12;   // P01x, I41xMsb
     const Yuv16Coeffs yc16 = yuv16_coeffs(matrix, f.bits, msb);   // used by the 16-bit 4:2:0 and 4:4:4 formats only

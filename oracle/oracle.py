@@ -460,6 +460,15 @@ def preprocess_frame(src: np.ndarray, cfg: PreprocessCfg, sw: int, sh: int, dw: 
     return dst
 
 
+def preprocess_frame_desc(src: np.ndarray, d: PreprocessDesc, f16: bool = False) -> np.ndarray:
+    """ko_preprocess_frame on a caller-built descriptor: any scale, pad and sampling, src = (dst - pad) / scale.
+    d.fmt is one of the FMT_* codes above (no YUV matrix bits); returns (3, dst_h, dst_w) f32 or f16."""
+    src = np.ascontiguousarray(src, np.uint8).reshape(-1)
+    dst = np.zeros((3, d.dst_h, d.dst_w), np.uint16 if f16 else np.float32)
+    assert lib().ko_preprocess_frame(_p(src), _p(dst), C.byref(d), int(f16), None) == 0
+    return dst.view(np.float16) if f16 else dst
+
+
 def preprocess_cpu_rgb_bilinear(src: np.ndarray, dw: int, dh: int, mode: int, mean, inv_std, pad_value: float,
                                 leaf: int = LEAF_X86) -> np.ndarray:
     src = np.ascontiguousarray(src, np.uint8)
