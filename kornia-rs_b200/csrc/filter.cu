@@ -15,10 +15,12 @@
 // Bit-exactness with the two-pass reference: each intermediate value is the same ascending,
 // unfused (-fmad=false) accumulation starting from +0.0.  A zero-filled halo element contributes
 // `acc += 0*k` = acc (acc can never be -0.0: it starts at +0.0 and x + (-x) rounds to +0.0), which
-// equals "tap skipped" for every finite tap.  (Non-finite taps × zero halo would differ; taps come
-// from finite Gaussian/Sobel tables.)
+// equals "tap skipped" for every finite tap.  A non-finite tap times the zero halo is NaN where the reference skips
+// the tap, so separable_filter with an inf or NaN tap runs the run-time-loop instance with `skip_oob` set: it sums
+// only the taps inside the image.
 #include <algorithm>
 
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <type_traits>
@@ -40,6 +42,7 @@ struct SepGeom {
     uint32_t cols, rows, C;
     uint32_t tw, th;          // tile size in pixels
     uint32_t tiles_x, tiles_y;
+    uint32_t skip_oob;        // 1: taps outside the image are skipped, not multiplied by the zero halo (KX = KY = 0 only)
 };
 
 // KX/KY > 0: compile-time tap counts (fully unrolled); 0: runtime loops.
@@ -95,7 +98,12 @@ __global__ void __launch_bounds__(256) sep_filter_fused_kernel(const float* __re
                     if (SOBEL) acc2 += v * taps.ky[t];
                 }
             } else {
-                for (int t = 0; t < kxn; ++t) {
+                int t0 = 0, t1 = kxn;
+                if (g.skip_oob) {   // tap t reads image column px + t
+                    const int px = x0 - hx + e / C;
+                    t0 = max(0, -px); t1 = min(kxn, (int)g.cols - px);
+                }
+                for (int t = t0; t < t1; ++t) {
                     const float v = srow[e + t * C];
                     acc += v * taps.kx[t];
                     if (SOBEL) acc2 += v * taps.ky[t];
@@ -123,7 +131,11 @@ __global__ void __launch_bounds__(256) sep_filter_fused_kernel(const float* __re
                     if (SOBEL) acc2 += s_mid2[(size_t)(r + t) * mid_w + e] * taps.kx[t];
                 }
             } else {
-                for (int t = 0; t < kyn; ++t) {
+                int t0 = 0, t1 = kyn;
+                if (g.skip_oob) {   // tap t reads image row gy - hy + t
+                    t0 = max(0, hy - gy); t1 = min(kyn, (int)g.rows + hy - gy);
+                }
+                for (int t = t0; t < t1; ++t) {
                     acc += s_mid[(size_t)(r + t) * mid_w + e] * taps.ky[t];
                     if (SOBEL) acc2 += s_mid2[(size_t)(r + t) * mid_w + e] * taps.kx[t];
                 }
@@ -541,12 +553,17 @@ static int launch_sep(cudaStream_t s, const float* src, size_t src_len, float* d
     for (uint32_t i = 0; i < kxn; ++i) taps.kx[i] = kx[i];
     for (uint32_t i = 0; i < kyn; ++i) taps.ky[i] = ky[i];
     taps.kxn = (int)kxn; taps.kyn = (int)kyn;
-    {
+    // the reference skips taps outside the image; the zero halo only stands in for that while every tap is finite
+    bool finite = true;
+    for (uint32_t i = 0; i < kxn; ++i) finite = finite && std::isfinite(kx[i]);
+    for (uint32_t i = 0; i < kyn; ++i) finite = finite && std::isfinite(ky[i]);
+    if (finite) {
         int st = KB200_OK;
         if (try_sep_stream(s, src, dst, taps, cols, rows, C, batch, sobel, &st)) return st;
     }
     SepGeom g;
     g.cols = cols; g.rows = rows; g.C = C;
+    g.skip_oob = finite ? 0u : 1u;
     g.tw = 64; g.th = 32;
     if (cols <= 32) g.tw = 32;
     if (rows <= 16) g.th = 16;
@@ -567,6 +584,7 @@ static int launch_sep(cudaStream_t s, const float* src, size_t src_len, float* d
         if (kxn == 3) return launch_sep_instance<3, 3, true>(s, src, dst, taps, g, batch, smem);
         return launch_sep_instance<5, 5, true>(s, src, dst, taps, g, batch, smem);
     }
+    if (!finite) return launch_sep_instance<0, 0, false>(s, src, dst, taps, g, batch, smem);
     if (kxn == 3 && kyn == 3) return launch_sep_instance<3, 3, false>(s, src, dst, taps, g, batch, smem);
     if (kxn == 5 && kyn == 5) return launch_sep_instance<5, 5, false>(s, src, dst, taps, g, batch, smem);
     if (kxn == 7 && kyn == 7) return launch_sep_instance<7, 7, false>(s, src, dst, taps, g, batch, smem);
