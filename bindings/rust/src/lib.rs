@@ -156,6 +156,8 @@ pub mod ffi {
         pub fn kb200_preprocess_f16(stream: *mut c_void, desc: *const kb200_preprocess_desc, frames: *const *const u8, frame_len: *const usize, batch: u32, dst: *mut u16, dst_len: usize) -> c_int;
         pub fn kb200_preprocess_strided_f32(stream: *mut c_void, desc: *const kb200_preprocess_desc, base: *const u8, base_len: usize, frame_stride: usize, batch: u32, dst: *mut f32, dst_len: usize) -> c_int;
         pub fn kb200_preprocess_strided_f16(stream: *mut c_void, desc: *const kb200_preprocess_desc, base: *const u8, base_len: usize, frame_stride: usize, batch: u32, dst: *mut u16, dst_len: usize) -> c_int;
+        pub fn kb200_preprocess_bf16(stream: *mut c_void, desc: *const kb200_preprocess_desc, frames: *const *const u8, frame_len: *const usize, batch: u32, dst: *mut u16, dst_len: usize) -> c_int;
+        pub fn kb200_preprocess_strided_bf16(stream: *mut c_void, desc: *const kb200_preprocess_desc, base: *const u8, base_len: usize, frame_stride: usize, batch: u32, dst: *mut u16, dst_len: usize) -> c_int;
         pub fn kb200_selftest_div255(stream: *mut c_void, mismatches_dev: *mut u64) -> c_int;
         pub fn kb200_selftest_div2(stream: *mut c_void, count: u64, seed: u32, mismatches_dev: *mut u64) -> c_int;
 
@@ -181,6 +183,9 @@ pub mod ffi {
         pub fn kb200_preprocess_host(pipeline: *mut kb200_host_pipeline, stream: *mut c_void, desc: *const kb200_preprocess_desc,
                                      host_base: *const u8, base_len: usize, frame_stride: usize, batch: u32, host_dst: *mut c_void,
                                      dst_len: usize, out_f16: c_int) -> c_int;
+        pub fn kb200_preprocess_host_format(pipeline: *mut kb200_host_pipeline, stream: *mut c_void, desc: *const kb200_preprocess_desc,
+                                            host_base: *const u8, base_len: usize, frame_stride: usize, batch: u32, host_dst: *mut c_void,
+                                            dst_len: usize, out_format: c_int) -> c_int;
     }
 }
 
@@ -219,7 +224,7 @@ pub const LEAF_SCALAR: c_int = 0;
 pub const LEAF_X86_AVX2_FMA: c_int = 1;
 pub const LEAF_NEON: c_int = 2;
 
-/// `out_format` of `kb200_resize_normalize_chw_u8_host` (kb200_out_format): the CHW element type.  16-bit values are the
+/// `out_format` of `kb200_resize_normalize_chw_u8_host` and `kb200_preprocess_host_format` (kb200_out_format): the CHW element type.  16-bit values are the
 /// f32 result rounded once to nearest-even, stored as their raw bits.
 pub const OUT_F32: c_int = 0;
 pub const OUT_F16: c_int = 1;
@@ -470,6 +475,42 @@ pub fn launch_preprocess_batch_f32(
     })
 }
 
+/// Same as `launch_preprocess_batch_f32`, `dst` holding bfloat16 bits: each value the f32 result rounded to nearest even
+/// (an extension beyond the reference, which writes f32 and f16 only).
+pub fn launch_preprocess_batch_bf16(
+    stream: &Arc<CudaStream>, desc: &ffi::kb200_preprocess_desc, frames: &[&CudaSlice<u8>], dst: &mut CudaSlice<u16>,
+) -> Result<(), Kb200Error> {
+    bind(stream.context())?;
+    let mut guards = Vec::with_capacity(frames.len());
+    let mut ptrs: Vec<*const u8> = Vec::with_capacity(frames.len());
+    let lens: Vec<usize> = frames.iter().map(|f| f.len()).collect();
+    for f in frames {
+        let (p, g) = f.device_ptr(stream);
+        ptrs.push(p as *const u8);
+        guards.push(g);
+    }
+    let dst_len = dst.len();
+    let (dp, _g1) = dst.device_ptr_mut(stream);
+    check(unsafe {
+        ffi::kb200_preprocess_bf16(stream.cu_stream() as *mut c_void, desc, ptrs.as_ptr(), lens.as_ptr(), frames.len() as u32, dp as *mut u16, dst_len)
+    })
+}
+
+/// `batch` frames at `frame_stride`-byte steps in `frames` (a capture ring buffer) -> [batch, 3, dst_h, dst_w] bfloat16 bits.
+pub fn launch_preprocess_strided_bf16(
+    stream: &Arc<CudaStream>, desc: &ffi::kb200_preprocess_desc, frames: &CudaSlice<u8>, frame_stride: usize, batch: u32,
+    dst: &mut CudaSlice<u16>,
+) -> Result<(), Kb200Error> {
+    bind(stream.context())?;
+    let (sp, _g0) = frames.device_ptr(stream);
+    let (src_len, dst_len) = (frames.len(), dst.len());
+    let (dp, _g1) = dst.device_ptr_mut(stream);
+    check(unsafe {
+        ffi::kb200_preprocess_strided_bf16(stream.cu_stream() as *mut c_void, desc, sp as *const u8, src_len, frame_stride, batch, dp as *mut u16,
+                                           dst_len)
+    })
+}
+
 
 /// Staging ring for the HOST-buffer form of `resize_normalize_to_tensor_u8_to_f32_bilinear` (resize/fused.rs:147):
 /// host `&Image<u8,3>` in, host CHW tensor out, executed on the GPU.  One per device; calls only enqueue.
@@ -529,6 +570,20 @@ impl HostPipeline {
             ffi::kb200_resize_normalize_chw_u8_host(self.raw, stream.cu_stream() as *mut c_void, src.as_ptr(), src.len(),
                                                     dst.as_mut_ptr() as *mut c_void, dst.len(), src_size.0, src_size.1, dst_size.0,
                                                     dst_size.1, batch, scale.as_ptr(), bias.as_ptr(), LEAF_X86_AVX2_FMA, out_format)
+        })
+    }
+
+    /// Camera preprocess from host frames: `batch` raw frames at `frame_stride`-byte steps in `frames` -> `dst`, the raw bits
+    /// of [batch, 3, dst_h, dst_w] values of `out_format` (OUT_F32: 4 bytes each; OUT_F16, OUT_BF16: 2).  Both should be
+    /// page-locked.  Enqueue-only: synchronise `stream` before reading `dst`.
+    pub fn preprocess(
+        &mut self, stream: &Arc<CudaStream>, desc: &ffi::kb200_preprocess_desc, frames: &[u8], frame_stride: usize, batch: u32, dst: &mut [u8],
+        out_format: c_int,
+    ) -> Result<(), Kb200Error> {
+        let elem = if out_format == OUT_F32 { 4 } else { 2 };
+        check(unsafe {
+            ffi::kb200_preprocess_host_format(self.raw, stream.cu_stream() as *mut c_void, desc, frames.as_ptr(), frames.len(), frame_stride,
+                                              batch, dst.as_mut_ptr() as *mut c_void, dst.len() / elem, out_format)
         })
     }
 

@@ -120,6 +120,9 @@ def _declare(l: C.CDLL) -> None:
         "kb200_preprocess_strided_f32": ([vp, C.POINTER(PreprocessDesc), vp, sz, sz, u32, vp, sz], i),
         "kb200_preprocess_host": ([vp, vp, C.POINTER(PreprocessDesc), vp, sz, sz, u32, vp, sz, i], i),
         "kb200_preprocess_strided_f16": ([vp, C.POINTER(PreprocessDesc), vp, sz, sz, u32, vp, sz], i),
+        "kb200_preprocess_bf16": ([vp, C.POINTER(PreprocessDesc), C.POINTER(vp), C.POINTER(sz), u32, vp, sz], i),
+        "kb200_preprocess_strided_bf16": ([vp, C.POINTER(PreprocessDesc), vp, sz, sz, u32, vp, sz], i),
+        "kb200_preprocess_host_format": ([vp, vp, C.POINTER(PreprocessDesc), vp, sz, sz, u32, vp, sz, i], i),
     }
     for name, (args, res) in sig.items():
         fn = getattr(l, name)  # AttributeError if the symbol is missing: fail loudly

@@ -35,7 +35,7 @@ using namespace kb200;
 namespace kb200 {   // preprocess.cu
 int preprocess_validate(const kb200_preprocess_desc* desc);
 size_t preprocess_frame_bytes(const kb200_preprocess_desc& d);
-int preprocess_launch_strided(cudaStream_t s, const kb200_preprocess_desc& d, const uint8_t* base, size_t stride, uint32_t batch, void* dst, bool f16);
+int preprocess_launch_strided(cudaStream_t s, const kb200_preprocess_desc& d, const uint8_t* base, size_t stride, uint32_t batch, void* dst, int out);
 }
 
 namespace {
@@ -185,14 +185,16 @@ KB200_API int kb200_resize_normalize_chw_u8_f32_host(kb200_host_pipeline* pipe, 
 
 // Host-buffer form of Preprocessor::run_raw_batch (preprocess.rs:1234; the reference's Python Preprocessor pins and
 // uploads camera frames itself, kornia-py/src/cuda_ext/mod.rs:700-760): `batch` raw frames at host_base + i*frame_stride
-// (page-locked memory for overlap) -> host tensor [batch,3,dst_h,dst_w] f32 or binary16.  Chunks of frames ride the same
-// stream ring as the fused resize: upload -> fused preprocess kernel (one launch per chunk) -> download.
-KB200_API int kb200_preprocess_host(kb200_host_pipeline* pipe, kb200_stream_t stream, const kb200_preprocess_desc* desc,
-                                    const uint8_t* host_base, size_t base_len, size_t frame_stride, uint32_t batch, void* host_dst,
-                                    size_t dst_len, int out_f16) {
+// (page-locked memory for overlap) -> host tensor [batch,3,dst_h,dst_w] of `out_format` (f32, binary16 or bfloat16).  Chunks
+// of frames ride the same stream ring as the fused resize: upload -> fused preprocess kernel (one launch per chunk) -> download.
+KB200_API int kb200_preprocess_host_format(kb200_host_pipeline* pipe, kb200_stream_t stream, const kb200_preprocess_desc* desc,
+                                           const uint8_t* host_base, size_t base_len, size_t frame_stride, uint32_t batch,
+                                           void* host_dst, size_t dst_len, int out_format) {
     KB200_TRY(check_ptr("pipeline", pipe));
     KB200_TRY(preprocess_validate(desc));
     KB200_TRY(check_ptr("base", host_base)); KB200_TRY(check_ptr("dst", host_dst));
+    if (out_format != KB200_OUT_F32 && out_format != KB200_OUT_F16 && out_format != KB200_OUT_BF16)
+        return fail(KB200_ERR_INVALID_ARGUMENT, "unknown output format %d", out_format);
     if (batch == 0) return fail(KB200_ERR_INVALID_ARGUMENT, "batch must be non-zero");
     const size_t need = preprocess_frame_bytes(*desc);
     if (frame_stride < need && batch > 1) return fail(KB200_ERR_INVALID_SOURCE, "frame stride %zu smaller than a frame (%zu bytes)", frame_stride, need);
@@ -203,7 +205,7 @@ KB200_API int kb200_preprocess_host(kb200_host_pipeline* pipe, kb200_stream_t st
     KB200_TRY(check_slice("dst", dst_len, dst_frame_elems * batch));
     pipe->h2d_bytes = pipe->d2h_bytes = 0;
     KB200_CUDA(cudaSetDevice(pipe->device));
-    const size_t elem = out_f16 ? 2 : 4;
+    const size_t elem = out_format == KB200_OUT_F32 ? sizeof(float) : sizeof(uint16_t);
     const size_t dst_frame = dst_frame_elems * elem;
     const size_t dev_stride = (need + 15) & ~(size_t)15;      // staged frames 16-byte aligned (the NV12 fast paths want aligned bases)
     const size_t per_chunk = std::min<size_t>(std::min(pipe->src_bytes / dev_stride, pipe->dst_bytes / dst_frame), 256);
@@ -223,7 +225,7 @@ KB200_API int kb200_preprocess_host(kb200_host_pipeline* pipe, kb200_stream_t st
         const uint8_t* hs = host_base + (size_t)f0 * frame_stride;
         if (frame_stride == need && dev_stride == need) KB200_CUDA(cudaMemcpyAsync(pipe->src[k], hs, need * n, cudaMemcpyHostToDevice, s));
         else KB200_CUDA(cudaMemcpy2DAsync(pipe->src[k], dev_stride, hs, frame_stride, need, n, cudaMemcpyHostToDevice, s));
-        KB200_TRY(preprocess_launch_strided(s, *desc, pipe->src[k], dev_stride, n, pipe->dst[k], out_f16 != 0));
+        KB200_TRY(preprocess_launch_strided(s, *desc, pipe->src[k], dev_stride, n, pipe->dst[k], out_format));
         KB200_CUDA(cudaMemcpyAsync(static_cast<uint8_t*>(host_dst) + (size_t)f0 * dst_frame, pipe->dst[k], dst_frame * n, cudaMemcpyDeviceToHost, s));
         pipe->h2d_bytes += need * n;
         pipe->d2h_bytes += dst_frame * n;
@@ -234,6 +236,13 @@ KB200_API int kb200_preprocess_host(kb200_host_pipeline* pipe, kb200_stream_t st
         KB200_CUDA(cudaStreamWaitEvent(user, pipe->done[k], 0));
     }
     return KB200_OK;
+}
+
+KB200_API int kb200_preprocess_host(kb200_host_pipeline* pipe, kb200_stream_t stream, const kb200_preprocess_desc* desc,
+                                    const uint8_t* host_base, size_t base_len, size_t frame_stride, uint32_t batch, void* host_dst,
+                                    size_t dst_len, int out_f16) {
+    return kb200_preprocess_host_format(pipe, stream, desc, host_base, base_len, frame_stride, batch, host_dst, dst_len,
+                                        out_f16 ? KB200_OUT_F16 : KB200_OUT_F32);
 }
 
 }  // extern "C"

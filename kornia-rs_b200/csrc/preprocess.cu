@@ -1,7 +1,7 @@
 // preprocess.cu — the fused camera preprocess (a12; BASELINE config 3): raw frame (RGB/BGR/RGBA/
 // Gray/NV12/YUYV, tight or pitched; beyond the reference also NV21/I420/YV12/UYVY/YVYU, the 8- and 16-bit Bayer
 // mosaics, the 10- and 12-bit 4:2:0 video P010/P012/I010/I012 and the 4:4:4 video I444/I410/I412/I410Msb/I412Msb) →
-// letterbox/stretch resample → (v/255 - mean) * inv_std → planar CHW f32 or f16, for a whole batch in ONE launch.
+// letterbox/stretch resample → (v/255 - mean) * inv_std → planar CHW f32, f16 or bf16, for a whole batch in ONE launch.
 // The 4:2:0 formats share the NV12 kernels (templated on the chroma layout); the 4:2:2 formats take the generic kernel.
 // A Bayer tap is the demosaiced pixel at the tap's coordinate (bayer.cuh); Bayer frames take the generic kernel, except
 // the identity geometry, which has its own fast kernel.  A 16-bit Bayer tap is normalised against the white level
@@ -26,6 +26,7 @@
 // One exact shortcut: when ax == 0 the x1 taps are multiplied by zero — `t00 + (t10-t00)*0` is t00
 // bit-for-bit for the finite decoded values — so those taps are not fetched (same for ay == 0).  At
 // integer scales (1080p NV12 → 1080p CHW, config 3a) that removes 3 of the 4 decodes per pixel.
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
 #include <cctype>
@@ -231,7 +232,7 @@ __device__ __forceinline__ float pre_lanczos_w(float dd) {
 }
 
 // SAMP: kb200_interp — 0 nearest, 1 bilinear, 3 Lanczos-3 (6x6 taps, clamp-to-edge, weights renormalised by their sum)
-template <bool F16, int SAMP, bool PTRS, int TAP>
+template <int OUT, int SAMP, bool PTRS, int TAP>
 __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                  const __grid_constant__ PreFrames fr, void* __restrict__ dst,
                                                                  uint32_t frame0, const SrcFormat sf, const TapCoeffs<TAP> yc) {
@@ -309,9 +310,12 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
     const float o1 = (q1 - d.mean[1]) * d.inv_std[1];
     const float o2 = (q2 - d.mean[2]) * d.inv_std[2];
     const size_t out = (size_t)(frame0 + f) * 3 * pixels + i;
-    if (F16) {
+    if constexpr (OUT == KB200_OUT_F16) {
         unsigned short* o = reinterpret_cast<unsigned short*>(dst);
         o[out] = f2h_ref(o0); o[out + pixels] = f2h_ref(o1); o[out + 2 * (size_t)pixels] = f2h_ref(o2);
+    } else if constexpr (OUT == KB200_OUT_BF16) {
+        __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(dst);
+        o[out] = __float2bfloat16_rn(o0); o[out + pixels] = __float2bfloat16_rn(o1); o[out + 2 * (size_t)pixels] = __float2bfloat16_rn(o2);
     } else {
         float* o = reinterpret_cast<float*>(dst);
         o[out] = o0; o[out + pixels] = o1; o[out + 2 * (size_t)pixels] = o2;
@@ -328,9 +332,16 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
 //   * `px / 255.0f` for the INTEGER px in [0,255] is evaluated as q = px*c; e = fma(-q,255,px); q' = fma(e,c,q)
 //     with c = RN(1/255): Markstein's correction gives the correctly rounded quotient (verified for all 256
 //     values, tests/test_abi_and_host.py) — identical bits to the IEEE division the reference performs.
-template <bool F16>
+// OUT: the kb200_out_format of dst.  A bfloat16 value is the f32 one rounded to nearest even (__floats2bfloat162_rn, two
+// values per conversion), stored like binary16 as one 8-byte word.
+template <int OUT>
 __device__ __forceinline__ void nv12_store4(void* __restrict__ dst, size_t idx, const float v[4]) {
-    if (F16) {
+    if constexpr (OUT == KB200_OUT_BF16) {
+        const __nv_bfloat162 lo = __floats2bfloat162_rn(v[0], v[1]), hi = __floats2bfloat162_rn(v[2], v[3]);
+        uint2 w;
+        memcpy(&w.x, &lo, 4); memcpy(&w.y, &hi, 4);
+        *reinterpret_cast<uint2*>(reinterpret_cast<unsigned short*>(dst) + idx) = w;
+    } else if constexpr (OUT == KB200_OUT_F16) {
         unsigned short hbits[4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
@@ -363,7 +374,7 @@ template <> struct YuvSample<uint16_t> { using Coeffs = Yuv16Coeffs; };
 // 16-bit words (T = uint16_t): LDG.64 of 4 Y words per row; P01x one LDG.64 of the 2 chroma pairs, I01x 2 U words and
 // 2 V words (LDG.32 each; w % 4 == 0 and even h keep them 4-B aligned in an 8-B aligned frame).  A pixel is normalised
 // as (px / W - mean) * inv_std with the IEEE division, like a 16-bit Bayer tap.
-template <bool F16, bool PTRS, int L, typename T>
+template <int OUT, bool PTRS, int L, typename T>
 __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                          const __grid_constant__ PreFrames fr, void* __restrict__ dst,
                                                                          uint32_t frame0, uint32_t groups_per_row, uint32_t items,
@@ -409,9 +420,9 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const _
                 b4[i] = (div_white((float)b, wl) - m2) * i2;
             }
             const size_t o = base + (size_t)row * w;
-            nv12_store4<F16>(dst, o, r4);
-            nv12_store4<F16>(dst, o + plane, g4);
-            nv12_store4<F16>(dst, o + 2 * plane, b4);
+            nv12_store4<OUT>(dst, o, r4);
+            nv12_store4<OUT>(dst, o + plane, g4);
+            nv12_store4<OUT>(dst, o + 2 * plane, b4);
         }
     } else {
         const uint32_t y0w = __ldg(reinterpret_cast<const uint32_t*>(src + (size_t)(2u * rp) * w + x));
@@ -450,9 +461,9 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const _
                 b4[i] = norm_int_px(b, m2, i2);
             }
             const size_t o = base + (size_t)row * w;
-            nv12_store4<F16>(dst, o, r4);
-            nv12_store4<F16>(dst, o + plane, g4);
-            nv12_store4<F16>(dst, o + 2 * plane, b4);
+            nv12_store4<OUT>(dst, o, r4);
+            nv12_store4<OUT>(dst, o + plane, g4);
+            nv12_store4<OUT>(dst, o + 2 * plane, b4);
         }
     }
 }
@@ -461,7 +472,7 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const _
 // Every pixel has its own chroma, so one thread = 4 columns of one row: one lane-contiguous load from each of the Y, U
 // and V planes (LDG.32 of 4 bytes, LDG.64 of 4 words: w % 4 == 0 and a frame aligned to that load align every plane's
 // rows), 3 x nv12_store4.  Bytes are normalised as in the 4:2:0 kernel (norm_int_px), words by W through div_white.
-template <bool F16, bool PTRS, typename T>
+template <int OUT, bool PTRS, typename T>
 __global__ void __launch_bounds__(128) preprocess_yuv444_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                          const __grid_constant__ PreFrames fr, void* __restrict__ dst,
                                                                          uint32_t frame0, uint32_t groups_per_row, uint32_t items,
@@ -507,9 +518,9 @@ __global__ void __launch_bounds__(128) preprocess_yuv444_identity_kernel(const _
         }
     }
     const size_t o = (size_t)(frame0 + f) * 3 * plane + p;
-    nv12_store4<F16>(dst, o, r4);
-    nv12_store4<F16>(dst, o + plane, g4);
-    nv12_store4<F16>(dst, o + 2 * plane, b4);
+    nv12_store4<OUT>(dst, o, r4);
+    nv12_store4<OUT>(dst, o + plane, g4);
+    nv12_store4<OUT>(dst, o + 2 * plane, b4);
 }
 
 // ── Bayer identity fast path (the config-3a shape from a Bayer mosaic: scale 1, no pad, same size) ──────────────
@@ -520,7 +531,7 @@ __global__ void __launch_bounds__(128) preprocess_yuv444_identity_kernel(const _
 // Packed samples (T = BayerPacked<BITS>): a thread's 4 columns are BITS / 2 bytes of a row, read as the aligned 8-byte
 // word that holds their first byte and, when they run past it, the next one (L1-allocating: the neighbouring lanes read
 // the same words), then unpacked into the words of the 16-bit kernel (bayer_unpack).  Rows and frames 16-B aligned.
-template <bool F16, bool PTRS, typename T, int P>
+template <int OUT, bool PTRS, typename T, int P>
 __global__ void __launch_bounds__(128) preprocess_bayer_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                         const __grid_constant__ PreFrames fr, void* __restrict__ dst,
                                                                         uint32_t frame0, uint32_t groups_per_row, uint32_t items, uint32_t bits) {
@@ -568,9 +579,9 @@ __global__ void __launch_bounds__(128) preprocess_bayer_identity_kernel(const __
     float r4[4], g4[4], b4[4];
     auto store_row = [&](uint32_t y) {
         const size_t o = base + (size_t)y * w;
-        nv12_store4<F16>(dst, o, r4);
-        nv12_store4<F16>(dst, o + plane, g4);
-        nv12_store4<F16>(dst, o + 2 * plane, b4);
+        nv12_store4<OUT>(dst, o, r4);
+        nv12_store4<OUT>(dst, o + plane, g4);
+        nv12_store4<OUT>(dst, o + 2 * plane, b4);
     };
     // 8-bit: px / 255 by the exact 3-instruction form (norm_int_px); 16-bit and packed: px / W, the IEEE division
     auto norm = [&](const int r[4], const int gg[4], const int b[4]) {
@@ -616,7 +627,7 @@ static constexpr int NV12_ROWS = 8;  // destination rows per thread: the x-side 
 
 // L: a 4:2:0 layout or YUV444 (yuv_tap); T: the sample type (YuvSample).  A pixel of 16-bit words is normalised as
 // (px / W - mean) * inv_std with the IEEE division, interpolated or not.
-template <bool F16, bool BILINEAR, bool PTRS, int L, typename T>
+template <int OUT, bool BILINEAR, bool PTRS, int L, typename T>
 __global__ void __launch_bounds__(128) preprocess_yuv_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                              const __grid_constant__ PreFrames fr, const __grid_constant__ Nv12Args na,
                                                              void* __restrict__ dst, uint32_t frame0, const typename YuvSample<T>::Coeffs yc) {
@@ -721,9 +732,9 @@ __global__ void __launch_bounds__(128) preprocess_yuv_kernel(const __grid_consta
                 }
             }
         }
-        nv12_store4<F16>(dst, obase, o[0]);
-        nv12_store4<F16>(dst, obase + plane, o[1]);
-        nv12_store4<F16>(dst, obase + 2 * plane, o[2]);
+        nv12_store4<OUT>(dst, obase, o[0]);
+        nv12_store4<OUT>(dst, obase + plane, o[1]);
+        nv12_store4<OUT>(dst, obase + 2 * plane, o[2]);
     }
 }
 
@@ -841,73 +852,73 @@ static int validate_desc(const kb200_preprocess_desc* dp) {
 }
 
 // The fast kernels of layout L (4:2:0, or YUV444) and sample type T, for one launch of <= 256 frames.
-template <bool F16, int L, typename T = uint8_t>
+template <int OUT, int L, typename T = uint8_t>
 static void launch_yuv_fast(cudaStream_t s, bool identity, bool bil, const kb200_preprocess_desc& d, const typename YuvSample<T>::Coeffs& yc,
                             const PreFrames& fr, bool ptrs, const Nv12Args& nv, void* dst, uint32_t f0, uint32_t nb, uint32_t id_groups,
                             size_t id_items) {
     if (identity) {
         dim3 grid(div_up(id_items, 128), nb);
         if constexpr (L == YUV444) {
-            if (ptrs) preprocess_yuv444_identity_kernel<F16, true, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
-            else preprocess_yuv444_identity_kernel<F16, false, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
+            if (ptrs) preprocess_yuv444_identity_kernel<OUT, true, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
+            else preprocess_yuv444_identity_kernel<OUT, false, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
         } else {
-            if (ptrs) preprocess_yuv420_identity_kernel<F16, true, L, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
-            else preprocess_yuv420_identity_kernel<F16, false, L, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
+            if (ptrs) preprocess_yuv420_identity_kernel<OUT, true, L, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
+            else preprocess_yuv420_identity_kernel<OUT, false, L, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
         }
         return;
     }
     dim3 grid(div_up(nv.groups, 128), div_up((size_t)d.dst_h, NV12_ROWS), nb);
-#define KB200_YUV_LAUNCH(BIL, PT) preprocess_yuv_kernel<F16, BIL, PT, L, T><<<grid, 128, 0, s>>>(d, fr, nv, dst, f0, yc)
+#define KB200_YUV_LAUNCH(BIL, PT) preprocess_yuv_kernel<OUT, BIL, PT, L, T><<<grid, 128, 0, s>>>(d, fr, nv, dst, f0, yc)
     if (bil) { if (ptrs) KB200_YUV_LAUNCH(true, true); else KB200_YUV_LAUNCH(true, false); }
     else     { if (ptrs) KB200_YUV_LAUNCH(false, true); else KB200_YUV_LAUNCH(false, false); }
 #undef KB200_YUV_LAUNCH
 }
 
 // The Bayer identity kernel of sample type T and pattern P, for one launch of <= 256 frames.
-template <bool F16, typename T, int P>
+template <int OUT, typename T, int P>
 static void launch_bayer_identity(cudaStream_t s, const kb200_preprocess_desc& d, const PreFrames& fr, bool ptrs, void* dst, uint32_t f0,
                                   uint32_t nb, uint32_t id_groups, size_t id_items, uint32_t bits) {
     dim3 grid(div_up(id_items, 128), nb);
-    if (ptrs) preprocess_bayer_identity_kernel<F16, true, T, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, bits);
-    else preprocess_bayer_identity_kernel<F16, false, T, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, bits);
+    if (ptrs) preprocess_bayer_identity_kernel<OUT, true, T, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, bits);
+    else preprocess_bayer_identity_kernel<OUT, false, T, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, bits);
 }
 
-template <bool F16, bool PTRS, int TAP>
+template <int OUT, bool PTRS, int TAP>
 static void launch_generic(cudaStream_t s, dim3 grid, const kb200_preprocess_desc& d, const SrcFormat& f, const TapCoeffs<TAP>& yc,
                            const PreFrames& fr, void* dst, uint32_t f0) {
-    if (d.sampling == KB200_INTERP_LANCZOS) preprocess_generic_kernel<F16, KB200_INTERP_LANCZOS, PTRS, TAP><<<grid, 256, 0, s>>>(d, fr, dst, f0, f, yc);
-    else if (d.sampling == KB200_INTERP_BILINEAR) preprocess_generic_kernel<F16, KB200_INTERP_BILINEAR, PTRS, TAP><<<grid, 256, 0, s>>>(d, fr, dst, f0, f, yc);
-    else preprocess_generic_kernel<F16, KB200_INTERP_NEAREST, PTRS, TAP><<<grid, 256, 0, s>>>(d, fr, dst, f0, f, yc);
+    if (d.sampling == KB200_INTERP_LANCZOS) preprocess_generic_kernel<OUT, KB200_INTERP_LANCZOS, PTRS, TAP><<<grid, 256, 0, s>>>(d, fr, dst, f0, f, yc);
+    else if (d.sampling == KB200_INTERP_BILINEAR) preprocess_generic_kernel<OUT, KB200_INTERP_BILINEAR, PTRS, TAP><<<grid, 256, 0, s>>>(d, fr, dst, f0, f, yc);
+    else preprocess_generic_kernel<OUT, KB200_INTERP_NEAREST, PTRS, TAP><<<grid, 256, 0, s>>>(d, fr, dst, f0, f, yc);
 }
 
-template <bool F16, bool PTRS>
+template <int OUT, bool PTRS>
 static void launch_generic_for(cudaStream_t s, dim3 grid, const kb200_preprocess_desc& d, const SrcFormat& f, const YuvCoeffs& yc,
                                const Yuv16Coeffs& yc16, const PreFrames& fr, void* dst, uint32_t f0) {
     if (f.family == SRC_BAYER) {
-        if (f.packed) launch_generic<F16, PTRS, TAP_BAYER_PACKED>(s, grid, d, f, yc, fr, dst, f0);
-        else if (f.words) launch_generic<F16, PTRS, TAP_BAYER16>(s, grid, d, f, yc, fr, dst, f0);
-        else launch_generic<F16, PTRS, TAP_BAYER>(s, grid, d, f, yc, fr, dst, f0);
+        if (f.packed) launch_generic<OUT, PTRS, TAP_BAYER_PACKED>(s, grid, d, f, yc, fr, dst, f0);
+        else if (f.words) launch_generic<OUT, PTRS, TAP_BAYER16>(s, grid, d, f, yc, fr, dst, f0);
+        else launch_generic<OUT, PTRS, TAP_BAYER>(s, grid, d, f, yc, fr, dst, f0);
     } else if (f.family == SRC_YUV444) {
-        if (f.words) launch_generic<F16, PTRS, TAP_YUV444_16>(s, grid, d, f, yc16, fr, dst, f0);
-        else launch_generic<F16, PTRS, TAP_YUV444>(s, grid, d, f, yc, fr, dst, f0);
+        if (f.words) launch_generic<OUT, PTRS, TAP_YUV444_16>(s, grid, d, f, yc16, fr, dst, f0);
+        else launch_generic<OUT, PTRS, TAP_YUV444>(s, grid, d, f, yc, fr, dst, f0);
     } else if (f.words) {
-        launch_generic<F16, PTRS, TAP_YUV16>(s, grid, d, f, yc16, fr, dst, f0);
+        launch_generic<OUT, PTRS, TAP_YUV16>(s, grid, d, f, yc16, fr, dst, f0);
     } else if (f.family == SRC_YUV420) {
         switch (f.layout) {
-            case YUV420_NV12: launch_generic<F16, PTRS, TAP_YUV420 + YUV420_NV12>(s, grid, d, f, yc, fr, dst, f0); break;
-            case YUV420_NV21: launch_generic<F16, PTRS, TAP_YUV420 + YUV420_NV21>(s, grid, d, f, yc, fr, dst, f0); break;
-            case YUV420_I420: launch_generic<F16, PTRS, TAP_YUV420 + YUV420_I420>(s, grid, d, f, yc, fr, dst, f0); break;
-            default: launch_generic<F16, PTRS, TAP_YUV420 + YUV420_YV12>(s, grid, d, f, yc, fr, dst, f0); break;
+            case YUV420_NV12: launch_generic<OUT, PTRS, TAP_YUV420 + YUV420_NV12>(s, grid, d, f, yc, fr, dst, f0); break;
+            case YUV420_NV21: launch_generic<OUT, PTRS, TAP_YUV420 + YUV420_NV21>(s, grid, d, f, yc, fr, dst, f0); break;
+            case YUV420_I420: launch_generic<OUT, PTRS, TAP_YUV420 + YUV420_I420>(s, grid, d, f, yc, fr, dst, f0); break;
+            default: launch_generic<OUT, PTRS, TAP_YUV420 + YUV420_YV12>(s, grid, d, f, yc, fr, dst, f0); break;
         }
     } else if (f.family == SRC_YUV422) {
-        launch_generic<F16, PTRS, TAP_YUV422>(s, grid, d, f, yc, fr, dst, f0);
+        launch_generic<OUT, PTRS, TAP_YUV422>(s, grid, d, f, yc, fr, dst, f0);
     } else {
-        launch_generic<F16, PTRS, TAP_RGB>(s, grid, d, f, yc, fr, dst, f0);
+        launch_generic<OUT, PTRS, TAP_RGB>(s, grid, d, f, yc, fr, dst, f0);
     }
 }
 
 // d: a validated descriptor with the plain format code; matrix: its kb200_yuv_matrix
-template <bool F16>
+template <int OUT>
 static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, int matrix, const uint8_t* const* frames, const uint8_t* base,
                              size_t stride, uint32_t batch, void* dst) {
     const SrcFormat f = src_format(d.fmt);
@@ -933,7 +944,7 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, int
     const size_t id_rows = bayer ? bayer_row_pairs((uint32_t)d.src_h) : f.family == SRC_YUV444 ? (size_t)d.src_h : (size_t)d.src_h / 2;
     const size_t id_items = (size_t)id_groups * id_rows;   // threads of 4 columns x (2 rows, or 1 row of 4:4:4)
     if (id_items > 0x7FFFFFFFull) identity = false;
-    // 4:2:0 general fast path: vector stores need dst_w % 4 == 0 and a 16-B (f32) / 8-B (f16) aligned destination.  Its
+    // 4:2:0 general fast path: vector stores need dst_w % 4 == 0 and a 16-B (f32) / 8-B (f16, bf16) aligned destination.  Its
     // NV12 / NV21 tap reads a chroma pair as one 16-bit word (yuv_tap), so those frames must start 2-B aligned; frames at
     // odd addresses take the generic kernel, which reads the pair's two bytes.
     const bool pair_loads = f.family == SRC_YUV420 && !f.words && (f.layout == YUV420_NV12 || f.layout == YUV420_NV21);
@@ -955,10 +966,10 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, int
             auto launch = [&](auto sample) {   // the kernel of the format's pattern for samples of the type of `sample`
                 using T = decltype(sample);
                 switch (f.pattern) {
-                    case KB200_BAYER_RGGB: launch_bayer_identity<F16, T, KB200_BAYER_RGGB>(s, d, fr, p, dst, f0, nb, id_groups, id_items, f.bits); break;
-                    case KB200_BAYER_BGGR: launch_bayer_identity<F16, T, KB200_BAYER_BGGR>(s, d, fr, p, dst, f0, nb, id_groups, id_items, f.bits); break;
-                    case KB200_BAYER_GRBG: launch_bayer_identity<F16, T, KB200_BAYER_GRBG>(s, d, fr, p, dst, f0, nb, id_groups, id_items, f.bits); break;
-                    default: launch_bayer_identity<F16, T, KB200_BAYER_GBRG>(s, d, fr, p, dst, f0, nb, id_groups, id_items, f.bits); break;
+                    case KB200_BAYER_RGGB: launch_bayer_identity<OUT, T, KB200_BAYER_RGGB>(s, d, fr, p, dst, f0, nb, id_groups, id_items, f.bits); break;
+                    case KB200_BAYER_BGGR: launch_bayer_identity<OUT, T, KB200_BAYER_BGGR>(s, d, fr, p, dst, f0, nb, id_groups, id_items, f.bits); break;
+                    case KB200_BAYER_GRBG: launch_bayer_identity<OUT, T, KB200_BAYER_GRBG>(s, d, fr, p, dst, f0, nb, id_groups, id_items, f.bits); break;
+                    default: launch_bayer_identity<OUT, T, KB200_BAYER_GBRG>(s, d, fr, p, dst, f0, nb, id_groups, id_items, f.bits); break;
                 }
             };
             if (!f.packed && f.words) launch(uint16_t{});
@@ -971,25 +982,25 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, int
         }
         if (identity || yuv420_fast) {
             if (f.family == SRC_YUV444) {
-                if (f.words) launch_yuv_fast<F16, YUV444, uint16_t>(s, identity, bil, d, yc16, fr, p, nv, dst, f0, nb, id_groups, id_items);
-                else launch_yuv_fast<F16, YUV444>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items);
+                if (f.words) launch_yuv_fast<OUT, YUV444, uint16_t>(s, identity, bil, d, yc16, fr, p, nv, dst, f0, nb, id_groups, id_items);
+                else launch_yuv_fast<OUT, YUV444>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items);
             } else if (f.words) {
-                if (f.layout == YUV420_I420) launch_yuv_fast<F16, YUV420_I420, uint16_t>(s, identity, bil, d, yc16, fr, p, nv, dst, f0, nb, id_groups, id_items);
-                else launch_yuv_fast<F16, YUV420_NV12, uint16_t>(s, identity, bil, d, yc16, fr, p, nv, dst, f0, nb, id_groups, id_items);
+                if (f.layout == YUV420_I420) launch_yuv_fast<OUT, YUV420_I420, uint16_t>(s, identity, bil, d, yc16, fr, p, nv, dst, f0, nb, id_groups, id_items);
+                else launch_yuv_fast<OUT, YUV420_NV12, uint16_t>(s, identity, bil, d, yc16, fr, p, nv, dst, f0, nb, id_groups, id_items);
             } else {
                 switch (f.layout) {
-                    case YUV420_NV12: launch_yuv_fast<F16, YUV420_NV12>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
-                    case YUV420_NV21: launch_yuv_fast<F16, YUV420_NV21>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
-                    case YUV420_I420: launch_yuv_fast<F16, YUV420_I420>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
-                    default: launch_yuv_fast<F16, YUV420_YV12>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                    case YUV420_NV12: launch_yuv_fast<OUT, YUV420_NV12>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                    case YUV420_NV21: launch_yuv_fast<OUT, YUV420_NV21>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                    case YUV420_I420: launch_yuv_fast<OUT, YUV420_I420>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
+                    default: launch_yuv_fast<OUT, YUV420_YV12>(s, identity, bil, d, yc, fr, p, nv, dst, f0, nb, id_groups, id_items); break;
                 }
             }
             KB200_TRY(check_launch(identity ? f.identity_kernel : f.fast_kernel));
             continue;
         }
         dim3 grid(div_up(pixels, 256), nb);
-        if (p) launch_generic_for<F16, true>(s, grid, d, f, yc, yc16, fr, dst, f0);
-        else launch_generic_for<F16, false>(s, grid, d, f, yc, yc16, fr, dst, f0);
+        if (p) launch_generic_for<OUT, true>(s, grid, d, f, yc, yc16, fr, dst, f0);
+        else launch_generic_for<OUT, false>(s, grid, d, f, yc, yc16, fr, dst, f0);
         KB200_TRY(check_launch("preprocess_generic_kernel"));
     }
     return KB200_OK;
@@ -998,13 +1009,16 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, int
 // used by the host-buffer pipeline (host_pipeline.cu): frames already staged at base + i*stride on the device
 int preprocess_validate(const kb200_preprocess_desc* desc) { return validate_desc(desc); }
 size_t preprocess_frame_bytes(const kb200_preprocess_desc& d) { return src_bytes(plain_desc(d)); }
-int preprocess_launch_strided(cudaStream_t s, const kb200_preprocess_desc& desc, const uint8_t* base, size_t stride, uint32_t batch, void* dst, bool f16) {
+// out: a kb200_out_format the caller has checked
+int preprocess_launch_strided(cudaStream_t s, const kb200_preprocess_desc& desc, const uint8_t* base, size_t stride, uint32_t batch, void* dst, int out) {
     const kb200_preprocess_desc d = plain_desc(desc);
     const int m = yuv_matrix(desc);
-    return f16 ? launch_preprocess<true>(s, d, m, nullptr, base, stride, batch, dst) : launch_preprocess<false>(s, d, m, nullptr, base, stride, batch, dst);
+    if (out == KB200_OUT_F16) return launch_preprocess<KB200_OUT_F16>(s, d, m, nullptr, base, stride, batch, dst);
+    if (out == KB200_OUT_BF16) return launch_preprocess<KB200_OUT_BF16>(s, d, m, nullptr, base, stride, batch, dst);
+    return launch_preprocess<KB200_OUT_F32>(s, d, m, nullptr, base, stride, batch, dst);
 }
 
-template <bool F16>
+template <int OUT>
 static int preprocess_entry(kb200_stream_t stream, const kb200_preprocess_desc* raw_desc, const uint8_t* const* frames,
                             const size_t* frame_len, const uint8_t* base, size_t base_len, size_t stride,
                             uint32_t batch, void* dst, size_t dst_len) {
@@ -1034,7 +1048,7 @@ static int preprocess_entry(kb200_stream_t stream, const kb200_preprocess_desc* 
     }
     // BatchMismatch / BadOutputShape: dst must hold [batch,3,H,W]
     KB200_TRY(check_slice("dst", dst_len, (size_t)batch * 3 * desc->dst_w * desc->dst_h));
-    return launch_preprocess<F16>(as_stream(stream), *desc, yuv_matrix(*raw_desc), frames, base, stride, batch, dst);
+    return launch_preprocess<OUT>(as_stream(stream), *desc, yuv_matrix(*raw_desc), frames, base, stride, batch, dst);
 }
 
 __global__ void selftest_div255_kernel(unsigned long long* mismatches) {
@@ -1073,20 +1087,29 @@ KB200_API size_t kb200_preprocess_src_bytes(const kb200_preprocess_desc* desc) {
 KB200_API int kb200_preprocess_f32(kb200_stream_t stream, const kb200_preprocess_desc* desc, const uint8_t* const* frames,
                                    const size_t* frame_len, uint32_t batch, float* dst, size_t dst_len) {
     if (!frames) return fail(KB200_ERR_INVALID_ARGUMENT, "null pointer for 'frames'");
-    return preprocess_entry<false>(stream, desc, frames, frame_len, nullptr, 0, 0, batch, dst, dst_len);
+    return preprocess_entry<KB200_OUT_F32>(stream, desc, frames, frame_len, nullptr, 0, 0, batch, dst, dst_len);
 }
 KB200_API int kb200_preprocess_f16(kb200_stream_t stream, const kb200_preprocess_desc* desc, const uint8_t* const* frames,
                                    const size_t* frame_len, uint32_t batch, uint16_t* dst, size_t dst_len) {
     if (!frames) return fail(KB200_ERR_INVALID_ARGUMENT, "null pointer for 'frames'");
-    return preprocess_entry<true>(stream, desc, frames, frame_len, nullptr, 0, 0, batch, dst, dst_len);
+    return preprocess_entry<KB200_OUT_F16>(stream, desc, frames, frame_len, nullptr, 0, 0, batch, dst, dst_len);
+}
+KB200_API int kb200_preprocess_bf16(kb200_stream_t stream, const kb200_preprocess_desc* desc, const uint8_t* const* frames,
+                                    const size_t* frame_len, uint32_t batch, uint16_t* dst, size_t dst_len) {
+    if (!frames) return fail(KB200_ERR_INVALID_ARGUMENT, "null pointer for 'frames'");
+    return preprocess_entry<KB200_OUT_BF16>(stream, desc, frames, frame_len, nullptr, 0, 0, batch, dst, dst_len);
 }
 KB200_API int kb200_preprocess_strided_f32(kb200_stream_t stream, const kb200_preprocess_desc* desc, const uint8_t* base,
                                            size_t base_len, size_t frame_stride, uint32_t batch, float* dst, size_t dst_len) {
-    return preprocess_entry<false>(stream, desc, nullptr, nullptr, base, base_len, frame_stride, batch, dst, dst_len);
+    return preprocess_entry<KB200_OUT_F32>(stream, desc, nullptr, nullptr, base, base_len, frame_stride, batch, dst, dst_len);
 }
 KB200_API int kb200_preprocess_strided_f16(kb200_stream_t stream, const kb200_preprocess_desc* desc, const uint8_t* base,
                                            size_t base_len, size_t frame_stride, uint32_t batch, uint16_t* dst, size_t dst_len) {
-    return preprocess_entry<true>(stream, desc, nullptr, nullptr, base, base_len, frame_stride, batch, dst, dst_len);
+    return preprocess_entry<KB200_OUT_F16>(stream, desc, nullptr, nullptr, base, base_len, frame_stride, batch, dst, dst_len);
+}
+KB200_API int kb200_preprocess_strided_bf16(kb200_stream_t stream, const kb200_preprocess_desc* desc, const uint8_t* base,
+                                            size_t base_len, size_t frame_stride, uint32_t batch, uint16_t* dst, size_t dst_len) {
+    return preprocess_entry<KB200_OUT_BF16>(stream, desc, nullptr, nullptr, base, base_len, frame_stride, batch, dst, dst_len);
 }
 
 }  // extern "C"

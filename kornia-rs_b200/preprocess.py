@@ -26,6 +26,12 @@ from .imgproc import YuvMatrix
 IMAGENET_MEAN = (0.485, 0.456, 0.406)  # preprocess.rs:93
 IMAGENET_STD = (0.229, 0.224, 0.225)   # preprocess.rs:95
 
+# The output dtype of each kb200_out_format, indexed by it.  The Preprocessor's internal `out` arguments are these codes,
+# so False and True still mean f32 and f16.
+_OUT_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
+_TABLE_ENTRIES = ("kb200_preprocess_f32", "kb200_preprocess_f16", "kb200_preprocess_bf16")
+_STRIDED_ENTRIES = ("kb200_preprocess_strided_f32", "kb200_preprocess_strided_f16", "kb200_preprocess_strided_bf16")
+
 
 class PreprocessError(Exception):
     """preprocess.rs:252-332; `kind` names the variant."""
@@ -370,7 +376,7 @@ class Preprocessor:
         return d
 
     @staticmethod
-    def _validate_dst(dst: torch.Tensor, expected_n: int, f16: bool) -> None:
+    def _validate_dst(dst: torch.Tensor, expected_n: int, out: int) -> None:
         shape = tuple(dst.shape)
         if dst.dim() != 4 or shape[1] != 3 or (expected_n == 1 and shape[0] != 1):  # :805-808
             raise PreprocessError("BadOutputShape", f"destination tensor must be [1, 3, H, W], got {list(shape)}")
@@ -379,11 +385,11 @@ class Preprocessor:
                                   dst_n=shape[0], frames=expected_n)
         if not dst.is_cuda:
             raise PreprocessError("NotDeviceTensor", "CUDA preprocessor requires a device-resident destination tensor")
-        want = torch.float16 if f16 else torch.float32
+        want = _OUT_DTYPES[out]
         if dst.dtype != want or not dst.is_contiguous():
             raise PreprocessError("BadOutputShape", f"destination tensor must be contiguous {want}, got {dst.dtype}")
 
-    def _launch(self, desc, frames: Sequence[torch.Tensor], dst: torch.Tensor, f16: bool) -> None:
+    def _launch(self, desc, frames: Sequence[torch.Tensor], dst: torch.Tensor, out: int) -> None:
         dev = dst.device
         for f in frames:
             if not f.is_cuda:
@@ -395,7 +401,7 @@ class Preprocessor:
         ptrs = (C.c_void_p * n)(*[f.data_ptr() for f in frames])
         lens = (C.c_size_t * n)(*[f.numel() * f.element_size() for f in frames])
         l = _lib.lib()
-        fn = l.kb200_preprocess_f16 if f16 else l.kb200_preprocess_f32
+        fn = getattr(l, _TABLE_ENTRIES[out])
         st = fn(torch.cuda.current_stream(dev).cuda_stream, C.byref(desc), ptrs, lens, n, dst.data_ptr(), dst.numel())
         if st != _lib.OK:
             kind = {_lib.ERR_INVALID_SOURCE: "InvalidRawSource", _lib.ERR_DIMS_TOO_LARGE: "DimensionsTooLarge"}.get(st, "Cuda")
@@ -415,7 +421,7 @@ class Preprocessor:
                                   format=f, width=w, height=h, got=got, need=need)
 
     # ── typed entries (interleaved RGB/BGR[A] images) ───────────────────────
-    def _run_typed(self, src: Image, dst: torch.Tensor, f16: bool) -> None:
+    def _run_typed(self, src: Image, dst: torch.Tensor, out: int) -> None:
         c = src.num_channels()
         if c not in (3, 4):
             raise PreprocessError("UnsupportedChannels", f"unsupported source channel count {c} (expected 3 or 4)")
@@ -423,12 +429,12 @@ class Preprocessor:
         self._validate_typed_format(c)
         if not src.is_device:
             raise PreprocessError("NotDeviceImage", "CUDA preprocessor requires a device-resident source image")
-        self._validate_dst(dst, 1, f16)
+        self._validate_dst(dst, 1, out)
         if src.dtype != torch.uint8 or src.is_batched:
             raise PreprocessError("UnsupportedChannels", "typed run() takes one u8 HWC image")
         w, h = src.width(), src.height()
         desc = self._desc(w, h, w * c, c, self._fmt.fmt_code(), dst.shape[3], dst.shape[2])
-        self._launch(desc, [src.data], dst, f16)
+        self._launch(desc, [src.data], dst, out)
 
     @staticmethod
     def _validate_dst_shape_only(dst: torch.Tensor) -> None:
@@ -438,59 +444,85 @@ class Preprocessor:
 
     def run(self, src: Image, dst: torch.Tensor) -> None:
         """preprocess.rs:887 — `src` u8 HWC C∈{3,4} → `dst` [1,3,H,W] f32."""
-        self._run_typed(src, dst, False)
+        self._run_typed(src, dst, _lib.OUT_F32)
 
     def run_f16(self, src: Image, dst: torch.Tensor) -> None:
         """preprocess.rs:1086."""
-        self._run_typed(src, dst, True)
+        self._run_typed(src, dst, _lib.OUT_F16)
+
+    def run_bf16(self, src: Image, dst: torch.Tensor) -> None:
+        """`run` into a torch.bfloat16 `dst`: each value is the f32 result rounded to nearest even (beyond the reference,
+        which writes f32 and f16 only)."""
+        self._run_typed(src, dst, _lib.OUT_BF16)
 
     # ── pitched surfaces ────────────────────────────────────────────────────
-    def _run_surface(self, src: PitchedSurface, dst: torch.Tensor, f16: bool) -> None:
+    def _run_surface(self, src: PitchedSurface, dst: torch.Tensor, out: int) -> None:
         src.validate()
-        self._validate_dst(dst, 1, f16)
+        self._validate_dst(dst, 1, out)
         if not self._fmt.interleaved():  # :1150-1156
             raise PreprocessError("FormatNeedsRawBuffer", f"source format {self._fmt!r} needs run_raw (raw device buffer), not the typed run()")
         desc = self._desc(src.width, src.height, src.row_pitch, src.channels, self._fmt.fmt_code(), dst.shape[3], dst.shape[2])
-        self._launch(desc, [src.data], dst, f16)
+        self._launch(desc, [src.data], dst, out)
 
     def run_surface(self, src: PitchedSurface, dst: torch.Tensor) -> None:
         """preprocess.rs:1112."""
-        self._run_surface(src, dst, False)
+        self._run_surface(src, dst, _lib.OUT_F32)
 
     def run_surface_f16(self, src: PitchedSurface, dst: torch.Tensor) -> None:
-        self._run_surface(src, dst, True)
+        self._run_surface(src, dst, _lib.OUT_F16)
+
+    def run_surface_bf16(self, src: PitchedSurface, dst: torch.Tensor) -> None:
+        self._run_surface(src, dst, _lib.OUT_BF16)
 
     # ── raw camera buffers ──────────────────────────────────────────────────
-    def _run_raw_batch(self, frames: Sequence[torch.Tensor], src_w: int, src_h: int, dst: torch.Tensor, f16: bool,
+    def _run_raw_batch(self, frames: Sequence[torch.Tensor], src_w: int, src_h: int, dst: torch.Tensor, out: int,
                        single: bool) -> None:
-        self._validate_dst(dst, 1 if single else len(frames), f16)
+        self._validate_dst(dst, 1 if single else len(frames), out)
         for f in frames:
             self._validate_raw(f.numel() * f.element_size(), src_w, src_h)
         fmt = self._fmt
         desc = self._desc(src_w, src_h, fmt.pitch(src_w), fmt.bpp(), fmt.fmt_code(), dst.shape[3], dst.shape[2])
-        self._launch(desc, list(frames), dst, f16)
+        self._launch(desc, list(frames), dst, out)
 
     def run_raw(self, src: torch.Tensor, src_w: int, src_h: int, dst: torch.Tensor) -> None:
         """preprocess.rs:1184 — one raw device frame in the builder's SourceFormat → [1,3,H,W]."""
-        self._run_raw_batch([src], src_w, src_h, dst, False, True)
+        self._run_raw_batch([src], src_w, src_h, dst, _lib.OUT_F32, True)
 
     def run_raw_f16(self, src: torch.Tensor, src_w: int, src_h: int, dst: torch.Tensor) -> None:
-        self._run_raw_batch([src], src_w, src_h, dst, True, True)
+        self._run_raw_batch([src], src_w, src_h, dst, _lib.OUT_F16, True)
+
+    def run_raw_bf16(self, src: torch.Tensor, src_w: int, src_h: int, dst: torch.Tensor) -> None:
+        self._run_raw_batch([src], src_w, src_h, dst, _lib.OUT_BF16, True)
 
     def run_raw_batch(self, frames: Sequence[torch.Tensor], src_w: int, src_h: int, dst: torch.Tensor) -> None:
         """preprocess.rs:1234 — N same-sized raw frames → [N,3,H,W], ONE launch (≤256 frames per launch)."""
-        self._run_raw_batch(frames, src_w, src_h, dst, False, False)
+        self._run_raw_batch(frames, src_w, src_h, dst, _lib.OUT_F32, False)
 
     def run_raw_batch_f16(self, frames: Sequence[torch.Tensor], src_w: int, src_h: int, dst: torch.Tensor) -> None:
-        self._run_raw_batch(frames, src_w, src_h, dst, True, False)
+        self._run_raw_batch(frames, src_w, src_h, dst, _lib.OUT_F16, False)
+
+    def run_raw_batch_bf16(self, frames: Sequence[torch.Tensor], src_w: int, src_h: int, dst: torch.Tensor) -> None:
+        self._run_raw_batch(frames, src_w, src_h, dst, _lib.OUT_BF16, False)
+
+    @staticmethod
+    def _out_format(f16: bool, dtype) -> int:
+        """The kb200_out_format of run_raw_host / run_raw_strided: `dtype` when given, else `f16` decides."""
+        if dtype is None:
+            return _lib.OUT_F16 if f16 else _lib.OUT_F32
+        if dtype not in _OUT_DTYPES:
+            raise PreprocessError("BadOutputShape", f"unsupported output dtype {dtype} (expected torch.float32, torch.float16 or torch.bfloat16)")
+        if f16 and dtype != torch.float16:
+            raise PreprocessError("BadOutputShape", f"f16=True conflicts with dtype={dtype}")
+        return _OUT_DTYPES.index(dtype)
 
     def run_raw_host(self, host_frames: torch.Tensor, src_w: int, src_h: int, dst_size: tuple[int, int], out: torch.Tensor | None = None,
-                     f16: bool = False, pipeline=None) -> torch.Tensor:
+                     f16: bool = False, pipeline=None, *, dtype: torch.dtype | None = None) -> torch.Tensor:
         """HOST camera frames in, HOST tensor out — what the reference's Python `Preprocessor` does around its kernel (pinned
         staging, upload, launch: kornia-py/src/cuda_ext/mod.rs:700-760), as one call: `host_frames` is a [N, frame_bytes] uint8
         host tensor, or [N, w*h] uint16 for the 16-bit Bayer formats, [N, w*h*3/2] uint16 for P010 / P012 / I010 / I012 and
         [N, 3*w*h] uint16 for I410 / I412 / I410Msb / I412Msb (page-locked
-        for overlap), the result a [N,3,H,W] f32 / f16 host tensor (pinned when allocated here).
+        for overlap), the result a [N,3,H,W] host tensor (pinned when allocated here) of `dtype`: torch.float32, torch.float16 or
+        torch.bfloat16; without `dtype`, f16 when `f16`, else f32.
         Chunks ride a `HostPipeline` ring: upload -> ONE fused launch per chunk -> download.  Enqueue-only: synchronise the
         current stream of the pipeline's device before reading the result."""
         from . import imgproc
@@ -503,7 +535,8 @@ class Preprocessor:
         n, stride = t.shape[0], t.shape[1] * t.element_size()   # bytes
         self._validate_raw(stride, src_w, src_h)
         dw, dh = dst_size
-        want = torch.float16 if f16 else torch.float32
+        fmt_out = self._out_format(f16, dtype)
+        want = _OUT_DTYPES[fmt_out]
         if out is None:
             out = torch.empty((n, 3, dh, dw), dtype=want, pin_memory=True)
         if out.is_cuda or out.dtype != want or not out.is_contiguous() or tuple(out.shape) != (n, 3, dh, dw):
@@ -512,19 +545,21 @@ class Preprocessor:
         desc = self._desc(src_w, src_h, fmt.pitch(src_w), fmt.bpp(), fmt.fmt_code(), dw, dh)
         pipe = imgproc._pipeline_for(pipeline)
         _lib.set_device(pipe.device.index)
-        st = _lib.lib().kb200_preprocess_host(pipe._h, torch.cuda.current_stream(pipe.device).cuda_stream, C.byref(desc), t.data_ptr(), n * stride,
-                                             stride, n, out.data_ptr(), out.numel(), 1 if f16 else 0)
+        st = _lib.lib().kb200_preprocess_host_format(pipe._h, torch.cuda.current_stream(pipe.device).cuda_stream, C.byref(desc), t.data_ptr(),
+                                                    n * stride, stride, n, out.data_ptr(), out.numel(), fmt_out)
         if st != _lib.OK:
             kind = {_lib.ERR_INVALID_SOURCE: "InvalidRawSource"}.get(st, "Cuda")
             raise PreprocessError(kind, _lib.last_error())
         return out
 
     def run_raw_strided(self, base: torch.Tensor, frame_stride: int, batch: int, src_w: int, src_h: int,
-                        dst: torch.Tensor, f16: bool = False) -> None:
+                        dst: torch.Tensor, f16: bool = False, *, dtype: torch.dtype | None = None) -> None:
         """Frames at `base + i*frame_stride` bytes (a capture ring buffer): no pointer table.  `base` may be uint8 or, for
         the formats of 16-bit samples (16-bit Bayer, P010 / P012 / I010 / I012, I410 / I412 / I410Msb / I412Msb), uint16: its
-        length is counted in bytes."""
-        self._validate_dst(dst, batch, f16)
+        length is counted in bytes.  `dst` is of `dtype` (torch.float32, torch.float16 or torch.bfloat16); without `dtype`,
+        float16 when `f16`, else float32."""
+        out = self._out_format(f16, dtype)
+        self._validate_dst(dst, batch, out)
         fmt = self._fmt
         nbytes = base.numel() * base.element_size()
         self._validate_raw(min(frame_stride, nbytes) if batch > 1 else nbytes, src_w, src_h)
@@ -534,7 +569,7 @@ class Preprocessor:
         dev = dst.device
         _lib.set_device(dev.index)
         l = _lib.lib()
-        fn = l.kb200_preprocess_strided_f16 if f16 else l.kb200_preprocess_strided_f32
+        fn = getattr(l, _STRIDED_ENTRIES[out])
         st = fn(torch.cuda.current_stream(dev).cuda_stream, C.byref(desc), base.data_ptr(), nbytes, frame_stride, batch,
                 dst.data_ptr(), dst.numel())
         if st != _lib.OK:
