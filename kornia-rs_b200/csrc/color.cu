@@ -101,6 +101,16 @@ __device__ __forceinline__ uint32_t pack_sat2(int hi, int lo, uint32_t upper) {
 // four saturated bytes, b0 in the low byte
 __device__ __forceinline__ uint32_t pack_sat4(int b0, int b1, int b2, int b3) { return pack_sat2(b1, b0, pack_sat2(b3, b2, 0u)); }
 
+// 48 bytes of interleaved 16-bit RGB, r0 g0 b0 r1 ..., two samples per 32-bit word, from rgb[channel][pixel] of 8 pixels.
+__device__ __forceinline__ void pack_rgb48_u16(const int (&rgb)[3][8], uint4 o[3]) {
+    uint32_t w[12];
+#pragma unroll
+    for (int m = 0; m < 12; ++m) w[m] = (uint32_t)rgb[(2 * m) % 3][(2 * m) / 3] | ((uint32_t)rgb[(2 * m + 1) % 3][(2 * m + 1) / 3] << 16);
+    o[0] = make_uint4(w[0], w[1], w[2], w[3]);
+    o[1] = make_uint4(w[4], w[5], w[6], w[7]);
+    o[2] = make_uint4(w[8], w[9], w[10], w[11]);
+}
+
 __device__ __forceinline__ void pack_rgb16(const uint32_t yw[4], const ChromaTerms ct[8], const YuvCoeffs& yc, uint4 out[3]) {
     uint32_t w[12];
 #pragma unroll
@@ -132,6 +142,23 @@ __device__ __forceinline__ void store_rgb48_coalesced(uint4* __restrict__ warp_d
     __syncwarp();
     stg_stream_u4(warp_dst + lane, a); stg_stream_u4(warp_dst + 32 + lane, b); stg_stream_u4(warp_dst + 64 + lane, c);
 }
+
+// The warp runs of the row-wise vector decoders: thread gx of a grid row owns COLS columns, so a warp owns 32 * COLS
+// contiguous columns of one row and 1536 contiguous output bytes.  A kernel returns when its warp is past the row
+// (gx0 * COLS >= width); a ragged last warp of a row stores its active threads' 48 B directly.
+template <uint32_t COLS>
+struct WarpRun {
+    uint32_t gx, lane, gx0;   // the thread's column group, its lane and its warp's first group
+    bool full_warp, active;
+    __device__ __forceinline__ explicit WarpRun(uint32_t width)
+        : gx(blockIdx.x * blockDim.x + threadIdx.x), lane(threadIdx.x & 31u), gx0(gx - lane),
+          full_warp((gx0 + 32) * COLS <= width), active(gx * COLS < width) {}
+    // d: the warp's run; stage: the warp's 1536-B scratch (store_rgb48_coalesced)
+    __device__ __forceinline__ void store(uint4* __restrict__ d, uint4* __restrict__ stage, const uint4 o[3]) const {
+        if (full_warp) store_rgb48_coalesced(d, stage, lane, o);
+        else if (active) { stg_stream_u4(d + 3 * lane, o[0]); stg_stream_u4(d + 3 * lane + 1, o[1]); stg_stream_u4(d + 3 * lane + 2, o[2]); }
+    }
+};
 
 // One thread: 16 luma columns x 2 rows (one chroma row) — 16 B Y (top), 16 B Y (bottom) and the 8 chroma pairs: one
 // 16-B load of the interleaved row (NV12 / NV21), or 8 B of the U plane and 8 B of the V plane (I420 / YV12; with
@@ -269,12 +296,7 @@ __global__ void __launch_bounds__(128) rgb_from_yuv420_u16_vec(const uint16_t* _
 #pragma unroll
         for (int j = 0; j < 8; ++j)
             decode_rgb16(yy_term16(yuv16_code(yw[j >> 1] >> (16 * (j & 1)), k), k), ct[j >> 1], k.white, rgb[0][j], rgb[1][j], rgb[2][j]);
-        uint32_t w[12];
-#pragma unroll
-        for (int m = 0; m < 12; ++m) w[m] = (uint32_t)rgb[(2 * m) % 3][(2 * m) / 3] | ((uint32_t)rgb[(2 * m + 1) % 3][(2 * m + 1) / 3] << 16);
-        o[0] = make_uint4(w[0], w[1], w[2], w[3]);
-        o[1] = make_uint4(w[4], w[5], w[6], w[7]);
-        o[2] = make_uint4(w[8], w[9], w[10], w[11]);
+        pack_rgb48_u16(rgb, o);
     };
     uint4 o[3];
     uint4* d0 = reinterpret_cast<uint4*>(out + ((size_t)(2 * cy) * width + (size_t)gx0 * 8) * 3);       // this warp's 1536-B run, top row
@@ -323,18 +345,14 @@ __global__ void rgb_from_yuv420_u16_generic(const uint16_t* __restrict__ src, ui
 __global__ void __launch_bounds__(128) rgb_from_i444_vec16(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, uint32_t width,
                                                            uint32_t height, const YuvCoeffs yc) {
     __shared__ uint4 stage[4][96];
-    const uint32_t gx = blockIdx.x * blockDim.x + threadIdx.x;  // 16-column group
-    const uint32_t lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
-    const uint32_t gx0 = gx - lane;                             // first group of this warp
-    if (gx0 * 16 >= width) return;                              // whole warp out of the row
-    const bool full_warp = (gx0 + 32) * 16 <= width;
-    const bool active = gx * 16 < width;
+    const WarpRun<16> run(width);
+    if (run.gx0 * 16 >= width) return;   // whole warp out of the row
     const size_t plane = (size_t)width * height;
     const uint8_t* frame = src + (size_t)blockIdx.z * plane * 3;
     const size_t row = (size_t)blockIdx.y * width;
     uint4 yv = make_uint4(0, 0, 0, 0), uv = yv, vv = yv;
-    if (active) {
-        const size_t p = row + (size_t)gx * 16;
+    if (run.active) {
+        const size_t p = row + (size_t)run.gx * 16;
         yv = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + p));
         uv = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + plane + p));
         vv = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + 2 * plane + p));
@@ -355,27 +373,21 @@ __global__ void __launch_bounds__(128) rgb_from_i444_vec16(const uint8_t* __rest
         w[3 * k + 2] = pack_sat4(b[2], r[3], g[3], b[3]);
     }
     const uint4 o[3] = {make_uint4(w[0], w[1], w[2], w[3]), make_uint4(w[4], w[5], w[6], w[7]), make_uint4(w[8], w[9], w[10], w[11])};
-    uint4* d = reinterpret_cast<uint4*>(dst + (size_t)blockIdx.z * plane * 3 + (row + (size_t)gx0 * 16) * 3);   // this warp's 1536-B run
-    if (full_warp) store_rgb48_coalesced(d, stage[wid], lane, o);
-    else if (active) { stg_stream_u4(d + 3 * lane, o[0]); stg_stream_u4(d + 3 * lane + 1, o[1]); stg_stream_u4(d + 3 * lane + 2, o[2]); }
+    run.store(reinterpret_cast<uint4*>(dst + (size_t)blockIdx.z * plane * 3 + (row + (size_t)run.gx0 * 16) * 3), stage[threadIdx.x >> 5], o);
 }
 
 // The depth, code position and matrix arrive in Yuv16Coeffs, so one kernel serves I410, I412, I410Msb and I412Msb.
 __global__ void __launch_bounds__(128) rgb_from_i41x_vec(const uint16_t* __restrict__ src, uint16_t* __restrict__ dst, uint32_t width,
                                                          uint32_t height, const Yuv16Coeffs k) {
     __shared__ uint4 stage[4][96];
-    const uint32_t gx = blockIdx.x * blockDim.x + threadIdx.x;  // 8-column group
-    const uint32_t lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
-    const uint32_t gx0 = gx - lane;                             // first group of this warp
-    if (gx0 * 8 >= width) return;                               // whole warp out of the row
-    const bool full_warp = (gx0 + 32) * 8 <= width;
-    const bool active = gx * 8 < width;
+    const WarpRun<8> run(width);
+    if (run.gx0 * 8 >= width) return;   // whole warp out of the row
     const size_t plane = (size_t)width * height;
     const uint16_t* frame = src + (size_t)blockIdx.z * plane * 3;
     const size_t row = (size_t)blockIdx.y * width;
     uint4 yv = make_uint4(0, 0, 0, 0), uv = yv, vv = yv;
-    if (active) {
-        const size_t p = row + (size_t)gx * 8;
+    if (run.active) {
+        const size_t p = row + (size_t)run.gx * 8;
         yv = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + p));
         uv = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + plane + p));
         vv = ldg_stream_u4(reinterpret_cast<const uint4*>(frame + 2 * plane + p));
@@ -388,13 +400,9 @@ __global__ void __launch_bounds__(128) rgb_from_i41x_vec(const uint16_t* __restr
         const ChromaTerms t = chroma_terms16(yuv16_code(uw[j >> 1] >> sh, k), yuv16_code(vw[j >> 1] >> sh, k), k);
         decode_rgb16(yy_term16(yuv16_code(yw[j >> 1] >> sh, k), k), t, k.white, rgb[0][j], rgb[1][j], rgb[2][j]);
     }
-    uint32_t w[12];   // 8 pixels -> 24 samples r0 g0 b0 r1 ..., two per 32-bit word
-#pragma unroll
-    for (int m = 0; m < 12; ++m) w[m] = (uint32_t)rgb[(2 * m) % 3][(2 * m) / 3] | ((uint32_t)rgb[(2 * m + 1) % 3][(2 * m + 1) / 3] << 16);
-    const uint4 o[3] = {make_uint4(w[0], w[1], w[2], w[3]), make_uint4(w[4], w[5], w[6], w[7]), make_uint4(w[8], w[9], w[10], w[11])};
-    uint4* d = reinterpret_cast<uint4*>(dst + (size_t)blockIdx.z * plane * 3 + (row + (size_t)gx0 * 8) * 3);   // this warp's 1536-B run
-    if (full_warp) store_rgb48_coalesced(d, stage[wid], lane, o);
-    else if (active) { stg_stream_u4(d + 3 * lane, o[0]); stg_stream_u4(d + 3 * lane + 1, o[1]); stg_stream_u4(d + 3 * lane + 2, o[2]); }
+    uint4 o[3];
+    pack_rgb48_u16(rgb, o);
+    run.store(reinterpret_cast<uint4*>(dst + (size_t)blockIdx.z * plane * 3 + (row + (size_t)run.gx0 * 8) * 3), stage[threadIdx.x >> 5], o);
 }
 
 // Generic fallbacks (any width, unaligned bases; words 2-B aligned): one thread per pixel.
@@ -608,20 +616,68 @@ static inline unsigned stream_grid(size_t items, unsigned block, unsigned ctas_p
     return (unsigned)std::max<size_t>(1, std::min(want, cap));
 }
 
-// The kernels of each layout, indexed by kb200_yuv420_layout / kb200_yuv422_layout, and the names they report through
-// kb200_last_kernel().
-struct Yuv420Kernels {
-    const char* layout;
-    void (*vec16)(const uint8_t*, uint8_t*, uint32_t, uint32_t, size_t, YuvCoeffs);
-    void (*generic)(const uint8_t*, uint8_t*, uint32_t, uint32_t, size_t, YuvCoeffs);
-    const char *vec16_name, *generic_name;
+// The argument checks the decoders share.
+static int check_matrix(int matrix) {
+    if (matrix < KB200_YUV_BT601_LIMITED || matrix > KB200_YUV_BT709_FULL) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown YUV matrix %d", matrix);
+    return KB200_OK;
+}
+static int check_words(const char* what, const void* p) {   // a buffer of 16-bit samples
+    if (reinterpret_cast<uintptr_t>(p) & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "'%s' is not 2-byte aligned (16-bit samples)", what);
+    return KB200_OK;
+}
+static int check_batch(uint32_t batch) {   // one frame per gridDim.z
+    if (batch > 65535u) return fail(KB200_ERR_INVALID_ARGUMENT, "batch %u exceeds 65535", batch);
+    return KB200_OK;
+}
+
+// The kernels of one decoder that has a vector kernel, and the names they report through kb200_last_kernel().  Both
+// take (src, dst, width, height, A...).
+template <typename S, typename D, typename... A>
+struct DecodeKernels {
+    void (*vec)(const S*, D*, uint32_t, uint32_t, A...);
+    void (*generic)(const S*, D*, uint32_t, uint32_t, A...);
+    const char *vec_name, *generic_name;
 };
-static const Yuv420Kernels YUV420_KERNELS[4] = {
-    {"NV12", rgb_from_yuv420_vec16<YUV420_NV12>, rgb_from_yuv420_generic<YUV420_NV12>, "rgb_from_nv12_vec16", "rgb_from_nv12_generic"},
-    {"NV21", rgb_from_yuv420_vec16<YUV420_NV21>, rgb_from_yuv420_generic<YUV420_NV21>, "rgb_from_nv21_vec16", "rgb_from_nv21_generic"},
-    {"I420", rgb_from_yuv420_vec16<YUV420_I420>, rgb_from_yuv420_generic<YUV420_I420>, "rgb_from_i420_vec16", "rgb_from_i420_generic"},
-    {"YV12", rgb_from_yuv420_vec16<YUV420_YV12>, rgb_from_yuv420_generic<YUV420_YV12>, "rgb_from_yv12_vec16", "rgb_from_yv12_generic"},
+
+// The launch of a DecodeKernels row (arguments already checked).  The vector kernel when the format's gate `fits` holds,
+// both bases are 16-B aligned and its `rows` grid rows fit gridDim.y: each thread owns `cols` columns of a grid row, the
+// threads of a row are CTAs of up to 128.  The fallback otherwise, one thread per `step` x `step` pixels (1, or 2 for the
+// 8-bit 4:2:0 kernel's 2x2 blocks) over a (width, height, batch) grid of 32 x 8 CTAs.
+template <typename S, typename D, typename... A>
+static int launch_decoder(const DecodeKernels<S, D, A...>& k, kb200_stream_t stream, bool fits, uint32_t cols, uint32_t rows, uint32_t step,
+                          const S* src, D* dst, uint32_t width, uint32_t height, uint32_t batch, A... args) {
+    cudaStream_t s = as_stream(stream);
+    if (fits && aligned16(src) && aligned16(dst) && rows <= 65535u) {
+        const unsigned groups = width / cols;
+        const unsigned bx = groups >= 128 ? 128 : 32 * ((groups + 31) / 32);
+        dim3 grid(div_up(groups, bx), rows, batch);
+        k.vec<<<grid, bx, 0, s>>>(src, dst, width, height, args...);
+        return check_launch(k.vec_name);
+    }
+    dim3 block(32, 8), grid(div_up(width / step, 32), div_up(height / step, 8), batch);
+    k.generic<<<grid, block, 0, s>>>(src, dst, width, height, args...);
+    return check_launch(k.generic_name);
+}
+
+// 8-bit 4:2:0, indexed by kb200_yuv420_layout.
+static const char* const YUV420_LAYOUTS[4] = {"NV12", "NV21", "I420", "YV12"};
+static const DecodeKernels<uint8_t, uint8_t, size_t, YuvCoeffs> YUV420_KERNELS[4] = {
+    {rgb_from_yuv420_vec16<YUV420_NV12>, rgb_from_yuv420_generic<YUV420_NV12>, "rgb_from_nv12_vec16", "rgb_from_nv12_generic"},
+    {rgb_from_yuv420_vec16<YUV420_NV21>, rgb_from_yuv420_generic<YUV420_NV21>, "rgb_from_nv21_vec16", "rgb_from_nv21_generic"},
+    {rgb_from_yuv420_vec16<YUV420_I420>, rgb_from_yuv420_generic<YUV420_I420>, "rgb_from_i420_vec16", "rgb_from_i420_generic"},
+    {rgb_from_yuv420_vec16<YUV420_YV12>, rgb_from_yuv420_generic<YUV420_YV12>, "rgb_from_yv12_vec16", "rgb_from_yv12_generic"},
 };
+// 16-bit 4:2:0, indexed by kb200_yuv420_u16_layout.
+static const DecodeKernels<uint16_t, uint16_t, Yuv16Coeffs> YUV420_U16_KERNELS[2] = {
+    {rgb_from_yuv420_u16_vec<KB200_YUV420_P01X>, rgb_from_yuv420_u16_generic<KB200_YUV420_P01X>, "rgb_from_p01x_vec", "rgb_from_p01x_generic"},
+    {rgb_from_yuv420_u16_vec<KB200_YUV420_I01X>, rgb_from_yuv420_u16_generic<KB200_YUV420_I01X>, "rgb_from_i01x_vec", "rgb_from_i01x_generic"},
+};
+static const DecodeKernels<uint8_t, uint8_t, YuvCoeffs> YUV444_KERNELS = {rgb_from_i444_vec16, rgb_from_i444_generic,
+                                                                          "rgb_from_i444_vec16", "rgb_from_i444_generic"};
+static const DecodeKernels<uint16_t, uint16_t, Yuv16Coeffs> YUV444_U16_KERNELS = {rgb_from_i41x_vec, rgb_from_i41x_generic,
+                                                                                  "rgb_from_i41x_vec", "rgb_from_i41x_generic"};
+
+// 4:2:2, indexed by kb200_yuv422_layout.  These kernels walk the batch flat in 2-pixel groups, so they have a row of their own.
 struct Yuv422Kernels {
     const char* layout;
     void (*vec16)(const uint4*, uint4*, size_t, YuvCoeffs);
@@ -635,12 +691,7 @@ static const Yuv422Kernels YUV422_KERNELS[3] = {
 };
 // The Bayer kernels of each sample type, indexed by kb200_bayer_pattern.
 static const char* const BAYER_PATTERNS[4] = {"RGGB", "BGGR", "GRBG", "GBRG"};
-template <typename T>
-struct BayerKernels {
-    void (*vec)(const T*, typename BayerSample<T>::Word*, uint32_t, uint32_t);
-    void (*generic)(const T*, typename BayerSample<T>::Word*, uint32_t, uint32_t);
-    const char *vec_name, *generic_name;
-};
+template <typename T> using BayerKernels = DecodeKernels<T, typename BayerSample<T>::Word>;
 static const BayerKernels<uint8_t> BAYER_KERNELS_U8[4] = {
     {rgb_from_bayer_vec<uint8_t, KB200_BAYER_RGGB>, rgb_from_bayer_generic<uint8_t, KB200_BAYER_RGGB>, "rgb_from_bayer_rggb_vec16", "rgb_from_bayer_rggb_generic"},
     {rgb_from_bayer_vec<uint8_t, KB200_BAYER_BGGR>, rgb_from_bayer_generic<uint8_t, KB200_BAYER_BGGR>, "rgb_from_bayer_bggr_vec16", "rgb_from_bayer_bggr_generic"},
@@ -660,24 +711,13 @@ template <typename T>
 static int launch_rgb_from_bayer(const BayerKernels<T> (&table)[4], kb200_stream_t stream, const T* src, size_t src_len, T* dst,
                                  size_t dst_len, uint32_t width, uint32_t height, uint32_t batch, int pattern) {
     if (pattern < KB200_BAYER_RGGB || pattern > KB200_BAYER_GBRG) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown Bayer pattern %d", pattern);
-    const BayerKernels<T>& k = table[pattern];
     KB200_TRY(check_geometry(width, height, width, height, batch));
     if (width < 3 || height < 3) return fail(KB200_ERR_INVALID_ARGUMENT, "Bayer %s needs at least 3x3 pixels, got %ux%u", BAYER_PATTERNS[pattern], width, height);
-    if (batch > 65535u) return fail(KB200_ERR_INVALID_ARGUMENT, "batch %u exceeds 65535", batch);
+    KB200_TRY(check_batch(batch));
     const size_t frame = (size_t)width * height;
     KB200_TRY(check_slice("src", src_len, frame * batch)); KB200_TRY(check_slice("dst", dst_len, frame * 3 * batch));
-    cudaStream_t s = as_stream(stream);
     constexpr uint32_t S = BayerSample<T>::VEC_COLS;
-    if ((width % S) == 0 && aligned16(src) && aligned16(dst) && bayer_row_pairs(height) <= 65535u) {
-        const unsigned groups = width / S;
-        const unsigned bx = groups >= 128 ? 128 : 32 * ((groups + 31) / 32);
-        dim3 grid(div_up(groups, bx), bayer_row_pairs(height), batch);
-        k.vec<<<grid, bx, 0, s>>>(src, dst, width, height);
-        return check_launch(k.vec_name);
-    }
-    dim3 block(32, 8), grid(div_up(width, 32), div_up(height, 8), batch);
-    k.generic<<<grid, block, 0, s>>>(src, dst, width, height);
-    return check_launch(k.generic_name);
+    return launch_decoder(table[pattern], stream, width % S == 0, S, bayer_row_pairs(height), 1, src, dst, width, height, batch);
 }
 
 // The packed decoders, by depth (10, 12, 14 bits) and pattern.
@@ -701,7 +741,6 @@ template <int BITS>
 static int launch_rgb_from_bayer_packed(const BayerKernels<BayerPacked<BITS>> (&table)[4], kb200_stream_t stream, const uint8_t* src,
                                         size_t src_len, uint16_t* dst, size_t dst_len, uint32_t width, uint32_t height, uint32_t batch,
                                         int pattern) {
-    const BayerKernels<BayerPacked<BITS>>& k = table[pattern];
     KB200_TRY(check_geometry(width, height, width, height, batch));
     if (width < 3 || height < 3)
         return fail(KB200_ERR_INVALID_ARGUMENT, "Bayer %s%dP needs at least 3x3 pixels, got %ux%u", BAYER_PATTERNS[pattern], BITS, width, height);
@@ -709,21 +748,11 @@ static int launch_rgb_from_bayer_packed(const BayerKernels<BayerPacked<BITS>> (&
     if (width % G)
         return fail(KB200_ERR_INVALID_ARGUMENT, "Bayer %s%dP needs a width that is a multiple of %u (whole %d-byte groups), got %u",
                     BAYER_PATTERNS[pattern], BITS, G, bayer_packed_group_bytes(BITS), width);
-    if (batch > 65535u) return fail(KB200_ERR_INVALID_ARGUMENT, "batch %u exceeds 65535", batch);
+    KB200_TRY(check_batch(batch));
     const size_t frame = (size_t)width * BITS / 8 * height;
     KB200_TRY(check_slice("src", src_len, frame * batch)); KB200_TRY(check_slice("dst", dst_len, (size_t)width * height * 3 * batch));
-    cudaStream_t s = as_stream(stream);
-    const BayerPacked<BITS>* p = reinterpret_cast<const BayerPacked<BITS>*>(src);
-    if (((size_t)width * BITS) % 128 == 0 && aligned16(src) && aligned16(dst) && bayer_row_pairs(height) <= 65535u) {
-        const unsigned groups = width / 8;
-        const unsigned bx = groups >= 128 ? 128 : 32 * ((groups + 31) / 32);
-        dim3 grid(div_up(groups, bx), bayer_row_pairs(height), batch);
-        k.vec<<<grid, bx, 0, s>>>(p, dst, width, height);
-        return check_launch(k.vec_name);
-    }
-    dim3 block(32, 8), grid(div_up(width, 32), div_up(height, 8), batch);
-    k.generic<<<grid, block, 0, s>>>(p, dst, width, height);
-    return check_launch(k.generic_name);
+    return launch_decoder(table[pattern], stream, ((size_t)width * BITS) % 128 == 0, 8, bayer_row_pairs(height), 1,
+                          reinterpret_cast<const BayerPacked<BITS>*>(src), dst, width, height, batch);
 }
 
 // ── RGB8 → YUYV / NV12 encode (SURVEY §8(f) #4) ─────────────────────────────────────────────
@@ -826,112 +855,67 @@ KB200_API int kb200_rgb_from_yuv420_u8_matrix(kb200_stream_t stream, const uint8
                                               size_t dst_len, uint32_t width, uint32_t height, uint32_t batch, int layout, int matrix) {
     KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
     if (layout < KB200_YUV420_NV12 || layout > KB200_YUV420_YV12) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown 4:2:0 layout %d", layout);
-    if (matrix < KB200_YUV_BT601_LIMITED || matrix > KB200_YUV_BT709_FULL) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown YUV matrix %d", matrix);
-    const YuvCoeffs& yc = YUV_COEFFS[matrix];
-    const Yuv420Kernels& k = YUV420_KERNELS[layout];
+    KB200_TRY(check_matrix(matrix));
     KB200_TRY(check_geometry(width, height, width, height, batch));
-    if ((width & 1u) || (height & 1u)) return fail(KB200_ERR_INVALID_ARGUMENT, "%s needs even dimensions, got %ux%u", k.layout, width, height);
-    if (batch > 65535u) return fail(KB200_ERR_INVALID_ARGUMENT, "batch %u exceeds 65535", batch);
-    const size_t frame = (size_t)width * height * 3 / 2, out_frame = (size_t)width * height * 3;
-    KB200_TRY(check_slice("src", src_len, frame * batch)); KB200_TRY(check_slice("dst", dst_len, out_frame * batch));
-    cudaStream_t s = as_stream(stream);
-    if ((width % 16u) == 0 && aligned16(src) && aligned16(dst) && (frame % 16u) == 0 && height / 2 <= 65535u) {
-        const unsigned groups = width / 16;
-        const unsigned bx = groups >= 128 ? 128 : 32 * ((groups + 31) / 32);
-        dim3 grid(div_up(groups, bx), height / 2, batch);
-        k.vec16<<<grid, bx, 0, s>>>(src, dst, width, height, frame, yc);
-        return check_launch(k.vec16_name);
-    }
-    dim3 block(32, 8), grid(div_up(width / 2, 32), div_up(height / 2, 8), batch);
-    k.generic<<<grid, block, 0, s>>>(src, dst, width, height, frame, yc);
-    return check_launch(k.generic_name);
+    if ((width & 1u) || (height & 1u)) return fail(KB200_ERR_INVALID_ARGUMENT, "%s needs even dimensions, got %ux%u", YUV420_LAYOUTS[layout], width, height);
+    KB200_TRY(check_batch(batch));
+    const size_t frame = (size_t)width * height * 3 / 2;
+    KB200_TRY(check_slice("src", src_len, frame * batch)); KB200_TRY(check_slice("dst", dst_len, (size_t)width * height * 3 * batch));
+    // w % 16 == 0, h even: every frame is a multiple of 16 B
+    return launch_decoder(YUV420_KERNELS[layout], stream, width % 16u == 0, 16, height / 2, 2, src, dst, width, height, batch, frame, YUV_COEFFS[matrix]);
 }
 
 KB200_API int kb200_rgb_from_yuv420_u16(kb200_stream_t stream, const uint16_t* src, size_t src_len, uint16_t* dst, size_t dst_len,
                                         uint32_t width, uint32_t height, uint32_t batch, int layout, int bits, int matrix) {
     KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
-    if (reinterpret_cast<uintptr_t>(src) & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "'src' is not 2-byte aligned (16-bit samples)");
-    if (reinterpret_cast<uintptr_t>(dst) & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "'dst' is not 2-byte aligned (16-bit samples)");
+    KB200_TRY(check_words("src", src)); KB200_TRY(check_words("dst", dst));
     if (layout != KB200_YUV420_P01X && layout != KB200_YUV420_I01X) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown 16-bit 4:2:0 layout %d", layout);
     if (bits != 10 && bits != 12) return fail(KB200_ERR_INVALID_ARGUMENT, "16-bit 4:2:0 samples are 10 or 12 bits, got %d", bits);
-    if (matrix < KB200_YUV_BT601_LIMITED || matrix > KB200_YUV_BT709_FULL) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown YUV matrix %d", matrix);
+    KB200_TRY(check_matrix(matrix));
     const bool planar = layout == KB200_YUV420_I01X;
-    const Yuv16Coeffs k = yuv16_coeffs(matrix, bits, !planar);
     char name[8];
     snprintf(name, sizeof name, "%c01%d", planar ? 'I' : 'P', bits - 10);
     KB200_TRY(check_geometry(width, height, width, height, batch));
     if ((width & 1u) || (height & 1u)) return fail(KB200_ERR_INVALID_ARGUMENT, "%s needs even dimensions, got %ux%u", name, width, height);
-    if (batch > 65535u) return fail(KB200_ERR_INVALID_ARGUMENT, "batch %u exceeds 65535", batch);
+    KB200_TRY(check_batch(batch));
     const size_t plane = (size_t)width * height;
     KB200_TRY(check_slice("src", src_len, plane * 3 / 2 * batch)); KB200_TRY(check_slice("dst", dst_len, plane * 3 * batch));
-    cudaStream_t s = as_stream(stream);
-    if ((width % 8u) == 0 && aligned16(src) && aligned16(dst) && height / 2 <= 65535u) {   // w % 8 == 0, h even: every frame 16-B aligned
-        const unsigned groups = width / 8;
-        const unsigned bx = groups >= 128 ? 128 : 32 * ((groups + 31) / 32);
-        dim3 grid(div_up(groups, bx), height / 2, batch);
-        if (planar) rgb_from_yuv420_u16_vec<KB200_YUV420_I01X><<<grid, bx, 0, s>>>(src, dst, width, height, k);
-        else rgb_from_yuv420_u16_vec<KB200_YUV420_P01X><<<grid, bx, 0, s>>>(src, dst, width, height, k);
-        return check_launch(planar ? "rgb_from_i01x_vec" : "rgb_from_p01x_vec");
-    }
-    dim3 block(32, 8), grid(div_up(width, 32), div_up(height, 8), batch);
-    if (planar) rgb_from_yuv420_u16_generic<KB200_YUV420_I01X><<<grid, block, 0, s>>>(src, dst, width, height, k);
-    else rgb_from_yuv420_u16_generic<KB200_YUV420_P01X><<<grid, block, 0, s>>>(src, dst, width, height, k);
-    return check_launch(planar ? "rgb_from_i01x_generic" : "rgb_from_p01x_generic");
+    // w % 8 == 0, h even: every frame 16-B aligned
+    return launch_decoder(YUV420_U16_KERNELS[layout], stream, width % 8u == 0, 8, height / 2, 1, src, dst, width, height, batch,
+                          yuv16_coeffs(matrix, bits, !planar));
 }
 
 KB200_API int kb200_rgb_from_yuv444_u8(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst, size_t dst_len,
                                        uint32_t width, uint32_t height, uint32_t batch, int matrix) {
     KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
-    if (matrix < KB200_YUV_BT601_LIMITED || matrix > KB200_YUV_BT709_FULL) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown YUV matrix %d", matrix);
-    const YuvCoeffs& yc = YUV_COEFFS[matrix];
+    KB200_TRY(check_matrix(matrix));
     KB200_TRY(check_geometry(width, height, width, height, batch));
-    if (batch > 65535u) return fail(KB200_ERR_INVALID_ARGUMENT, "batch %u exceeds 65535", batch);
+    KB200_TRY(check_batch(batch));
     const size_t plane = (size_t)width * height;
     KB200_TRY(check_slice("src", src_len, plane * 3 * batch)); KB200_TRY(check_slice("dst", dst_len, plane * 3 * batch));
-    cudaStream_t s = as_stream(stream);
-    if ((width % 16u) == 0 && aligned16(src) && aligned16(dst) && height <= 65535u) {
-        const unsigned groups = width / 16;
-        const unsigned bx = groups >= 128 ? 128 : 32 * ((groups + 31) / 32);
-        dim3 grid(div_up(groups, bx), height, batch);
-        rgb_from_i444_vec16<<<grid, bx, 0, s>>>(src, dst, width, height, yc);
-        return check_launch("rgb_from_i444_vec16");
-    }
-    dim3 block(32, 8), grid(div_up(width, 32), div_up(height, 8), batch);
-    rgb_from_i444_generic<<<grid, block, 0, s>>>(src, dst, width, height, yc);
-    return check_launch("rgb_from_i444_generic");
+    return launch_decoder(YUV444_KERNELS, stream, width % 16u == 0, 16, height, 1, src, dst, width, height, batch, YUV_COEFFS[matrix]);
 }
 
 KB200_API int kb200_rgb_from_yuv444_u16(kb200_stream_t stream, const uint16_t* src, size_t src_len, uint16_t* dst, size_t dst_len,
                                         uint32_t width, uint32_t height, uint32_t batch, int layout, int bits, int matrix) {
     KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
-    if (reinterpret_cast<uintptr_t>(src) & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "'src' is not 2-byte aligned (16-bit samples)");
-    if (reinterpret_cast<uintptr_t>(dst) & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "'dst' is not 2-byte aligned (16-bit samples)");
+    KB200_TRY(check_words("src", src)); KB200_TRY(check_words("dst", dst));
     if (layout != KB200_YUV444_I41X && layout != KB200_YUV444_I41X_MSB) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown 16-bit 4:4:4 layout %d", layout);
     if (bits != 10 && bits != 12) return fail(KB200_ERR_INVALID_ARGUMENT, "16-bit 4:4:4 samples are 10 or 12 bits, got %d", bits);
-    if (matrix < KB200_YUV_BT601_LIMITED || matrix > KB200_YUV_BT709_FULL) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown YUV matrix %d", matrix);
-    const Yuv16Coeffs k = yuv16_coeffs(matrix, bits, layout == KB200_YUV444_I41X_MSB);
+    KB200_TRY(check_matrix(matrix));
     KB200_TRY(check_geometry(width, height, width, height, batch));
-    if (batch > 65535u) return fail(KB200_ERR_INVALID_ARGUMENT, "batch %u exceeds 65535", batch);
+    KB200_TRY(check_batch(batch));
     const size_t plane = (size_t)width * height;
     KB200_TRY(check_slice("src", src_len, plane * 3 * batch)); KB200_TRY(check_slice("dst", dst_len, plane * 3 * batch));
-    cudaStream_t s = as_stream(stream);
-    if ((width % 8u) == 0 && aligned16(src) && aligned16(dst) && height <= 65535u) {
-        const unsigned groups = width / 8;
-        const unsigned bx = groups >= 128 ? 128 : 32 * ((groups + 31) / 32);
-        dim3 grid(div_up(groups, bx), height, batch);
-        rgb_from_i41x_vec<<<grid, bx, 0, s>>>(src, dst, width, height, k);
-        return check_launch("rgb_from_i41x_vec");
-    }
-    dim3 block(32, 8), grid(div_up(width, 32), div_up(height, 8), batch);
-    rgb_from_i41x_generic<<<grid, block, 0, s>>>(src, dst, width, height, k);
-    return check_launch("rgb_from_i41x_generic");
+    return launch_decoder(YUV444_U16_KERNELS, stream, width % 8u == 0, 8, height, 1, src, dst, width, height, batch,
+                          yuv16_coeffs(matrix, bits, layout == KB200_YUV444_I41X_MSB));
 }
 
 KB200_API int kb200_rgb_from_yuv422_u8_matrix(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint8_t* dst,
                                               size_t dst_len, uint32_t width, uint32_t height, uint32_t batch, int layout, int matrix) {
     KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
     if (layout < KB200_YUV422_YUYV || layout > KB200_YUV422_YVYU) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown 4:2:2 layout %d", layout);
-    if (matrix < KB200_YUV_BT601_LIMITED || matrix > KB200_YUV_BT709_FULL) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown YUV matrix %d", matrix);
+    KB200_TRY(check_matrix(matrix));
     const YuvCoeffs& yc = YUV_COEFFS[matrix];
     const Yuv422Kernels& k = YUV422_KERNELS[layout];
     KB200_TRY(check_geometry(width, height, width, height, batch));
@@ -985,15 +969,14 @@ KB200_API int kb200_rgb_from_bayer_u8(kb200_stream_t stream, const uint8_t* src,
 KB200_API int kb200_rgb_from_bayer_u16(kb200_stream_t stream, const uint16_t* src, size_t src_len, uint16_t* dst,
                                        size_t dst_len, uint32_t width, uint32_t height, uint32_t batch, int pattern) {
     KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
-    if (reinterpret_cast<uintptr_t>(src) & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "'src' is not 2-byte aligned (16-bit samples)");
-    if (reinterpret_cast<uintptr_t>(dst) & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "'dst' is not 2-byte aligned (16-bit samples)");
+    KB200_TRY(check_words("src", src)); KB200_TRY(check_words("dst", dst));
     return launch_rgb_from_bayer(BAYER_KERNELS_U16, stream, src, src_len, dst, dst_len, width, height, batch, pattern);
 }
 
 KB200_API int kb200_rgb_from_bayer_packed(kb200_stream_t stream, const uint8_t* src, size_t src_len, uint16_t* dst, size_t dst_len,
                                           uint32_t width, uint32_t height, uint32_t batch, int pattern, int bits) {
     KB200_TRY(check_ptr("src", src)); KB200_TRY(check_ptr("dst", dst));
-    if (reinterpret_cast<uintptr_t>(dst) & 1u) return fail(KB200_ERR_INVALID_ARGUMENT, "'dst' is not 2-byte aligned (16-bit samples)");
+    KB200_TRY(check_words("dst", dst));
     if (pattern < KB200_BAYER_RGGB || pattern > KB200_BAYER_GBRG) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown Bayer pattern %d", pattern);
     switch (bits) {
         case 10: return launch_rgb_from_bayer_packed<10>(BAYER_KERNELS_10P, stream, src, src_len, dst, dst_len, width, height, batch, pattern);
