@@ -27,6 +27,7 @@
 
 #include "kb200_common.cuh"
 #include "pair_math.cuh"
+#include "tma_ring.cuh"
 
 namespace kb200 {
 
@@ -152,7 +153,7 @@ __global__ void __launch_bounds__(256) sep_filter_fused_kernel(const float* __re
 // issue-bound, far below the HBM roofline.  Here:
 //   * work unit = (image, strip of 512*NV floats of a row, chunk of `rows_per_chunk` rows); a CTA walks its
 //     strip top-down.  Each input row segment (strip + 16-B-rounded halo) is copied global -> shared by
-//     the TMA engine (cp.async.bulk 1-D) into an mbarrier ring by a producer warp — every input row is
+//     the TMA engine (tma::load_1d) into an mbarrier ring by a producer warp — every input row is
 //     read once per chunk (+ K-1 halo rows per chunk), nothing is staged twice horizontally.
 //   * a consumer thread owns NV float4 columns of the strip (tid, tid+128, …; each lane-contiguous).  Per row it
 //     reads its outputs' horizontal support as NF4 aligned LDS.128, forms the horizontal results in registers,
@@ -170,33 +171,6 @@ struct SepStreamParams {
     uint32_t strips, chunks, rows_per_chunk, nunits;
     uint32_t slot_floats;  // floats per stage slot
 };
-
-__device__ __forceinline__ uint32_t ss_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void ss_mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(ss_smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void ss_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(ss_smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void ss_mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(ss_smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void ss_mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "SS_WAIT_LOOP:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra SS_WAIT_DONE;\n"
-        "bra SS_WAIT_LOOP;\n"
-        "SS_WAIT_DONE:\n"
-        "}\n" ::"r"(ss_smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void ss_tma_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(ss_smem_u32(smem_dst)),
-                 "l"(gmem_src), "r"(bytes), "r"(ss_smem_u32(bar))
-                 : "memory");
-}
 
 // Sobel taps are compile-time constants (filter/kernels.rs:55-72): D = derivative, S = smoothing.
 template <int K> struct SobelTaps;
@@ -300,8 +274,8 @@ __global__ void __launch_bounds__(SS2<NV>::THREADS) sep_filter_stream2_kernel(co
     const uint32_t tid = threadIdx.x;
     const uint32_t nst = R.stages;
     if (tid == 0) {
-        for (uint32_t s = 0; s < nst; ++s) { ss_mbar_init(&full_bar[s], 1); ss_mbar_init(&empty_bar[s], G::COLS4 / 32); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        for (uint32_t s = 0; s < nst; ++s) { tma::mbar_init(&full_bar[s], 1); tma::mbar_init(&empty_bar[s], G::COLS4 / 32); }
+        tma::mbar_fence_init();
     }
     __syncthreads();
     const size_t img_floats = (size_t)P.rowlen * P.rows;
@@ -321,14 +295,14 @@ __global__ void __launch_bounds__(SS2<NV>::THREADS) sep_filter_stream2_kernel(co
             const int y_first = (int)(chunk * P.rows_per_chunk), y_end = min(y_first + (int)P.rows_per_chunk, (int)P.rows);
             const float* base = src + (size_t)img * img_floats + g0;
             for (int iy = y_first - HY; iy < y_end + (KY - 1 - HY); ++iy) {
-                if (!first_lap) ss_mbar_wait(&empty_bar[stage], phase ^ 1u);
+                if (!first_lap) tma::mbar_wait(&empty_bar[stage], phase ^ 1u);
                 const bool valid = iy >= 0 && iy < (int)P.rows;
                 row_valid[stage] = valid ? 1 : 0;
                 if (valid) {
-                    ss_mbar_expect_tx(&full_bar[stage], bytes);
-                    ss_tma_load_1d(ss_smem + (size_t)stage * P.slot_floats + slot_off, base + (size_t)iy * P.rowlen, bytes, &full_bar[stage]);
+                    tma::mbar_expect_tx(&full_bar[stage], bytes);
+                    tma::load_1d(ss_smem + (size_t)stage * P.slot_floats + slot_off, base + (size_t)iy * P.rowlen, bytes, &full_bar[stage]);
                 } else {
-                    ss_mbar_arrive(&full_bar[stage]);
+                    tma::mbar_arrive(&full_bar[stage]);
                 }
                 if (++stage == nst) { stage = 0; phase ^= 1u; first_lap = false; }
             }
@@ -365,7 +339,7 @@ __global__ void __launch_bounds__(SS2<NV>::THREADS) sep_filter_stream2_kernel(co
 #pragma unroll
             for (int s = 0; s < KY; ++s) {   // unrolled: window slot indices are compile-time
                 if (iy >= iy_end) break;
-                ss_mbar_wait(&full_bar[stage], phase);
+                tma::mbar_wait(&full_bar[stage], phase);
                 const bool valid = row_valid[stage] != 0;
                 const float4* sp = reinterpret_cast<const float4*>(ss_smem + (size_t)stage * P.slot_floats) + tid;
 #pragma unroll
@@ -400,7 +374,7 @@ __global__ void __launch_bounds__(SS2<NV>::THREADS) sep_filter_stream2_kernel(co
                     if (SOBEL) { winB[s][v][0] = ss_pack(hB[0], hB[1]); winB[s][v][1] = ss_pack(hB[2], hB[3]); }
                 }
                 __syncwarp();
-                if (lane0) ss_mbar_arrive(&empty_bar[stage]);
+                if (lane0) tma::mbar_arrive(&empty_bar[stage]);
                 if (++stage == nst) { stage = 0; phase ^= 1u; }
                 // the row that just became complete: r = iy - (KY-1-HY); its window is slots s+1 … s+KY (mod KY), oldest first
                 if (iy - (KY - 1 - HY) >= y_first) {

@@ -232,7 +232,7 @@ __global__ void __launch_bounds__(256) blur_u8_tile_w_kernel(const uint8_t* __re
 // The tile kernel above pays two block-wide phase changes, a (64+K-1)^2 / 64^2 halo and a shared-memory round trip of the
 // intermediate per tile.  This is the u8 twin of sep_filter_stream2 (filter.cu): a unit is
 // (image, strip of 128*NV words of a row, chunk of rows); every source row span is copied ONCE global -> shared by the
-// TMA engine (cp.async.bulk, mbarrier ring, producer lane; rows clamped = the reference's replicate border in y); a
+// TMA engine (tma::load_1d, mbarrier ring, producer lane; rows clamped = the reference's replicate border in y); a
 // consumer thread owns NV word columns: the H pass reads the words around its column (compile-time funnel shifts per tap,
 // two 16-bit lanes per register as above), its result goes — split into even and odd bytes — into a K-deep rotating REGISTER
 // window, and as soon as the window is full the V pass emits one lane-contiguous STG.32 per column.  The u8 intermediate never

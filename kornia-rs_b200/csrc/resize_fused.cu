@@ -17,6 +17,7 @@
 
 #include "kb200_common.cuh"
 #include "resize_fused.cuh"
+#include "tma_ring.cuh"
 
 namespace kb200 {
 
@@ -233,7 +234,7 @@ KB200_API void kb200_resize_row_plan(uint32_t src_h, uint32_t dst_h, uint32_t* p
 //   * work unit = (image, column tile of TW destination columns, chunk of RC destination rows); CTAs are
 //     persistent and walk their units with carry arithmetic (no integer division in the loop).
 //   * per destination row, the source rows it taps are copied — only the byte span [x0(first col), x1(last col)]
-//     the column tile touches, rounded out to 16 B — global -> shared by the TMA engine (cp.async.bulk 1-D, SASS
+//     the column tile touches, rounded out to 16 B — global -> shared by the TMA engine (tma::load_1d, SASS
 //     UBLKCP), completion counted on an mbarrier (expect_tx).  Source rows with no (or a zero) weight are never
 //     addressed: 2 of every 3 at scale 3.
 //   * a short ring (3 stages), one destination row per stage, running continuously across units.  Warp 4 is the
@@ -259,35 +260,6 @@ struct FusedStagedParams {
     uint32_t dtx, dcy, dimg;
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_LOOP:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra WAIT_DONE;\n"
-        "bra WAIT_LOOP;\n"
-        "WAIT_DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-// 1-D bulk copy global -> shared::cta through the TMA engine; bytes % 16 == 0, both addresses 16-B aligned.
-__device__ __forceinline__ void tma_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_dst)),
-                 "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
-
 // half-pixel source coordinate of the fused path — resize/fused.rs:196-201 (unfused mul/add)
 __device__ __forceinline__ void fused_axis(uint32_t d, float scale, uint32_t src_len, uint32_t* i0, uint32_t* i1, float* w) {
     const float f = fmaxf(((float)d + 0.5f) * scale - 0.5f, 0.0f);
@@ -296,24 +268,6 @@ __device__ __forceinline__ void fused_axis(uint32_t d, float scale, uint32_t src
     *i1 = min(a + 1u, src_len - 1u);
     *w = f - (float)a;
 }
-
-// (tx, chunk, img) walk: advance by one CTA stride without dividing.
-struct UnitWalk {
-    uint32_t tx, cy, img;
-    __device__ __forceinline__ void init(uint32_t u, const FusedStagedParams& P) {
-        const uint32_t per_img = P.tiles_x * P.chunks_y;
-        img = u / per_img;
-        const uint32_t t = u - img * per_img;
-        cy = t / P.tiles_x;
-        tx = t - cy * P.tiles_x;
-    }
-    __device__ __forceinline__ void advance(const FusedStagedParams& P) {
-        tx += P.dtx; cy += P.dcy; img += P.dimg;
-        if (tx >= P.tiles_x) { tx -= P.tiles_x; ++cy; }
-        if (cy >= P.chunks_y) { cy -= P.chunks_y; ++img; }
-        if (cy >= P.chunks_y) { cy -= P.chunks_y; ++img; }
-    }
-};
 
 // Several destination columns per thread + per-launch specialisation.
 //
@@ -410,12 +364,12 @@ __global__ void __launch_bounds__(FR_THREADS) fused_rows_kernel(const uint8_t* _
     const size_t plane = (size_t)p.dw * p.dh;
 
     if (tid == 0) {
-        for (uint32_t s = 0; s < nst; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], FR_CT / 32); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        for (uint32_t s = 0; s < nst; ++s) { tma::mbar_init(&full_bar[s], 1); tma::mbar_init(&empty_bar[s], FR_CT / 32); }
+        tma::mbar_fence_init();
     }
     __syncthreads();
 
-    UnitWalk w;
+    tma::UnitWalk<FusedStagedParams> w;
     w.init(blockIdx.x, P);
     uint32_t stage = 0, phase = 0;  // ring position, running continuously across units
 
@@ -435,16 +389,16 @@ __global__ void __launch_bounds__(FR_THREADS) fused_rows_kernel(const uint8_t* _
             const uint8_t* frame = src + (size_t)w.img * frame_bytes + b0;
             const uint32_t y_first = w.cy * P.rows_per_chunk, y_end = min(y_first + P.rows_per_chunk, p.dh);
             for (uint32_t dy = y_first; dy < y_end; ++dy) {
-                if (!first_lap) mbar_wait(&empty_bar[stage], phase ^ 1u);  // consumers drained the previous tenant
+                if (!first_lap) tma::mbar_wait(&empty_bar[stage], phase ^ 1u);  // consumers drained the previous tenant
                 uint32_t y0, y1;
                 float wy;
                 fused_axis(dy, p.scale_y, p.sh, &y0, &y1, &wy);
                 uint8_t* sbase = smem_raw + (size_t)stage * R.stage_bytes;
                 const bool two = (MODE == FR_BOX) || ((MODE == FR_GENERAL) && (wy != 0.0f));  // a zero-weight y1 row is never fetched
                 if (MODE == FR_GENERAL) wy_s[stage] = wy;  // before the arrive(release): covered by the consumers' acquire on `full`
-                mbar_expect_tx(&full_bar[stage], two ? bytes * 2u : bytes);
-                tma_load_1d(sbase, frame + (size_t)fused_row_slot(p, y0) * P.row_bytes, bytes, &full_bar[stage]);
-                if (two) tma_load_1d(sbase + P.slot_bytes, frame + (size_t)fused_row_slot(p, y1) * P.row_bytes, bytes, &full_bar[stage]);
+                tma::mbar_expect_tx(&full_bar[stage], two ? bytes * 2u : bytes);
+                tma::load_1d(sbase, frame + (size_t)fused_row_slot(p, y0) * P.row_bytes, bytes, &full_bar[stage]);
+                if (two) tma::load_1d(sbase + P.slot_bytes, frame + (size_t)fused_row_slot(p, y1) * P.row_bytes, bytes, &full_bar[stage]);
                 if (++stage == nst) { stage = 0; phase ^= 1u; first_lap = false; }
             }
         }
@@ -483,7 +437,7 @@ __global__ void __launch_bounds__(FR_THREADS) fused_rows_kernel(const uint8_t* _
         T* out1 = out0 + plane;
         T* out2 = out1 + plane;
         for (uint32_t dy = y_first; dy < y_end; ++dy) {
-            mbar_wait(&full_bar[stage], phase);
+            tma::mbar_wait(&full_bar[stage], phase);
             const uint8_t* sbase = smem_raw + (size_t)stage * R.stage_bytes;
             const float wy = (MODE == FR_GENERAL) ? wy_s[stage] : 0.0f;
 #pragma unroll
@@ -494,7 +448,7 @@ __global__ void __launch_bounds__(FR_THREADS) fused_rows_kernel(const uint8_t* _
             }
             out0 += p.dw; out1 += p.dw; out2 += p.dw;
             __syncwarp();
-            if (lane0) mbar_arrive(&empty_bar[stage]);
+            if (lane0) tma::mbar_arrive(&empty_bar[stage]);
             if (++stage == nst) { stage = 0; phase ^= 1u; }
         }
     }
@@ -502,7 +456,7 @@ __global__ void __launch_bounds__(FR_THREADS) fused_rows_kernel(const uint8_t* _
 
 // Full-row point mode.  The tiled schedule above cuts every source row into ~2.4 KB spans (five CTAs per row at 4K, each
 // refetching its 16-B-rounded edges) and every plane row into 1 KB pieces, walked by a few persistent CTAs per SM.  Here
-// a CTA of 256 threads owns one (image, destination row) over the whole width: one `cp.async.bulk` copies the whole tapped
+// a CTA of 256 threads owns one (image, destination row) over the whole width: one `tma::load_1d` copies the whole tapped
 // source row into shared memory, then the CTA writes the three whole plane rows and exits.  With ~12 KB of shared memory,
 // 256 threads and <= 32 registers, 8 CTAs are resident per SM, so the hardware scheduler keeps many rows in flight in
 // different phases (copy / compute / store) without a ring.  On the headline (H100) this was 4-5 % faster than the tiled
@@ -530,17 +484,17 @@ __global__ void __launch_bounds__(FRR_CT) fused_point_rows_kernel(const uint8_t*
         uint32_t y0, y1;
         float wy;
         fused_axis(dy, p.scale_y, p.sh, &y0, &y1, &wy);  // point mode: wy == 0 on every row, y0 is the only tap
-        mbar_init(&bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        mbar_expect_tx(&bar, row_bytes);
-        tma_load_1d(row_s, src + ((size_t)img * p.src_rows + fused_row_slot(p, y0)) * row_bytes, row_bytes, &bar);
+        tma::mbar_init(&bar, 1);
+        tma::mbar_fence_init();
+        tma::mbar_expect_tx(&bar, row_bytes);
+        tma::load_1d(row_s, src + ((size_t)img * p.src_rows + fused_row_slot(p, y0)) * row_bytes, row_bytes, &bar);
     }
     __syncthreads();   // the mbarrier is initialised before anyone waits on it
     const float s0 = p.scale[0], s1 = p.scale[1], s2 = p.scale[2];
     const float o0 = p.bias[0], o1 = p.bias[1], o2 = p.bias[2];
     const size_t plane = (size_t)p.dw * p.dh;
     FrrVec<T>* out0 = reinterpret_cast<FrrVec<T>*>(dst + (size_t)img * plane * 3 + (size_t)dy * p.dw) + tid;
-    mbar_wait(&bar, 0);
+    tma::mbar_wait(&bar, 0);
 #pragma unroll
     for (int j = 0; j < NPX; ++j) {
         const uint32_t xb = (tid + (uint32_t)j * FRR_CT) * FRR_V;
@@ -698,10 +652,7 @@ int launch_fused_resize_rows(cudaStream_t s, const uint8_t* src, T* dst, const F
     R.stages = stages;
     R.stage_bytes = stage_bytes;
     const unsigned grid = (unsigned)std::min<size_t>(nunits, ctas);
-    P.dtx = grid % P.tiles_x;
-    const uint32_t g = grid / P.tiles_x;
-    P.dcy = g % P.chunks_y;
-    P.dimg = g / P.chunks_y;
+    tma::carry_strides(grid, P);
     const bool allfma = p.fma_bulk >= p.dw;
     cudaError_t e;
     if (mode == FR_POINT) e = fr_launch_npx<T, FR_POINT>(npx, allfma, grid, smem, s, src, dst, R);

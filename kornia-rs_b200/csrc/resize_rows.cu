@@ -7,7 +7,7 @@
 //   * work unit = (image, tile of TW = 128*NPX destination columns, chunk of destination rows); persistent CTAs walk
 //     their units with carry arithmetic.
 //   * per destination row the TWO source rows it taps (y0, y1) are copied — only the float span the column tile
-//     touches, rounded out to 16 B — global -> shared by the TMA engine (`cp.async.bulk`, SASS UBLKCP) into a short
+//     touches, rounded out to 16 B — global -> shared by the TMA engine (`tma::load_1d`, SASS UBLKCP) into a short
 //     mbarrier ring filled by a producer lane; every source byte is fetched once per column tile, in whole lines.
 //     Zero-weight taps ARE fetched (f32 sources may hold inf/NaN and 0*inf must stay NaN, unlike the u8 fused path).
 //   * 4 consumer warps; a thread owns NPX lane-contiguous destination columns for the whole unit: the x-side of the
@@ -51,23 +51,6 @@ __device__ __forceinline__ void rr_axis(uint32_t i, float a, float b, uint32_t l
     *f = s - (float)k;
 }
 
-struct RRWalk {
-    uint32_t tx, cy, img;
-    __device__ __forceinline__ void init(uint32_t u, const ResizeRowsParams& P) {
-        const uint32_t per_img = P.tiles_x * P.chunks_y;
-        img = u / per_img;
-        const uint32_t t = u - img * per_img;
-        cy = t / P.tiles_x;
-        tx = t - cy * P.tiles_x;
-    }
-    __device__ __forceinline__ void advance(const ResizeRowsParams& P) {
-        tx += P.dtx; cy += P.dcy; img += P.dimg;
-        if (tx >= P.tiles_x) { tx -= P.tiles_x; ++cy; }
-        if (cy >= P.chunks_y) { cy -= P.chunks_y; ++img; }
-        if (cy >= P.chunks_y) { cy -= P.chunks_y; ++img; }
-    }
-};
-
 // span of source floats a column tile taps: [b0, b1), 4-float aligned (row_floats % 4 == 0)
 __device__ __forceinline__ void rr_span(uint32_t dx0, uint32_t dx1, const ResizeRowsParams& P, uint32_t* b0, uint32_t* b1) {
     uint32_t xa, xb, t;
@@ -101,7 +84,7 @@ __global__ void __launch_bounds__(RR_THREADS) resize_rows_f32_kernel(const float
     }
     __syncthreads();
 
-    RRWalk w;
+    tma::UnitWalk<ResizeRowsParams> w;
     w.init(blockIdx.x, P);
     uint32_t stage = 0, phase = 0;
 
@@ -283,10 +266,7 @@ int launch_resize_rows_f32(int mode, cudaStream_t s, const float* src, float* ds
     if (nunits > 0x7FFFFFFFull) return KB200_OK;
     P.nunits = (uint32_t)nunits;
     const unsigned grid = (unsigned)std::min<size_t>(nunits, ctas);
-    P.dtx = grid % P.tiles_x;
-    const uint32_t g = grid / P.tiles_x;
-    P.dcy = g % P.chunks_y;
-    P.dimg = g / P.chunks_y;
+    tma::carry_strides(grid, P);
     cudaError_t e = npx == 1 ? rr_launch<1>(mode, grid, smem, s, src, dst, P) : (npx == 2 ? rr_launch<2>(mode, grid, smem, s, src, dst, P) : rr_launch<3>(mode, grid, smem, s, src, dst, P));
     if (e != cudaSuccess) return fail(KB200_ERR_CUDA, "cudaFuncSetAttribute failed: %s", cudaGetErrorString(e));
     KB200_TRY(check_launch("resize_rows_f32_kernel"));

@@ -7,7 +7,7 @@
 //   * work unit = (image, tile of TW = 128*NPX destination columns, chunk of destination rows); persistent CTAs.
 //   * the inverse map of a near-identity homography / small rotation sends a destination row segment to a thin BAND of
 //     source rows that slides down by about one row per destination row.  A producer warp walks that band: every source
-//     row span the tile needs is copied global -> shared exactly once by the TMA engine (`cp.async.bulk`, SASS UBLKCP)
+//     row span the tile needs is copied global -> shared exactly once by the TMA engine (`tma::load_1d`, SASS UBLKCP)
 //     into a ring of NSLOT row slots (slot = load sequence number mod NSLOT), completion counted on the slot's `full`
 //     mbarrier; consumers release a slot (`empty` mbarrier) when the band has moved past its row.  Bytes in flight per SM
 //     are set by the ring, not by the thread count, and every DRAM access is a whole-line bulk copy.
@@ -51,7 +51,7 @@ __global__ void __launch_bounds__(WS_THREADS) warp_stream_kernel(const float* __
     }
     __syncthreads();
 
-    WSWalk w;
+    tma::UnitWalk<WarpStreamParams> w;
     w.init(blockIdx.x, P);
     // Load sequence numbers: the q-th row this CTA loads lives in slot q & smask, phase (q / nslot) & 1.  Within a unit,
     // source row r has q = qbase + (r - r0) with r0 the unit's first resident row; qbase continues across units.
@@ -200,10 +200,7 @@ static int ws_launch(cudaStream_t s, const float* src, float* dst, WarpStreamPar
     if (nunits > 0x7FFFFFFFull) return KB200_OK;
     P.nunits = (uint32_t)nunits;
     const unsigned grid = (unsigned)std::min<size_t>(nunits, ctas);
-    P.dtx = grid % P.tiles_x;
-    const uint32_t g = grid / P.tiles_x;
-    P.dcy = g % P.chunks_y;
-    P.dimg = g / P.chunks_y;
+    tma::carry_strides(grid, P);
     kern<<<grid, WS_THREADS, smem, s>>>(src, dst, P);
     KB200_TRY(check_launch("warp_stream_kernel"));
     *handled = true;

@@ -24,23 +24,6 @@ struct WarpStreamParams {
     uint32_t dtx, dcy, dimg;
 };
 
-struct WSWalk {
-    uint32_t tx, cy, img;
-    __device__ __forceinline__ void init(uint32_t u, const WarpStreamParams& P) {
-        const uint32_t per_img = P.tiles_x * P.chunks_y;
-        img = u / per_img;
-        const uint32_t t = u - img * per_img;
-        cy = t / P.tiles_x;
-        tx = t - cy * P.tiles_x;
-    }
-    __device__ __forceinline__ void advance(const WarpStreamParams& P) {
-        tx += P.dtx; cy += P.dcy; img += P.dimg;
-        if (tx >= P.tiles_x) { tx -= P.tiles_x; ++cy; }
-        if (cy >= P.chunks_y) { cy -= P.chunks_y; ++img; }
-        if (cy >= P.chunks_y) { cy -= P.chunks_y; ++img; }
-    }
-};
-
 // approximate inverse map (schedule / span planning only — results never depend on it)
 template <bool PERSPECTIVE>
 __device__ __forceinline__ bool ws_plan_coord(const float* __restrict__ m, float x, float y, float* sx, float* sy) {
@@ -145,7 +128,7 @@ __device__ __forceinline__ void ws_producer(const float* __restrict__ src, const
     const int nslot = (int)P.nslot;
     const uint32_t smask = P.nslot - 1u;
     const size_t src_img = (size_t)P.row_floats * P.sh;
-    WSWalk w;
+    tma::UnitWalk<WarpStreamParams> w;
     w.init(blockIdx.x, P);
     uint32_t qbase = 0;
     for (uint32_t u = blockIdx.x; u < P.nunits; u += gridDim.x, w.advance(P)) {

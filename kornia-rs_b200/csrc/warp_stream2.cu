@@ -97,7 +97,7 @@ __global__ void __launch_bounds__(WS_THREADS) warp_stream2_kernel(const float* _
     const float fsw = (float)P.sw, fsh = (float)P.sh;
     const uint32_t ring_u32 = tma::smem_u32(ring);
     const uint32_t slot_bytes = P.slot_floats * 4u;
-    WSWalk w;
+    tma::UnitWalk<WarpStreamParams> w;
     w.init(blockIdx.x, P);
     uint32_t qbase = 0, obuf = 0;
     for (uint32_t u = blockIdx.x; u < P.nunits; u += gridDim.x, w.advance(P)) {
@@ -300,10 +300,7 @@ int ws2_launch(cudaStream_t s, const float* src, float* dst, WarpStreamParams& P
     if (nunits > 0x7FFFFFFFull) return KB200_OK;
     P.nunits = (uint32_t)nunits;
     const unsigned grid = (unsigned)std::min<size_t>(nunits, ctas);
-    P.dtx = grid % P.tiles_x;
-    const uint32_t g = grid / P.tiles_x;
-    P.dcy = g % P.chunks_y;
-    P.dimg = g / P.chunks_y;
+    tma::carry_strides(grid, P);
     WarpStream2Args A;
     A.p = P; A.neg_zero = -0.0f; A.one = 1.0f;
     kern<<<grid, WS_THREADS, smem, s>>>(src, dst, A);
