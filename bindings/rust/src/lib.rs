@@ -48,6 +48,19 @@ pub mod ffi {
 
     const _: () = assert!(std::mem::size_of::<kb200_preprocess_desc>() == 80);
 
+    /// include/kornia_b200.h `kb200_roi` — region (x, y, w, h) of frame `frame`, 20 bytes, C layout.
+    #[repr(C)]
+    #[derive(Clone, Copy, Debug, Default)]
+    pub struct kb200_roi {
+        pub frame: i32,
+        pub x: i32,
+        pub y: i32,
+        pub w: i32,
+        pub h: i32,
+    }
+
+    const _: () = assert!(std::mem::size_of::<kb200_roi>() == 20);
+
     extern "C" {
         pub fn kb200_version() -> c_int;
         pub fn kb200_last_kernel() -> *const c_char;
@@ -158,6 +171,7 @@ pub mod ffi {
         pub fn kb200_preprocess_strided_f16(stream: *mut c_void, desc: *const kb200_preprocess_desc, base: *const u8, base_len: usize, frame_stride: usize, batch: u32, dst: *mut u16, dst_len: usize) -> c_int;
         pub fn kb200_preprocess_bf16(stream: *mut c_void, desc: *const kb200_preprocess_desc, frames: *const *const u8, frame_len: *const usize, batch: u32, dst: *mut u16, dst_len: usize) -> c_int;
         pub fn kb200_preprocess_strided_bf16(stream: *mut c_void, desc: *const kb200_preprocess_desc, base: *const u8, base_len: usize, frame_stride: usize, batch: u32, dst: *mut u16, dst_len: usize) -> c_int;
+        pub fn kb200_preprocess_rois(stream: *mut c_void, desc: *const kb200_preprocess_desc, mode: c_int, frames: *const *const u8, frame_len: *const usize, n_frames: u32, rois: *const kb200_roi, n_rois: u32, dst: *mut c_void, dst_len: usize, out_format: c_int) -> c_int;
         pub fn kb200_selftest_div255(stream: *mut c_void, mismatches_dev: *mut u64) -> c_int;
         pub fn kb200_selftest_div2(stream: *mut c_void, count: u64, seed: u32, mismatches_dev: *mut u64) -> c_int;
 
@@ -472,6 +486,29 @@ pub fn launch_preprocess_batch_f32(
     let (dp, _g1) = dst.device_ptr_mut(stream);
     check(unsafe {
         ffi::kb200_preprocess_f32(stream.cu_stream() as *mut c_void, desc, ptrs.as_ptr(), lens.as_ptr(), frames.len() as u32, dp as *mut f32, dst_len)
+    })
+}
+
+/// Crop-and-resize `rois` of `frames` into `dst` ([rois.len(), 3, dst_h, dst_w] f32) with `mode` (0 Letterbox, 1 Stretch):
+/// one launch per 80 regions.  Replaces a caller's loop of one `launch_view` per crop (an extension beyond the reference).
+pub fn launch_preprocess_rois(
+    stream: &Arc<CudaStream>, desc: &ffi::kb200_preprocess_desc, mode: i32, frames: &[&CudaSlice<u8>], rois: &[ffi::kb200_roi],
+    dst: &mut CudaSlice<f32>,
+) -> Result<(), Kb200Error> {
+    bind(stream.context())?;
+    let mut guards = Vec::with_capacity(frames.len());
+    let mut ptrs: Vec<*const u8> = Vec::with_capacity(frames.len());
+    let lens: Vec<usize> = frames.iter().map(|f| f.len()).collect();
+    for f in frames {
+        let (p, g) = f.device_ptr(stream);
+        ptrs.push(p as *const u8);
+        guards.push(g);
+    }
+    let dst_len = dst.len();
+    let (dp, _g1) = dst.device_ptr_mut(stream);
+    check(unsafe {
+        ffi::kb200_preprocess_rois(stream.cu_stream() as *mut c_void, desc, mode, ptrs.as_ptr(), lens.as_ptr(), frames.len() as u32, rois.as_ptr(),
+                                   rois.len() as u32, dp as *mut c_void, dst_len, 0)
     })
 }
 

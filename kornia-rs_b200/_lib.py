@@ -29,6 +29,11 @@ class PreprocessDesc(C.Structure):
     ]
 
 
+class Roi(C.Structure):
+    """kb200_roi: region (x, y, w, h) of frame `frame`"""
+    _fields_ = [("frame", C.c_int32), ("x", C.c_int32), ("y", C.c_int32), ("w", C.c_int32), ("h", C.c_int32)]
+
+
 _lib = None
 _tls = threading.local()
 
@@ -123,6 +128,7 @@ def _declare(l: C.CDLL) -> None:
         "kb200_preprocess_bf16": ([vp, C.POINTER(PreprocessDesc), C.POINTER(vp), C.POINTER(sz), u32, vp, sz], i),
         "kb200_preprocess_strided_bf16": ([vp, C.POINTER(PreprocessDesc), vp, sz, sz, u32, vp, sz], i),
         "kb200_preprocess_host_format": ([vp, vp, C.POINTER(PreprocessDesc), vp, sz, sz, u32, vp, sz, i], i),
+        "kb200_preprocess_rois": ([vp, C.POINTER(PreprocessDesc), i, C.POINTER(vp), C.POINTER(sz), u32, C.POINTER(Roi), u32, vp, sz, i], i),
     }
     for name, (args, res) in sig.items():
         fn = getattr(l, name)  # AttributeError if the symbol is missing: fail loudly

@@ -1,0 +1,252 @@
+// preprocess.cuh — what the camera preprocess's two sources share: preprocess.cu (one affine per frame, the batch entries)
+// and preprocess_roi.cu (one affine per region of a frame, kb200_preprocess_rois): the source-format facts, the taps
+// (fetch_px), the Lanczos weight, the normalising divisions, the stores, the fast resampler's arguments, the host rules of
+// the descriptor and the kernel-selection switches.  The arithmetic is documented in preprocess.cu's header.
+#pragma once
+
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
+#include <type_traits>
+
+#include "bayer.cuh"
+#include "kb200_common.cuh"
+#include "yuv.cuh"
+
+namespace kb200 {
+
+struct PreFrames {
+    const uint8_t* base;  // strided mode
+    size_t stride;
+    const uint8_t* ptr[256];  // pointer-table mode
+};
+
+// preprocess.rs:461-484 — manual RNE f32 -> binary16 (kept bit-identical, including its rule that
+// any exp >= 31 input with a nonzero mantissa gets the quiet bit).
+__device__ __forceinline__ unsigned short f2h_ref(float f) {
+    const unsigned int x = __float_as_uint(f);
+    const unsigned int sign = (x >> 16) & 0x8000u;
+    const int exp = (int)((x >> 23) & 0xFFu) - 127 + 15;
+    unsigned int man = x & 0x7FFFFFu;
+    if (exp >= 31) {
+        const unsigned int nan_bit = (man != 0u) ? 0x0200u : 0u;
+        return (unsigned short)(sign | 0x7C00u | nan_bit);
+    }
+    if (exp <= 0) {
+        if (exp < -10) return (unsigned short)sign;
+        man |= 0x800000u;
+        const unsigned int shift = (unsigned int)(14 - exp);
+        unsigned short h = (unsigned short)(sign | (man >> shift));
+        const unsigned int rem = man & ((1u << shift) - 1u);
+        const unsigned int mid = 1u << (shift - 1u);
+        if (rem > mid || (rem == mid && (h & 1u))) h++;
+        return h;
+    }
+    unsigned short h = (unsigned short)(sign | ((unsigned int)exp << 10) | (man >> 13));
+    const unsigned int rem = man & 0x1FFFu;
+    if (rem > 0x1000u || (rem == 0x1000u && (h & 1u))) h++;
+    return h;
+}
+
+// `p / 255.0f`, exactly: q = p*c; e = fma(-q, 255, p); q' = fma(e, c, q) with c = RN(1/255) (Markstein's correction).
+// Verified bit-identical to the IEEE division for EVERY float in [0, 256) by kb200_selftest_div255 (1.13e9 inputs,
+// tests/test_gpu_parity.py::test_div255_identity_exhaustive); every px here is a decoded or interpolated value in [0, 255].
+__device__ __forceinline__ float div255_exact(float p) {
+    const float c = 0.00392156885936856269836f;  // 0x3b808081
+    const float q = p * c;
+    const float e = fmaf(-q, 255.0f, p);
+    return fmaf(e, c, q);
+}
+
+// The facts of one source format code (kb200_src_fmt without the matrix bits), from SRC_FORMATS below.  Every host
+// function reads them from here; the generic kernel takes its format's as an argument.
+enum SrcFamily { SRC_NONE, SRC_RGB, SRC_GRAY, SRC_YUV420, SRC_YUV422, SRC_BAYER, SRC_YUV444 };
+struct SrcFormat {
+    int code = -1;
+    const char* name = nullptr;   // the SourceFormat name in messages; nullptr: the code is not a format
+    SrcFamily family = SRC_NONE;
+    int layout = 0;    // SRC_RGB: 0 RGB, 1 BGR order; SRC_YUV420: kb200_yuv420_layout (P01x NV12's, I01x I420's); SRC_YUV422: kb200_yuv422_layout;
+                       // SRC_YUV444: kb200_yuv444_u16_layout (I41x's code position; 0 for I444)
+    int pattern = 0;   // SRC_BAYER: kb200_bayer_pattern
+    int bits = 8;      // bits per sample
+    bool words = false;    // one little-endian 16-bit word per sample
+    bool packed = false;   // MIPI CSI-2 packed samples (bits / 8 bytes each)
+    const char* identity_kernel = nullptr;   // kb200_last_kernel() names of the format's fast kernels, nullptr: none
+    const char* fast_kernel = nullptr;
+    __host__ __device__ float white() const { return (float)((1u << bits) - 1u); }   // the white level W = 2^bits - 1
+};
+
+// p / W of a 16-bit YUV tap, bit for bit the IEEE quotient __fdiv_rn(p, W) (W = 1023 or 4095), but the division never sees
+// a zero dividend: 0 / W is p itself (+0 or -0, since W > 0), so a zero p is returned as it is and 1 is divided in its
+// place.  A zero operand fails the fast-path check (FCHK) of __fdiv_rn and enters its slow-path subroutine, and decoded
+// video is full of codes clamped to 0 (blacks, out-of-gamut chroma), so without this most warps took the subroutine on
+// some lane.
+__device__ __forceinline__ float div_white(float p, float w) {
+    const bool zero = p == 0.0f;
+    const float q = __fdiv_rn(zero ? 1.0f : p, w);
+    return zero ? p : q;
+}
+
+// The taps an instantiation of the generic kernel reads: interleaved RGB / BGR or gray bytes, 4:2:2, the 16-bit words of
+// P01x / I01x, a Bayer mosaic of bytes, 16-bit words or packed samples, 8-bit 4:2:0 in one layout (TAP_YUV420 +
+// kb200_yuv420_layout), 8-bit 4:4:4 (TAP_YUV444, the same tap in the YUV444 layout) or the 16-bit words of I41x
+// (TAP_YUV444_16).  Within a kind the format's layout is a uniform branch.  The 4:2:0 layouts get an instantiation
+// each: with the four taps in one kernel, its Lanczos loop no longer unrolls and spills; for the same reason 4:4:4 is not
+// a branch of TAP_YUV16.  TapCoeffs: the coefficient argument, the Q16 set with its code extraction for the 16-bit words
+// (as in the fast kernels), the Q20 set otherwise.
+static constexpr int TAP_RGB = 0, TAP_YUV422 = 1, TAP_YUV16 = 2, TAP_BAYER = 3, TAP_BAYER16 = 4, TAP_BAYER_PACKED = 5, TAP_YUV420 = 6;
+static constexpr int TAP_YUV444 = TAP_YUV420 + YUV444, TAP_YUV444_16 = TAP_YUV444 + 1;
+template <int TAP> constexpr bool tap_words = TAP == TAP_YUV16 || TAP == TAP_YUV444_16;   // YUV taps of 16-bit words
+template <int TAP> using TapCoeffs = std::conditional_t<tap_words<TAP>, Yuv16Coeffs, YuvCoeffs>;
+
+template <int TAP>
+__device__ __forceinline__ void fetch_px(const uint8_t* __restrict__ src, int x, int y, const kb200_preprocess_desc& d, const SrcFormat& f,
+                                         const TapCoeffs<TAP>& yc, float px[3]) {  // :510-530
+    if constexpr (TAP == TAP_RGB) {
+        if (f.family == SRC_GRAY) {
+            const float v = (float)src[(long long)y * d.src_pitch + x];
+            px[0] = v; px[1] = v; px[2] = v;
+            return;
+        }
+        const uint8_t* p = src + (long long)y * d.src_pitch + x * d.src_bpp;
+        if (f.layout == 0) { px[0] = (float)p[0]; px[1] = (float)p[1]; px[2] = (float)p[2]; }
+        else { px[0] = (float)p[2]; px[1] = (float)p[1]; px[2] = (float)p[0]; }
+        return;
+    }
+    int rgb[3];
+    if constexpr (TAP == TAP_BAYER || TAP == TAP_BAYER16) {   // src_pitch is in bytes (even for 16-bit samples)
+        using T = std::conditional_t<TAP == TAP_BAYER16, uint16_t, uint8_t>;
+        bayer_px(reinterpret_cast<const T*>(src), (size_t)d.src_pitch / sizeof(T), d.src_w, d.src_h, x, y, f.pattern, rgb);
+    } else if constexpr (TAP == TAP_BAYER_PACKED) {
+        bayer_px_packed(src, (size_t)d.src_pitch, d.src_w, d.src_h, x, y, f.pattern, f.bits, rgb);
+    } else if constexpr (TAP == TAP_YUV16) {
+        if (f.layout == YUV420_I420) yuv_tap<YUV420_I420>(src, x, y, d.src_w, d.src_h, yc, rgb);
+        else yuv_tap<YUV420_NV12>(src, x, y, d.src_w, d.src_h, yc, rgb);
+    } else if constexpr (TAP == TAP_YUV444_16) {
+        yuv_tap<YUV444>(src, x, y, d.src_w, d.src_h, yc, rgb);
+    } else if constexpr (TAP >= TAP_YUV420) {
+        yuv_tap<TAP - TAP_YUV420, false>(src, x, y, d.src_w, d.src_h, yc, rgb);
+    } else {
+        switch (f.layout) {
+            case YUV422_YUYV: yuv422_tap<YUV422_YUYV>(src, x, y, d.src_pitch, yc, rgb); break;
+            case YUV422_UYVY: yuv422_tap<YUV422_UYVY>(src, x, y, d.src_pitch, yc, rgb); break;
+            default: yuv422_tap<YUV422_YVYU>(src, x, y, d.src_pitch, yc, rgb); break;
+        }
+    }
+    px[0] = (float)rgb[0]; px[1] = (float)rgb[1]; px[2] = (float)rgb[2];
+}
+
+// preprocess.rs:481-488 (kernel source): 1-D Lanczos-3 weight — the CUDA math library's sinf, like the reference kernel
+__device__ __forceinline__ float pre_lanczos_w(float dd) {
+    const float ad = fabsf(dd);
+    if (ad < 1e-6f) return 1.0f;
+    if (ad >= 3.0f) return 0.0f;
+    const float pd = 3.14159265358979f * dd;
+    return __fdiv_rn(3.0f * sinf(pd) * sinf(__fdiv_rn(pd, 3.0f)), pd * pd);
+}
+
+// OUT: the kb200_out_format of dst.  A bfloat16 value is the f32 one rounded to nearest even (__floats2bfloat162_rn, two
+// values per conversion), stored like binary16 as one 8-byte word.
+template <int OUT>
+__device__ __forceinline__ void nv12_store4(void* __restrict__ dst, size_t idx, const float v[4]) {
+    if constexpr (OUT == KB200_OUT_BF16) {
+        const __nv_bfloat162 lo = __floats2bfloat162_rn(v[0], v[1]), hi = __floats2bfloat162_rn(v[2], v[3]);
+        uint2 w;
+        memcpy(&w.x, &lo, 4); memcpy(&w.y, &hi, 4);
+        *reinterpret_cast<uint2*>(reinterpret_cast<unsigned short*>(dst) + idx) = w;
+    } else if constexpr (OUT == KB200_OUT_F16) {
+        unsigned short hbits[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            // hardware RNE == the reference's manual RNE for every finite value below the f16 overflow threshold;
+            // beyond it (and for NaN) defer to the reference's own bit rules
+            hbits[i] = (fabsf(v[i]) < 65504.0f) ? __half_as_ushort(__float2half_rn(v[i])) : f2h_ref(v[i]);
+        }
+        uint2 w;
+        w.x = hbits[0] | ((uint32_t)hbits[1] << 16); w.y = hbits[2] | ((uint32_t)hbits[3] << 16);
+        *reinterpret_cast<uint2*>(reinterpret_cast<unsigned short*>(dst) + idx) = w;
+    } else {
+        stg_stream_f4(reinterpret_cast<float4*>(reinterpret_cast<float*>(dst) + idx), make_float4(v[0], v[1], v[2], v[3]));
+    }
+}
+
+__device__ __forceinline__ float norm_int_px(int r, float m, float is) { return (div255_exact((float)r) - m) * is; }
+
+struct Nv12Args {
+    float pad_norm[3];  // ((pad_value / 255) - mean) * inv_std, evaluated on the host in f32
+    uint32_t groups;    // ceil(dst_w / 4)
+};
+
+static constexpr int NV12_ROWS = 8;  // destination rows per thread: the x-side of the sampler is computed once for all of them
+
+// ── host side ───────────────────────────────────────────────────────────────────────────────────────────────────────────
+// The rules of the descriptor, in preprocess.cu.
+SrcFormat src_format(int fmt);   // the facts of a plain format code; name == nullptr: not a format
+kb200_preprocess_desc plain_desc(const kb200_preprocess_desc& d);   // the format code without its YUV matrix bits
+int yuv_matrix(const kb200_preprocess_desc& raw);
+size_t src_bytes(const kb200_preprocess_desc& d);    // d: a plain descriptor
+int validate_desc(const kb200_preprocess_desc* dp);  // the raw descriptor an entry was given
+
+// The Q16 coefficient set of a format of 16-bit YUV words (P01x, I01x, I41x) decoded with `matrix`.
+inline Yuv16Coeffs yuv16_coeffs_of(const SrcFormat& f, int matrix) {
+    const bool msb = f.family == SRC_YUV444 ? f.layout == KB200_YUV444_I41X_MSB : f.layout == YUV420_NV12;   // P01x, I41xMsb
+    return yuv16_coeffs(matrix, f.bits, msb);
+}
+
+// The fast resampler's arguments: the normalised pad value (BODY :610-612 on the host, f32, unfused) and the 4-column groups of a row.
+inline Nv12Args nv12_args(const kb200_preprocess_desc& d) {
+    Nv12Args nv{};
+    nv.groups = (uint32_t)(d.dst_w + 3) / 4u;
+    for (int c = 0; c < 3; ++c) nv.pad_norm[c] = (d.pad_value / 255.0f - d.mean[c]) * d.inv_std[c];
+    return nv;
+}
+
+template <int V> using IntC = std::integral_constant<int, V>;
+
+// Calls launch(IntC<TAP>{}, coeffs) with the generic kernels' tap kind for format f and that tap's coefficient set.
+template <class Launch>
+void with_tap(const SrcFormat& f, const YuvCoeffs& yc, const Yuv16Coeffs& yc16, Launch&& launch) {
+    if (f.family == SRC_BAYER) {
+        if (f.packed) launch(IntC<TAP_BAYER_PACKED>{}, yc);
+        else if (f.words) launch(IntC<TAP_BAYER16>{}, yc);
+        else launch(IntC<TAP_BAYER>{}, yc);
+    } else if (f.family == SRC_YUV444) {
+        if (f.words) launch(IntC<TAP_YUV444_16>{}, yc16);
+        else launch(IntC<TAP_YUV444>{}, yc);
+    } else if (f.words) {
+        launch(IntC<TAP_YUV16>{}, yc16);
+    } else if (f.family == SRC_YUV420) {
+        switch (f.layout) {
+            case YUV420_NV12: launch(IntC<TAP_YUV420 + YUV420_NV12>{}, yc); break;
+            case YUV420_NV21: launch(IntC<TAP_YUV420 + YUV420_NV21>{}, yc); break;
+            case YUV420_I420: launch(IntC<TAP_YUV420 + YUV420_I420>{}, yc); break;
+            default: launch(IntC<TAP_YUV420 + YUV420_YV12>{}, yc); break;
+        }
+    } else if (f.family == SRC_YUV422) {
+        launch(IntC<TAP_YUV422>{}, yc);
+    } else {
+        launch(IntC<TAP_RGB>{}, yc);
+    }
+}
+
+// Calls launch(IntC<L>{}, T{}, coeffs) with the fast kernels' layout L (4:2:0, or YUV444) and sample type T for a format
+// that has fast kernels (SrcFormat::fast_kernel), and their coefficient set.
+template <class Launch>
+void with_yuv_layout(const SrcFormat& f, const YuvCoeffs& yc, const Yuv16Coeffs& yc16, Launch&& launch) {
+    if (f.family == SRC_YUV444) {
+        if (f.words) launch(IntC<YUV444>{}, uint16_t{}, yc16);
+        else launch(IntC<YUV444>{}, uint8_t{}, yc);
+    } else if (f.words) {
+        if (f.layout == YUV420_I420) launch(IntC<YUV420_I420>{}, uint16_t{}, yc16);
+        else launch(IntC<YUV420_NV12>{}, uint16_t{}, yc16);
+    } else {
+        switch (f.layout) {
+            case YUV420_NV12: launch(IntC<YUV420_NV12>{}, uint8_t{}, yc); break;
+            case YUV420_NV21: launch(IntC<YUV420_NV21>{}, uint8_t{}, yc); break;
+            case YUV420_I420: launch(IntC<YUV420_I420>{}, uint8_t{}, yc); break;
+            default: launch(IntC<YUV420_YV12>{}, uint8_t{}, yc); break;
+        }
+    }
+}
+
+}  // namespace kb200

@@ -575,3 +575,57 @@ class Preprocessor:
         if st != _lib.OK:
             kind = {_lib.ERR_INVALID_SOURCE: "InvalidRawSource"}.get(st, "Cuda")
             raise PreprocessError(kind, _lib.last_error())
+
+    # ── regions of interest ─────────────────────────────────────────────────
+    def run_rois(self, frames: Sequence[torch.Tensor], src_w: int, src_h: int, rois, dst: torch.Tensor) -> None:
+        """Crop-and-resize regions of raw device frames in the builder's SourceFormat: region i = (frame, x, y, w, h), the
+        rectangle (x, y, w, h) of frames[frame], is resampled into dst[i] with the builder's mode (its affine is the one a
+        w x h frame gets), sampling, normalisation, pad value and YUV matrix; taps are clamped to the region and decode at
+        frame coordinates.  `rois`: a sequence of (frame, x, y, w, h), or an integer CPU tensor [M, 5].  `dst`: a contiguous
+        device [M, 3, H, W] tensor of torch.float32, torch.float16 or torch.bfloat16, which selects the output.  One launch per
+        80 regions.  A region outside its frame (or naming a frame that is not there) raises PreprocessError("InvalidRoi")."""
+        if isinstance(rois, torch.Tensor):
+            if rois.is_cuda or rois.dim() != 2 or rois.shape[1] != 5 or rois.dtype.is_floating_point or rois.dtype.is_complex or rois.dtype == torch.bool:
+                raise PreprocessError("InvalidRoi", f"rois must be an integer CPU tensor [M, 5], got {rois.dtype} {list(rois.shape)} on {rois.device}")
+            table = [tuple(int(v) for v in r) for r in rois.tolist()]
+        else:
+            table = [tuple(r) for r in rois]
+            if any(len(r) != 5 or not all(isinstance(v, int) or (isinstance(v, torch.Tensor) and v.dim() == 0) for v in r) for r in table):
+                raise PreprocessError("InvalidRoi", "each region must be (frame, x, y, w, h) of integers")
+            table = [tuple(int(v) for v in r) for r in table]
+        lim = 2 ** 31
+        if not table:
+            raise PreprocessError("InvalidRoi", "no regions given")
+        if any(not -lim <= v < lim for r in table for v in r):
+            raise PreprocessError("InvalidRoi", "region values must fit in 32-bit signed integers")
+        for i, (k, x, y, w, h) in enumerate(table):   # the C entry's region rules, checked here so that the kind is InvalidRoi
+            if not 0 <= k < len(frames):
+                raise PreprocessError("InvalidRoi", f"region {i}: frame index {k} is outside [0, {len(frames)})", region=i)
+            if x < 0 or y < 0:
+                raise PreprocessError("InvalidRoi", f"region {i}: origin ({x}, {y}) is negative", region=i)
+            if w < 1 or h < 1:
+                raise PreprocessError("InvalidRoi", f"region {i}: size {w}x{h} is empty", region=i)
+            if x + w > src_w or y + h > src_h:
+                raise PreprocessError("InvalidRoi", f"region {i}: ({x}, {y}) + {w}x{h} reaches outside the {src_w}x{src_h} frame", region=i)
+        if dst.dtype not in _OUT_DTYPES:
+            raise PreprocessError("BadOutputShape", f"unsupported output dtype {dst.dtype} (expected torch.float32, torch.float16 or torch.bfloat16)")
+        out = _OUT_DTYPES.index(dst.dtype)
+        self._validate_dst(dst, len(table), out)
+        for f in frames:
+            self._validate_raw(f.numel() * f.element_size(), src_w, src_h)
+            if not f.is_cuda:
+                raise PreprocessError("NotDeviceImage", "CUDA preprocessor requires a device-resident source image")
+            if f.device != dst.device:
+                raise PreprocessError("Cuda", "CUDA error: source and destination are on different CUDA devices")
+        fmt = self._fmt
+        desc = self._desc(src_w, src_h, fmt.pitch(src_w), fmt.bpp(), fmt.fmt_code(), dst.shape[3], dst.shape[2])
+        n, m = len(frames), len(table)
+        ptrs = (C.c_void_p * max(n, 1))(*[f.data_ptr() for f in frames])
+        lens = (C.c_size_t * max(n, 1))(*[f.numel() * f.element_size() for f in frames])
+        regions = (_lib.Roi * m)(*[_lib.Roi(*r) for r in table])
+        _lib.set_device(dst.device.index)
+        st = _lib.lib().kb200_preprocess_rois(torch.cuda.current_stream(dst.device).cuda_stream, C.byref(desc), self._mode.value, ptrs, lens, n,
+                                              regions, m, dst.data_ptr(), dst.numel(), out)
+        if st != _lib.OK:
+            kind = {_lib.ERR_INVALID_SOURCE: "InvalidRawSource", _lib.ERR_DIMS_TOO_LARGE: "DimensionsTooLarge"}.get(st, "Cuda")
+            raise PreprocessError(kind, ("CUDA error: " if kind == "Cuda" else "") + _lib.last_error())
