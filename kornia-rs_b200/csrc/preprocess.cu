@@ -33,8 +33,7 @@
 
 namespace kb200 {
 
-// SAMP: kb200_interp — 0 nearest, 1 bilinear, 3 Lanczos-3 (6x6 taps, clamp-to-edge, weights renormalised by their sum).
-// preprocess_roi.cu restates this body (generic_pixel) with a region's geometry: a change to a sampling rule goes there too.
+// One thread per output pixel of frame frame0 + blockIdx.y; SAMP: kb200_interp (generic_pixel).
 template <int OUT, int SAMP, bool PTRS, int TAP>
 __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                  const __grid_constant__ PreFrames fr, void* __restrict__ dst,
@@ -45,84 +44,9 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
     const uint32_t f = blockIdx.y;
     const uint8_t* src = PTRS ? fr.ptr[f] : fr.base + (size_t)(frame0 + f) * fr.stride;
     const int ox = i % d.dst_w, oy = i / d.dst_w;
-    const float sx = __fdiv_rn((float)ox - d.pad_x, d.scale_x);
-    const float sy = __fdiv_rn((float)oy - d.pad_y, d.scale_y);
-    const bool inside = !(sx < 0.0f || sy < 0.0f || sx >= (float)d.src_w || sy >= (float)d.src_h);
-    float px[3];
-    if (inside) {
-        if (SAMP == KB200_INTERP_LANCZOS) {   // preprocess.rs:565-590 sample_lanczos: acc += w * t (unfused), one division per channel
-            const int x0 = (int)floorf(sx), y0 = (int)floorf(sy);
-            float acc0 = 0.0f, acc1 = 0.0f, acc2 = 0.0f, wsum = 0.0f;
-            for (int j = -2; j <= 3; ++j) {
-                const int yj = y0 + j;
-                const float wy = pre_lanczos_w(sy - (float)yj);
-                const int ycl = min(max(yj, 0), d.src_h - 1);
-                for (int ii = -2; ii <= 3; ++ii) {
-                    const int xi = x0 + ii;
-                    const float w = wy * pre_lanczos_w(sx - (float)xi);
-                    const int xc = min(max(xi, 0), d.src_w - 1);
-                    float t[3];
-                    fetch_px<TAP>(src, xc, ycl, d, sf, yc, t);
-                    acc0 += w * t[0]; acc1 += w * t[1]; acc2 += w * t[2];
-                    wsum += w;
-                }
-            }
-            px[0] = __fdiv_rn(acc0, wsum); px[1] = __fdiv_rn(acc1, wsum); px[2] = __fdiv_rn(acc2, wsum);
-        } else if (SAMP == KB200_INTERP_BILINEAR) {
-            int x0 = (int)floorf(sx), y0 = (int)floorf(sy);
-            const float ax = sx - (float)x0, ay = sy - (float)y0;
-            const int x1 = min(x0 + 1, d.src_w - 1), y1 = min(y0 + 1, d.src_h - 1);
-            x0 = max(x0, 0); y0 = max(y0, 0);
-            float t00[3], t10[3], t01[3], t11[3];
-            fetch_px<TAP>(src, x0, y0, d, sf, yc, t00);
-            const bool need_x = ax != 0.0f, need_y = ay != 0.0f;
-            if (need_x) fetch_px<TAP>(src, x1, y0, d, sf, yc, t10);
-            if (need_y) {
-                fetch_px<TAP>(src, x0, y1, d, sf, yc, t01);
-                if (need_x) fetch_px<TAP>(src, x1, y1, d, sf, yc, t11);
-            }
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-                const float top = need_x ? t00[c] + (t10[c] - t00[c]) * ax : t00[c];
-                if (need_y) {
-                    const float bot = need_x ? t01[c] + (t11[c] - t01[c]) * ax : t01[c];
-                    px[c] = top + (bot - top) * ay;
-                } else {
-                    px[c] = top;
-                }
-            }
-        } else {
-            const int xn = min(max((int)roundf(sx), 0), d.src_w - 1);
-            const int yn = min(max((int)roundf(sy), 0), d.src_h - 1);
-            fetch_px<TAP>(src, xn, yn, d, sf, yc, px);
-        }
-    } else {
-        px[0] = d.pad_value; px[1] = d.pad_value; px[2] = d.pad_value;
-    }
-    float q0, q1, q2;
-    if (tap_words<TAP> && inside) {   // px / W, the IEEE quotient (div_white: no zero dividend reaches the division)
-        const float wl = sf.white();
-        q0 = div_white(px[0], wl); q1 = div_white(px[1], wl); q2 = div_white(px[2], wl);
-    } else if ((TAP == TAP_BAYER16 || TAP == TAP_BAYER_PACKED) && inside) {   // px / W: taps up to 65535 and Lanczos overshoot, so the IEEE division
-        const float wl = sf.white();
-        q0 = __fdiv_rn(px[0], wl); q1 = __fdiv_rn(px[1], wl); q2 = __fdiv_rn(px[2], wl);
-    } else if (inside && SAMP != KB200_INTERP_LANCZOS) { q0 = div255_exact(px[0]); q1 = div255_exact(px[1]); q2 = div255_exact(px[2]); }
-    else if (inside) { q0 = __fdiv_rn(px[0], 255.0f); q1 = __fdiv_rn(px[1], 255.0f); q2 = __fdiv_rn(px[2], 255.0f); }  // Lanczos overshoots [0, 255]
-    else { q0 = __fdiv_rn(px[0], 255.0f); q1 = q0; q2 = q0; }  // pad_value is caller-supplied: plain IEEE division
-    const float o0 = (q0 - d.mean[0]) * d.inv_std[0];
-    const float o1 = (q1 - d.mean[1]) * d.inv_std[1];
-    const float o2 = (q2 - d.mean[2]) * d.inv_std[2];
-    const size_t out = (size_t)(frame0 + f) * 3 * pixels + i;
-    if constexpr (OUT == KB200_OUT_F16) {
-        unsigned short* o = reinterpret_cast<unsigned short*>(dst);
-        o[out] = f2h_ref(o0); o[out + pixels] = f2h_ref(o1); o[out + 2 * (size_t)pixels] = f2h_ref(o2);
-    } else if constexpr (OUT == KB200_OUT_BF16) {
-        __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(dst);
-        o[out] = __float2bfloat16_rn(o0); o[out + pixels] = __float2bfloat16_rn(o1); o[out + 2 * (size_t)pixels] = __float2bfloat16_rn(o2);
-    } else {
-        float* o = reinterpret_cast<float*>(dst);
-        o[out] = o0; o[out + pixels] = o1; o[out + 2 * (size_t)pixels] = o2;
-    }
+    float o[3];
+    generic_pixel<SAMP, TAP>(src, ox, oy, d, sf, yc, FrameGeom{d}, o);
+    generic_store<OUT>(dst, (size_t)(frame0 + f) * 3 * pixels + i, pixels, o);
 }
 
 // ── NV12 identity fast path (config 3a: 1080p NV12 → [N,3,1080,1920], scale 1, no pad) ─────────────────────
@@ -389,9 +313,7 @@ __global__ void __launch_bounds__(128) preprocess_bayer_identity_kernel(const __
 //     (1080p → 640 letterbox is exactly 3:1) that is ONE decode per pixel;
 //   * a pixel that was not interpolated is an integer 0..255, whose `px / 255.0f` is the 3-instruction exact
 //     form (norm_int_px); interpolated pixels use the IEEE division.
-// L: a 4:2:0 layout or YUV444 (yuv_tap); T: the sample type (YuvSample).  A pixel of 16-bit words is normalised as
-// (px / W - mean) * inv_std with the IEEE division, interpolated or not.
-// preprocess_roi.cu restates this body (yuv_resample) with a region's geometry: a change to a sampling rule goes there too.
+// The sampler is yuv_resample (preprocess.cuh), here over frame frame0 + blockIdx.z.
 template <int OUT, bool BILINEAR, bool PTRS, int L, typename T>
 __global__ void __launch_bounds__(128) preprocess_yuv_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                              const __grid_constant__ PreFrames fr, const __grid_constant__ Nv12Args na,
@@ -399,108 +321,8 @@ __global__ void __launch_bounds__(128) preprocess_yuv_kernel(const __grid_consta
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= na.groups) return;
     const uint32_t f = blockIdx.z;
-    const int ox0 = (int)g * 4;
-    const int w = d.src_w, h = d.src_h;
     const uint8_t* src = PTRS ? fr.ptr[f] : fr.base + (size_t)(frame0 + f) * fr.stride;
-    const size_t plane = (size_t)d.dst_w * d.dst_h;
-    // x-side, once: plan_pixel + sample_* coordinate rules (preprocess.rs:437-448, :534-563)
-    int xa[4], xb[4];
-    float ax[4];
-    bool xin[4];
-    bool any_in = false;
-    // 16-bit samples and 4:4:4: the four divisions first, so that only their quotients are live across the slow-path calls
-    // they may make (the interleaved form spilled in the f16 bilinear instantiations); the 8-bit 4:2:0 kernels keep the
-    // interleaved form
-    constexpr bool SX_FIRST = sizeof(T) == 2 || L == YUV444;
-    [[maybe_unused]] float sx16[4];
-    if constexpr (SX_FIRST) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) sx16[j] = __fdiv_rn((float)(ox0 + j) - d.pad_x, d.scale_x);
-    }
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const float sx = SX_FIRST ? sx16[j] : __fdiv_rn((float)(ox0 + j) - d.pad_x, d.scale_x);
-        xin[j] = !(sx < 0.0f || sx >= (float)w);
-        any_in = any_in || xin[j];
-        if (BILINEAR) {
-            const int x0 = (int)floorf(sx);
-            ax[j] = sx - (float)x0;
-            xb[j] = min(x0 + 1, w - 1);
-            xa[j] = max(x0, 0);
-        } else {
-            xa[j] = min(max((int)roundf(sx), 0), w - 1);
-            xb[j] = xa[j]; ax[j] = 0.0f;
-        }
-    }
-    const int oy_first = (int)blockIdx.y * NV12_ROWS;
-#pragma unroll 1
-    for (int r = 0; r < NV12_ROWS; ++r) {
-        const int oy = oy_first + r;
-        if (oy >= d.dst_h) break;
-        const size_t obase = (size_t)(frame0 + f) * 3 * plane + (size_t)oy * d.dst_w + ox0;
-        float o[3][4];
-        const float sy = __fdiv_rn((float)oy - d.pad_y, d.scale_y);
-        const bool row_in = !(sy < 0.0f || sy >= (float)h);
-        if (!(row_in && any_in)) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) { o[0][j] = na.pad_norm[0]; o[1][j] = na.pad_norm[1]; o[2][j] = na.pad_norm[2]; }
-        } else {
-            int y0, y1 = 0;
-            float ay = 0.0f;
-            if (BILINEAR) {
-                y0 = (int)floorf(sy);
-                ay = sy - (float)y0;
-                y1 = min(y0 + 1, h - 1);
-                y0 = max(y0, 0);
-            } else {
-                y0 = min(max((int)roundf(sy), 0), h - 1);
-            }
-            const bool need_y = BILINEAR && ay != 0.0f;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                if (!xin[j]) { o[0][j] = na.pad_norm[0]; o[1][j] = na.pad_norm[1]; o[2][j] = na.pad_norm[2]; continue; }
-                int t00[3];
-                yuv_tap<L>(src, xa[j], y0, w, h, yc, t00);
-                const bool need_x = BILINEAR && ax[j] != 0.0f;
-                float px[3];
-                if (!need_x && !need_y) {  // the sample IS the decoded tap (exact, see header)
-                    px[0] = (float)t00[0]; px[1] = (float)t00[1]; px[2] = (float)t00[2];
-                } else {
-                    int t10[3] = {0, 0, 0}, t01[3] = {0, 0, 0}, t11[3] = {0, 0, 0};
-                    if (need_x) yuv_tap<L>(src, xb[j], y0, w, h, yc, t10);
-                    if (need_y) {
-                        yuv_tap<L>(src, xa[j], y1, w, h, yc, t01);
-                        if (need_x) yuv_tap<L>(src, xb[j], y1, w, h, yc, t11);
-                    }
-#pragma unroll
-                    for (int c = 0; c < 3; ++c) {
-                        const float a = (float)t00[c];
-                        const float top = need_x ? a + ((float)t10[c] - a) * ax[j] : a;
-                        if (need_y) {
-                            const float cc = (float)t01[c];
-                            const float bot = need_x ? cc + ((float)t11[c] - cc) * ax[j] : cc;
-                            px[c] = top + (bot - top) * ay;
-                        } else {
-                            px[c] = top;
-                        }
-                    }
-                }
-                if constexpr (sizeof(T) == 2) {
-                    const float wl = (float)yc.white;
-                    o[0][j] = (div_white(px[0], wl) - d.mean[0]) * d.inv_std[0];
-                    o[1][j] = (div_white(px[1], wl) - d.mean[1]) * d.inv_std[1];
-                    o[2][j] = (div_white(px[2], wl) - d.mean[2]) * d.inv_std[2];
-                } else {
-                    o[0][j] = (div255_exact(px[0]) - d.mean[0]) * d.inv_std[0];
-                    o[1][j] = (div255_exact(px[1]) - d.mean[1]) * d.inv_std[1];
-                    o[2][j] = (div255_exact(px[2]) - d.mean[2]) * d.inv_std[2];
-                }
-            }
-        }
-        nv12_store4<OUT>(dst, obase, o[0]);
-        nv12_store4<OUT>(dst, obase + plane, o[1]);
-        nv12_store4<OUT>(dst, obase + 2 * plane, o[2]);
-    }
+    yuv_resample<OUT, BILINEAR, L, T>(FrameGeom{d}, src, d, na, dst, frame0 + f, (int)g * 4, yc);
 }
 
 // One row per format code.  A Bayer code is 16 + pattern (8-bit samples), 32 + 4*k + pattern (16-bit words, k = 0..3 for
@@ -616,6 +438,18 @@ int validate_desc(const kb200_preprocess_desc* dp) {
     return KB200_OK;
 }
 
+int check_frame_table(const kb200_preprocess_desc& d, const uint8_t* const* frames, const size_t* frame_len, uint32_t n) {
+    const SrcFormat f = src_format(d.fmt);
+    const size_t need = src_bytes(d);
+    for (uint32_t i = 0; i < n; ++i) {
+        if (!frames[i]) return fail(KB200_ERR_INVALID_ARGUMENT, "null frame pointer at index %u", i);
+        if (f.words && (reinterpret_cast<uintptr_t>(frames[i]) & 1u)) return fail(KB200_ERR_INVALID_SOURCE, "%s frame %u is not 2-byte aligned", f.name, i);
+        if (frame_len && frame_len[i] < need)  // InvalidRawSource{got,need}, preprocess.rs:1287-1300
+            return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source at %dx%d (got %zu bytes, need %zu)", d.src_w, d.src_h, frame_len[i], need);
+    }
+    return KB200_OK;
+}
+
 // The fast kernels of layout L (4:2:0, or YUV444) and sample type T, for one launch of <= 256 frames.
 template <int OUT, int L, typename T = uint8_t>
 static void launch_yuv_fast(cudaStream_t s, bool identity, bool bil, const kb200_preprocess_desc& d, const typename YuvSample<T>::Coeffs& yc,
@@ -676,25 +510,14 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, int
     // 16-bit words, 16 B for packed Bayer.
     const uint32_t row_align = f.packed ? BayerSample<BayerPacked<12>>::ID_ALIGN
                                         : f.words ? BayerSample<uint16_t>::ID_ALIGN : BayerSample<uint8_t>::ID_ALIGN;
-    auto frames_aligned = [&](uint32_t a) {   // every frame of the call starts a-byte aligned
-        if (!frames) return ((reinterpret_cast<uintptr_t>(base) & (a - 1)) == 0) && (stride % a == 0);
-        for (uint32_t k = 0; k < batch; ++k)
-            if (reinterpret_cast<uintptr_t>(frames[k]) & (a - 1)) return false;
-        return true;
-    };
     bool identity = !lanczos && f.identity_kernel && d.scale_x == 1.0f && d.scale_y == 1.0f && d.pad_x == 0.0f && d.pad_y == 0.0f &&
                     d.dst_w == d.src_w && d.dst_h == d.src_h && (d.src_w % 4) == 0 && (d.src_pitch % row_align) == 0 && aligned16(dst) &&
-                    frames_aligned(row_align);
+                    frames_aligned(frames, base, stride, batch, row_align);
     const uint32_t id_groups = (uint32_t)d.src_w / 4u;
     const size_t id_rows = bayer ? bayer_row_pairs((uint32_t)d.src_h) : f.family == SRC_YUV444 ? (size_t)d.src_h : (size_t)d.src_h / 2;
     const size_t id_items = (size_t)id_groups * id_rows;   // threads of 4 columns x (2 rows, or 1 row of 4:4:4)
     if (id_items > 0x7FFFFFFFull) identity = false;
-    // 4:2:0 general fast path: vector stores need dst_w % 4 == 0 and a 16-B (f32) / 8-B (f16, bf16) aligned destination.  Its
-    // NV12 / NV21 tap reads a chroma pair as one 16-bit word (yuv_tap), so those frames must start 2-B aligned; frames at
-    // odd addresses take the generic kernel, which reads the pair's two bytes.
-    const bool pair_loads = f.family == SRC_YUV420 && !f.words && (f.layout == YUV420_NV12 || f.layout == YUV420_NV21);
-    const bool yuv420_fast = !lanczos && f.fast_kernel && (d.dst_w % 4) == 0 && aligned16(dst) && d.dst_h <= 65535 * NV12_ROWS &&
-                             (!pair_loads || frames_aligned(2));
+    const bool yuv420_fast = yuv_resampler_ok(f, d, dst, frames_aligned(frames, base, stride, batch, 2));
     const YuvCoeffs& yc = YUV_COEFFS[matrix];
     const Yuv16Coeffs yc16 = yuv16_coeffs_of(f, matrix);   // used by the 16-bit 4:2:0 and 4:4:4 formats only
     const Nv12Args nv = nv12_args(d);
@@ -764,13 +587,7 @@ static int preprocess_entry(kb200_stream_t stream, const kb200_preprocess_desc* 
     if (f.words && !frames && ((reinterpret_cast<uintptr_t>(base) & 1u) || (batch > 1 && (stride & 1u))))
         return fail(KB200_ERR_INVALID_SOURCE, "%s frames must start 2-byte aligned (base %p, stride %zu)", f.name, (const void*)base, stride);
     if (frames) {
-        for (uint32_t i = 0; i < batch; ++i) {
-            if (!frames[i]) return fail(KB200_ERR_INVALID_ARGUMENT, "null frame pointer at index %u", i);
-            if (f.words && (reinterpret_cast<uintptr_t>(frames[i]) & 1u))
-                return fail(KB200_ERR_INVALID_SOURCE, "%s frame %u is not 2-byte aligned", f.name, i);
-            if (frame_len && frame_len[i] < need)  // InvalidRawSource{got,need}, preprocess.rs:1287-1300
-                return fail(KB200_ERR_INVALID_SOURCE, "invalid raw source at %dx%d (got %zu bytes, need %zu)", desc->src_w, desc->src_h, frame_len[i], need);
-        }
+        KB200_TRY(check_frame_table(*desc, frames, frame_len, batch));
     } else {
         KB200_TRY(check_ptr("base", base));
         if (stride < need && batch > 1) return fail(KB200_ERR_INVALID_SOURCE, "frame stride %zu smaller than a frame (%zu bytes)", stride, need);

@@ -1,7 +1,8 @@
 // preprocess.cuh — what the camera preprocess's two sources share: preprocess.cu (one affine per frame, the batch entries)
 // and preprocess_roi.cu (one affine per region of a frame, kb200_preprocess_rois): the source-format facts, the taps
-// (fetch_px), the Lanczos weight, the normalising divisions, the stores, the fast resampler's arguments, the host rules of
-// the descriptor and the kernel-selection switches.  The arithmetic is documented in preprocess.cu's header.
+// (fetch_px), the Lanczos weight, the normalising divisions, the stores, the two sampler bodies over a frame's or a
+// region's geometry, the fast resampler's arguments and launch rule, the host rules of the descriptor and the
+// kernel-selection switches.  The arithmetic is documented in preprocess.cu's header.
 #pragma once
 
 #include <cuda_bf16.h>
@@ -179,6 +180,236 @@ struct Nv12Args {
 
 static constexpr int NV12_ROWS = 8;  // destination rows per thread: the x-side of the sampler is computed once for all of them
 
+// ── the sampler bodies ──────────────────────────────────────────────────────────────────────────────────────────────────
+// generic_pixel and yuv_resample sample a source rectangle through a geometry G, which gives the source coordinate of an
+// output column / row (sx, sy: IEEE division, plan_pixel :437-448), the rectangle's extent (w, h: the inside test and the
+// tap clamps) and its origin in the frame (x0, y0: added to every tap, so that taps decode at frame coordinates), and, for
+// yuv_resample's row loop, all three of a row at once (row).  FrameGeom is a whole frame under the descriptor's affine;
+// RoiGeom (preprocess_roi.cu) is one region of a frame under its own.
+
+// The row side of yuv_resample: the source row of an output row, the extent it is tested and clamped against, the origin.
+struct GeomRow {
+    float sy;
+    int h, y0;
+};
+
+struct FrameGeom {
+    const kb200_preprocess_desc& d;
+    int rows;   // d.src_h, read once: see row()
+    __device__ __forceinline__ explicit FrameGeom(const kb200_preprocess_desc& desc) : d(desc), rows(desc.src_h) {}
+    __device__ __forceinline__ float sx(int ox) const { return __fdiv_rn((float)ox - d.pad_x, d.scale_x); }
+    __device__ __forceinline__ float sy(int oy) const { return __fdiv_rn((float)oy - d.pad_y, d.scale_y); }
+    __device__ __forceinline__ int w() const { return d.src_w; }
+    __device__ __forceinline__ int h() const { return d.src_h; }
+    __device__ __forceinline__ int x0() const { return 0; }
+    __device__ __forceinline__ int y0() const { return 0; }
+    // The height comes from the copy taken at construction, so the row loop holds it as one value.  Read through d after
+    // each row's stores (whose inline asm clobbers memory), it is reloaded in the body's own optimisation, and every
+    // preprocess_yuv_kernel instantiation compiled to a different predicate order and register assignment.
+    __device__ __forceinline__ GeomRow row(int oy) const { return {sy(oy), rows, 0}; }
+};
+
+// Output pixel (ox, oy) of the rectangle g of the frame at src, sampled with SAMP (kb200_interp — 0 nearest, 1 bilinear,
+// 3 Lanczos-3: 6x6 taps, clamp-to-edge, weights renormalised by their sum) and normalised into o.
+template <int SAMP, int TAP, class G>
+__device__ __forceinline__ void generic_pixel(const uint8_t* __restrict__ src, int ox, int oy, const kb200_preprocess_desc& d, const SrcFormat& sf,
+                                              const TapCoeffs<TAP>& yc, const G& g, float o[3]) {
+    const float sx = g.sx(ox);
+    const float sy = g.sy(oy);
+    const bool inside = !(sx < 0.0f || sy < 0.0f || sx >= (float)g.w() || sy >= (float)g.h());
+    float px[3];
+    if (inside) {
+        if (SAMP == KB200_INTERP_LANCZOS) {   // preprocess.rs:565-590 sample_lanczos: acc += w * t (unfused), one division per channel
+            const int x0 = (int)floorf(sx), y0 = (int)floorf(sy);
+            float acc0 = 0.0f, acc1 = 0.0f, acc2 = 0.0f, wsum = 0.0f;
+            for (int j = -2; j <= 3; ++j) {
+                const int yj = y0 + j;
+                const float wy = pre_lanczos_w(sy - (float)yj);
+                const int ycl = min(max(yj, 0), g.h() - 1);
+                for (int ii = -2; ii <= 3; ++ii) {
+                    const int xi = x0 + ii;
+                    const float w = wy * pre_lanczos_w(sx - (float)xi);
+                    const int xc = min(max(xi, 0), g.w() - 1);
+                    float t[3];
+                    fetch_px<TAP>(src, g.x0() + xc, g.y0() + ycl, d, sf, yc, t);
+                    acc0 += w * t[0]; acc1 += w * t[1]; acc2 += w * t[2];
+                    wsum += w;
+                }
+            }
+            px[0] = __fdiv_rn(acc0, wsum); px[1] = __fdiv_rn(acc1, wsum); px[2] = __fdiv_rn(acc2, wsum);
+        } else if (SAMP == KB200_INTERP_BILINEAR) {
+            int x0 = (int)floorf(sx), y0 = (int)floorf(sy);
+            const float ax = sx - (float)x0, ay = sy - (float)y0;
+            const int x1 = g.x0() + min(x0 + 1, g.w() - 1), y1 = g.y0() + min(y0 + 1, g.h() - 1);
+            x0 = g.x0() + max(x0, 0); y0 = g.y0() + max(y0, 0);
+            float t00[3], t10[3], t01[3], t11[3];
+            fetch_px<TAP>(src, x0, y0, d, sf, yc, t00);
+            const bool need_x = ax != 0.0f, need_y = ay != 0.0f;
+            if (need_x) fetch_px<TAP>(src, x1, y0, d, sf, yc, t10);
+            if (need_y) {
+                fetch_px<TAP>(src, x0, y1, d, sf, yc, t01);
+                if (need_x) fetch_px<TAP>(src, x1, y1, d, sf, yc, t11);
+            }
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const float top = need_x ? t00[c] + (t10[c] - t00[c]) * ax : t00[c];
+                if (need_y) {
+                    const float bot = need_x ? t01[c] + (t11[c] - t01[c]) * ax : t01[c];
+                    px[c] = top + (bot - top) * ay;
+                } else {
+                    px[c] = top;
+                }
+            }
+        } else {
+            const int xn = g.x0() + min(max((int)roundf(sx), 0), g.w() - 1);
+            const int yn = g.y0() + min(max((int)roundf(sy), 0), g.h() - 1);
+            fetch_px<TAP>(src, xn, yn, d, sf, yc, px);
+        }
+    } else {
+        px[0] = d.pad_value; px[1] = d.pad_value; px[2] = d.pad_value;
+    }
+    float q0, q1, q2;
+    if (tap_words<TAP> && inside) {   // px / W, the IEEE quotient (div_white: no zero dividend reaches the division)
+        const float wl = sf.white();
+        q0 = div_white(px[0], wl); q1 = div_white(px[1], wl); q2 = div_white(px[2], wl);
+    } else if ((TAP == TAP_BAYER16 || TAP == TAP_BAYER_PACKED) && inside) {   // px / W: taps up to 65535 and Lanczos overshoot, so the IEEE division
+        const float wl = sf.white();
+        q0 = __fdiv_rn(px[0], wl); q1 = __fdiv_rn(px[1], wl); q2 = __fdiv_rn(px[2], wl);
+    } else if (inside && SAMP != KB200_INTERP_LANCZOS) { q0 = div255_exact(px[0]); q1 = div255_exact(px[1]); q2 = div255_exact(px[2]); }
+    else if (inside) { q0 = __fdiv_rn(px[0], 255.0f); q1 = __fdiv_rn(px[1], 255.0f); q2 = __fdiv_rn(px[2], 255.0f); }  // Lanczos overshoots [0, 255]
+    else { q0 = __fdiv_rn(px[0], 255.0f); q1 = q0; q2 = q0; }  // pad_value is caller-supplied: plain IEEE division
+    o[0] = (q0 - d.mean[0]) * d.inv_std[0];
+    o[1] = (q1 - d.mean[1]) * d.inv_std[1];
+    o[2] = (q2 - d.mean[2]) * d.inv_std[2];
+}
+
+// The three planes of one pixel: element `out` of plane 0 of a CHW image of `pixels` pixels per plane.
+template <int OUT>
+__device__ __forceinline__ void generic_store(void* __restrict__ dst, size_t out, int pixels, const float o[3]) {
+    if constexpr (OUT == KB200_OUT_F16) {
+        unsigned short* p = reinterpret_cast<unsigned short*>(dst);
+        p[out] = f2h_ref(o[0]); p[out + pixels] = f2h_ref(o[1]); p[out + 2 * (size_t)pixels] = f2h_ref(o[2]);
+    } else if constexpr (OUT == KB200_OUT_BF16) {
+        __nv_bfloat16* p = reinterpret_cast<__nv_bfloat16*>(dst);
+        p[out] = __float2bfloat16_rn(o[0]); p[out + pixels] = __float2bfloat16_rn(o[1]); p[out + 2 * (size_t)pixels] = __float2bfloat16_rn(o[2]);
+    } else {
+        float* p = reinterpret_cast<float*>(dst);
+        p[out] = o[0]; p[out + pixels] = o[1]; p[out + 2 * (size_t)pixels] = o[2];
+    }
+}
+
+// The fast resampler: the 4 output columns ox0 .. ox0 + 3 of the NV12_ROWS rows from blockIdx.y * NV12_ROWS of output
+// image `img`, sampled from the rectangle geo of the frame at src.  The frame's w x h (the descriptor's) address its planes
+// in yuv_tap; geo's extent sets the inside test and the clamps.  L: a 4:2:0 layout or YUV444 (yuv_tap); T: the sample type
+// (YuvSample).  A pixel of 16-bit words is normalised as (px / W - mean) * inv_std with the IEEE division, interpolated or not.
+template <int OUT, bool BILINEAR, int L, typename T, class G>
+__device__ __forceinline__ void yuv_resample(const G& geo, const uint8_t* __restrict__ src, const kb200_preprocess_desc& d, const Nv12Args& na,
+                                             void* __restrict__ dst, uint32_t img, int ox0, const typename YuvSample<T>::Coeffs& yc) {
+    const int w = d.src_w, h = d.src_h;
+    const int rw = geo.w();
+    const size_t plane = (size_t)d.dst_w * d.dst_h;
+    // x-side, once: plan_pixel + sample_* coordinate rules (preprocess.rs:437-448, :534-563)
+    int xa[4], xb[4];
+    float ax[4];
+    bool xin[4];
+    bool any_in = false;
+    // 16-bit samples and 4:4:4: the four divisions first, so that only their quotients are live across the slow-path calls
+    // they may make (the interleaved form spilled in the f16 bilinear instantiations); the 8-bit 4:2:0 kernels keep the
+    // interleaved form
+    constexpr bool SX_FIRST = sizeof(T) == 2 || L == YUV444;
+    [[maybe_unused]] float sx16[4];
+    if constexpr (SX_FIRST) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) sx16[j] = geo.sx(ox0 + j);
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const float sx = SX_FIRST ? sx16[j] : geo.sx(ox0 + j);
+        xin[j] = !(sx < 0.0f || sx >= (float)rw);
+        any_in = any_in || xin[j];
+        if (BILINEAR) {
+            const int x0 = (int)floorf(sx);
+            ax[j] = sx - (float)x0;
+            xb[j] = geo.x0() + min(x0 + 1, rw - 1);
+            xa[j] = geo.x0() + max(x0, 0);
+        } else {
+            xa[j] = geo.x0() + min(max((int)roundf(sx), 0), rw - 1);
+            xb[j] = xa[j]; ax[j] = 0.0f;
+        }
+    }
+    const int oy_first = (int)blockIdx.y * NV12_ROWS;
+#pragma unroll 1
+    for (int r = 0; r < NV12_ROWS; ++r) {
+        const int oy = oy_first + r;
+        if (oy >= d.dst_h) break;
+        const size_t obase = (size_t)img * 3 * plane + (size_t)oy * d.dst_w + ox0;
+        float o[3][4];
+        const GeomRow gr = geo.row(oy);
+        const float sy = gr.sy;
+        const int rh = gr.h, ry = gr.y0;
+        const bool row_in = !(sy < 0.0f || sy >= (float)rh);
+        if (!(row_in && any_in)) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) { o[0][j] = na.pad_norm[0]; o[1][j] = na.pad_norm[1]; o[2][j] = na.pad_norm[2]; }
+        } else {
+            int y0, y1 = 0;
+            float ay = 0.0f;
+            if (BILINEAR) {
+                y0 = (int)floorf(sy);
+                ay = sy - (float)y0;
+                y1 = ry + min(y0 + 1, rh - 1);
+                y0 = ry + max(y0, 0);
+            } else {
+                y0 = ry + min(max((int)roundf(sy), 0), rh - 1);
+            }
+            const bool need_y = BILINEAR && ay != 0.0f;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                if (!xin[j]) { o[0][j] = na.pad_norm[0]; o[1][j] = na.pad_norm[1]; o[2][j] = na.pad_norm[2]; continue; }
+                int t00[3];
+                yuv_tap<L>(src, xa[j], y0, w, h, yc, t00);
+                const bool need_x = BILINEAR && ax[j] != 0.0f;
+                float px[3];
+                if (!need_x && !need_y) {  // the sample IS the decoded tap (exact, see preprocess.cu's header)
+                    px[0] = (float)t00[0]; px[1] = (float)t00[1]; px[2] = (float)t00[2];
+                } else {
+                    int t10[3] = {0, 0, 0}, t01[3] = {0, 0, 0}, t11[3] = {0, 0, 0};
+                    if (need_x) yuv_tap<L>(src, xb[j], y0, w, h, yc, t10);
+                    if (need_y) {
+                        yuv_tap<L>(src, xa[j], y1, w, h, yc, t01);
+                        if (need_x) yuv_tap<L>(src, xb[j], y1, w, h, yc, t11);
+                    }
+#pragma unroll
+                    for (int c = 0; c < 3; ++c) {
+                        const float a = (float)t00[c];
+                        const float top = need_x ? a + ((float)t10[c] - a) * ax[j] : a;
+                        if (need_y) {
+                            const float cc = (float)t01[c];
+                            const float bot = need_x ? cc + ((float)t11[c] - cc) * ax[j] : cc;
+                            px[c] = top + (bot - top) * ay;
+                        } else {
+                            px[c] = top;
+                        }
+                    }
+                }
+                if constexpr (sizeof(T) == 2) {
+                    const float wl = (float)yc.white;
+                    o[0][j] = (div_white(px[0], wl) - d.mean[0]) * d.inv_std[0];
+                    o[1][j] = (div_white(px[1], wl) - d.mean[1]) * d.inv_std[1];
+                    o[2][j] = (div_white(px[2], wl) - d.mean[2]) * d.inv_std[2];
+                } else {
+                    o[0][j] = (div255_exact(px[0]) - d.mean[0]) * d.inv_std[0];
+                    o[1][j] = (div255_exact(px[1]) - d.mean[1]) * d.inv_std[1];
+                    o[2][j] = (div255_exact(px[2]) - d.mean[2]) * d.inv_std[2];
+                }
+            }
+        }
+        nv12_store4<OUT>(dst, obase, o[0]);
+        nv12_store4<OUT>(dst, obase + plane, o[1]);
+        nv12_store4<OUT>(dst, obase + 2 * plane, o[2]);
+    }
+}
+
 // ── host side ───────────────────────────────────────────────────────────────────────────────────────────────────────────
 // The rules of the descriptor, in preprocess.cu.
 SrcFormat src_format(int fmt);   // the facts of a plain format code; name == nullptr: not a format
@@ -186,6 +417,28 @@ kb200_preprocess_desc plain_desc(const kb200_preprocess_desc& d);   // the forma
 int yuv_matrix(const kb200_preprocess_desc& raw);
 size_t src_bytes(const kb200_preprocess_desc& d);    // d: a plain descriptor
 int validate_desc(const kb200_preprocess_desc* dp);  // the raw descriptor an entry was given
+// The checks of a table of n frame pointers (frame_len: their lengths, or nullptr): none null, every frame of 16-bit samples
+// 2-byte aligned, every length >= src_bytes(d).  d: a plain descriptor.
+int check_frame_table(const kb200_preprocess_desc& d, const uint8_t* const* frames, const size_t* frame_len, uint32_t n);
+
+// Every frame of a call starts a-byte aligned: the n frames of the pointer table `frames`, or, when it is nullptr, the
+// frames at base + k * stride.
+inline bool frames_aligned(const uint8_t* const* frames, const uint8_t* base, size_t stride, uint32_t n, uint32_t a) {
+    if (!frames) return ((reinterpret_cast<uintptr_t>(base) & (a - 1)) == 0) && (stride % a == 0);
+    for (uint32_t k = 0; k < n; ++k)
+        if (reinterpret_cast<uintptr_t>(frames[k]) & (a - 1)) return false;
+    return true;
+}
+
+// Whether the fast resampler (yuv_resample) takes a call of format f (plain descriptor d) into dst: a format with fast
+// kernels, not Lanczos, and vector stores, which need dst_w % 4 == 0 and a 16-B (f32) / 8-B (f16, bf16) aligned
+// destination.  The NV12 / NV21 tap reads a chroma pair as one 16-bit word (yuv_tap), so those frames must start 2-B
+// aligned (frames_even); frames at odd addresses take the generic kernel, which reads the pair's two bytes.
+inline bool yuv_resampler_ok(const SrcFormat& f, const kb200_preprocess_desc& d, const void* dst, bool frames_even) {
+    const bool pair_loads = f.family == SRC_YUV420 && !f.words && (f.layout == YUV420_NV12 || f.layout == YUV420_NV21);
+    return d.sampling != KB200_INTERP_LANCZOS && f.fast_kernel && (d.dst_w % 4) == 0 && aligned16(dst) && d.dst_h <= 65535 * NV12_ROWS &&
+           (!pair_loads || frames_even);
+}
 
 // The Q16 coefficient set of a format of 16-bit YUV words (P01x, I01x, I41x) decoded with `matrix`.
 inline Yuv16Coeffs yuv16_coeffs_of(const SrcFormat& f, int matrix) {
