@@ -61,6 +61,17 @@ pub mod ffi {
 
     const _: () = assert!(std::mem::size_of::<kb200_roi>() == 20);
 
+    /// include/kornia_b200.h `kb200_warp_roi` — frame `frame` through the forward map `m` (row-major 3x3, frame -> output
+    /// pixel coordinates), 40 bytes, C layout.
+    #[repr(C)]
+    #[derive(Clone, Copy, Debug, Default)]
+    pub struct kb200_warp_roi {
+        pub frame: i32,
+        pub m: [f32; 9],
+    }
+
+    const _: () = assert!(std::mem::size_of::<kb200_warp_roi>() == 40);
+
     extern "C" {
         pub fn kb200_version() -> c_int;
         pub fn kb200_last_kernel() -> *const c_char;
@@ -172,6 +183,7 @@ pub mod ffi {
         pub fn kb200_preprocess_bf16(stream: *mut c_void, desc: *const kb200_preprocess_desc, frames: *const *const u8, frame_len: *const usize, batch: u32, dst: *mut u16, dst_len: usize) -> c_int;
         pub fn kb200_preprocess_strided_bf16(stream: *mut c_void, desc: *const kb200_preprocess_desc, base: *const u8, base_len: usize, frame_stride: usize, batch: u32, dst: *mut u16, dst_len: usize) -> c_int;
         pub fn kb200_preprocess_rois(stream: *mut c_void, desc: *const kb200_preprocess_desc, mode: c_int, frames: *const *const u8, frame_len: *const usize, n_frames: u32, rois: *const kb200_roi, n_rois: u32, dst: *mut c_void, dst_len: usize, out_format: c_int) -> c_int;
+        pub fn kb200_preprocess_warps(stream: *mut c_void, desc: *const kb200_preprocess_desc, frames: *const *const u8, frame_len: *const usize, n_frames: u32, warps: *const kb200_warp_roi, n_warps: u32, dst: *mut c_void, dst_len: usize, out_format: c_int) -> c_int;
         pub fn kb200_selftest_div255(stream: *mut c_void, mismatches_dev: *mut u64) -> c_int;
         pub fn kb200_selftest_div2(stream: *mut c_void, count: u64, seed: u32, mismatches_dev: *mut u64) -> c_int;
 
@@ -509,6 +521,30 @@ pub fn launch_preprocess_rois(
     check(unsafe {
         ffi::kb200_preprocess_rois(stream.cu_stream() as *mut c_void, desc, mode, ptrs.as_ptr(), lens.as_ptr(), frames.len() as u32, rois.as_ptr(),
                                    rois.len() as u32, dp as *mut c_void, dst_len, 0)
+    })
+}
+
+/// Rotated and perspective crops: `warps[i]` is frame `warps[i].frame` through its forward map (frame -> output pixel
+/// coordinates), sampled into `dst` ([warps.len(), 3, dst_h, dst_w] f32) with the descriptor's sampling (Nearest or
+/// Bilinear) and normalisation: one launch per 72 regions (an extension beyond the reference).
+pub fn launch_preprocess_warps(
+    stream: &Arc<CudaStream>, desc: &ffi::kb200_preprocess_desc, frames: &[&CudaSlice<u8>], warps: &[ffi::kb200_warp_roi],
+    dst: &mut CudaSlice<f32>,
+) -> Result<(), Kb200Error> {
+    bind(stream.context())?;
+    let mut guards = Vec::with_capacity(frames.len());
+    let mut ptrs: Vec<*const u8> = Vec::with_capacity(frames.len());
+    let lens: Vec<usize> = frames.iter().map(|f| f.len()).collect();
+    for f in frames {
+        let (p, g) = f.device_ptr(stream);
+        ptrs.push(p as *const u8);
+        guards.push(g);
+    }
+    let dst_len = dst.len();
+    let (dp, _g1) = dst.device_ptr_mut(stream);
+    check(unsafe {
+        ffi::kb200_preprocess_warps(stream.cu_stream() as *mut c_void, desc, ptrs.as_ptr(), lens.as_ptr(), frames.len() as u32, warps.as_ptr(),
+                                    warps.len() as u32, dp as *mut c_void, dst_len, 0)
     })
 }
 

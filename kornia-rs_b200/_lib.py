@@ -34,6 +34,11 @@ class Roi(C.Structure):
     _fields_ = [("frame", C.c_int32), ("x", C.c_int32), ("y", C.c_int32), ("w", C.c_int32), ("h", C.c_int32)]
 
 
+class WarpRoi(C.Structure):
+    """kb200_warp_roi: frame `frame` through the forward map `m` (row-major 3x3, frame -> output pixel coordinates)"""
+    _fields_ = [("frame", C.c_int32), ("m", C.c_float * 9)]
+
+
 _lib = None
 _tls = threading.local()
 
@@ -129,6 +134,7 @@ def _declare(l: C.CDLL) -> None:
         "kb200_preprocess_strided_bf16": ([vp, C.POINTER(PreprocessDesc), vp, sz, sz, u32, vp, sz], i),
         "kb200_preprocess_host_format": ([vp, vp, C.POINTER(PreprocessDesc), vp, sz, sz, u32, vp, sz, i], i),
         "kb200_preprocess_rois": ([vp, C.POINTER(PreprocessDesc), i, C.POINTER(vp), C.POINTER(sz), u32, C.POINTER(Roi), u32, vp, sz, i], i),
+        "kb200_preprocess_warps": ([vp, C.POINTER(PreprocessDesc), C.POINTER(vp), C.POINTER(sz), u32, C.POINTER(WarpRoi), u32, vp, sz, i], i),
     }
     for name, (args, res) in sig.items():
         fn = getattr(l, name)  # AttributeError if the symbol is missing: fail loudly

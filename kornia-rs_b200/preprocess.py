@@ -629,3 +629,81 @@ class Preprocessor:
         if st != _lib.OK:
             kind = {_lib.ERR_INVALID_SOURCE: "InvalidRawSource", _lib.ERR_DIMS_TOO_LARGE: "DimensionsTooLarge"}.get(st, "Cuda")
             raise PreprocessError(kind, ("CUDA error: " if kind == "Cuda" else "") + _lib.last_error())
+
+    # ── rotated and perspective regions ─────────────────────────────────────
+    def run_warps(self, frames: Sequence[torch.Tensor], src_w: int, src_h: int, frame_index, matrices, dst: torch.Tensor) -> None:
+        """Rotated and perspective crops of raw device frames in the builder's SourceFormat: region i is frames[frame_index[i]]
+        through the FORWARD map matrices[i] (frame pixel coordinates -> output pixel coordinates, as cv2.warpAffine /
+        warpPerspective without WARP_INVERSE_MAP; a 2x3 map gets the row (0, 0, 1)), sampled into dst[i] with the builder's
+        sampling (Nearest or Bilinear), normalisation, pad value and YUV matrix.  The builder's mode does not apply: the map
+        is the geometry.  `frame_index`: a sequence of ints or an integer CPU tensor [M]; `matrices`: a CPU tensor or nested
+        sequence [M, 2, 3] or [M, 3, 3], converted to float32; `dst`: a contiguous device [M, 3, H, W] tensor of
+        torch.float32, torch.float16 or torch.bfloat16, which selects the output.  A bad frame index, a map of another shape,
+        with a non-finite entry or singular raises PreprocessError("InvalidWarp", region=i); Lanczos sampling raises
+        "UnsupportedSampling"."""
+        import math
+
+        if self._sampling not in (InterpolationMode.Nearest, InterpolationMode.Bilinear):
+            raise PreprocessError("UnsupportedSampling", f"unsupported sampling mode {self._sampling!r} for warped regions (expected Nearest or Bilinear)")
+        if isinstance(frame_index, torch.Tensor):
+            if (frame_index.is_cuda or frame_index.dim() != 1 or frame_index.dtype.is_floating_point or frame_index.dtype.is_complex
+                    or frame_index.dtype == torch.bool):
+                raise PreprocessError("InvalidWarp", f"frame_index must be an integer CPU tensor [M], got {frame_index.dtype} "
+                                      f"{list(frame_index.shape)} on {frame_index.device}")
+            index = [int(v) for v in frame_index.tolist()]
+        else:
+            index = list(frame_index)
+            if not all(isinstance(v, int) or (isinstance(v, torch.Tensor) and v.dim() == 0 and not v.dtype.is_floating_point) for v in index):
+                raise PreprocessError("InvalidWarp", "frame_index must hold integers")
+            index = [int(v) for v in index]
+        if not index:
+            raise PreprocessError("InvalidWarp", "no regions given")
+        if isinstance(matrices, torch.Tensor):
+            if matrices.is_cuda or matrices.dim() != 3 or tuple(matrices.shape[1:]) not in ((2, 3), (3, 3)):
+                raise PreprocessError("InvalidWarp", f"matrices must be a CPU tensor [M, 2, 3] or [M, 3, 3], got {list(matrices.shape)} on {matrices.device}")
+            maps = list(matrices.to(torch.float32).unbind(0))
+        else:
+            maps = []
+            for i, mi in enumerate(matrices):
+                try:
+                    t = torch.as_tensor(mi, dtype=torch.float32)
+                except (TypeError, ValueError, RuntimeError) as e:
+                    raise PreprocessError("InvalidWarp", f"region {i}: the map is not a 2x3 or 3x3 array of numbers ({e})", region=i) from None
+                if tuple(t.shape) not in ((2, 3), (3, 3)):
+                    raise PreprocessError("InvalidWarp", f"region {i}: the map has shape {list(t.shape)} (expected 2x3 or 3x3)", region=i)
+                maps.append(t)
+        if len(maps) != len(index):
+            raise PreprocessError("InvalidWarp", f"{len(maps)} maps for {len(index)} frame indices")
+        table = []
+        for i, (k, mi) in enumerate(zip(index, maps)):   # the C entry's region rules, checked here so that the kind is InvalidWarp
+            if not 0 <= k < len(frames):
+                raise PreprocessError("InvalidWarp", f"region {i}: frame index {k} is outside [0, {len(frames)})", region=i)
+            flat = mi.reshape(-1).tolist() + ([0.0, 0.0, 1.0] if mi.shape[0] == 2 else [])
+            if not all(math.isfinite(v) for v in flat):
+                raise PreprocessError("InvalidWarp", f"region {i}: the map has a non-finite entry", region=i)
+            table.append((k, flat))
+        if dst.dtype not in _OUT_DTYPES:
+            raise PreprocessError("BadOutputShape", f"unsupported output dtype {dst.dtype} (expected torch.float32, torch.float16 or torch.bfloat16)")
+        out = _OUT_DTYPES.index(dst.dtype)
+        self._validate_dst(dst, len(table), out)
+        for f in frames:
+            self._validate_raw(f.numel() * f.element_size(), src_w, src_h)
+            if not f.is_cuda:
+                raise PreprocessError("NotDeviceImage", "CUDA preprocessor requires a device-resident source image")
+            if f.device != dst.device:
+                raise PreprocessError("Cuda", "CUDA error: source and destination are on different CUDA devices")
+        fmt = self._fmt
+        desc = self._desc(src_w, src_h, fmt.pitch(src_w), fmt.bpp(), fmt.fmt_code(), dst.shape[3], dst.shape[2])
+        n, m = len(frames), len(table)
+        ptrs = (C.c_void_p * max(n, 1))(*[f.data_ptr() for f in frames])
+        lens = (C.c_size_t * max(n, 1))(*[f.numel() * f.element_size() for f in frames])
+        warps = (_lib.WarpRoi * m)(*[_lib.WarpRoi(k, (C.c_float * 9)(*flat)) for k, flat in table])
+        _lib.set_device(dst.device.index)
+        st = _lib.lib().kb200_preprocess_warps(torch.cuda.current_stream(dst.device).cuda_stream, C.byref(desc), ptrs, lens, n, warps, m,
+                                               dst.data_ptr(), dst.numel(), out)
+        if st != _lib.OK:
+            msg = _lib.last_error()
+            if st == _lib.ERR_SINGULAR_MATRIX:   # "region <i>: ..." (preprocess_warp.cu invert_warp)
+                raise PreprocessError("InvalidWarp", msg, region=int(msg.split(":")[0].split()[1]))
+            kind = {_lib.ERR_INVALID_SOURCE: "InvalidRawSource", _lib.ERR_DIMS_TOO_LARGE: "DimensionsTooLarge"}.get(st, "Cuda")
+            raise PreprocessError(kind, ("CUDA error: " if kind == "Cuda" else "") + msg)
