@@ -72,6 +72,17 @@ pub mod ffi {
 
     const _: () = assert!(std::mem::size_of::<kb200_warp_roi>() == 40);
 
+    /// include/kornia_b200.h `kb200_remap_roi` — frame `frame` resampled through map `map` of the call's map arrays,
+    /// 8 bytes, C layout.
+    #[repr(C)]
+    #[derive(Clone, Copy, Debug, Default)]
+    pub struct kb200_remap_roi {
+        pub frame: i32,
+        pub map: i32,
+    }
+
+    const _: () = assert!(std::mem::size_of::<kb200_remap_roi>() == 8);
+
     extern "C" {
         pub fn kb200_version() -> c_int;
         pub fn kb200_last_kernel() -> *const c_char;
@@ -184,6 +195,7 @@ pub mod ffi {
         pub fn kb200_preprocess_strided_bf16(stream: *mut c_void, desc: *const kb200_preprocess_desc, base: *const u8, base_len: usize, frame_stride: usize, batch: u32, dst: *mut u16, dst_len: usize) -> c_int;
         pub fn kb200_preprocess_rois(stream: *mut c_void, desc: *const kb200_preprocess_desc, mode: c_int, frames: *const *const u8, frame_len: *const usize, n_frames: u32, rois: *const kb200_roi, n_rois: u32, dst: *mut c_void, dst_len: usize, out_format: c_int) -> c_int;
         pub fn kb200_preprocess_warps(stream: *mut c_void, desc: *const kb200_preprocess_desc, frames: *const *const u8, frame_len: *const usize, n_frames: u32, warps: *const kb200_warp_roi, n_warps: u32, dst: *mut c_void, dst_len: usize, out_format: c_int) -> c_int;
+        pub fn kb200_preprocess_remap(stream: *mut c_void, desc: *const kb200_preprocess_desc, frames: *const *const u8, frame_len: *const usize, n_frames: u32, map_x: *const f32, map_y: *const f32, map_len: usize, n_maps: u32, regions: *const kb200_remap_roi, n_regions: u32, dst: *mut c_void, dst_len: usize, out_format: c_int) -> c_int;
         pub fn kb200_selftest_div255(stream: *mut c_void, mismatches_dev: *mut u64) -> c_int;
         pub fn kb200_selftest_div2(stream: *mut c_void, count: u64, seed: u32, mismatches_dev: *mut u64) -> c_int;
 
@@ -203,6 +215,9 @@ pub mod ffi {
                               channels: u32, batch: u32) -> c_int;
         pub fn kb200_generate_correction_map_polynomial(stream: *mut c_void, intrinsic: *const f64, distortion: *const f64, width: u32,
                                                         height: u32, map_x: *mut f32, map_y: *mut f32, map_len: usize) -> c_int;
+        pub fn kb200_generate_correction_map_polynomial_to(stream: *mut c_void, intrinsic: *const f64, distortion: *const f64,
+                                                           new_intrinsic: *const f64, width: u32, height: u32, map_x: *mut f32,
+                                                           map_y: *mut f32, map_len: usize) -> c_int;
         pub fn kb200_fused_pipeline_u8_f32(stream: *mut c_void, src: *const u8, src_len: usize, dst: *mut f32, dst_len: usize, src_w: u32,
                                            src_h: u32, dst_w: u32, dst_h: u32, batch: u32, maps: c_int, scale: *const f32, bias: *const f32,
                                            sink: c_int) -> c_int;
@@ -545,6 +560,35 @@ pub fn launch_preprocess_warps(
     check(unsafe {
         ffi::kb200_preprocess_warps(stream.cu_stream() as *mut c_void, desc, ptrs.as_ptr(), lens.as_ptr(), frames.len() as u32, warps.as_ptr(),
                                     warps.len() as u32, dp as *mut c_void, dst_len, 0)
+    })
+}
+
+/// Frames resampled through dense coordinate maps (lens undistortion, rig rectification): `regions[i]` is frame
+/// `regions[i].frame` sampled at the coordinates of map `regions[i].map` of `map_x` / `map_y` ([n_maps, dst_h, dst_w] f32)
+/// into `dst` ([regions.len(), 3, dst_h, dst_w] f32) with the descriptor's sampling (Nearest or Bilinear) and
+/// normalisation; coordinates outside the frame take the pad value.  One launch per 192 regions (an extension beyond the
+/// reference).
+pub fn launch_preprocess_remap(
+    stream: &Arc<CudaStream>, desc: &ffi::kb200_preprocess_desc, frames: &[&CudaSlice<u8>], map_x: &CudaSlice<f32>, map_y: &CudaSlice<f32>,
+    n_maps: u32, regions: &[ffi::kb200_remap_roi], dst: &mut CudaSlice<f32>,
+) -> Result<(), Kb200Error> {
+    bind(stream.context())?;
+    let mut guards = Vec::with_capacity(frames.len());
+    let mut ptrs: Vec<*const u8> = Vec::with_capacity(frames.len());
+    let lens: Vec<usize> = frames.iter().map(|f| f.len()).collect();
+    for f in frames {
+        let (p, g) = f.device_ptr(stream);
+        ptrs.push(p as *const u8);
+        guards.push(g);
+    }
+    let map_len = map_x.len().min(map_y.len());
+    let (mx, _gx) = map_x.device_ptr(stream);
+    let (my, _gy) = map_y.device_ptr(stream);
+    let dst_len = dst.len();
+    let (dp, _g1) = dst.device_ptr_mut(stream);
+    check(unsafe {
+        ffi::kb200_preprocess_remap(stream.cu_stream() as *mut c_void, desc, ptrs.as_ptr(), lens.as_ptr(), frames.len() as u32, mx as *const f32,
+                                    my as *const f32, map_len, n_maps, regions.as_ptr(), regions.len() as u32, dp as *mut c_void, dst_len, 0)
     })
 }
 

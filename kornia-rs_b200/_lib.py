@@ -39,6 +39,11 @@ class WarpRoi(C.Structure):
     _fields_ = [("frame", C.c_int32), ("m", C.c_float * 9)]
 
 
+class RemapRoi(C.Structure):
+    """kb200_remap_roi: frame `frame` resampled through map `map` of the call's map arrays"""
+    _fields_ = [("frame", C.c_int32), ("map", C.c_int32)]
+
+
 _lib = None
 _tls = threading.local()
 
@@ -62,6 +67,7 @@ def _declare(l: C.CDLL) -> None:
         "kb200_resize_lanczos_scratch_len": ([u32, u32, u32, u32], sz),
         "kb200_resize_lanczos_f32_c3": ([vp, vp, sz, vp, sz, vp, sz, u32, u32, u32, u32, u32], i),
         "kb200_generate_correction_map_polynomial": ([vp, C.POINTER(C.c_double), C.POINTER(C.c_double), u32, u32, vp, vp, sz], i),
+        "kb200_generate_correction_map_polynomial_to": ([vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double), u32, u32, vp, vp, sz], i),
         "kb200_fused_pipeline_u8_f32": ([vp, vp, sz, vp, sz, u32, u32, u32, u32, u32, i, fp, fp, i], i),
         "kb200_pyrdown_f32": ([vp, vp, sz, vp, sz, u32, u32, u32, u32], i),
         "kb200_pyrup_f32": ([vp, vp, sz, vp, sz, u32, u32, u32, u32], i),
@@ -135,6 +141,8 @@ def _declare(l: C.CDLL) -> None:
         "kb200_preprocess_host_format": ([vp, vp, C.POINTER(PreprocessDesc), vp, sz, sz, u32, vp, sz, i], i),
         "kb200_preprocess_rois": ([vp, C.POINTER(PreprocessDesc), i, C.POINTER(vp), C.POINTER(sz), u32, C.POINTER(Roi), u32, vp, sz, i], i),
         "kb200_preprocess_warps": ([vp, C.POINTER(PreprocessDesc), C.POINTER(vp), C.POINTER(sz), u32, C.POINTER(WarpRoi), u32, vp, sz, i], i),
+        "kb200_preprocess_remap": ([vp, C.POINTER(PreprocessDesc), C.POINTER(vp), C.POINTER(sz), u32, vp, vp, sz, u32, C.POINTER(RemapRoi), u32, vp, sz, i],
+                                   i),
     }
     for name, (args, res) in sig.items():
         fn = getattr(l, name)  # AttributeError if the symbol is missing: fail loudly

@@ -11,7 +11,9 @@
 
 namespace kb200 {
 
-struct DistortArgs { double intr[4]; double dist[8]; };
+// intr: the camera the map distorts with (fx, fy, cx, cy); out: the camera of the output pixels (fx', fy', cx', cy'), intr
+// itself for the reference's map.
+struct DistortArgs { double intr[4]; double dist[8]; double out[4]; };
 
 __global__ void __launch_bounds__(256) correction_map_kernel(float* __restrict__ map_x, float* __restrict__ map_y, uint32_t w, uint32_t h,
                                                              const __grid_constant__ DistortArgs A) {
@@ -19,8 +21,8 @@ __global__ void __launch_bounds__(256) correction_map_kernel(float* __restrict__
     if (px >= w || py >= h) return;
     const double fx = A.intr[0], fy = A.intr[1], cx = A.intr[2], cy = A.intr[3];
     const double k1 = A.dist[0], k2 = A.dist[1], k3 = A.dist[2], k4 = A.dist[3], k5 = A.dist[4], k6 = A.dist[5], p1 = A.dist[6], p2 = A.dist[7];
-    const double x = __ddiv_rn((double)px - cx, fx);
-    const double y = __ddiv_rn((double)py - cy, fy);
+    const double x = __ddiv_rn((double)px - A.out[2], A.out[0]);
+    const double y = __ddiv_rn((double)py - A.out[3], A.out[1]);
     const double r2 = x * x + y * y;
     const double r4 = r2 * r2;
     const double r6 = r4 * r2;
@@ -40,17 +42,24 @@ using namespace kb200;
 
 extern "C" {
 
-KB200_API int kb200_generate_correction_map_polynomial(kb200_stream_t stream, const double intrinsic[4], const double distortion[8], uint32_t width,
-                                                       uint32_t height, float* map_x, float* map_y, size_t map_len) {
-    KB200_TRY(check_ptr("intrinsic", intrinsic)); KB200_TRY(check_ptr("distortion", distortion));
+KB200_API int kb200_generate_correction_map_polynomial_to(kb200_stream_t stream, const double intrinsic[4], const double distortion[8],
+                                                          const double new_intrinsic[4], uint32_t width, uint32_t height, float* map_x,
+                                                          float* map_y, size_t map_len) {
+    KB200_TRY(check_ptr("intrinsic", intrinsic)); KB200_TRY(check_ptr("distortion", distortion)); KB200_TRY(check_ptr("new_intrinsic", new_intrinsic));
     KB200_TRY(check_ptr("map_x", map_x)); KB200_TRY(check_ptr("map_y", map_y));
     if (width == 0 || height == 0) return fail(KB200_ERR_INVALID_ARGUMENT, "image dimensions must be non-zero");
     KB200_TRY(check_slice("map", map_len, (size_t)width * height));
     DistortArgs A;
     for (int i = 0; i < 4; ++i) A.intr[i] = intrinsic[i];
     for (int i = 0; i < 8; ++i) A.dist[i] = distortion[i];
+    for (int i = 0; i < 4; ++i) A.out[i] = new_intrinsic[i];
     correction_map_kernel<<<dim3(div_up(width, 32), div_up(height, 8)), dim3(32, 8), 0, as_stream(stream)>>>(map_x, map_y, width, height, A);
     return check_launch("correction_map_kernel");
+}
+
+KB200_API int kb200_generate_correction_map_polynomial(kb200_stream_t stream, const double intrinsic[4], const double distortion[8], uint32_t width,
+                                                       uint32_t height, float* map_x, float* map_y, size_t map_len) {
+    return kb200_generate_correction_map_polynomial_to(stream, intrinsic, distortion, intrinsic, width, height, map_x, map_y, map_len);
 }
 
 }  // extern "C"

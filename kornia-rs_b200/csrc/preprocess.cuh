@@ -209,6 +209,21 @@ struct FrameGeom {
     __device__ __forceinline__ GeomRow row(int oy) const { return {sy(oy), rows, 0}; }
 };
 
+// One output pixel's sample point as a geometry for generic_pixel, which then samples and normalises it exactly as it does
+// a pixel of a whole frame: the caller's frame coordinate, or (-1, -1) when the caller found it outside, so that
+// generic_pixel's inside test (0 <= s < extent) agrees with the caller's; the extent is the frame's and the origin 0.
+// generic_pixel's ox / oy arguments are not read.  The warp and remap region entries sample through it.
+struct WarpPoint {
+    float x, y;
+    int fw, fh;
+    __device__ __forceinline__ float sx(int) const { return x; }
+    __device__ __forceinline__ float sy(int) const { return y; }
+    __device__ __forceinline__ int w() const { return fw; }
+    __device__ __forceinline__ int h() const { return fh; }
+    __device__ __forceinline__ int x0() const { return 0; }
+    __device__ __forceinline__ int y0() const { return 0; }
+};
+
 // Output pixel (ox, oy) of the rectangle g of the frame at src, sampled with SAMP (kb200_interp — 0 nearest, 1 bilinear,
 // 3 Lanczos-3: 6x6 taps, clamp-to-edge, weights renormalised by their sum) and normalised into o.
 template <int SAMP, int TAP, class G>

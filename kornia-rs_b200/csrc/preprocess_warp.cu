@@ -36,25 +36,11 @@ static_assert(sizeof(PreWarp) == 48, "PreWarp is 48 bytes");
 static_assert(sizeof(kb200_preprocess_desc) + sizeof(PreWarps) + sizeof(SrcFormat) + sizeof(Yuv16Coeffs) + 16 <= 4096,
               "the warp kernels' parameters must fit the classic 4 KB parameter block");
 
-// One output pixel's sample point as a geometry for generic_pixel (preprocess.cuh), which then samples and normalises it
-// exactly as it does a pixel of a whole frame: the coordinate warp_coord gave it, or (-1, -1) when warp_coord found it
-// outside, so that generic_pixel's inside test (0 <= s < extent) agrees with warp_coord's; the extent is the frame's and
-// the origin 0.  generic_pixel's ox / oy arguments are not read.
-struct WarpPoint {
-    float x, y;
-    int fw, fh;
-    __device__ __forceinline__ float sx(int) const { return x; }
-    __device__ __forceinline__ float sy(int) const { return y; }
-    __device__ __forceinline__ int w() const { return fw; }
-    __device__ __forceinline__ int h() const { return fh; }
-    __device__ __forceinline__ int x0() const { return 0; }
-    __device__ __forceinline__ int y0() const { return 0; }
-};
-
 // The largest float below the positive integer n.
 __device__ __forceinline__ float below(int n) { return __int_as_float(__float_as_int((float)n) - 1); }
 
-// Output pixel (ox, oy) of region r, normalised into o.  warp_coord's degenerate-axis rule judges an axis whose step is
+// Output pixel (ox, oy) of region r, normalised into o, sampled through WarpPoint (preprocess.cuh) at the coordinate
+// warp_coord gives it.  warp_coord's degenerate-axis rule judges an axis whose step is
 // below 1e-6 on its row constant, so an inside coordinate can sit a hair outside [0, src_w) x [0, src_h); it is clamped
 // into [0, below(src_w)] x [0, below(src_h)] before sampling, which leaves every other inside coordinate as it is.  The
 // clamped value samples what its nearest frame pixel holds: x0 = x1 = W - 1 above W - 1, and nearest rounds it to W - 1.

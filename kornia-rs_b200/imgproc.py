@@ -12,7 +12,7 @@ from __future__ import annotations
 
 import ctypes as C
 import enum
-from typing import Sequence
+from typing import Optional, Sequence
 
 import torch
 
@@ -863,18 +863,26 @@ def build_pyramid(src: Image, max_level: int) -> list[Image]:
 
 
 # ── calibration: undistort maps (calibration/distortion.rs) ──────────────────
-def generate_correction_map_polynomial(intrinsic: Sequence[float], distortion: Sequence[float], size: ImageSize, device) -> tuple[Image, Image]:
+def generate_correction_map_polynomial(intrinsic: Sequence[float], distortion: Sequence[float], size: ImageSize, device,
+                                       new_intrinsic: Optional[Sequence[float]] = None) -> tuple[Image, Image]:
     """calibration/distortion.rs:135 — (map_x, map_y), each an H x W x 1 f32 device Image, for `remap`: the distorted source
     coordinate of every destination pixel under the polynomial (Brown-Conrady rational) model.  `intrinsic` = (fx, fy, cx,
     cy) of CameraIntrinsic, `distortion` = (k1, k2, k3, k4, k5, k6, p1, p2) of PolynomialDistortion.  Generated on the
-    device — the reference builds the maps on the host and uploads them."""
-    if len(intrinsic) != 4 or len(distortion) != 8:
-        raise ValueError("intrinsic = (fx, fy, cx, cy), distortion = (k1..k6, p1, p2)")
+    device — the reference builds the maps on the host and uploads them.  `new_intrinsic` = (fx', fy', cx', cy'), cv2's
+    newCameraMatrix: the camera of the output pixels, so that `size` can be the output's own (a 640 x 640 model input of a
+    1080p camera); None uses `intrinsic`, the reference's map."""
+    if len(intrinsic) != 4 or len(distortion) != 8 or (new_intrinsic is not None and len(new_intrinsic) != 4):
+        raise ValueError("intrinsic = (fx, fy, cx, cy), distortion = (k1..k6, p1, p2), new_intrinsic = (fx, fy, cx, cy) or None")
     dev = torch.device(device)
     _lib.set_device(dev.index if dev.index is not None else torch.cuda.current_device())
     mx = Image.zeros_cuda(size, 1, torch.float32, dev)
     my = Image.zeros_cuda(size, 1, torch.float32, dev)
-    _check(_lib.lib().kb200_generate_correction_map_polynomial(_stream(dev), (C.c_double * 4)(*[float(v) for v in intrinsic]),
-                                                              (C.c_double * 8)(*[float(v) for v in distortion]), size.width, size.height,
-                                                              mx.data.data_ptr(), my.data.data_ptr(), mx.numel()))
+    intr = (C.c_double * 4)(*[float(v) for v in intrinsic])
+    dist = (C.c_double * 8)(*[float(v) for v in distortion])
+    if new_intrinsic is None:
+        _check(_lib.lib().kb200_generate_correction_map_polynomial(_stream(dev), intr, dist, size.width, size.height, mx.data.data_ptr(),
+                                                                  my.data.data_ptr(), mx.numel()))
+    else:
+        _check(_lib.lib().kb200_generate_correction_map_polynomial_to(_stream(dev), intr, dist, (C.c_double * 4)(*[float(v) for v in new_intrinsic]),
+                                                                     size.width, size.height, mx.data.data_ptr(), my.data.data_ptr(), mx.numel()))
     return mx, my

@@ -707,3 +707,87 @@ class Preprocessor:
                 raise PreprocessError("InvalidWarp", msg, region=int(msg.split(":")[0].split()[1]))
             kind = {_lib.ERR_INVALID_SOURCE: "InvalidRawSource", _lib.ERR_DIMS_TOO_LARGE: "DimensionsTooLarge"}.get(st, "Cuda")
             raise PreprocessError(kind, ("CUDA error: " if kind == "Cuda" else "") + msg)
+
+    # ── dense coordinate maps ───────────────────────────────────────────────
+    @staticmethod
+    def _remap_map(name: str, m) -> torch.Tensor:
+        """A map argument of run_remap as a [K, H, W] tensor: a tensor [H, W] or [K, H, W], or an H x W x 1 Image."""
+        if isinstance(m, Image):
+            m = m.data
+            if m.dim() != 3 or m.shape[2] != 1:
+                raise PreprocessError("InvalidMap", f"{name} must be a one-channel H x W x 1 Image, got {list(m.shape)}")
+            m = m[..., 0]
+        if not isinstance(m, torch.Tensor):
+            raise PreprocessError("InvalidMap", f"{name} must be a device tensor or an Image, got {type(m).__name__}")
+        if m.dim() not in (2, 3) or m.numel() == 0:
+            raise PreprocessError("InvalidMap", f"{name} must be [H, W] or [K, H, W], got {list(m.shape)}")
+        if m.dtype != torch.float32 or not m.is_cuda or not m.is_contiguous():
+            raise PreprocessError("InvalidMap", f"{name} must be a contiguous float32 device tensor, got {m.dtype} on {m.device}")
+        if m.data_ptr() % 4:
+            raise PreprocessError("InvalidMap", f"{name} must be 4-byte aligned")
+        return m if m.dim() == 3 else m.unsqueeze(0)
+
+    def run_remap(self, frames: Sequence[torch.Tensor], src_w: int, src_h: int, map_x, map_y, dst: torch.Tensor, regions=None) -> None:
+        """Raw device frames in the builder's SourceFormat resampled through dense coordinate maps (lens undistortion, rig
+        rectification, fisheye views): region i = (frame k, map j) writes dst[i], output pixel (x, y) sampled at frame
+        coordinate (map_x[j, y, x], map_y[j, y, x]) with the builder's sampling (Nearest or Bilinear), normalisation, pad
+        value and YUV matrix.  A coordinate outside [0, src_w) x [0, src_h) (NaN included) takes the pad value.  The
+        builder's mode does not apply: the map is the geometry.  `map_x` / `map_y`: contiguous float32 device tensors
+        [H, W] or [K, H, W] of the same shape, or the Images generate_correction_map_polynomial returns; H x W is dst's.
+        `regions`: a sequence of (frame, map) pairs or an integer CPU tensor [M, 2]; None is (i, 0) for every frame.
+        `dst`: a contiguous device [M, 3, H, W] tensor of torch.float32, torch.float16 or torch.bfloat16, which selects the
+        output.  A bad region raises PreprocessError("InvalidMap", region=i); a map of the wrong shape, dtype, device or
+        alignment raises "InvalidMap"; Lanczos sampling raises "UnsupportedSampling"."""
+        if self._sampling not in (InterpolationMode.Nearest, InterpolationMode.Bilinear):
+            raise PreprocessError("UnsupportedSampling", f"unsupported sampling mode {self._sampling!r} for remapped regions (expected Nearest or Bilinear)")
+        mx, my = self._remap_map("map_x", map_x), self._remap_map("map_y", map_y)
+        if mx.shape != my.shape or mx.device != my.device:
+            raise PreprocessError("InvalidMap", f"map_x {list(mx.shape)} on {mx.device} and map_y {list(my.shape)} on {my.device} differ")
+        k, mh, mw = mx.shape
+        if regions is None:
+            table = [(i, 0) for i in range(len(frames))]
+        elif isinstance(regions, torch.Tensor):
+            if (regions.is_cuda or regions.dim() != 2 or regions.shape[1] != 2 or regions.dtype.is_floating_point or regions.dtype.is_complex
+                    or regions.dtype == torch.bool):
+                raise PreprocessError("InvalidMap", f"regions must be an integer CPU tensor [M, 2], got {regions.dtype} {list(regions.shape)} on {regions.device}")
+            table = [(int(a), int(b)) for a, b in regions.tolist()]
+        else:
+            table = []
+            for i, q in enumerate(regions):
+                q = tuple(q) if isinstance(q, (tuple, list)) else None
+                if q is None or len(q) != 2 or not all(isinstance(v, int) and not isinstance(v, bool) for v in q):
+                    raise PreprocessError("InvalidMap", f"region {i}: expected a (frame, map) pair of integers", region=i)
+                table.append(q)
+        if not table:
+            raise PreprocessError("InvalidMap", "no regions given")
+        for i, (f, j) in enumerate(table):   # the C entry's region rules, checked here so that the kind is InvalidMap
+            if not 0 <= f < len(frames):
+                raise PreprocessError("InvalidMap", f"region {i}: frame index {f} is outside [0, {len(frames)})", region=i)
+            if not 0 <= j < k:
+                raise PreprocessError("InvalidMap", f"region {i}: map index {j} is outside [0, {k})", region=i)
+        if dst.dtype not in _OUT_DTYPES:
+            raise PreprocessError("BadOutputShape", f"unsupported output dtype {dst.dtype} (expected torch.float32, torch.float16 or torch.bfloat16)")
+        out = _OUT_DTYPES.index(dst.dtype)
+        self._validate_dst(dst, len(table), out)
+        if (dst.shape[2], dst.shape[3]) != (mh, mw):
+            raise PreprocessError("InvalidMap", f"the maps are {mh} x {mw} (H x W) but dst is {dst.shape[2]} x {dst.shape[3]}")
+        if mx.device != dst.device:
+            raise PreprocessError("InvalidMap", f"the maps are on {mx.device} but dst is on {dst.device}")
+        for f in frames:
+            self._validate_raw(f.numel() * f.element_size(), src_w, src_h)
+            if not f.is_cuda:
+                raise PreprocessError("NotDeviceImage", "CUDA preprocessor requires a device-resident source image")
+            if f.device != dst.device:
+                raise PreprocessError("Cuda", "CUDA error: source and destination are on different CUDA devices")
+        fmt = self._fmt
+        desc = self._desc(src_w, src_h, fmt.pitch(src_w), fmt.bpp(), fmt.fmt_code(), mw, mh)
+        n, m = len(frames), len(table)
+        ptrs = (C.c_void_p * max(n, 1))(*[f.data_ptr() for f in frames])
+        lens = (C.c_size_t * max(n, 1))(*[f.numel() * f.element_size() for f in frames])
+        rois = (_lib.RemapRoi * m)(*[_lib.RemapRoi(f, j) for f, j in table])
+        _lib.set_device(dst.device.index)
+        st = _lib.lib().kb200_preprocess_remap(torch.cuda.current_stream(dst.device).cuda_stream, C.byref(desc), ptrs, lens, n, mx.data_ptr(),
+                                               my.data_ptr(), mx.numel(), k, rois, m, dst.data_ptr(), dst.numel(), out)
+        if st != _lib.OK:
+            kind = {_lib.ERR_INVALID_SOURCE: "InvalidRawSource", _lib.ERR_DIMS_TOO_LARGE: "DimensionsTooLarge"}.get(st, "Cuda")
+            raise PreprocessError(kind, ("CUDA error: " if kind == "Cuda" else "") + _lib.last_error())
