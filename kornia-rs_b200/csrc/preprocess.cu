@@ -450,6 +450,28 @@ int check_frame_table(const kb200_preprocess_desc& d, const uint8_t* const* fram
     return KB200_OK;
 }
 
+int check_region_call(const kb200_preprocess_desc* desc, const int* mode, const char* point, int out_format, kb200_preprocess_desc* raw,
+                      kb200_preprocess_desc* plain) {
+    if (!desc) return fail(KB200_ERR_INVALID_ARGUMENT, "null preprocess descriptor");
+    *raw = *desc;   // each region gets its own geometry: the descriptor's scale and pad are not used
+    raw->scale_x = raw->scale_y = 1.0f;
+    raw->pad_x = raw->pad_y = 0.0f;
+    KB200_TRY(validate_desc(raw));
+    if (mode && *mode != 0 && *mode != 1) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown resize mode %d (expected 0 Letterbox or 1 Stretch)", *mode);
+    if (point && raw->sampling == KB200_INTERP_LANCZOS)
+        return fail(KB200_ERR_UNSUPPORTED, "unsupported sampling mode %d for %s (expected Nearest or Bilinear)", raw->sampling, point);
+    if (out_format != KB200_OUT_F32 && out_format != KB200_OUT_F16 && out_format != KB200_OUT_BF16)
+        return fail(KB200_ERR_INVALID_ARGUMENT, "unknown output format %d (expected 0 f32, 1 f16 or 2 bf16)", out_format);
+    *plain = plain_desc(*raw);
+    return KB200_OK;
+}
+
+int check_region_frame(uint32_t i, int32_t frame, uint32_t n_frames) {
+    if (frame < 0 || (uint32_t)frame >= n_frames)
+        return fail(KB200_ERR_INVALID_ARGUMENT, "region %u: frame index %d is outside [0, %u)", i, frame, n_frames);
+    return KB200_OK;
+}
+
 // The fast kernels of layout L (4:2:0, or YUV444) and sample type T, for one launch of <= 256 frames.
 template <int OUT, int L, typename T = uint8_t>
 static void launch_yuv_fast(cudaStream_t s, bool identity, bool bil, const kb200_preprocess_desc& d, const typename YuvSample<T>::Coeffs& yc,
@@ -565,11 +587,9 @@ int preprocess_validate(const kb200_preprocess_desc* desc) { return validate_des
 size_t preprocess_frame_bytes(const kb200_preprocess_desc& d) { return src_bytes(plain_desc(d)); }
 // out: a kb200_out_format the caller has checked
 int preprocess_launch_strided(cudaStream_t s, const kb200_preprocess_desc& desc, const uint8_t* base, size_t stride, uint32_t batch, void* dst, int out) {
-    const kb200_preprocess_desc d = plain_desc(desc);
-    const int m = yuv_matrix(desc);
-    if (out == KB200_OUT_F16) return launch_preprocess<KB200_OUT_F16>(s, d, m, nullptr, base, stride, batch, dst);
-    if (out == KB200_OUT_BF16) return launch_preprocess<KB200_OUT_BF16>(s, d, m, nullptr, base, stride, batch, dst);
-    return launch_preprocess<KB200_OUT_F32>(s, d, m, nullptr, base, stride, batch, dst);
+    return with_out_format(out, [&](auto o) {
+        return launch_preprocess<decltype(o)::value>(s, plain_desc(desc), yuv_matrix(desc), nullptr, base, stride, batch, dst);
+    });
 }
 
 template <int OUT>

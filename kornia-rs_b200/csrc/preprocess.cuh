@@ -1,8 +1,8 @@
-// preprocess.cuh — what the camera preprocess's two sources share: preprocess.cu (one affine per frame, the batch entries)
-// and preprocess_roi.cu (one affine per region of a frame, kb200_preprocess_rois): the source-format facts, the taps
+// preprocess.cuh — what the camera preprocess's sources share: preprocess.cu (one affine per frame, the batch entries)
+// and the region entries (preprocess_roi.cu, preprocess_warp.cu, preprocess_remap.cu): the source-format facts, the taps
 // (fetch_px), the Lanczos weight, the normalising divisions, the stores, the two sampler bodies over a frame's or a
-// region's geometry, the fast resampler's arguments and launch rule, the host rules of the descriptor and the
-// kernel-selection switches.  The arithmetic is documented in preprocess.cu's header.
+// region's geometry, the fast resampler's arguments and launch rule, the host rules of the descriptor and of a region
+// call, and the kernel-selection and output-format switches.  The arithmetic is documented in preprocess.cu's header.
 #pragma once
 
 #include <cuda_bf16.h>
@@ -435,6 +435,15 @@ int validate_desc(const kb200_preprocess_desc* dp);  // the raw descriptor an en
 // The checks of a table of n frame pointers (frame_len: their lengths, or nullptr): none null, every frame of 16-bit samples
 // 2-byte aligned, every length >= src_bytes(d).  d: a plain descriptor.
 int check_frame_table(const kb200_preprocess_desc& d, const uint8_t* const* frames, const size_t* frame_len, uint32_t n);
+// The checks a region entry (kb200_preprocess_rois, _warps, _remap) starts with, in this order: a descriptor is given; its
+// rules hold (validate_desc) with its scale and pad taken as the identity, since each region brings its own geometry; the
+// resize mode of the entry that takes one (mode; nullptr for the others) is known; a point-sampled entry refuses Lanczos
+// (point: the noun its message names the regions by, "warped regions"; nullptr: Lanczos is sampled); the output format
+// is known.  raw: that descriptor; plain: its plain_desc.
+int check_region_call(const kb200_preprocess_desc* desc, const int* mode, const char* point, int out_format, kb200_preprocess_desc* raw,
+                      kb200_preprocess_desc* plain);
+// The first rule of every region entry's per-region loop: region i's frame index names one of the n_frames frames.
+int check_region_frame(uint32_t i, int32_t frame, uint32_t n_frames);
 
 // Every frame of a call starts a-byte aligned: the n frames of the pointer table `frames`, or, when it is nullptr, the
 // frames at base + k * stride.
@@ -453,6 +462,13 @@ inline bool yuv_resampler_ok(const SrcFormat& f, const kb200_preprocess_desc& d,
     const bool pair_loads = f.family == SRC_YUV420 && !f.words && (f.layout == YUV420_NV12 || f.layout == YUV420_NV21);
     return d.sampling != KB200_INTERP_LANCZOS && f.fast_kernel && (d.dst_w % 4) == 0 && aligned16(dst) && d.dst_h <= 65535 * NV12_ROWS &&
            (!pair_loads || frames_even);
+}
+
+// Whether the warp and remap region kernels' 4-column stores (nv12_store4) can write dst in output format out: whole
+// 4-column groups and a destination 16-B (f32) / 8-B (f16, bf16) aligned.
+inline bool vector_dst_ok(const kb200_preprocess_desc& d, const void* dst, int out) {
+    const uintptr_t a = out == KB200_OUT_F32 ? 15u : 7u;
+    return d.dst_w % 4 == 0 && (reinterpret_cast<uintptr_t>(dst) & a) == 0;
 }
 
 // The Q16 coefficient set of a format of 16-bit YUV words (P01x, I01x, I41x) decoded with `matrix`.
@@ -495,6 +511,14 @@ void with_tap(const SrcFormat& f, const YuvCoeffs& yc, const Yuv16Coeffs& yc16, 
     } else {
         launch(IntC<TAP_RGB>{}, yc);
     }
+}
+
+// Returns launch(IntC<OUT>{}) for the kb200_out_format out, one the caller has checked.
+template <class Launch>
+int with_out_format(int out, Launch&& launch) {
+    if (out == KB200_OUT_F16) return launch(IntC<KB200_OUT_F16>{});
+    if (out == KB200_OUT_BF16) return launch(IntC<KB200_OUT_BF16>{});
+    return launch(IntC<KB200_OUT_F32>{});
 }
 
 // Calls launch(IntC<L>{}, T{}, coeffs) with the fast kernels' layout L (4:2:0, or YUV444) and sample type T for a format

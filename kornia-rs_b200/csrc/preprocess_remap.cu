@@ -87,20 +87,15 @@ __global__ void __launch_bounds__(256) preprocess_remap_generic_kernel(const __g
     generic_store<OUT>(dst, (size_t)(r0 + r) * 3 * pixels + i, pixels, o);
 }
 
-// The vector kernel's rule: whole 4-column groups, maps its float4 loads can address (every map then starts 16-B aligned
-// too: a map is dst_w * dst_h floats) and a destination its 16-B (f32) / 8-B (f16, bf16) stores can address.
-static bool remap_vector_ok(const kb200_preprocess_desc& d, const float* map_x, const float* map_y, const void* dst, int out_format) {
-    const uintptr_t a = out_format == KB200_OUT_F32 ? 15u : 7u;
-    return d.dst_w % 4 == 0 && aligned16(map_x) && aligned16(map_y) && (reinterpret_cast<uintptr_t>(dst) & a) == 0;
-}
-
 // d: a validated descriptor with the plain format code; frames, maps and regions: checked by the entry
 template <int OUT>
 static int launch_remap(cudaStream_t s, const kb200_preprocess_desc& d, int matrix, const uint8_t* const* frames, const float* map_x,
                         const float* map_y, const kb200_remap_roi* regions, uint32_t n_regions, void* dst) {
     const SrcFormat f = src_format(d.fmt);
     const bool bil = d.sampling == KB200_INTERP_BILINEAR;
-    const bool vec = remap_vector_ok(d, map_x, map_y, dst, OUT);
+    // the vector kernel's rule: its stores' (vector_dst_ok), and maps its float4 loads can address (every map then starts
+    // 16-B aligned too: a map is dst_w * dst_h floats)
+    const bool vec = vector_dst_ok(d, dst, OUT) && aligned16(map_x) && aligned16(map_y);
     const YuvCoeffs& yc = YUV_COEFFS[matrix];
     const Yuv16Coeffs yc16 = yuv16_coeffs_of(f, matrix);   // used by the 16-bit YUV formats only
     const size_t plane = (size_t)d.dst_w * d.dst_h;
@@ -137,15 +132,8 @@ extern "C" {
 KB200_API int kb200_preprocess_remap(kb200_stream_t stream, const kb200_preprocess_desc* desc, const uint8_t* const* frames, const size_t* frame_len,
                                      uint32_t n_frames, const float* map_x, const float* map_y, size_t map_len, uint32_t n_maps,
                                      const kb200_remap_roi* regions, uint32_t n_regions, void* dst, size_t dst_len, int out_format) {
-    if (!desc) return fail(KB200_ERR_INVALID_ARGUMENT, "null preprocess descriptor");
-    kb200_preprocess_desc raw = *desc;   // the map is the geometry: the descriptor's scale and pad are not used
-    raw.scale_x = raw.scale_y = 1.0f;
-    raw.pad_x = raw.pad_y = 0.0f;
-    KB200_TRY(validate_desc(&raw));
-    if (raw.sampling == KB200_INTERP_LANCZOS)
-        return fail(KB200_ERR_UNSUPPORTED, "unsupported sampling mode %d for remapped regions (expected Nearest or Bilinear)", raw.sampling);
-    if (out_format != KB200_OUT_F32 && out_format != KB200_OUT_F16 && out_format != KB200_OUT_BF16)
-        return fail(KB200_ERR_INVALID_ARGUMENT, "unknown output format %d (expected 0 f32, 1 f16 or 2 bf16)", out_format);
+    kb200_preprocess_desc raw, d;
+    KB200_TRY(check_region_call(desc, nullptr, "remapped regions", out_format, &raw, &d));
     KB200_TRY(check_ptr("frames", frames));
     KB200_TRY(check_ptr("regions", regions));
     KB200_TRY(check_ptr("map_x", map_x));
@@ -154,11 +142,9 @@ KB200_API int kb200_preprocess_remap(kb200_stream_t stream, const kb200_preproce
     if (n_regions == 0) return fail(KB200_ERR_INVALID_ARGUMENT, "n_regions must be non-zero");
     if (n_maps == 0) return fail(KB200_ERR_INVALID_ARGUMENT, "n_maps must be non-zero");
     if (!aligned4(map_x) || !aligned4(map_y)) return fail(KB200_ERR_INVALID_ARGUMENT, "map_x and map_y must be 4-byte aligned float arrays");
-    const kb200_preprocess_desc d = plain_desc(raw);
     for (uint32_t i = 0; i < n_regions; ++i) {
         const kb200_remap_roi& q = regions[i];
-        if (q.frame < 0 || (uint32_t)q.frame >= n_frames)
-            return fail(KB200_ERR_INVALID_ARGUMENT, "region %u: frame index %d is outside [0, %u)", i, q.frame, n_frames);
+        KB200_TRY(check_region_frame(i, q.frame, n_frames));
         if (q.map < 0 || (uint32_t)q.map >= n_maps)
             return fail(KB200_ERR_INVALID_ARGUMENT, "region %u: map index %d is outside [0, %u)", i, q.map, n_maps);
     }
@@ -166,11 +152,9 @@ KB200_API int kb200_preprocess_remap(kb200_stream_t stream, const kb200_preproce
     const size_t plane = (size_t)d.dst_w * d.dst_h;   // < 2^31 (validate_desc), so the products below fit 64 bits
     KB200_TRY(check_slice("map", map_len, (size_t)n_maps * plane));
     KB200_TRY(check_slice("dst", dst_len, (size_t)n_regions * 3 * plane));
-    const cudaStream_t s = as_stream(stream);
-    const int m = yuv_matrix(raw);
-    if (out_format == KB200_OUT_F16) return launch_remap<KB200_OUT_F16>(s, d, m, frames, map_x, map_y, regions, n_regions, dst);
-    if (out_format == KB200_OUT_BF16) return launch_remap<KB200_OUT_BF16>(s, d, m, frames, map_x, map_y, regions, n_regions, dst);
-    return launch_remap<KB200_OUT_F32>(s, d, m, frames, map_x, map_y, regions, n_regions, dst);
+    return with_out_format(out_format, [&](auto o) {
+        return launch_remap<decltype(o)::value>(as_stream(stream), d, yuv_matrix(raw), frames, map_x, map_y, regions, n_regions, dst);
+    });
 }
 
 }  // extern "C"

@@ -141,23 +141,15 @@ extern "C" {
 KB200_API int kb200_preprocess_rois(kb200_stream_t stream, const kb200_preprocess_desc* desc, int mode, const uint8_t* const* frames,
                                     const size_t* frame_len, uint32_t n_frames, const kb200_roi* rois, uint32_t n_rois, void* dst,
                                     size_t dst_len, int out_format) {
-    if (!desc) return fail(KB200_ERR_INVALID_ARGUMENT, "null preprocess descriptor");
-    kb200_preprocess_desc raw = *desc;   // each region gets its own affine: the descriptor's scale and pad are not used
-    raw.scale_x = raw.scale_y = 1.0f;
-    raw.pad_x = raw.pad_y = 0.0f;
-    KB200_TRY(validate_desc(&raw));
-    if (mode != 0 && mode != 1) return fail(KB200_ERR_INVALID_ARGUMENT, "unknown resize mode %d (expected 0 Letterbox or 1 Stretch)", mode);
-    if (out_format != KB200_OUT_F32 && out_format != KB200_OUT_F16 && out_format != KB200_OUT_BF16)
-        return fail(KB200_ERR_INVALID_ARGUMENT, "unknown output format %d (expected 0 f32, 1 f16 or 2 bf16)", out_format);
+    kb200_preprocess_desc raw, d;
+    KB200_TRY(check_region_call(desc, &mode, nullptr, out_format, &raw, &d));
     KB200_TRY(check_ptr("frames", frames));
     KB200_TRY(check_ptr("rois", rois));
     KB200_TRY(check_ptr("dst", dst));
     if (n_rois == 0) return fail(KB200_ERR_INVALID_ARGUMENT, "n_rois must be non-zero");
-    const kb200_preprocess_desc d = plain_desc(raw);
     for (uint32_t i = 0; i < n_rois; ++i) {
         const kb200_roi& q = rois[i];
-        if (q.frame < 0 || (uint32_t)q.frame >= n_frames)
-            return fail(KB200_ERR_INVALID_ARGUMENT, "region %u: frame index %d is outside [0, %u)", i, q.frame, n_frames);
+        KB200_TRY(check_region_frame(i, q.frame, n_frames));
         if (q.x < 0 || q.y < 0) return fail(KB200_ERR_INVALID_ARGUMENT, "region %u: origin (%d, %d) is negative", i, q.x, q.y);
         if (q.w < 1 || q.h < 1) return fail(KB200_ERR_INVALID_ARGUMENT, "region %u: size %dx%d is empty", i, q.w, q.h);
         if ((int64_t)q.x + q.w > d.src_w || (int64_t)q.y + q.h > d.src_h)
@@ -166,11 +158,9 @@ KB200_API int kb200_preprocess_rois(kb200_stream_t stream, const kb200_preproces
     }
     KB200_TRY(check_frame_table(d, frames, frame_len, n_frames));
     KB200_TRY(check_slice("dst", dst_len, (size_t)n_rois * 3 * d.dst_w * d.dst_h));
-    const cudaStream_t s = as_stream(stream);
-    const int m = yuv_matrix(raw);
-    if (out_format == KB200_OUT_F16) return launch_rois<KB200_OUT_F16>(s, d, m, mode, frames, n_frames, rois, n_rois, dst);
-    if (out_format == KB200_OUT_BF16) return launch_rois<KB200_OUT_BF16>(s, d, m, mode, frames, n_frames, rois, n_rois, dst);
-    return launch_rois<KB200_OUT_F32>(s, d, m, mode, frames, n_frames, rois, n_rois, dst);
+    return with_out_format(out_format, [&](auto o) {
+        return launch_rois<decltype(o)::value>(as_stream(stream), d, yuv_matrix(raw), mode, frames, n_frames, rois, n_rois, dst);
+    });
 }
 
 }  // extern "C"

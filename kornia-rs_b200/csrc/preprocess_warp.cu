@@ -113,19 +113,13 @@ static int invert_warp(uint32_t i, const kb200_warp_roi& q, float inv[9], bool* 
     return KB200_OK;
 }
 
-// The vector kernel's rule: whole 4-column groups and a destination its 16-B (f32) / 8-B (f16, bf16) stores can address.
-static bool warp_vector_ok(const kb200_preprocess_desc& d, const void* dst, int out_format) {
-    const uintptr_t a = out_format == KB200_OUT_F32 ? 15u : 7u;
-    return d.dst_w % 4 == 0 && (reinterpret_cast<uintptr_t>(dst) & a) == 0;
-}
-
 // d: a validated descriptor with the plain format code; frames and warps: checked by the entry
 template <int OUT>
 static int launch_warps(cudaStream_t s, const kb200_preprocess_desc& d, int matrix, const uint8_t* const* frames, const kb200_warp_roi* warps,
                         uint32_t n_warps, void* dst) {
     const SrcFormat f = src_format(d.fmt);
     const bool bil = d.sampling == KB200_INTERP_BILINEAR;
-    const bool vec = warp_vector_ok(d, dst, OUT);
+    const bool vec = vector_dst_ok(d, dst, OUT);
     const YuvCoeffs& yc = YUV_COEFFS[matrix];
     const Yuv16Coeffs yc16 = yuv16_coeffs_of(f, matrix);   // used by the 16-bit YUV formats only
     const size_t items = vec ? (size_t)(d.dst_w / 4) * d.dst_h : (size_t)d.dst_w * d.dst_h;
@@ -162,35 +156,23 @@ extern "C" {
 
 KB200_API int kb200_preprocess_warps(kb200_stream_t stream, const kb200_preprocess_desc* desc, const uint8_t* const* frames, const size_t* frame_len,
                                      uint32_t n_frames, const kb200_warp_roi* warps, uint32_t n_warps, void* dst, size_t dst_len, int out_format) {
-    if (!desc) return fail(KB200_ERR_INVALID_ARGUMENT, "null preprocess descriptor");
-    kb200_preprocess_desc raw = *desc;   // each region's map is its geometry: the descriptor's scale and pad are not used
-    raw.scale_x = raw.scale_y = 1.0f;
-    raw.pad_x = raw.pad_y = 0.0f;
-    KB200_TRY(validate_desc(&raw));
-    if (raw.sampling == KB200_INTERP_LANCZOS)
-        return fail(KB200_ERR_UNSUPPORTED, "unsupported sampling mode %d for warped regions (expected Nearest or Bilinear)", raw.sampling);
-    if (out_format != KB200_OUT_F32 && out_format != KB200_OUT_F16 && out_format != KB200_OUT_BF16)
-        return fail(KB200_ERR_INVALID_ARGUMENT, "unknown output format %d (expected 0 f32, 1 f16 or 2 bf16)", out_format);
+    kb200_preprocess_desc raw, d;
+    KB200_TRY(check_region_call(desc, nullptr, "warped regions", out_format, &raw, &d));
     KB200_TRY(check_ptr("frames", frames));
     KB200_TRY(check_ptr("warps", warps));
     KB200_TRY(check_ptr("dst", dst));
     if (n_warps == 0) return fail(KB200_ERR_INVALID_ARGUMENT, "n_warps must be non-zero");
-    const kb200_preprocess_desc d = plain_desc(raw);
     for (uint32_t i = 0; i < n_warps; ++i) {
-        const kb200_warp_roi& q = warps[i];
-        if (q.frame < 0 || (uint32_t)q.frame >= n_frames)
-            return fail(KB200_ERR_INVALID_ARGUMENT, "region %u: frame index %d is outside [0, %u)", i, q.frame, n_frames);
+        KB200_TRY(check_region_frame(i, warps[i].frame, n_frames));
         float inv[9];
         bool persp;
-        KB200_TRY(invert_warp(i, q, inv, &persp));
+        KB200_TRY(invert_warp(i, warps[i], inv, &persp));
     }
     KB200_TRY(check_frame_table(d, frames, frame_len, n_frames));
     KB200_TRY(check_slice("dst", dst_len, (size_t)n_warps * 3 * d.dst_w * d.dst_h));
-    const cudaStream_t s = as_stream(stream);
-    const int m = yuv_matrix(raw);
-    if (out_format == KB200_OUT_F16) return launch_warps<KB200_OUT_F16>(s, d, m, frames, warps, n_warps, dst);
-    if (out_format == KB200_OUT_BF16) return launch_warps<KB200_OUT_BF16>(s, d, m, frames, warps, n_warps, dst);
-    return launch_warps<KB200_OUT_F32>(s, d, m, frames, warps, n_warps, dst);
+    return with_out_format(out_format, [&](auto o) {
+        return launch_warps<decltype(o)::value>(as_stream(stream), d, yuv_matrix(raw), frames, warps, n_warps, dst);
+    });
 }
 
 }  // extern "C"

@@ -390,19 +390,27 @@ class Preprocessor:
             raise PreprocessError("BadOutputShape", f"destination tensor must be contiguous {want}, got {dst.dtype}")
 
     def _launch(self, desc, frames: Sequence[torch.Tensor], dst: torch.Tensor, out: int) -> None:
+        self._call(frames, dst, lambda s, ptrs, lens, n: getattr(_lib.lib(), _TABLE_ENTRIES[out])(
+            s, C.byref(desc), ptrs, lens, n, dst.data_ptr(), dst.numel()))
+
+    def _call(self, frames: Sequence[torch.Tensor], dst: torch.Tensor, entry, src_wh: tuple[int, int] | None = None) -> None:
+        """One call of a frame-table entry: each frame is checked (its raw size against src_wh = (src_w, src_h) when given,
+        then that it is on dst's device), entry(stream, frame pointers, frame lengths, frame count) runs on the current
+        stream of dst's device, and a status other than OK is raised.  The region entries build their descriptor inside
+        `entry`, so that its DimensionsTooLarge comes after the frame checks."""
         dev = dst.device
         for f in frames:
+            if src_wh:
+                self._validate_raw(f.numel() * f.element_size(), *src_wh)
             if not f.is_cuda:
                 raise PreprocessError("NotDeviceImage", "CUDA preprocessor requires a device-resident source image")
             if f.device != dev:
                 raise PreprocessError("Cuda", "CUDA error: source and destination are on different CUDA devices")
         _lib.set_device(dev.index)
         n = len(frames)
-        ptrs = (C.c_void_p * n)(*[f.data_ptr() for f in frames])
-        lens = (C.c_size_t * n)(*[f.numel() * f.element_size() for f in frames])
-        l = _lib.lib()
-        fn = getattr(l, _TABLE_ENTRIES[out])
-        st = fn(torch.cuda.current_stream(dev).cuda_stream, C.byref(desc), ptrs, lens, n, dst.data_ptr(), dst.numel())
+        ptrs = (C.c_void_p * max(n, 1))(*[f.data_ptr() for f in frames])
+        lens = (C.c_size_t * max(n, 1))(*[f.numel() * f.element_size() for f in frames])
+        st = entry(torch.cuda.current_stream(dev).cuda_stream, ptrs, lens, n)
         if st != _lib.OK:
             kind = {_lib.ERR_INVALID_SOURCE: "InvalidRawSource", _lib.ERR_DIMS_TOO_LARGE: "DimensionsTooLarge"}.get(st, "Cuda")
             raise PreprocessError(kind, ("CUDA error: " if kind == "Cuda" else "") + _lib.last_error())
@@ -607,28 +615,14 @@ class Preprocessor:
                 raise PreprocessError("InvalidRoi", f"region {i}: size {w}x{h} is empty", region=i)
             if x + w > src_w or y + h > src_h:
                 raise PreprocessError("InvalidRoi", f"region {i}: ({x}, {y}) + {w}x{h} reaches outside the {src_w}x{src_h} frame", region=i)
-        if dst.dtype not in _OUT_DTYPES:
-            raise PreprocessError("BadOutputShape", f"unsupported output dtype {dst.dtype} (expected torch.float32, torch.float16 or torch.bfloat16)")
-        out = _OUT_DTYPES.index(dst.dtype)
+        out = self._out_format(False, dst.dtype)
         self._validate_dst(dst, len(table), out)
-        for f in frames:
-            self._validate_raw(f.numel() * f.element_size(), src_w, src_h)
-            if not f.is_cuda:
-                raise PreprocessError("NotDeviceImage", "CUDA preprocessor requires a device-resident source image")
-            if f.device != dst.device:
-                raise PreprocessError("Cuda", "CUDA error: source and destination are on different CUDA devices")
-        fmt = self._fmt
-        desc = self._desc(src_w, src_h, fmt.pitch(src_w), fmt.bpp(), fmt.fmt_code(), dst.shape[3], dst.shape[2])
-        n, m = len(frames), len(table)
-        ptrs = (C.c_void_p * max(n, 1))(*[f.data_ptr() for f in frames])
-        lens = (C.c_size_t * max(n, 1))(*[f.numel() * f.element_size() for f in frames])
-        regions = (_lib.Roi * m)(*[_lib.Roi(*r) for r in table])
-        _lib.set_device(dst.device.index)
-        st = _lib.lib().kb200_preprocess_rois(torch.cuda.current_stream(dst.device).cuda_stream, C.byref(desc), self._mode.value, ptrs, lens, n,
-                                              regions, m, dst.data_ptr(), dst.numel(), out)
-        if st != _lib.OK:
-            kind = {_lib.ERR_INVALID_SOURCE: "InvalidRawSource", _lib.ERR_DIMS_TOO_LARGE: "DimensionsTooLarge"}.get(st, "Cuda")
-            raise PreprocessError(kind, ("CUDA error: " if kind == "Cuda" else "") + _lib.last_error())
+        regions = (_lib.Roi * len(table))(*[_lib.Roi(*r) for r in table])
+
+        def call(s, ptrs, lens, n):
+            desc = self._desc(src_w, src_h, self._fmt.pitch(src_w), self._fmt.bpp(), self._fmt.fmt_code(), dst.shape[3], dst.shape[2])
+            return _lib.lib().kb200_preprocess_rois(s, C.byref(desc), self._mode.value, ptrs, lens, n, regions, len(table), dst.data_ptr(), dst.numel(), out)
+        self._call(frames, dst, call, (src_w, src_h))
 
     # ── rotated and perspective regions ─────────────────────────────────────
     def run_warps(self, frames: Sequence[torch.Tensor], src_w: int, src_h: int, frame_index, matrices, dst: torch.Tensor) -> None:
@@ -682,31 +676,18 @@ class Preprocessor:
             if not all(math.isfinite(v) for v in flat):
                 raise PreprocessError("InvalidWarp", f"region {i}: the map has a non-finite entry", region=i)
             table.append((k, flat))
-        if dst.dtype not in _OUT_DTYPES:
-            raise PreprocessError("BadOutputShape", f"unsupported output dtype {dst.dtype} (expected torch.float32, torch.float16 or torch.bfloat16)")
-        out = _OUT_DTYPES.index(dst.dtype)
+        out = self._out_format(False, dst.dtype)
         self._validate_dst(dst, len(table), out)
-        for f in frames:
-            self._validate_raw(f.numel() * f.element_size(), src_w, src_h)
-            if not f.is_cuda:
-                raise PreprocessError("NotDeviceImage", "CUDA preprocessor requires a device-resident source image")
-            if f.device != dst.device:
-                raise PreprocessError("Cuda", "CUDA error: source and destination are on different CUDA devices")
-        fmt = self._fmt
-        desc = self._desc(src_w, src_h, fmt.pitch(src_w), fmt.bpp(), fmt.fmt_code(), dst.shape[3], dst.shape[2])
-        n, m = len(frames), len(table)
-        ptrs = (C.c_void_p * max(n, 1))(*[f.data_ptr() for f in frames])
-        lens = (C.c_size_t * max(n, 1))(*[f.numel() * f.element_size() for f in frames])
-        warps = (_lib.WarpRoi * m)(*[_lib.WarpRoi(k, (C.c_float * 9)(*flat)) for k, flat in table])
-        _lib.set_device(dst.device.index)
-        st = _lib.lib().kb200_preprocess_warps(torch.cuda.current_stream(dst.device).cuda_stream, C.byref(desc), ptrs, lens, n, warps, m,
-                                               dst.data_ptr(), dst.numel(), out)
-        if st != _lib.OK:
-            msg = _lib.last_error()
+        warps = (_lib.WarpRoi * len(table))(*[_lib.WarpRoi(k, (C.c_float * 9)(*flat)) for k, flat in table])
+
+        def call(s, ptrs, lens, n):
+            desc = self._desc(src_w, src_h, self._fmt.pitch(src_w), self._fmt.bpp(), self._fmt.fmt_code(), dst.shape[3], dst.shape[2])
+            st = _lib.lib().kb200_preprocess_warps(s, C.byref(desc), ptrs, lens, n, warps, len(table), dst.data_ptr(), dst.numel(), out)
             if st == _lib.ERR_SINGULAR_MATRIX:   # "region <i>: ..." (preprocess_warp.cu invert_warp)
+                msg = _lib.last_error()
                 raise PreprocessError("InvalidWarp", msg, region=int(msg.split(":")[0].split()[1]))
-            kind = {_lib.ERR_INVALID_SOURCE: "InvalidRawSource", _lib.ERR_DIMS_TOO_LARGE: "DimensionsTooLarge"}.get(st, "Cuda")
-            raise PreprocessError(kind, ("CUDA error: " if kind == "Cuda" else "") + msg)
+            return st
+        self._call(frames, dst, call, (src_w, src_h))
 
     # ── dense coordinate maps ───────────────────────────────────────────────
     @staticmethod
@@ -765,29 +746,16 @@ class Preprocessor:
                 raise PreprocessError("InvalidMap", f"region {i}: frame index {f} is outside [0, {len(frames)})", region=i)
             if not 0 <= j < k:
                 raise PreprocessError("InvalidMap", f"region {i}: map index {j} is outside [0, {k})", region=i)
-        if dst.dtype not in _OUT_DTYPES:
-            raise PreprocessError("BadOutputShape", f"unsupported output dtype {dst.dtype} (expected torch.float32, torch.float16 or torch.bfloat16)")
-        out = _OUT_DTYPES.index(dst.dtype)
+        out = self._out_format(False, dst.dtype)
         self._validate_dst(dst, len(table), out)
         if (dst.shape[2], dst.shape[3]) != (mh, mw):
             raise PreprocessError("InvalidMap", f"the maps are {mh} x {mw} (H x W) but dst is {dst.shape[2]} x {dst.shape[3]}")
         if mx.device != dst.device:
             raise PreprocessError("InvalidMap", f"the maps are on {mx.device} but dst is on {dst.device}")
-        for f in frames:
-            self._validate_raw(f.numel() * f.element_size(), src_w, src_h)
-            if not f.is_cuda:
-                raise PreprocessError("NotDeviceImage", "CUDA preprocessor requires a device-resident source image")
-            if f.device != dst.device:
-                raise PreprocessError("Cuda", "CUDA error: source and destination are on different CUDA devices")
-        fmt = self._fmt
-        desc = self._desc(src_w, src_h, fmt.pitch(src_w), fmt.bpp(), fmt.fmt_code(), mw, mh)
-        n, m = len(frames), len(table)
-        ptrs = (C.c_void_p * max(n, 1))(*[f.data_ptr() for f in frames])
-        lens = (C.c_size_t * max(n, 1))(*[f.numel() * f.element_size() for f in frames])
-        rois = (_lib.RemapRoi * m)(*[_lib.RemapRoi(f, j) for f, j in table])
-        _lib.set_device(dst.device.index)
-        st = _lib.lib().kb200_preprocess_remap(torch.cuda.current_stream(dst.device).cuda_stream, C.byref(desc), ptrs, lens, n, mx.data_ptr(),
-                                               my.data_ptr(), mx.numel(), k, rois, m, dst.data_ptr(), dst.numel(), out)
-        if st != _lib.OK:
-            kind = {_lib.ERR_INVALID_SOURCE: "InvalidRawSource", _lib.ERR_DIMS_TOO_LARGE: "DimensionsTooLarge"}.get(st, "Cuda")
-            raise PreprocessError(kind, ("CUDA error: " if kind == "Cuda" else "") + _lib.last_error())
+        rois = (_lib.RemapRoi * len(table))(*[_lib.RemapRoi(f, j) for f, j in table])
+
+        def call(s, ptrs, lens, n):
+            desc = self._desc(src_w, src_h, self._fmt.pitch(src_w), self._fmt.bpp(), self._fmt.fmt_code(), mw, mh)
+            return _lib.lib().kb200_preprocess_remap(s, C.byref(desc), ptrs, lens, n, mx.data_ptr(), my.data_ptr(), mx.numel(), k, rois, len(table),
+                                                     dst.data_ptr(), dst.numel(), out)
+        self._call(frames, dst, call, (src_w, src_h))
