@@ -13,42 +13,15 @@ import numpy as np
 import pytest
 import torch
 
+from harness import dev, make_pre, offset_buf, oracle_cfg, raw_bytes
+from restate import PATTERNS, PATTERN_CODE, demosaic
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
-
-PATTERNS = ("RGGB", "BGGR", "GRBG", "GBRG")
-CODE = {p: i for i, p in enumerate(PATTERNS)}                  # kb200_bayer_pattern
-R_AT = {"RGGB": (0, 0), "BGGR": (1, 1), "GRBG": (1, 0), "GBRG": (0, 1)}   # (column, row) parity of the R site
 
 
 def fmt_name(pattern):
     return "Bayer" + pattern.capitalize()
-
-
-# ── the restatement: numpy arrays or torch tensors [..., h, w] uint8 -> [..., h, w, 3] uint8 ──
-def demosaic(raw, pattern):
-    is_t = isinstance(raw, torch.Tensor)
-    h, w = raw.shape[-2:]
-    p = raw.to(torch.int32) if is_t else raw.astype(np.int32)
-    rx, ry = R_AT[pattern]
-    ar = (lambda n: torch.arange(n, device=raw.device)) if is_t else np.arange
-    cx, cy = ar(w).clip(1, w - 2), ar(h).clip(1, h - 2)
-
-    def at(dy, dx):
-        return p[..., cy + dy, :][..., cx + dx]
-
-    c, n, s, wv, e = at(0, 0), at(-1, 0), at(1, 0), at(0, -1), at(0, 1)
-    d = at(-1, -1) + at(-1, 1) + at(1, -1) + at(1, 1)
-    g4, d4, h2, v2 = (n + s + wv + e + 2) >> 2, (d + 2) >> 2, (wv + e + 1) >> 1, (n + s + 1) >> 1
-    px, py = (cx & 1)[None, :], (cy & 1)[:, None]
-    rsite, bsite = (px == rx) & (py == ry), (px != rx) & (py != ry)
-    grow = ~rsite & ~bsite & (py == ry)    # a G on an R row has R left and right
-    where = torch.where if is_t else np.where
-    r = where(rsite, c, where(bsite, d4, where(grow, h2, v2)))
-    b = where(bsite, c, where(rsite, d4, where(grow, v2, h2)))
-    g = where(rsite | bsite, g4, c)
-    out = (torch.stack if is_t else np.stack)([r, g, b], -1)
-    return out.to(torch.uint8) if is_t else out.astype(np.uint8)
 
 
 # ═══ CPU ═══════════════════════════════════════════════════════════════════════════════════════════════════════
@@ -87,7 +60,7 @@ def test_validation_without_a_gpu(kb):
     for bad in (-1, 4):
         assert l.kb200_rgb_from_bayer_u8(None, p, 4096, p, 4096, 4, 4, 1, bad) == _lib.ERR_INVALID_ARGUMENT
         assert _lib.last_error() == f"unknown Bayer pattern {bad}"
-    for p_name, code in CODE.items():
+    for p_name, code in PATTERN_CODE.items():
         for w, h in ((2, 7), (7, 2), (2, 2)):
             assert l.kb200_rgb_from_bayer_u8(None, p, 4096, p, 4096, w, h, 1, code) == _lib.ERR_INVALID_ARGUMENT
             assert _lib.last_error() == f"Bayer {p_name} needs at least 3x3 pixels, got {w}x{h}"
@@ -120,19 +93,8 @@ def test_validation_without_a_gpu(kb):
 
 
 # ═══ GPU ═══════════════════════════════════════════════════════════════════════════════════════════════════════
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-def offset_u8(dev, n, off):
-    """A u8 device buffer of n bytes whose data pointer is `off` bytes past the start of a fresh (aligned) allocation."""
-    return torch.empty(n + off, dtype=torch.uint8, device=dev)[off:]
-
-
 def run_decode(kb, dev, pattern, raw_dev, w, h, n, dst_off=0):
-    out = offset_u8(dev, n * h * w * 3, dst_off)
+    out = offset_buf(dev, n * h * w * 3, dst_off, torch.uint8)
     out.fill_(0xCD)
     kb.imgproc.rgb_from_bayer(raw_dev, kb.Image(out.view(n, h, w, 3)), kb.imgproc.BayerPattern[pattern])
     return out.view(n, h, w, 3), kb._lib.last_kernel()
@@ -150,8 +112,8 @@ DECODE_CASES = [(p, c) for p in PATTERNS for c in CASES]
 @pytest.mark.parametrize("pattern,case", DECODE_CASES, ids=[f"{p}-{'x'.join(map(str, c))}" for p, c in DECODE_CASES])
 def test_decode_bayer(kb, dev, pattern, case):
     w, h, n, soff, doff = case
-    raws = np.random.default_rng(w * 7919 + h * 31 + n + 1000 * CODE[pattern]).integers(0, 256, (n, h, w), dtype=np.uint8)
-    src = offset_u8(dev, n * w * h, soff)
+    raws = np.random.default_rng(w * 7919 + h * 31 + n + 1000 * PATTERN_CODE[pattern]).integers(0, 256, (n, h, w), dtype=np.uint8)
+    src = offset_buf(dev, n * w * h, soff, torch.uint8)
     src.copy_(torch.from_numpy(raws.reshape(-1)))
     got, kern = run_decode(kb, dev, pattern, src.view(n, w * h), w, h, n, doff)
     vec = w % 16 == 0 and soff % 16 == 0 and doff % 16 == 0
@@ -165,7 +127,7 @@ def test_decode_bayer(kb, dev, pattern, case):
 @pytest.mark.parametrize("pattern", PATTERNS)
 def test_decode_bayer_1080p_batch(kb, dev, pattern):
     w, h, n = 1920, 1080, 256
-    g = torch.Generator(device=dev).manual_seed(0x1080 + CODE[pattern])
+    g = torch.Generator(device=dev).manual_seed(0x1080 + PATTERN_CODE[pattern])
     raw = torch.randint(0, 256, (n, h * w), dtype=torch.uint8, device=dev, generator=g)
     got, kern = run_decode(kb, dev, pattern, raw, w, h, n)
     assert kern == f"rgb_from_bayer_{pattern.lower()}_vec16"
@@ -180,26 +142,10 @@ GEOMS = [(8, 6, 7, 5), (64, 48, 40, 40), (64, 48, 64, 48), (30, 20, 61, 47), (12
          (96, 54, 32, 32), (32, 24, 64, 48), (192, 108, 64, 36), (37, 21, 37, 21), (20, 3, 20, 3)]   # test_yuv_layouts' + odd sizes
 
 
-def raw_bytes(n, k=0):
-    return ((np.arange(n, dtype=np.int64) * 7 + 13) % 251 + 31 * k).astype(np.uint8)
-
-
 def expected_preprocess_kernel(pattern, sampling, w, h, dw, dh):
     if sampling != "Lanczos" and (dw, dh) == (w, h) and w % 4 == 0:
         return f"preprocess_bayer_{pattern.lower()}_identity_kernel"
     return "preprocess_generic_kernel"
-
-
-def make_pre(kb, fmt, mode, sampling):
-    return (kb.Preprocessor.builder().source_format(kb.SourceFormat[fmt]).mode(kb.ResizeMode[mode])
-            .sampling(kb.InterpolationMode[sampling]).normalize(kb.Normalize.imagenet()).pad_value(114).build_cuda())
-
-
-def oracle_rgb_cfg(kb, oracle, mode, sampling):
-    inv = tuple(float(np.float32(1.0) / np.float32(s)) for s in kb.IMAGENET_STD)
-    return oracle.PreprocessCfg(mode=oracle.LETTERBOX if mode == "Letterbox" else oracle.STRETCH, fmt=oracle.FMT_RGB,
-                                mean=kb.IMAGENET_MEAN, inv_std=inv, pad_value=114.0,
-                                sampling={"Bilinear": oracle.BILINEAR, "Nearest": oracle.NEAREST, "Lanczos": oracle.LANCZOS}[sampling])
 
 
 def device_twin(kb, dev, pattern, raw_dev, w, h):
@@ -218,11 +164,11 @@ def test_preprocess_bayer(kb, oracle, dev, pattern, mode, sampling, f16):
     """Every geometry: bit-equal to the device run on the RGB twin, with the kernel the dispatch promises; bit-equal to
     the oracle on the twin (Lanczos: within the tolerance of test_preprocess_lanczos_vs_oracle)."""
     pre, twin_pre = make_pre(kb, fmt_name(pattern), mode, sampling), make_pre(kb, "Rgb8", mode, sampling)
-    cfg = oracle_rgb_cfg(kb, oracle, mode, sampling)
+    cfg = oracle_cfg(kb, oracle, mode, sampling)
     dt, it = (torch.float16, torch.int16) if f16 else (torch.float32, torch.int32)
     for w, h, dw, dh in GEOMS:
         what = f"{pattern} {mode} {sampling} {'f16' if f16 else 'f32'} {(w, h, dw, dh)}"
-        raw = torch.from_numpy(raw_bytes(w * h, CODE[pattern])).to(dev)
+        raw = torch.from_numpy(raw_bytes(w * h, PATTERN_CODE[pattern])).to(dev)
         twin = device_twin(kb, dev, pattern, raw.view(1, -1), w, h)[0]
         np.testing.assert_array_equal(twin.cpu().numpy().reshape(h, w, 3), demosaic(raw.cpu().numpy().reshape(h, w), pattern))
         got = torch.full((1, 3, dh, dw), float("nan"), dtype=dt, device=dev)
@@ -250,7 +196,7 @@ def test_preprocess_bayer_identity_1080p(kb, oracle, dev, pattern, n):
     sides of the 256-frame launch split."""
     w, h = 1920, 1080
     nb = w * h
-    g = torch.Generator(device=dev).manual_seed(0x3A + CODE[pattern])
+    g = torch.Generator(device=dev).manual_seed(0x3A + PATTERN_CODE[pattern])
     ring = torch.randint(0, 256, (n, nb + 64), dtype=torch.uint8, device=dev, generator=g)   # padded strided slots
     frames = ring[:, :nb]
     twin = torch.cat([device_twin(kb, dev, pattern, frames[k0:k0 + 64].contiguous(), w, h) for k0 in range(0, n, 64)])
@@ -268,7 +214,7 @@ def test_preprocess_bayer_identity_1080p(kb, oracle, dev, pattern, n):
     pre.run_raw_strided(ring.view(-1), nb + 64, n, w, h, got)
     assert kb._lib.last_kernel() == kernel
     assert torch.equal(got.view(torch.int32), want.view(torch.int32))
-    cfg = oracle_rgb_cfg(kb, oracle, "Stretch", "Bilinear")
+    cfg = oracle_cfg(kb, oracle, "Stretch", "Bilinear")
     for k in sorted({0, 255, n - 1}):
         rgb = demosaic(frames[k].cpu().numpy().reshape(h, w), pattern)
         o = oracle.preprocess_frame(rgb, cfg, w, h, w, h)

@@ -13,111 +13,15 @@ import numpy as np
 import pytest
 import torch
 
+from harness import bayer16_identity, check_against_restatement, dev, make_pre, offset_buf, restated, to_dev16, to_np16
+from restate import DEPTHS, PATTERNS, PATTERN_CODE, demosaic, fmt_name
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 
-PATTERNS = ("RGGB", "BGGR", "GRBG", "GBRG")
-CODE = {p: i for i, p in enumerate(PATTERNS)}                  # kb200_bayer_pattern
-R_AT = {"RGGB": (0, 0), "BGGR": (1, 1), "GRBG": (1, 0), "GBRG": (0, 1)}   # (column, row) parity of the R site
-DEPTHS = (10, 12, 14, 16)
-
-
-def fmt_name(pattern, bits):
-    return f"Bayer{pattern.capitalize()}{bits}"
-
 
 def fmt_code(pattern, bits):
-    return 32 + 4 * DEPTHS.index(bits) + CODE[pattern]
-
-
-def white(bits):
-    return (1 << bits) - 1
-
-
-# ── the restatement: numpy arrays or torch tensors [..., h, w] uint16 -> [..., h, w, 3] uint16 ──
-# test_bayer.demosaic, generalised to 16-bit samples (int32 sums: 4 * 65535 + 2 does not fit 16 bits)
-def demosaic(raw, pattern):
-    is_t = isinstance(raw, torch.Tensor)
-    h, w = raw.shape[-2:]
-    p = raw.to(torch.int32) if is_t else raw.astype(np.int32)
-    rx, ry = R_AT[pattern]
-    ar = (lambda n: torch.arange(n, device=raw.device)) if is_t else np.arange
-    cx, cy = ar(w).clip(1, w - 2), ar(h).clip(1, h - 2)
-
-    def at(dy, dx):
-        return p[..., cy + dy, :][..., cx + dx]
-
-    c, n, s, wv, e = at(0, 0), at(-1, 0), at(1, 0), at(0, -1), at(0, 1)
-    d = at(-1, -1) + at(-1, 1) + at(1, -1) + at(1, 1)
-    g4, d4, h2, v2 = (n + s + wv + e + 2) >> 2, (d + 2) >> 2, (wv + e + 1) >> 1, (n + s + 1) >> 1
-    px, py = (cx & 1)[None, :], (cy & 1)[:, None]
-    rsite, bsite = (px == rx) & (py == ry), (px != rx) & (py != ry)
-    grow = ~rsite & ~bsite & (py == ry)    # a G on an R row has R left and right
-    where = torch.where if is_t else np.where
-    r = where(rsite, c, where(bsite, d4, where(grow, h2, v2)))
-    b = where(bsite, c, where(rsite, d4, where(grow, v2, h2)))
-    g = where(rsite | bsite, g4, c)
-    out = (torch.stack if is_t else np.stack)([r, g, b], -1)
-    return out.to(torch.uint16) if is_t else out.astype(np.uint16)
-
-
-# ── the oracle's ko_preprocess_frame restated for interleaved 16-bit RGB with a white level ──
-# Op for op in f32 (numpy rounds every operation; nothing is fused): plan_pixel, the three samplers, then
-# o = (px / W - mean) * inv_std inside the content, (pad / 255 - mean) * inv_std on the pad.
-F32 = np.float32
-
-
-def _lanczos_w(dd):
-    ad = np.abs(dd)
-    pd = F32(3.14159265358979) * dd
-    with np.errstate(divide="ignore", invalid="ignore"):
-        v = F32(3.0) * np.sin(pd) * np.sin(pd / F32(3.0)) / (pd * pd)
-    return np.where(ad < F32(1e-6), F32(1.0), np.where(ad >= F32(3.0), F32(0.0), v)).astype(F32)
-
-
-def preprocess_rgb16(rgb, bits, affine, dw, dh, sampling, mean, inv_std, pad_value, f16=False):
-    """rgb: (h, w, 3) uint16 -> (3, dh, dw) f32 (or f16 bits rounded to nearest even)."""
-    h, w = rgb.shape[:2]
-    sxs, sys_, padx, pady = (F32(v) for v in affine)
-    src = rgb.astype(F32)
-    sx = np.broadcast_to((np.arange(dw, dtype=F32) - padx) / sxs, (dh, dw))
-    sy = np.broadcast_to(((np.arange(dh, dtype=F32) - pady) / sys_)[:, None], (dh, dw))
-    inside = ~((sx < 0) | (sy < 0) | (sx >= F32(w)) | (sy >= F32(h)))
-
-    def tap(yi, xi):
-        return src[np.clip(yi, 0, h - 1), np.clip(xi, 0, w - 1)]
-
-    if sampling == "Nearest":
-        def roundf(v):
-            f = np.floor(v)
-            return (f + (v - f >= F32(0.5))).astype(np.int64)
-        px = tap(np.clip(roundf(sy), 0, h - 1), np.clip(roundf(sx), 0, w - 1))
-    elif sampling == "Bilinear":
-        x0, y0 = np.floor(sx).astype(np.int64), np.floor(sy).astype(np.int64)
-        ax, ay = (sx - x0.astype(F32))[..., None], (sy - y0.astype(F32))[..., None]
-        x1, y1 = np.minimum(x0 + 1, w - 1), np.minimum(y0 + 1, h - 1)
-        x0, y0 = np.maximum(x0, 0), np.maximum(y0, 0)
-        t00, t10, t01, t11 = tap(y0, x0), tap(y0, x1), tap(y1, x0), tap(y1, x1)
-        top = t00 + (t10 - t00) * ax
-        bot = t01 + (t11 - t01) * ax
-        px = top + (bot - top) * ay
-    else:
-        x0, y0 = np.floor(sx).astype(np.int64), np.floor(sy).astype(np.int64)
-        acc = np.zeros((dh, dw, 3), F32)
-        wsum = np.zeros((dh, dw), F32)
-        for j in range(-2, 4):
-            yj = y0 + j
-            wy = _lanczos_w(sy - yj.astype(F32))
-            for i in range(-2, 4):
-                xi = x0 + i
-                wt = wy * _lanczos_w(sx - xi.astype(F32))
-                acc = acc + wt[..., None] * tap(yj, xi)
-                wsum = wsum + wt
-        with np.errstate(divide="ignore", invalid="ignore"):
-            px = acc / wsum[..., None]
-    q = np.where(inside[..., None], px / F32(white(bits)), F32(pad_value) / F32(255.0))
-    o = ((q - np.asarray(mean, F32)) * np.asarray(inv_std, F32)).astype(F32).transpose(2, 0, 1)
-    return np.ascontiguousarray(o.astype(np.float16) if f16 else o)
+    return 32 + 4 * DEPTHS.index(bits) + PATTERN_CODE[pattern]
 
 
 # ═══ CPU ═══════════════════════════════════════════════════════════════════════════════════════════════════════
@@ -172,7 +76,7 @@ def test_validation_without_a_gpu(kb):
     assert _lib.last_error() == "'src' is not 2-byte aligned (16-bit samples)"
     assert l.kb200_rgb_from_bayer_u16(None, p, n, p + 3, n, 16, 4, 1, 0) == _lib.ERR_INVALID_ARGUMENT
     assert _lib.last_error() == "'dst' is not 2-byte aligned (16-bit samples)"
-    for p_name, code in CODE.items():
+    for p_name, code in PATTERN_CODE.items():
         for w, h in ((2, 7), (7, 2), (2, 2)):
             assert l.kb200_rgb_from_bayer_u16(None, p, n, p, n, w, h, 1, code) == _lib.ERR_INVALID_ARGUMENT
             assert _lib.last_error() == f"Bayer {p_name} needs at least 3x3 pixels, got {w}x{h}"
@@ -226,27 +130,8 @@ def test_u16_image_exports_a_typestr(kb):
 
 
 # ═══ GPU ═══════════════════════════════════════════════════════════════════════════════════════════════════════
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-def offset_u16(dev, n, off):
-    """A u16 device buffer of n samples whose data pointer is `off` samples past the start of a fresh allocation."""
-    return torch.empty(n + off, dtype=torch.uint16, device=dev)[off:]
-
-
-def to_dev16(a, dev):
-    return torch.from_numpy(np.ascontiguousarray(a).astype(np.int32)).to(dev).to(torch.uint16)
-
-
-def to_np16(t):
-    return t.to(torch.int32).cpu().numpy().astype(np.uint16)
-
-
 def run_decode(kb, dev, pattern, raw_dev, w, h, n, dst_off=0):
-    out = offset_u16(dev, n * h * w * 3, dst_off)
+    out = offset_buf(dev, n * h * w * 3, dst_off, torch.uint16)
     out.fill_(0xCDCD)
     kb.imgproc.rgb_from_bayer16(raw_dev, kb.Image(out.view(n, h, w, 3)), kb.imgproc.BayerPattern[pattern])
     return out.view(n, h, w, 3), kb._lib.last_kernel()
@@ -270,8 +155,8 @@ DECODE_CASES = [(p, c) for p in PATTERNS for c in CASES]
 def test_decode_bayer16(kb, dev, pattern, case):
     w, h, n, soff, doff = case
     bits = DEPTHS[(w + h) % 4]
-    raws = np.random.default_rng(w * 7919 + h * 31 + n + 1000 * CODE[pattern]).integers(0, 1 << bits, (n, h, w), dtype=np.uint16)
-    src = offset_u16(dev, n * w * h, soff)
+    raws = np.random.default_rng(w * 7919 + h * 31 + n + 1000 * PATTERN_CODE[pattern]).integers(0, 1 << bits, (n, h, w), dtype=np.uint16)
+    src = offset_buf(dev, n * w * h, soff, torch.uint16)
     src.copy_(to_dev16(raws.reshape(-1), dev))
     got, kern = run_decode(kb, dev, pattern, src.view(n, w * h), w, h, n, doff)
     assert kern == decode_kernel(pattern, w, soff, doff)
@@ -301,7 +186,7 @@ def test_decode_bayer16_extremes(kb, dev, pattern, w, h):
 @pytest.mark.parametrize("pattern", PATTERNS)
 def test_decode_bayer16_1080p_batch(kb, dev, pattern):
     w, h, n = 1920, 1080, 256
-    g = torch.Generator(device=dev).manual_seed(0x1016 + CODE[pattern])
+    g = torch.Generator(device=dev).manual_seed(0x1016 + PATTERN_CODE[pattern])
     raw = torch.randint(0, 1 << 16, (n, h * w), dtype=torch.int32, device=dev, generator=g).to(torch.uint16)
     got, kern = run_decode(kb, dev, pattern, raw, w, h, n)
     assert kern == f"rgb_from_bayer16_{pattern.lower()}_vec"
@@ -327,31 +212,6 @@ def expected_preprocess_kernel(pattern, sampling, w, h, dw, dh):
     return "preprocess_generic_kernel"
 
 
-def make_pre(kb, fmt, mode, sampling):
-    return (kb.Preprocessor.builder().source_format(kb.SourceFormat[fmt]).mode(kb.ResizeMode[mode])
-            .sampling(kb.InterpolationMode[sampling]).normalize(kb.Normalize.imagenet()).pad_value(114).build_cuda())
-
-
-def restated(kb, rgb, bits, mode, sampling, dw, dh, f16=False):
-    from kornia_rs_b200 import _lib
-
-    h, w = rgb.shape[:2]
-    a = (C.c_float * 4)()
-    _lib.lib().kb200_preprocess_affine(kb.ResizeMode[mode].value, w, h, dw, dh, a)
-    inv = tuple(F32(1.0) / F32(s) for s in kb.IMAGENET_STD)
-    return preprocess_rgb16(rgb, bits, tuple(a), dw, dh, sampling, kb.IMAGENET_MEAN, inv, 114.0, f16)
-
-
-def check_against_restatement(got, o, sampling, f16, what):
-    g = got.cpu().numpy()
-    if sampling == "Lanczos":
-        assert np.max(np.abs(g.astype(np.float32) - o.astype(np.float32))) <= (2e-3 if f16 else 1e-4), what
-    elif f16:
-        np.testing.assert_array_equal(g.view(np.uint16), o.view(np.uint16), what)
-    else:
-        np.testing.assert_array_equal(g.view(np.uint32), o.view(np.uint32), what)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("pattern,bits", FORMATS)
 @pytest.mark.parametrize("mode", ["Letterbox", "Stretch"])
@@ -364,23 +224,12 @@ def test_preprocess_bayer16(kb, dev, pattern, bits, mode, sampling, f16):
     dt = torch.float16 if f16 else torch.float32
     for w, h, dw, dh in GEOMS:
         what = f"{pattern}{bits} {mode} {sampling} {'f16' if f16 else 'f32'} {(w, h, dw, dh)}"
-        raw = raw_samples(w * h, bits, CODE[pattern])
+        raw = raw_samples(w * h, bits, PATTERN_CODE[pattern])
         got = torch.full((1, 3, dh, dw), float("nan"), dtype=dt, device=dev)
         (pre.run_raw_f16 if f16 else pre.run_raw)(to_dev16(raw, dev), w, h, got)
         assert kb._lib.last_kernel() == expected_preprocess_kernel(pattern, sampling, w, h, dw, dh), what
         o = restated(kb, demosaic(raw.reshape(h, w), pattern), bits, mode, sampling, dw, dh, f16 and sampling != "Lanczos")
         check_against_restatement(got[0], o, sampling, f16, what)
-
-
-def torch_identity(raw, pattern, bits, kb):
-    """Config 3a of 16-bit frames [n, h, w] on the device: the restatement's demosaic, then (px / W - mean) * inv_std
-    as separate IEEE f32 operations."""
-    # the divisor is a device tensor: torch turns division by a host scalar into a multiplication by its reciprocal
-    wl = torch.full((1,), float(white(bits)), dtype=torch.float32, device=raw.device)
-    rgb = demosaic(raw, pattern).to(torch.int32).to(torch.float32) / wl
-    mean = torch.tensor(kb.IMAGENET_MEAN, dtype=torch.float32, device=raw.device)
-    inv = torch.tensor(1.0, dtype=torch.float32) / torch.tensor(kb.IMAGENET_STD, dtype=torch.float32)
-    return ((rgb - mean) * inv.to(raw.device)).permute(0, 3, 1, 2)
 
 
 @pytest.mark.gpu
@@ -391,7 +240,7 @@ def test_preprocess_bayer16_identity_1080p(kb, dev, pattern, bits, n):
     pointer table and the strided entry, against the restatement for every frame."""
     w, h = 1920, 1080
     ns = w * h
-    g = torch.Generator(device=dev).manual_seed(0x3A16 + CODE[pattern])
+    g = torch.Generator(device=dev).manual_seed(0x3A16 + PATTERN_CODE[pattern])
     ring = torch.randint(0, 1 << bits, (n, ns + 32), dtype=torch.int32, device=dev, generator=g).to(torch.uint16)   # padded strided slots
     frames = ring[:, :ns]
     pre = kb.Preprocessor.builder().source_format(kb.SourceFormat[fmt_name(pattern, bits)]).mode(kb.ResizeMode.Stretch).normalize(kb.Normalize.imagenet()).build_cuda()
@@ -401,7 +250,7 @@ def test_preprocess_bayer16_identity_1080p(kb, dev, pattern, bits, n):
     def check(entry):
         assert kb._lib.last_kernel() == kernel, entry
         for k0 in range(0, n, 32):
-            want = torch_identity(frames[k0:k0 + 32].reshape(-1, h, w), pattern, bits, kb)
+            want = bayer16_identity(frames[k0:k0 + 32].reshape(-1, h, w), pattern, bits, kb)
             assert torch.equal(got[k0:k0 + 32].view(torch.int32), want.contiguous().view(torch.int32)), f"{entry} frames {k0}.."
 
     pre.run_raw_batch([frames[k] for k in range(n)], w, h, got)

@@ -2,7 +2,7 @@
 
 The packing only changes how samples are read from memory, so every check is against the frame's unpacked 16-bit twin:
 a packed frame must give the same bits as the same samples unpacked into one LSB-aligned word each, on every path —
-the decoder against `rgb_from_bayer16` and the numpy restatement of tests/test_bayer16.py, the preprocess against the
+the decoder against `rgb_from_bayer16` and the numpy restatement of tests/restate.py, the preprocess against the
 `BayerXxxNN` format of the same depth and the restated oracle.  A numpy / torch unpacker defines the packing and is
 pinned by a known-answer table.
 """
@@ -12,11 +12,11 @@ import numpy as np
 import pytest
 import torch
 
-from test_bayer16 import PATTERNS, CODE, check_against_restatement, demosaic, fmt_name, make_pre, restated, to_dev16, to_np16, torch_identity, white
+from harness import bayer16_identity, check_against_restatement, dev, make_pre, offset_buf, restated, to_dev16, to_np16
+from restate import GROUP, GROUP_BYTES, PATTERNS, PATTERN_CODE, demosaic, fmt_name, pack, unpack, white
+
 
 PDEPTHS = (10, 12, 14)
-GROUP = {10: 4, 12: 2, 14: 4}          # samples per group
-GROUP_BYTES = {10: 5, 12: 3, 14: 7}    # bytes per group
 
 
 def pfmt_name(pattern, bits):
@@ -24,40 +24,11 @@ def pfmt_name(pattern, bits):
 
 
 def pfmt_code(pattern, bits):
-    return 64 + 4 * PDEPTHS.index(bits) + CODE[pattern]
+    return 64 + 4 * PDEPTHS.index(bits) + PATTERN_CODE[pattern]
 
 
 def row_bytes(w, bits):
     return w * bits // 8
-
-
-# ── the packing, restated: numpy for the CPU side, numpy or torch for unpack ──
-def pack(samples, bits):
-    """[..., h, w] samples < 2^bits (numpy) -> [..., h, w*bits/8] uint8, each row packed on its own."""
-    g, gb, lo = GROUP[bits], GROUP_BYTES[bits], bits - 8
-    v = np.asarray(samples).astype(np.int64)
-    *lead, w = v.shape
-    assert w % g == 0
-    v = v.reshape(*lead, w // g, g)
-    field = np.zeros(v.shape[:-1], np.int64)
-    for j in range(g):
-        field |= (v[..., j] & ((1 << lo) - 1)) << (lo * j)
-    lo_bytes = np.stack([(field >> (8 * i)) & 0xFF for i in range(gb - g)], -1)
-    return np.concatenate([v >> lo, lo_bytes], -1).astype(np.uint8).reshape(*lead, w // g * gb)
-
-
-def unpack(raw, bits):
-    """[..., h, w*bits/8] uint8 (numpy array or torch tensor) -> [..., h, w] samples (int32)."""
-    g, gb, lo = GROUP[bits], GROUP_BYTES[bits], bits - 8
-    is_t = isinstance(raw, torch.Tensor)
-    b = raw.to(torch.int32) if is_t else raw.astype(np.int32)
-    *lead, nb = b.shape
-    b = b.reshape(*lead, nb // gb, gb)
-    field = b[..., g] * 0
-    for i in range(gb - g):
-        field = field | (b[..., g + i] << (8 * i))
-    out = (torch.stack if is_t else np.stack)([(b[..., j] << lo) | ((field >> (lo * j)) & ((1 << lo) - 1)) for j in range(g)], -1)
-    return out.reshape(*lead, nb // gb * g)
 
 
 KNOWN = [(10, [0xFF, 0x00, 0x80, 0x01, 0xE4], [1020, 1, 514, 7]),
@@ -123,7 +94,7 @@ def test_validation_without_a_gpu(kb):
         assert _lib.last_error() == f"packed Bayer samples are 10, 12 or 14 bits, got {bits}"
     assert l.kb200_rgb_from_bayer_packed(None, p, n, p + 1, n, 8, 4, 1, 0, 12) == _lib.ERR_INVALID_ARGUMENT
     assert _lib.last_error() == "'dst' is not 2-byte aligned (16-bit samples)"
-    for p_name, code in CODE.items():
+    for p_name, code in PATTERN_CODE.items():
         for bits in PDEPTHS:
             g, gb = GROUP[bits], GROUP_BYTES[bits]
             for w, h in ((4, 2), (2, 7), (2, 2)):
@@ -182,17 +153,6 @@ def test_validation_without_a_gpu(kb):
 
 
 # ═══ GPU ═══════════════════════════════════════════════════════════════════════════════════════════════════════
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-def offset_buf(dev, n, off, dtype):
-    """A device buffer of n elements whose data pointer is `off` elements past the start of a fresh allocation."""
-    return torch.empty(n + off, dtype=dtype, device=dev)[off:]
-
-
 def decode(kb, dev, pattern, bits, src, w, h, n, dst_off=0):
     out = offset_buf(dev, n * h * w * 3, dst_off, torch.uint16)
     out.fill_(0xCDCD)
@@ -234,7 +194,7 @@ def test_decode_packed(kb, dev, bits, pattern, size, offs):
     mosaic and to the restatement, with the kernel the dispatch promises."""
     w, h = size
     soff, doff = offs
-    v = contents(bits, w, h, w * 31 + h + 7 * bits + CODE[pattern])
+    v = contents(bits, w, h, w * 31 + h + 7 * bits + PATTERN_CODE[pattern])
     n = len(v)
     packed = pack(v, bits)
     src = offset_buf(dev, packed.size, soff, torch.uint8)
@@ -317,7 +277,7 @@ def test_preprocess_packed_identity_1080p(kb, dev, pattern, bits, n):
     table and the strided entry: every frame bit-equal to the device-unpacked samples normalised in torch."""
     w, h = 1920, 1080
     fb = row_bytes(w, bits) * h
-    g = torch.Generator(device=dev).manual_seed(0x3A0 + bits + CODE[pattern])
+    g = torch.Generator(device=dev).manual_seed(0x3A0 + bits + PATTERN_CODE[pattern])
     ring = torch.randint(0, 256, (n, fb + 32), dtype=torch.uint8, device=dev, generator=g)   # padded strided slots
     frames = ring[:, :fb]
     pre = (kb.Preprocessor.builder().source_format(kb.SourceFormat[pfmt_name(pattern, bits)]).mode(kb.ResizeMode.Stretch)
@@ -328,7 +288,7 @@ def test_preprocess_packed_identity_1080p(kb, dev, pattern, bits, n):
     def check(entry):
         assert kb._lib.last_kernel() == kernel, entry
         for k0 in range(0, n, 32):
-            want = torch_identity(unpack(frames[k0:k0 + 32].reshape(-1, h, row_bytes(w, bits)), bits), pattern, bits, kb)
+            want = bayer16_identity(unpack(frames[k0:k0 + 32].reshape(-1, h, row_bytes(w, bits)), bits), pattern, bits, kb)
             assert torch.equal(got[k0:k0 + 32].view(torch.int32), want.contiguous().view(torch.int32)), f"{entry} frames {k0}.."
 
     pre.run_raw_batch([frames[k] for k in range(n)], w, h, got)

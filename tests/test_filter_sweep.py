@@ -11,7 +11,7 @@ that only runs those.  So here:
     (separable_filter: equal lengths 3/5/7 with kx != ky and a non-palindromic kx, or random lengths 1-31, odd and even,
     mixed signs), sigma_x != sigma_y at equal sizes and (0, 0) auto sizes (gaussians), kx != ky (box), image size, batch,
     and buffers aligned or one element past a 16-byte boundary.  Hand-picked edge cases (EDGES) run the same way.
-  * Each case calls the C ABI directly, src inside test_footprint.Guarded poison, dst inside a Guarded region prefilled
+  * Each case calls the C ABI directly, src inside harness.Guarded poison, dst inside a Guarded region prefilled
     with NaN (f32) or 0xCD (u8).  The guards must keep their fill, no f32 output may be left at the fill, kb200_last_kernel()
     must be the kernel `plan` (a host mirror of launch_sep / launch_blur_u8) names, and every frame must equal the
     oracle bit for bit (f32: +0 / -0 and NaN payloads aside; infinities must match in sign).
@@ -28,10 +28,9 @@ import numpy as np
 import pytest
 import torch
 
-from test_footprint import Guarded
-from test_gpu_variants import assert_f32_equal
-from test_launch_shapes import knobs
-from test_oracle_golden import _q8_two_pass_numpy
+from harness import Guarded, assert_f32_bits_or_signed_zero, dev, knobs, lib
+from restate import _q8_two_pass_numpy
+
 
 BASE = 0x5F170000
 F32 = np.float32
@@ -423,17 +422,6 @@ assert len(EDGES) == len(_edges()), "edge case names must be unique"
 
 
 # ── the GPU run ─────────────────────────────────────────────────────────────────────────────────────────────────────
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
-def lib(kb):
-    return kb._lib.lib()
-
-
 def frame(c, k):
     rng = np.random.default_rng([c.seed, k])
     if c.u8:
@@ -470,7 +458,7 @@ def call(lib, c, src, dst, n):
 
 
 def assert_same_f32(got, want, what):
-    """Bit for bit, as assert_f32_equal, where both are finite; elsewhere the same non-finite class (NaN, +inf or -inf)."""
+    """Bit for bit, as assert_f32_bits_or_signed_zero, where both are finite; elsewhere the same non-finite class (NaN, +inf or -inf)."""
     got, want = got.reshape(-1), want.reshape(-1)
     fin_g, fin_w = np.isfinite(got), np.isfinite(want)
     cls = lambda a: np.where(np.isnan(a), 2, np.sign(np.nan_to_num(a, nan=0.0, posinf=1.0, neginf=-1.0)))
@@ -478,7 +466,7 @@ def assert_same_f32(got, want, what):
     if bad.size:
         raise AssertionError(f"{what}: {bad.size} elements differ in finiteness, first at element {bad[0]}: got {got[bad[0]]}, want {want[bad[0]]}")
     if fin_w.any():
-        assert_f32_equal(got[fin_w], want[fin_w], what)
+        assert_f32_bits_or_signed_zero(got[fin_w], want[fin_w], what)
 
 
 def run_case(kb, lib, dev, c):

@@ -10,7 +10,9 @@ import numpy as np
 import pytest
 import torch
 
-from test_launch_shapes import fused_schedule
+from harness import dev, knobs
+from restate import fused_schedule
+
 
 FRR_CT, FRR_V, FRR_MAX_NPX = 256, 4, 2
 
@@ -61,12 +63,6 @@ def test_full_rows_geometries(sw, sh, dw, dh, batch, npx):
 
 
 # ── device: every frame against the oracle and the tiled kernel ─────────────────────────────────────────────────
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
 def _bits(t):
     return t.view(torch.int32 if t.dtype == torch.float32 else torch.int16)
 
@@ -93,16 +89,11 @@ def test_full_rows_match_oracle(kb, oracle, dev, sw, sh, dw, dh, batch, npx, lea
         tiled = None
         for k in KNOBS:
             what = f"{sw}x{sh}->{dw}x{dh} x{batch} leaf {leaf} {dtype} {k}"
-            try:
-                for name, v in k.items():
-                    kb._lib.set_knob(name, v)
+            with knobs(kb, k):
                 out = kb.imgproc.resize_normalize_to_tensor_u8_bilinear(src, dw, dh, scale, bias, dtype, leaf=leaf)
                 assert kb._lib.last_kernel() == "fused_rows_kernel", what
-            finally:
-                for name in k:
-                    kb._lib.set_knob(name, 0)
             got = _bits(out).cpu()
-            # the oracle and the device may disagree on the sign of an exact zero (assert_f32_equal's rule)
+            # the oracle and the device may disagree on the sign of an exact zero (assert_f32_bits_or_signed_zero's rule)
             mag = 0x7FFFFFFF if dtype == torch.float32 else 0x7FFF
             differ = (got != want) & ~(((got & mag) == 0) & ((want & mag) == 0))
             for i in range(batch):

@@ -11,14 +11,11 @@ import numpy as np
 import pytest
 import torch
 
+from harness import dev
+from restate import NAMED_FUSED_MODES, fused_schedule
+
 HALF = [torch.float16, torch.bfloat16]
 gpu = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    return torch.device("cuda:0")
 
 
 def cu(a, dev):
@@ -38,7 +35,7 @@ def assert_same_bits(got, want, what=""):
 
 
 def assert_matches_oracle(got, want_f32, dtype, what=""):
-    """`got` (16-bit) against the oracle's f32 result rounded on the host; like assert_f32_equal, +0 and -0 are the same
+    """`got` (16-bit) against the oracle's f32 result rounded on the host; like assert_f32_bits_or_signed_zero, +0 and -0 are the same
     value (the oracle and the device may disagree on the sign of an exact zero)."""
     if dtype == torch.float16:
         w = np.asarray(want_f32, np.float32).astype(np.float16).view(np.int16)
@@ -77,8 +74,6 @@ def f32_then_cast(kb, src, dw, dh, scale, bias, dtype, **kw):
 @pytest.mark.parametrize("leaf", [0, 1])
 @pytest.mark.parametrize("dtype", HALF)
 def test_half_modes_named(kb, oracle, dev, sw, sh, dw, dh, kernel, leaf, dtype):
-    from test_gpu_variants import NAMED_FUSED_MODES
-    from test_launch_shapes import fused_schedule
 
     n = 2
     assert fused_schedule(sw, sh, dw, dh, n, torch.cuda.get_device_properties(dev).multi_processor_count).mode == NAMED_FUSED_MODES[(sw, sh, dw, dh)]

@@ -23,7 +23,9 @@ import pytest
 import torch
 
 import bench
-from test_gpu_variants import assert_f32_equal
+
+from harness import POOL, _one_omp_thread, compare_frames, dev, free_device_memory, knobs
+from restate import Schedule, _lround, _pick_npx, _walk, fused_schedule
 
 pytestmark = pytest.mark.gpu
 
@@ -31,136 +33,8 @@ f32 = np.float32
 
 
 @pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
 def sm_count(dev):
     return torch.cuda.get_device_properties(dev).multi_processor_count
-
-
-@contextlib.contextmanager
-def knobs(kb, values):
-    """Developer knobs (names contain dots, hence a dict), always reset to 0 (= the dispatcher's own choice)."""
-    try:
-        for name, v in values.items():
-            kb._lib.set_knob(name, v)
-        yield
-    finally:
-        for name in values:
-            kb._lib.set_knob(name, 0)
-
-
-def free_device_memory():
-    torch.cuda.synchronize()
-    torch.cuda.empty_cache()
-
-
-# ── host mirrors of the two tiled schedules ─────────────────────────────────────────────────────────────────────
-@dataclass
-class Schedule:
-    mode: str             # fused: POINT / BOX / YZERO / GENERAL, or "gather" when the staged kernel declines
-    npx: int = 0
-    stages: int = 0
-    per_sm: int = 0
-    tiles_x: int = 0
-    rows_per_chunk: int = 0
-    chunks_y: int = 0
-    nunits: int = 0
-    grid: int = 0
-    dtx: int = 0
-    dcy: int = 0
-    dimg: int = 0
-    dh: int = 0
-
-    @property
-    def staged(self):
-        return self.mode != "gather"
-
-    @property
-    def units_per_cta(self):
-        return -(-self.nunits // self.grid)
-
-    @property
-    def ragged(self):
-        """The last chunk of every image is shorter than the others."""
-        return self.dh % self.rows_per_chunk != 0
-
-    def regime(self):
-        return {"mode": self.mode, "multi": self.nunits > self.grid, "dimg": self.dimg >= 1, "ragged": self.ragged}
-
-    def __str__(self):
-        if not self.staged:
-            return "gather"
-        return (f"{self.mode} npx={self.npx} stages={self.stages} per_sm={self.per_sm} tiles={self.tiles_x} rc={self.rows_per_chunk} "
-                f"chunks={self.chunks_y} units={self.nunits} grid={self.grid} ({self.units_per_cta}/CTA) "
-                f"stride=({self.dtx},{self.dcy},{self.dimg})")
-
-
-def _lround(x):
-    return int(math.floor(x + 0.5))
-
-
-def _pick_npx(dw, order, tol):
-    npx, best = 1, 1e30
-    for o in order:
-        tw = 128 * o
-        waste = -(-dw // tw) * tw / dw
-        if waste < best - tol:
-            best, npx = waste, o
-    return npx
-
-
-def _walk(s, dh, batch, ctas, min_rc):
-    total_rows = dh * batch * s.tiles_x
-    s.rows_per_chunk = min(max(min_rc, total_rows // (ctas * 16)), dh)
-    s.chunks_y = -(-dh // s.rows_per_chunk)
-    s.nunits = s.tiles_x * s.chunks_y * batch
-    s.grid = min(s.nunits, ctas)
-    s.dtx = s.grid % s.tiles_x
-    g = s.grid // s.tiles_x
-    s.dcy, s.dimg = g % s.chunks_y, g // s.chunks_y
-    s.dh = dh
-    return s
-
-
-def _axis_weights_all_zero(dst_len, src_len, scale):
-    d = np.arange(dst_len, dtype=f32)
-    f = np.maximum((d + f32(0.5)) * f32(scale) - f32(0.5), f32(0))
-    a = np.minimum(f.astype(np.uint32), src_len - 1)
-    b = np.minimum(a + 1, src_len - 1)
-    return bool(np.all((b == a) | (f - a.astype(f32) == 0)))
-
-
-def fused_schedule(sw, sh, dw, dh, batch, sm, npx_knob=0, stages_knob=0, ctas_knob=0):
-    """launch_fused_resize_rows (csrc/resize_fused.cu) on the host.  The leaf and output type do not enter the schedule."""
-    row_bytes = sw * 3
-    sx, sy = f32(sw) / f32(dw), f32(sh) / f32(dh)
-    if row_bytes % 16 or sx > 6 or sw < 16:
-        return Schedule("gather")
-    yz = _axis_weights_all_zero(dh, sh, sy)
-    xz = yz and _axis_weights_all_zero(dw, sw, sx)
-    mode = "BOX" if (sw == 2 * dw and sh == 2 * dh) else ("POINT" if xz else ("YZERO" if yz else "GENERAL"))
-    npx = _pick_npx(dw, (2, 3, 1, 4, 5), 0.10 if mode == "GENERAL" else 0.02)
-    if 1 <= npx_knob <= 5:
-        npx = npx_knob
-    tw = 128 * npx
-    slot = int(((tw - 1) * float(sx) + 4.0) * 3.0) + 32
-    slot = min((slot + 127) & ~127, (row_bytes + 16 + 127) & ~127)
-    stage_bytes = slot * (2 if mode in ("GENERAL", "BOX") else 1)
-    stages = stages_knob if 2 <= stages_knob <= 16 else 3
-    per_sm = ctas_knob if ctas_knob > 0 else (4 if mode == "GENERAL" else _lround(36 * 1024 / (stages * stage_bytes)))
-    per_sm = max(2, min(per_sm, 8))
-    while per_sm > 2 and per_sm * (stages * stage_bytes + 1024) > 200 * 1024:
-        per_sm -= 1
-    if ctas_knob <= 0 and stages_knob <= 0 and per_sm == 2:
-        stages = min(16, max(3, int(18 * 1024 / stage_bytes)))
-    if stages < 3 or stage_bytes * stages > 200 * 1024:
-        return Schedule("gather")
-    s = Schedule(mode, npx=npx, stages=stages, per_sm=per_sm, tiles_x=-(-dw // tw))
-    return _walk(s, dh, batch, sm * per_sm, 8)
 
 
 def resize_rows_schedule(sw, sh, dw, dh, batch, sm, resident, npx_knob=0, stages_knob=0, ctas_knob=0):
@@ -187,49 +61,6 @@ def resize_rows_schedule(sw, sh, dw, dh, batch, sm, resident, npx_knob=0, stages
     per_sm = min(per_sm, resident)
     s = Schedule("rows", npx=npx, stages=stages, per_sm=per_sm, tiles_x=-(-dw // tw))
     return _walk(s, dh, batch, sm * per_sm, 8)
-
-
-# ── frame-by-frame comparison ───────────────────────────────────────────────────────────────────────────────────
-POOL = max(1, min(16, len(os.sched_getaffinity(0))))
-
-
-def _one_omp_thread(oracle):
-    oracle.set_threads(1)   # this worker's OpenMP teams: the pool is the parallelism
-
-
-def check_frame(got, want, rule, what):
-    """rule: "f32" = assert_f32_equal (bit-identical, +0 == -0); "exact" = equal elements (integers, 16-bit float bits);
-    a float = within that absolute tolerance (Lanczos: sinf of two math libraries)."""
-    got, want = np.asarray(got), np.asarray(want)
-    assert got.shape == want.shape, (what, got.shape, want.shape)
-    if rule == "f32":
-        bad = (got.view(np.uint32) != want.view(np.uint32)) & ~((got == 0) & (want == 0))
-        n = int(bad.sum())
-        if n:
-            assert_f32_equal(got, want, f"{what} ({n} of {got.size} elements differ)")
-    elif rule == "exact":
-        n = int((got != want).sum())
-        assert n == 0, f"{what}: {n} of {got.size} elements differ"
-    else:
-        n = int((~(np.abs(got.astype(np.float64) - want.astype(np.float64)) <= rule)).sum())
-        assert n == 0, f"{what}: {n} of {got.size} elements differ by more than {rule}"
-
-
-def compare_frames(oracle, n, want_fn, got_fn, rule, what):
-    """want_fn(i) -> the oracle's frame i (run in the pool, at most POOL frames ahead); got_fn(i) -> device frame i on the
-    host.  Either may return a tuple (several outputs of one frame).  Stops at the first frame that differs and names it."""
-    with ThreadPoolExecutor(POOL, initializer=_one_omp_thread, initargs=(oracle,)) as ex:
-        pending = deque(ex.submit(want_fn, i) for i in range(min(POOL, n)))
-        for i in range(n):
-            want = pending.popleft().result()
-            if i + POOL < n:
-                pending.append(ex.submit(want_fn, i + POOL))
-            got = got_fn(i)
-            if isinstance(want, tuple):
-                for k, (g, w) in enumerate(zip(got, want, strict=True)):
-                    check_frame(g, w, rule, f"{what} (output {k}): frame {i} of {n}")
-            else:
-                check_frame(got, want, rule, f"{what}: frame {i} of {n}")
 
 
 def first_bad_frame(bad):

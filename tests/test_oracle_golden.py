@@ -10,6 +10,8 @@ import os
 import numpy as np
 import pytest
 
+from restate import _q8_two_pass_numpy
+
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 
 
@@ -653,18 +655,6 @@ def _knuth_u8(n):
     """the reference tests' generator: ((i * 2654435761) >> 24) as u8 with usize wrapping (filter/ops.rs:1992-1994)"""
     i = np.arange(n, dtype=np.uint64)
     return (((i * np.uint64(2654435761)) & np.uint64(0xFFFFFFFFFFFFFFFF)) >> np.uint64(24)).astype(np.uint8)
-
-
-def _q8_two_pass_numpy(src, ikx, iky):
-    """Independent numpy restatement of the general path: replicate border, (acc+128)>>8 after EACH pass."""
-    rows, cols, c = src.shape
-    hx, hy = len(ikx) // 2, len(iky) // 2
-    p = np.pad(src.astype(np.uint32), ((0, 0), (hx, hx), (0, 0)), mode="edge")
-    h = sum(p[:, k:k + cols] * np.uint32(ikx[k]) for k in range(len(ikx)))
-    h = ((h + 128) >> 8).astype(np.uint32)
-    p = np.pad(h, ((hy, hy), (0, 0), (0, 0)), mode="edge")
-    v = sum(p[k:k + rows] * np.uint32(iky[k]) for k in range(len(iky)))
-    return ((v + 128) >> 8).astype(np.uint8)
 
 
 def test_quantize_kernel_256(oracle):

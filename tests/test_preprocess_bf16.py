@@ -23,9 +23,9 @@ import numpy as np
 import pytest
 import torch
 
-from test_footprint import Guarded, poison
-from test_preprocess_sweep import (BILINEAR, EDGES, GENERIC, LANCZOS, N_SWEEP, case, edge, expected_kernel, frame_bytes,
-                                   host_chunk)
+from harness import Guarded, dev, lib, poison
+from restate import BILINEAR, EDGES, FORMATS, GENERIC, LANCZOS, N_SWEEP, case, edge, expected_kernel, frame_bytes, host_chunk, row_bytes
+
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 OUT_F32, OUT_F16, OUT_BF16 = 0, 1, 2
@@ -55,17 +55,6 @@ def assert_bf16_matches(got_raw, f32_raw, what):
 def desc_of(c):
     from kornia_rs_b200._lib import PreprocessDesc
     return c.desc(PreprocessDesc)
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
-def lib(kb):
-    return kb._lib.lib()
 
 
 DEVICE_FN = {("table", OUT_F32): "kb200_preprocess_f32", ("table", OUT_F16): "kb200_preprocess_f16", ("table", OUT_BF16): "kb200_preprocess_bf16",
@@ -155,7 +144,6 @@ def test_bf16_sweep_covers_every_kernel():
     kernel."""
     cases = [case(i) for i in range(N_SWEEP)] + list(EDGES.values())
     ran = {(c.code, c.planned()) for c in cases}
-    from test_preprocess_sweep import FORMATS
     for code, f in FORMATS.items():
         assert {k for k in (f.identity, f.fast, GENERIC) if k} <= {k for cc, k in ran if cc == code}, f.name
     assert {c.entry for c in cases} == {"table", "strided", "host"}
@@ -415,7 +403,6 @@ FOOT_KERNEL = {"generic": GENERIC, "yuv420_identity": "preprocess_nv12_identity_
 
 def padding_mask(c):
     """True at the pitch padding bytes of a frame of case c."""
-    from test_preprocess_sweep import row_bytes
     m = np.zeros(c.need, bool)
     row = row_bytes(c.fmt, c.w, c.bpp)
     if c.pitch > row:

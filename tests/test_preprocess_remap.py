@@ -11,7 +11,7 @@ On the GPU:
     kb200_preprocess_warps on that map;
   * a seeded sweep (`mcase(i)`, a pure function of i, every format twice) of undistortion maps from the device generator
     (both entries), random smooth maps, per-pixel noise (NaN, +-inf, -0.0, 1e30, samples on 0, W - 1, the float below W
-    and W) and constant maps against the reference, each run into a test_footprint.Guarded destination with a 0xFF
+    and W) and constant maps against the reference, each run into a harness.Guarded destination with a 0xFF
     prefill, on the kernel a host mirror of the dispatch rule names, and again with dst and with the maps one element past
     a 16-byte boundary, where the generic kernel must give the same bytes;
   * several maps and an arbitrary (frame, map) table against one shared-map call per map, at region counts around the
@@ -31,18 +31,14 @@ import numpy as np
 import pytest
 import torch
 
-import test_preprocess_warp as tpw
-from test_footprint import Guarded
-from test_preprocess_roi import RCase, compare, load_frames, picture, place
-from test_preprocess_sweep import BILINEAR, CODES, FORMATS, LANCZOS, NEAREST, NORMS, SAMPLING_NAME, pad_step, row_bytes, size_rule, src_bytes, yuv
-from test_preprocess_warp import batch_entry, draw_map, inverse, make_case, smooth_rgb, warp_array, warp_coords
+from harness import Guarded, batch_entry, compare_region, dev, inverse, lib, load_frames, warp_array
+from restate import BILINEAR, CODES, ESZ, FORMATS, LANCZOS, NEAREST, NORMS, OUTS, RCase, SAMPLING_NAME, draw_map, make_case, pad_step, picture, place, remap_reference, row_bytes, size_rule, smooth_rgb, src_bytes, warp_coords, yuv
+
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BASE = 0x5E3A0000
 CHUNK = 192   # regions per launch (preprocess_remap.cu REMAP_CHUNK)
 VECTOR, GENERIC = "preprocess_remap_kernel", "preprocess_remap_generic_kernel"
-OUTS = ("f32", "f16", "bf16")
-ESZ = {"f32": 4, "f16": 2, "bf16": 2}
 INVALID, SLICE, UNSUPPORTED, INVALID_SOURCE = -1, -2, -4, -8
 F32 = np.float32
 KINDS = ("undistort", "undistort_to", "smooth", "noise", "constant")
@@ -52,20 +48,6 @@ KINDS = ("undistort", "undistort_to", "smooth", "noise", "constant")
 def expected_kernel(dw, out, dst, map_x, map_y):
     ok = dw % 4 == 0 and map_x % 16 == 0 and map_y % 16 == 0 and dst % (16 if out == "f32" else 8) == 0
     return VECTOR if ok else GENERIC
-
-
-# ── the reference ──────────────────────────────────────────────────────────────────────────────────────────────────────
-def inside_of(mx, my, w, h):
-    with np.errstate(invalid="ignore"):
-        return (mx >= 0) & (mx < F32(w)) & (my >= 0) & (my < F32(h))
-
-
-def remap_reference(pic, mx, my, sampling, norm, pad_value, out):
-    """(3, dh, dw) of one region through the map (mx, my) (float32 [dh, dw]): f32, or f16 bits for f16 output."""
-    h, w = pic[1].shape[:2]
-    coords = (mx, my, inside_of(mx, my, w, h), np.zeros(mx.shape, bool))
-    with mock.patch.object(tpw, "warp_coords", lambda *a: coords), np.errstate(invalid="ignore"):
-        return tpw.warp_reference(pic, None, False, mx.shape[1], mx.shape[0], sampling, norm, pad_value, out)
 
 
 def distort_map(intr, dist, new, dw, dh):
@@ -138,7 +120,7 @@ def draw_map_pair(rng, kind, w, h, dw, dh):
 # ── the cases ──────────────────────────────────────────────────────────────────────────────────────────────────────────
 @dataclass(frozen=True)
 class MCase:
-    base: object              # test_preprocess_sweep.Case: format, frame geometry, sampler, normalisation, pad value, dst size
+    base: object              # restate.Case: format, frame geometry, sampler, normalisation, pad value, dst size
     out: str
     n_frames: int
     offsets: tuple            # each frame's byte offset in one allocation (16-B aligned base)
@@ -198,17 +180,6 @@ def call(lib, c, ptrs, lens, map_x, map_y, map_len, n_maps, regions, dst_ptr, ds
     n = len(ptrs)
     return lib.kb200_preprocess_remap(stream, C.byref(d), (C.c_void_p * max(1, n))(*ptrs), (C.c_size_t * max(1, n))(*lens) if lens is not None else None,
                                       n, map_x, map_y, map_len, n_maps, region_array(regions), len(regions), dst_ptr, dst_len, OUTS.index(out))
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
-def lib(kb):
-    return kb._lib.lib()
 
 
 def generate(lib, dev, intr, dist, new, dw, dh):
@@ -280,7 +251,7 @@ def run_mcase(kb, lib, dev, mc):
         if k not in pics:
             pics[k] = picture(c, raws[k])
         want = remap_reference(pics[k], mx[j], my[j], c.sampling, c.norm, c.pad_value, mc.out)
-        compare(outs[0][i * fb:(i + 1) * fb], want, mc.rcase, f"{mc}: region {i} frame {k} map {j} ({mc.maps[j][0]})")
+        compare_region(outs[0][i * fb:(i + 1) * fb], want, mc.rcase, f"{mc}: region {i} frame {k} map {j} ({mc.maps[j][0]})")
     for o in outs[1:]:
         bad = np.flatnonzero(outs[0] != o)
         assert bad.size == 0, f"{mc}: the kernels differ in {bad.size} bytes"

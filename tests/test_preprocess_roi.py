@@ -3,13 +3,13 @@
 Region i = (k, x, y, w, h) must give:
   * for the whole frame (k, 0, 0, W, H), the bytes the batch entry gives frame k (test_whole_frame);
   * for any region, the bytes of the sweep's references (test_preprocess_sweep.reference's restatements: the oracle on the
-    decoded RGB8 picture, or test_bayer16.preprocess_rgb16 on the decoded 16-bit picture) run on the w x h crop at (x, y)
+    decoded RGB8 picture, or restate.preprocess_rgb16 on the decoded 16-bit picture) run on the w x h crop at (x, y)
     of frame k's decoded picture with kb200_preprocess_affine(mode, w, h, dst_w, dst_h) (test_sweep, `rcase(i)` a pure
     function of i); Lanczos within the sweep's tolerance.
 
 Every sweep case that does not sample with Lanczos runs a second time into a destination one element past a 16-byte
 boundary, which refuses the fast region kernels: the generic region kernel must give the same bits.  Destinations sit in
-test_footprint.Guarded with a 0xFF prefill; frames sit in one buffer with random bytes in their pitch padding, between them
+harness.Guarded with a 0xFF prefill; frames sit in one buffer with random bytes in their pitch padding, between them
 and around them.  The CPU tests cover the host validation (no region outside its frame ever reaches a device), the
 dispatch rule's coverage and run_rois' argument rules.
 """
@@ -20,21 +20,13 @@ import numpy as np
 import pytest
 import torch
 
-from test_bayer import demosaic as demosaic8
-from test_bayer16 import demosaic as demosaic16, preprocess_rgb16
-from test_bayer_packed import unpack
-from test_footprint import Guarded
-from test_preprocess_sweep import (BILINEAR, CODES, FORMATS, LANCZOS, NEAREST, NORMS, SAMPLING_NAME, Case, IMAGENET_INV, elem_align, frame_bytes,
-                                   oracle_rgb, pad_step, row_bytes, size_rule, src_bytes, yuv)
-from test_yuv16 import decode as decode_yuv16
-from test_yuv444 import decode8 as decode_yuv444, decode16 as decode_yuv444_16
-from test_yuv_matrix import MATRICES, decode as decode_yuv8
+from harness import Guarded, compare_region, dev, lib, load_frames, roi_array
+from restate import BILINEAR, CODES, Case, ESZ, FORMATS, LANCZOS, NEAREST, NORMS, OUTS, RCase, SAMPLING_NAME, pad_step, picture, place, region_reference, row_bytes, size_rule, src_bytes, yuv
+
 
 BASE = 0x2011F000
 CHUNK = 80   # regions per launch (preprocess_roi.cu ROI_CHUNK)
 GENERIC = "preprocess_roi_generic_kernel"
-OUTS = ("f32", "f16", "bf16")
-ESZ = {"f32": 4, "f16": 2, "bf16": 2}
 INVALID, SLICE, INVALID_SOURCE = -1, -2, -8
 F32 = np.float32
 
@@ -52,24 +44,8 @@ def expected_kernel(f, sampling, dw, dh, dst, frames):
     return GENERIC
 
 
-# ── the cases ──────────────────────────────────────────────────────────────────────────────────────────────────────────
-@dataclass(frozen=True)
-class RCase:
-    base: Case                # format, frame geometry, sampler, normalisation, pad value, dst size (f16 unused)
-    mode: int
-    out: str
-    n_frames: int
-    offsets: tuple            # each frame's byte offset in one allocation (16-B aligned base)
-    rois: tuple               # (k, x, y, w, h)
-
-    def kernel(self, dst=0):
-        return expected_kernel(self.base.fmt, self.base.sampling, self.base.dw, self.base.dh, dst, self.offsets)
-
-    def __str__(self):
-        c = self.base
-        r = self.rois if len(self.rois) <= 6 else self.rois[:6] + ("...",)
-        return (f"{c.name}: {c.fmt.name} matrix {c.matrix} bpp {c.bpp} {c.w}x{c.h} pitch {c.pitch} -> {c.dw}x{c.dh} mode {self.mode} "
-                f"{SAMPLING_NAME[c.sampling]} {self.out} norm {c.norm} pad {c.pad_value} frames {self.offsets} rois {r}")
+def roi_kernel(rc, dst=0):
+    return expected_kernel(rc.base.fmt, rc.base.sampling, rc.base.dw, rc.base.dh, dst, rc.offsets)
 
 
 def draw_rois(rng, w, h, n_frames, n):
@@ -91,20 +67,6 @@ def draw_rois(rng, w, h, n_frames, n):
                 y |= 1
         out.append((k, x, y, rw, rh))
     return tuple(out)
-
-
-def place(rng, f, need, n, odd=False):
-    """Frame offsets: even (and element-aligned), gaps between frames; `odd`: one frame of a byte format at an odd address."""
-    e = max(2, elem_align(f))
-    offs, at = [], 16
-    for _ in range(n):
-        at = -(-at // e) * e + e * int(rng.integers(0, 8))
-        offs.append(at)
-        at += need + e * int(rng.integers(1, 8))
-    if odd and elem_align(f) == 1:
-        k = int(rng.integers(0, n))
-        offs[k] += 1 - offs[k] % 2
-    return tuple(offs)
 
 
 def rcase(i):
@@ -152,101 +114,12 @@ def chunk_cases():
 CHUNKS = chunk_cases()
 
 
-# ── references ─────────────────────────────────────────────────────────────────────────────────────────────────────
-def picture(c, raw):
-    """Frame `raw` of case c decoded: (8, (h, w, 3) uint8) or (bits, (h, w, 3) uint16)."""
-    f, w, h = c.fmt, c.w, c.h
-    m = MATRICES[c.matrix]
-    rows = raw[:c.pitch * h].reshape(h, c.pitch)[:, :row_bytes(f, w, c.bpp)]
-    if f.family == "gray":
-        return 8, np.repeat(np.ascontiguousarray(rows)[:, :, None], 3, axis=2)
-    if f.family == "rgb":
-        px = np.ascontiguousarray(rows).reshape(h, w, c.bpp)[:, :, :3]
-        return 8, np.ascontiguousarray(px if f.code == 0 else px[:, :, ::-1])
-    if f.family in ("yuv420", "yuv422") and not f.words:
-        tight = raw if f.family == "yuv420" else np.ascontiguousarray(rows).reshape(-1)
-        return 8, np.asarray(decode_yuv8(tight, w, h, f.layout, m)).astype(np.uint8).reshape(h, w, 3)
-    if f.code == 11:
-        return 8, np.asarray(decode_yuv444(raw, w, h, m)).astype(np.uint8).reshape(h, w, 3)
-    if f.family == "bayer" and not f.words and not f.packed:
-        return 8, demosaic8(np.ascontiguousarray(rows), f.layout).astype(np.uint8)
-    if f.family == "bayer":
-        samples = np.ascontiguousarray(rows).view("<u2") if f.words else unpack(np.ascontiguousarray(rows), f.bits)
-        return f.bits, np.asarray(demosaic16(np.asarray(samples).astype(np.uint16), f.layout)).astype(np.uint16)
-    words = torch.from_numpy(raw.view("<u2").astype(np.int32))
-    rgb16 = (decode_yuv16 if f.family == "yuv420" else decode_yuv444_16)(words, w, h, f.name, m).numpy()
-    return f.bits, np.asarray(rgb16).astype(np.uint16).reshape(h, w, 3)
-
-
-def region_reference(rc, pic, roi):
-    """(3, dh, dw) of region roi: f32, or f16 bits for f16 output (Lanczos: f32, compared within a tolerance)."""
-    from oracle.oracle import preprocess_affine
-    c = rc.base
-    bits, arr = pic
-    _, x, y, w, h = roi
-    sx, sy, px, py = preprocess_affine(rc.mode, w, h, c.dw, c.dh)
-    h16 = rc.out == "f16" and c.sampling != LANCZOS
-    crop = np.ascontiguousarray(arr[y:y + h, x:x + w])
-    if bits == 8:
-        cc = replace(c, w=w, h=h, pitch=3 * w, scale_x=sx, scale_y=sy, pad_x=px, pad_y=py)
-        return oracle_rgb(cc, crop.reshape(-1), 0, 3, 3 * w, h16)
-    mean, inv = NORMS[c.norm]
-    return preprocess_rgb16(crop, bits, (sx, sy, px, py), c.dw, c.dh, SAMPLING_NAME[c.sampling], mean, inv, c.pad_value, h16)
-
-
-def compare(got, want, rc, what):
-    c = rc.base
-    if rc.out == "bf16" and c.sampling != LANCZOS:
-        want = torch.from_numpy(np.ascontiguousarray(want, np.float32)).to(torch.bfloat16).view(torch.int16).numpy()
-    if c.sampling == LANCZOS:
-        g = (torch.from_numpy(got.copy()).view(torch.bfloat16).float().numpy() if rc.out == "bf16"
-             else got.view(np.float16 if rc.out == "f16" else np.float32).astype(np.float32))
-        want = want.reshape(-1).astype(np.float32)
-        step = {"f32": 0.0, "f16": np.spacing(np.abs(want).astype(np.float16)).astype(np.float32),
-                "bf16": np.abs(want) * 2.0 ** -7 + 1e-38}[rc.out]
-        tol = 1e-4 * max(1.0, max(NORMS[c.norm][1]) / max(IMAGENET_INV)) + step
-        over = np.abs(g - want) - tol
-        assert over.max() <= 0, f"{what}: error {float(np.abs(g - want)[over.argmax()])} at element {int(over.argmax())}"
-    else:
-        w = np.ascontiguousarray(want).reshape(-1).view(np.uint8)
-        bad = np.flatnonzero(got != w)
-        assert bad.size == 0, f"{what}: {bad.size} bytes differ, first at byte {bad[0]}"
-
-
-# ── the call ─────────────────────────────────────────────────────────────────────────────────────────────────────────
-def roi_array(rois):
-    from kornia_rs_b200._lib import Roi
-    return (Roi * max(1, len(rois)))(*[Roi(*r) for r in rois])
-
-
 def call(lib, c, mode, ptrs, lens, rois, dst_ptr, dst_len, out, stream=None):
     from kornia_rs_b200._lib import PreprocessDesc
     d = c.desc(PreprocessDesc)
     n = len(ptrs)
     return lib.kb200_preprocess_rois(stream, C.byref(d), mode, (C.c_void_p * max(1, n))(*ptrs), (C.c_size_t * max(1, n))(*lens), n,
                                      roi_array(rois), len(rois), dst_ptr, dst_len, OUTS.index(out))
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
-def lib(kb):
-    return kb._lib.lib()
-
-
-def load_frames(dev, rc):
-    c = rc.base
-    need = c.need
-    raws = [frame_bytes(c, k) for k in range(rc.n_frames)]
-    span = rc.offsets[-1] + need + 16
-    image = np.random.default_rng(c.seed ^ 0xBAD).integers(0, 256, span, dtype=np.int64).astype(np.uint8)   # poisoned gaps
-    for s, r in zip(rc.offsets, raws):
-        image[s:s + need] = r
-    return raws, Guarded(dev, span).load("u8", image)
 
 
 def run_rcase(kb, lib, dev, rc):
@@ -265,7 +138,7 @@ def run_rcase(kb, lib, dev, rc):
         ran = kb._lib.last_kernel()
         torch.cuda.synchronize()
         want = expected_kernel(c.fmt, c.sampling, c.dw, c.dh, dst.ptr, ptrs)
-        assert ran == want == (rc.kernel(off) if off else ran), f"{rc}: dst +{off} B ran {ran}, the dispatch mirror says {want}"
+        assert ran == want == (roi_kernel(rc, off) if off else ran), f"{rc}: dst +{off} B ran {ran}, the dispatch mirror says {want}"
         for what, g in zip(("lead", "tail"), dst.guards()):
             assert (g == 0xFF).all(), f"{rc}: dst +{off} B: bytes written in the {what} guard"
         outs.append(dst.out())
@@ -277,10 +150,10 @@ def run_rcase(kb, lib, dev, rc):
     for i, roi in enumerate(rc.rois):
         if roi[0] not in pics:
             pics[roi[0]] = picture(c, raws[roi[0]])
-        compare(outs[0][i * fb:(i + 1) * fb], region_reference(rc, pics[roi[0]], roi), rc, f"{rc}: region {i} {roi}")
+        compare_region(outs[0][i * fb:(i + 1) * fb], region_reference(rc, pics[roi[0]], roi), rc, f"{rc}: region {i} {roi}")
     if len(outs) == 2:
         bad = np.flatnonzero(outs[0] != outs[1])
-        assert bad.size == 0, f"{rc}: {rc.kernel()} and {GENERIC} differ in {bad.size} bytes"
+        assert bad.size == 0, f"{rc}: {roi_kernel(rc)} and {GENERIC} differ in {bad.size} bytes"
 
 
 @pytest.mark.gpu
@@ -467,9 +340,9 @@ def test_dispatch_coverage():
     samplers, modes, dw4, outs, matrices, nmax = set(), set(), set(), set(), {}, 0
     for rc in cases:
         c = rc.base
-        kernels[c.code].add(rc.kernel())
-        kernels[c.code].add(rc.kernel(dst=ESZ[rc.out]))
-        assert rc.kernel(dst=ESZ[rc.out]) == GENERIC
+        kernels[c.code].add(roi_kernel(rc))
+        kernels[c.code].add(roi_kernel(rc, ESZ[rc.out]))
+        assert roi_kernel(rc, ESZ[rc.out]) == GENERIC
         samplers.add(c.sampling)
         modes.add(rc.mode)
         dw4.add(c.dw % 4)

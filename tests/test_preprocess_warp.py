@@ -12,7 +12,7 @@ On the GPU:
     degree rotations and both flips of RGB8 / BGR8 / Gray8 / I444 / I41x frames against the batch entry on the frame
     rotated on the host;
   * a seeded sweep (`wcase(i)`, a pure function of i, every format twice) of similarity, general affine and perspective
-    maps against the reference, each run into a test_footprint.Guarded destination with a 0xFF prefill, on the kernel a
+    maps against the reference, each run into a harness.Guarded destination with a 0xFF prefill, on the kernel a
     host mirror of the dispatch rule names, and again one element past a 16-byte boundary, where the generic kernel must
     give the same bytes;
   * region counts around the launch chunk, a captured graph, Preprocessor.run_warps with both matrix shapes;
@@ -28,17 +28,14 @@ import numpy as np
 import pytest
 import torch
 
-from test_footprint import Guarded
-from test_preprocess_roi import RCase, compare, load_frames, picture, place, roi_array
-from test_preprocess_sweep import (BILINEAR, CODES, FORMATS, LANCZOS, NEAREST, NORMS, SAMPLING_NAME, Case, frame_bytes, pad_step, row_bytes,
-                                   size_rule, src_bytes, yuv)
+from harness import Guarded, batch_entry, compare_region, dev, inverse, lib, load_frames, roi_array, warp_array
+from restate import BILINEAR, CODES, Case, ESZ, FORMATS, LANCZOS, NEAREST, NORMS, OUTS, RCase, SAMPLING_NAME, draw_map, forward_of, frame_bytes, make_case, pad_step, picture, place, row_bytes, size_rule, smooth_rgb, src_bytes, warp_coords, warp_reference, yuv
+
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BASE = 0x3A7F0000
 CHUNK = 72   # regions per launch (preprocess_warp.cu WARP_CHUNK)
 VECTOR, GENERIC = "preprocess_warp_kernel", "preprocess_warp_generic_kernel"
-OUTS = ("f32", "f16", "bf16")
-ESZ = {"f32": 4, "f16": 2, "bf16": 2}
 INVALID, SLICE, SINGULAR, UNSUPPORTED, INVALID_SOURCE = -1, -2, -3, -4, -8
 F32 = np.float32
 KINDS = ("similarity", "affine", "perspective", "edges", "wzero", "wcross", "rot90", "tiny")
@@ -47,137 +44,6 @@ KINDS = ("similarity", "affine", "perspective", "edges", "wzero", "wcross", "rot
 # ── the dispatch rule, restated (preprocess_warp.cu warp_vector_ok) ──────────────────────────────────────────────────
 def expected_kernel(dw, out, dst):
     return VECTOR if dw % 4 == 0 and dst % (16 if out == "f32" else 8) == 0 else GENERIC
-
-
-# ── the maps ───────────────────────────────────────────────────────────────────────────────────────────────────────────
-def forward_of(inv):
-    """The forward map (float32, row-major 9) whose float64 inverse is `inv` (3x3)."""
-    return tuple(float(v) for v in np.linalg.inv(np.asarray(inv, np.float64)).astype(F32).reshape(-1))
-
-
-def inverse(lib, m):
-    """(the library's f32 inverse of forward map m as a 3x3 float32 array, perspective?) — the entry's host computation."""
-    m = (C.c_float * 9)(*m)
-    out = (C.c_float * 9)()
-    persp = not (m[6] == 0.0 and m[7] == 0.0 and m[8] == 1.0)
-    if persp:
-        assert lib.kb200_invert_homography(m, out) == 0
-    else:
-        lib.kb200_invert_affine_transform(m, out)
-        out[6], out[7], out[8] = 0.0, 0.0, 1.0
-    return np.array(out[:], F32).reshape(3, 3), persp
-
-
-def draw_map(rng, kind, w, h, dw, dh):
-    """One forward map of `kind` for a w x h frame and a dw x dh output."""
-    if kind in ("similarity", "perspective", "rot90"):
-        ang = float(rng.uniform(-np.pi, np.pi)) if kind != "rot90" else float(np.pi / 2 * rng.integers(1, 4))
-        s = float(np.exp(rng.uniform(np.log(0.25), np.log(4.0))))
-        # frame point the output centre lands on: usually inside, sometimes past an edge
-        c = (float(rng.uniform(-0.3, 1.3) * w), float(rng.uniform(-0.3, 1.3) * h))
-        if kind == "rot90":   # get_rotation_matrix2d's float cos / sin: a ~1e-8 step on the axis it turns away, the degenerate rule
-            a, b = F32(np.cos(ang)) * F32(s), F32(np.sin(ang)) * F32(s)
-            m = [a, b, F32(dw / 2) - a * F32(c[0]) - b * F32(c[1]), -b, a, F32(dh / 2) + b * F32(c[0]) - a * F32(c[1]), 0, 0, 1]
-            return tuple(float(F32(v)) for v in m)
-        r = np.array([[np.cos(ang), -np.sin(ang)], [np.sin(ang), np.cos(ang)]]) / s   # output -> frame
-        inv = np.eye(3)
-        inv[:2, :2] = r
-        inv[:2, 2] = np.array(c) - r @ np.array([dw / 2, dh / 2])
-        if kind == "perspective":
-            p = np.eye(3)
-            p[2, :2] = rng.uniform(-0.03, 0.03, 2)
-            inv = inv @ p
-            if rng.random() < 0.2:   # an inverse of tiny scale: |w| < 1e-10 at every pixel, all pad
-                return tuple(float(F32(v) * F32(1e12)) for v in forward_of(inv))
-        return forward_of(inv)
-    if kind == "affine":
-        inv = np.eye(3)
-        inv[:2, :2] = rng.uniform(-2.0, 2.0, (2, 2))
-        while abs(np.linalg.det(inv[:2, :2])) < 0.05:
-            inv[:2, :2] = rng.uniform(-2.0, 2.0, (2, 2))
-        inv[:2, 2] = rng.uniform(-0.5, 1.5, 2) * (w, h)
-        return forward_of(inv)
-    if kind == "edges":
-        # a translation (or an x2 upscale, half-integer samples: nearest's ties) that puts column / row 0 of the output on
-        # 0, W - 1, the float below W or W
-        tx = [0.0, w - 1.0, float(np.nextafter(F32(w), F32(0))), float(w)][int(rng.integers(0, 4))]
-        ty = [0.0, h - 1.0, float(np.nextafter(F32(h), F32(0))), float(h)][int(rng.integers(0, 4))]
-        if rng.random() < 0.5:
-            tx, ty = (float(-rng.integers(0, dw)) + tx, ty) if rng.random() < 0.5 else (tx, float(-rng.integers(0, dh)) + ty)
-        s = 2.0 if rng.random() < 0.3 else 1.0
-        return (s, 0.0, -s * tx, 0.0, s, -s * ty, 0.0, 0.0, 1.0)
-    if kind == "wzero":
-        # w = x - c exactly (c a power of two): |w| < 1e-10 on column c, negative left of it
-        c = float(2 ** int(rng.integers(0, max(1, int(np.log2(max(dw - 1, 1))) + 1))))
-        t = rng.uniform(-0.5, 0.5, 2) * (w, h)
-        return (1.0, 0.0, float(F32(t[0])), 0.0, 1.0, float(F32(t[1])), 1.0 / c, 0.0, -1.0 / c) if rng.random() < 0.5 else \
-            (1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 1.0 / c, 0.0, -1.0 / c)
-    if kind == "wcross":
-        inv = np.eye(3)
-        inv[:2, :2] = rng.uniform(-1.5, 1.5, (2, 2))
-        inv[:2, 2] = rng.uniform(0, 1, 2) * (w, h)
-        gx, gy = rng.uniform(-2, 2, 2) / (dw, dh)
-        inv[2] = (gx, gy, -(gx * rng.uniform(0, dw) + gy * rng.uniform(0, dh)) + rng.uniform(-1e-3, 1e-3))
-        if abs(np.linalg.det(inv)) < 1e-6:
-            inv[2, 2] += 0.5
-        return forward_of(inv)
-    # "tiny": a map whose output is a few frame pixels, and the frame's corner regions
-    s = float(rng.choice([0.125, 0.25, 8.0]))
-    return (s, 0.0, -s * float(rng.integers(-2, w + 2)), 0.0, s, -s * float(rng.integers(-2, h + 2)), 0.0, 0.0, 1.0)
-
-
-# ── the reference ──────────────────────────────────────────────────────────────────────────────────────────────────────
-def warp_coords(inv, persp, dw, dh, w, h):
-    """warp_coord on inverse `inv` over a dw x dh output: (sx, sy, inside, |w| < 1e-10 mask), float32."""
-    x = np.arange(dw, dtype=F32)[None, :]
-    y = np.arange(dh, dtype=F32)[:, None]
-    m = inv.reshape(-1)
-    with np.errstate(all="ignore"):
-        if persp:
-            ww = (m[6] * x + m[7] * y) + m[8]
-            small = np.abs(ww) < F32(1e-10)
-            sx = ((m[0] * x + m[1] * y) + m[2]) / ww
-            sy = ((m[3] * x + m[4] * y) + m[5]) / ww
-            inside = ~small & (sx >= 0) & (sx < F32(w)) & (sy >= 0) & (sy < F32(h))
-        else:
-            sx0 = np.broadcast_to(m[1] * y + m[2], (dh, dw))
-            sy0 = np.broadcast_to(m[4] * y + m[5], (dh, dw))
-            sx = m[0] * x + sx0
-            sy = m[3] * x + sy0
-            ax = sx0 if abs(m[0]) < F32(1e-6) else sx
-            ay = sy0 if abs(m[3]) < F32(1e-6) else sy
-            inside = (ax >= 0) & (ax < F32(w)) & (ay >= 0) & (ay < F32(h))
-            small = np.zeros((dh, dw), bool)
-    return sx.astype(F32), sy.astype(F32), inside, small
-
-
-def warp_reference(pic, inv, persp, dw, dh, sampling, norm, pad_value, out):
-    """(3, dh, dw) of one region: f32, or f16 bits for f16 output."""
-    bits, arr = pic
-    h, w = arr.shape[:2]
-    sx, sy, inside, _ = warp_coords(inv, persp, dw, dh, w, h)
-    # the degenerate-axis clamp: [0, the float below W]; it moves no other inside coordinate
-    sx = np.where(inside, np.minimum(np.maximum(sx, F32(0)), np.nextafter(F32(w), F32(0))), F32(0))
-    sy = np.where(inside, np.minimum(np.maximum(sy, F32(0)), np.nextafter(F32(h), F32(0))), F32(0))
-    t = arr.astype(F32)
-    fx, fy = np.floor(sx), np.floor(sy)
-    if sampling == NEAREST:   # roundf: half away from zero, here on s >= 0
-        xn = np.clip(fx.astype(np.int64) + (sx - fx >= F32(0.5)), 0, w - 1)
-        yn = np.clip(fy.astype(np.int64) + (sy - fy >= F32(0.5)), 0, h - 1)
-        px = t[yn, xn]
-    else:
-        ax, ay = (sx - fx)[..., None], (sy - fy)[..., None]
-        x0, y0 = np.maximum(fx.astype(np.int64), 0), np.maximum(fy.astype(np.int64), 0)
-        x1, y1 = np.minimum(fx.astype(np.int64) + 1, w - 1), np.minimum(fy.astype(np.int64) + 1, h - 1)
-        top = t[y0, x0] + (t[y0, x1] - t[y0, x0]) * ax   # a zero weight adds exactly 0: the tap not read
-        bot = t[y1, x0] + (t[y1, x1] - t[y1, x0]) * ax
-        px = top + (bot - top) * ay
-    mean, inv_std = (np.array(v, F32) for v in NORMS[norm])
-    q = px / F32(255 if bits == 8 else (1 << bits) - 1)
-    o = (q - mean) * inv_std
-    padv = (F32(pad_value) / F32(255) - mean) * inv_std
-    o = np.where(inside[..., None], o, padv).astype(F32).transpose(2, 0, 1)
-    return np.ascontiguousarray(o.astype(np.float16) if out == "f16" else o)
 
 
 # ── the cases ──────────────────────────────────────────────────────────────────────────────────────────────────────────
@@ -201,11 +67,6 @@ class WCase:
         c = self.base
         return (f"{c.name}: {c.fmt.name} matrix {c.matrix} bpp {c.bpp} {c.w}x{c.h} pitch {c.pitch} -> {c.dw}x{c.dh} {SAMPLING_NAME[c.sampling]} "
                 f"{self.out} norm {c.norm} pad {c.pad_value} frames {self.offsets} {len(self.warps)} maps, first {self.warps[:2]}")
-
-
-def make_case(name, seed, code, matrix, bpp, w, h, pitch, dw, dh, sampling, norm, pad_value):
-    return Case(name, seed, code, matrix, bpp, w, h, pitch, "warp", 1.0, 1.0, 0.0, 0.0, dw, dh, sampling, False, "table", 1, (), None, 0, norm,
-                pad_value)
 
 
 def wcase(i):
@@ -256,29 +117,12 @@ def chunk_cases():
 CHUNKS = chunk_cases()
 
 
-# ── the call ─────────────────────────────────────────────────────────────────────────────────────────────────────────
-def warp_array(warps):
-    from kornia_rs_b200._lib import WarpRoi
-    return (WarpRoi * max(1, len(warps)))(*[WarpRoi(k, (C.c_float * 9)(*m)) for k, m in warps])
-
-
 def call(lib, c, ptrs, lens, warps, dst_ptr, dst_len, out, stream=None, desc=None):
     from kornia_rs_b200._lib import PreprocessDesc
     d = desc if desc is not None else c.desc(PreprocessDesc)
     n = len(ptrs)
     return lib.kb200_preprocess_warps(stream, C.byref(d), (C.c_void_p * max(1, n))(*ptrs), (C.c_size_t * max(1, n))(*lens) if lens is not None else None,
                                       n, warp_array(warps), len(warps), dst_ptr, dst_len, OUTS.index(out))
-
-
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
-def lib(kb):
-    return kb._lib.lib()
 
 
 def run_wcase(kb, lib, dev, wc):
@@ -310,7 +154,7 @@ def run_wcase(kb, lib, dev, wc):
             pics[k] = picture(c, raws[k])
         inv, persp = inverse(lib, fwd)
         want = warp_reference(pics[k], inv, persp, c.dw, c.dh, c.sampling, c.norm, c.pad_value, wc.out)
-        compare(outs[0][i * fb:(i + 1) * fb], want, wc.rcase, f"{wc}: region {i} frame {k} map {fwd}")
+        compare_region(outs[0][i * fb:(i + 1) * fb], want, wc.rcase, f"{wc}: region {i} frame {k} map {fwd}")
     bad = np.flatnonzero(outs[0] != outs[1])
     assert bad.size == 0, f"{wc}: {wc.kernel()} and {GENERIC} differ in {bad.size} bytes"
 
@@ -325,14 +169,6 @@ def test_sweep(kb, lib, dev, i):
 @pytest.mark.parametrize("name", [c.base.name for c in CHUNKS])
 def test_chunking(kb, lib, dev, name):
     run_wcase(kb, lib, dev, next(c for c in CHUNKS if c.base.name == name))
-
-
-def batch_entry(lib, c, out, ptrs, dst):
-    """The batch entry on the frames at ptrs with the descriptor's scale 1, pad 0 (Stretch of a frame to its own size)."""
-    from kornia_rs_b200._lib import PreprocessDesc
-    d = c.desc(PreprocessDesc)
-    fn = getattr(lib, f"kb200_preprocess_{out}")
-    return fn(None, C.byref(d), (C.c_void_p * len(ptrs))(*ptrs), None, len(ptrs), dst.data_ptr(), dst.numel() * dst.element_size() // ESZ[out])
 
 
 @pytest.mark.gpu
@@ -508,16 +344,6 @@ def test_python_run_warps(kb, lib, dev, fmt):
         for g in got:
             assert torch.equal(g.view(torch.uint8), want.view(torch.uint8)), (fmt, dtype)
         assert torch.equal(dst23.view(torch.uint8), want[affine].view(torch.uint8)), (fmt, dtype)
-
-
-def smooth_rgb(w, h, seed):
-    rng = np.random.default_rng(seed)
-    y, x = np.mgrid[0:h, 0:w].astype(np.float64)
-    chans = []
-    for _ in range(3):
-        a, b, p, q = rng.uniform(0.02, 0.08, 4)
-        chans.append(127.5 + 60 * np.sin(a * x + b * y + p * 10) + 50 * np.cos(q * x - a * y))
-    return np.clip(np.rint(np.stack(chans, axis=2)), 0, 255).astype(np.uint8)
 
 
 @pytest.mark.gpu

@@ -23,8 +23,9 @@ import numpy as np
 import pytest
 import torch
 
-from test_gpu_variants import cu, rot
-from test_launch_shapes import compare_frames, free_device_memory, knobs
+from harness import compare_frames, cu, dev, free_device_memory, knobs, rot
+from restate import NAMED_FUSED_MODES, _remap_maps, demosaic, filter_kernel, preprocess_rgb16
+
 
 F32 = np.float32
 FLT_MIN = float(np.finfo(np.float32).tiny)
@@ -233,12 +234,6 @@ def test_blur_taps_reach_the_u8_bound(oracle):
 
 
 # ═══ GPU ════════════════════════════════════════════════════════════════════════════════════════════════════════
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
 def stack(fn, src):
     return np.stack([fn(s) for s in src])
 
@@ -330,7 +325,6 @@ def test_warps_f32_values(kb, oracle, dev, kind):
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind", KINDS)
 def test_remap_f32_values(kb, oracle, dev, kind):
-    from test_gpu_parity import _remap_maps
     n, sw, sh, dw, dh = 2, 64, 48, 64, 40
     mx, my = _remap_maps(dw, dh, sw, sh, "swirl", np.random.default_rng(3))
     mxi, myi = kb.Image(cu(mx[..., None], dev)), kb.Image(cu(my[..., None], dev))
@@ -346,15 +340,6 @@ def test_remap_f32_values(kb, oracle, dev, kind):
 
 # ── filters ──
 FILTER_SHAPES = [(1100, 40, 1, 1), (700, 37, 3, 1), (97, 61, 3, 2), (33, 50, 4, 1), (5, 5, 1, 1)]
-
-
-def filter_kernel(w, c, op):
-    """try_sep_stream (csrc/filter.cu): rows of a whole number of float4 (>= 16 floats) and a streaming instance for
-    (C, K, sobel) -> the streaming kernel; everything else (and every kx != ky filter) -> the tile kernel."""
-    k = int(op[-1]) if op != "sep" else 0
-    inst = (op.startswith("gauss") and c in (1, 3, 4) and k in (3, 5, 7) and not (c == 4 and k == 7)) or \
-           (op.startswith("sobel") and c in (1, 3) and k in (3, 5))
-    return "sep_filter_stream2_kernel" if inst and (w * c) % 4 == 0 and w * c >= 16 else "sep_filter_fused_kernel"
 
 
 @pytest.mark.gpu
@@ -507,7 +492,6 @@ def test_min_max_values(kb, oracle, dev, kind):
 @pytest.mark.gpu
 @pytest.mark.parametrize("leaf", [0, 1])
 def test_fused_resize_extreme_scale_bias(kb, oracle, dev, leaf):
-    from test_gpu_variants import NAMED_FUSED_MODES
     n = 2
     params = [([3e38, 1e37, -2e36], [1e38, -3e38, 0.0]), ([1.0 / 255.0, -1.0, 0.0], [-0.0, -0.0, -0.0]),
               ([0.0, -0.0, 1e-40], [-0.0, 0.0, -1e-41])]
@@ -598,7 +582,6 @@ def test_preprocess_normalisation_values(kb, oracle, dev, param, f16):
     NV12 twin for the other 4:2:0 layouts, on the demosaiced RGB twin for Bayer).  Lanczos: the device's own unit-scale
     run gives q = px / 255 exactly (q - 0 = q, q * 1 = q), and the normalisation of q is restated in f32; the sinf of two
     math libraries keeps Lanczos taps from being compared with the oracle bit for bit (test_gpu_variants)."""
-    from test_bayer import demosaic
     dt = torch.float16 if f16 else torch.float32
     for label, fmt, mode, sampling, (w, h, dw, dh), kernel in PRE_KERNELS:
         bayer = fmt.startswith("Bayer")
@@ -635,9 +618,8 @@ def test_preprocess_normalisation_values(kb, oracle, dev, param, f16):
 @pytest.mark.parametrize("param", PARAMS, ids=PARAM_IDS)
 @pytest.mark.parametrize("f16", [False, True])
 def test_preprocess_bayer16_normalisation_values(kb, oracle, dev, param, f16):
-    """The 16-bit Bayer identity kernel and the generic Bayer16 kernel against the f32 restatement of test_bayer16.py
+    """The 16-bit Bayer identity kernel and the generic Bayer16 kernel against the f32 restatement in restate.py
     (samples over the whole 12-bit range), converted to f16 by the oracle's f2h (the reference's conversion rules)."""
-    from test_bayer16 import demosaic, preprocess_rgb16
     w, h, bits = 64, 48, 12
     raw = np.random.default_rng(0xB16).permutation(np.resize(np.arange(1 << bits, dtype=np.uint16), w * h))
     raw[:8] = (1 << bits) - 1

@@ -14,28 +14,15 @@ import numpy as np
 import pytest
 import torch
 
-from test_bayer16 import check_against_restatement, offset_u16, restated
+from harness import check_against_restatement, dev, make_pre, offset_buf, random_words, restated, yuv16_identity
+from restate import BITS, KR_KB, MATRICES, TABLE16, decode_yuv16, q16, white
+
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
-MATRICES = ("Bt601Limited", "Bt601Full", "Bt709Limited", "Bt709Full")   # kb200_yuv_matrix order
 FORMATS = ("P010", "P012", "I010", "I012")
 CODE = {"P010": 80, "P012": 81, "I010": 82, "I012": 83}
-BITS = {"P010": 10, "P012": 12, "I010": 10, "I012": 12}
 LAYOUT = {"P010": 0, "P012": 0, "I010": 1, "I012": 1}   # kb200_yuv420_u16_layout: P01X, I01X
-
-# ── the specification: (y_off, cy, cvr, cub, cug, cvg) per depth and matrix, Q16 ──
-TABLE16 = {
-    10: {"Bt601Limited": (64, 76533, 104905, 132590, -25750, -53435), "Bt601Full": (0, 65536, 91881, 116130, -22553, -46802),
-         "Bt709Limited": (64, 76533, 117835, 138846, -14017, -35027), "Bt709Full": (0, 65536, 103206, 121609, -12276, -30679)},
-    12: {"Bt601Limited": (256, 76590, 104982, 132687, -25769, -53475), "Bt601Full": (0, 65536, 91881, 116130, -22553, -46802),
-         "Bt709Limited": (256, 76590, 117921, 138947, -14027, -35053), "Bt709Full": (0, 65536, 103206, 121609, -12276, -30679)},
-}
-KR_KB = {"Bt601": (0.299, 0.114), "Bt709": (0.2126, 0.0722)}
-
-
-def white(bits):
-    return (1 << bits) - 1
 
 
 def float_coeffs16(m, bits):
@@ -46,39 +33,6 @@ def float_coeffs16(m, bits):
     full = m.endswith("Full")
     sy, sc = (1.0, 1.0) if full else (w / (219.0 * s), w / (224.0 * s))
     return (0 if full else 16 * s, sy, 2 * (1 - kr) * sc, 2 * (1 - kb_) * sc, -2 * kb_ * (1 - kb_) / kg * sc, -2 * kr * (1 - kr) / kg * sc)
-
-
-# ── the restatement (torch, any device; int64) ──
-def q16(y, u, v, m, bits):
-    """The Q16 decode of n-bit code tensors y, u, v with matrix m -> [..., 3] int64 codes 0..W."""
-    yo, cy, cvr, cub, cug, cvg = TABLE16[bits][m]
-    half = 1 << (bits - 1)
-    yy = (y - yo).clamp(min=0) * cy
-    u, v = u - half, v - half
-    r = (yy + cvr * v + (1 << 15)) >> 16
-    g = (yy + cug * u + cvg * v + (1 << 15)) >> 16
-    b = (yy + cub * u + (1 << 15)) >> 16
-    return torch.stack([r, g, b], -1).clamp(0, white(bits))
-
-
-def codes(words, fmt):
-    """16-bit words -> their n-bit codes (int64): the high bits of a P01x word, the low bits of an I01x word."""
-    wd = words.to(torch.int32).to(torch.int64) & 0xFFFF
-    bits = BITS[fmt]
-    return wd >> (16 - bits) if fmt[0] == "P" else wd & white(bits)
-
-
-def decode(raw, w, h, fmt, m):
-    """Frames [..., w*h*3/2] of 16-bit words -> [..., h, w, 3] int64, reading the layout directly (chroma replicated)."""
-    c = codes(raw, fmt)
-    lead = c.shape[:-1]
-    y, ch, q = c[..., :w * h].reshape(*lead, h, w), c[..., w * h:], (w // 2) * (h // 2)
-    u, v = (ch[..., 0::2], ch[..., 1::2]) if fmt[0] == "P" else (ch[..., :q], ch[..., q:])
-
-    def up(a):
-        return a.reshape(*lead, h // 2, w // 2).repeat_interleave(2, -2).repeat_interleave(2, -1)
-
-    return q16(y, up(u), up(v), m, BITS[fmt])
 
 
 def pack(yc, uc, vc, fmt, junk=None):
@@ -94,11 +48,6 @@ def pack(yc, uc, vc, fmt, junk=None):
         if junk is not None:
             words = words | ((junk << bits) & 0xFFFF)
     return words.to(torch.int32).to(torch.uint16)
-
-
-def random_words(shape, seed):
-    g = torch.Generator().manual_seed(seed)
-    return torch.randint(0, 1 << 16, shape, generator=g, dtype=torch.int32).to(torch.uint16)
 
 
 # ═══ CPU ═══════════════════════════════════════════════════════════════════════════════════════════════════════
@@ -266,14 +215,8 @@ def test_python_decoders_check_their_operands(kb):
 
 
 # ═══ GPU ═══════════════════════════════════════════════════════════════════════════════════════════════════════
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
 def run_decode(kb, dev, fmt, src, w, h, n, m, dst_off=0):
-    out = offset_u16(dev, n * h * w * 3, dst_off)
+    out = offset_buf(dev, n * h * w * 3, dst_off, torch.uint16)
     out.fill_(0xCDCD)
     getattr(kb.imgproc, f"rgb_from_{fmt.lower()}")(src, kb.Image(out.view(n, h, w, 3)), matrix=kb.YuvMatrix[m])
     return out.view(n, h, w, 3), kb._lib.last_kernel()
@@ -300,12 +243,12 @@ def test_decode(kb, dev, fmt, m):
     for w, h, n, soff, doff in DECODE_CASES:
         nw = w * h * 3 // 2
         raws = random_words((n, nw), w * 131 + h + 7 * n + 1000 * MATRICES.index(m) + 17 * CODE[fmt])
-        src = offset_u16(dev, n * nw, soff)
+        src = offset_buf(dev, n * nw, soff, torch.uint16)
         src.copy_(raws.reshape(-1).to(dev))
         got, kern = run_decode(kb, dev, fmt, src.view(n, nw), w, h, n, m, doff)
         what = f"{fmt} {m} {(w, h, n, soff, doff)}"
         assert kern == decode_kernel(fmt, w, soff, doff), what
-        want = decode(raws, w, h, fmt, m)
+        want = decode_yuv16(raws, w, h, fmt, m)
         assert torch.equal(got.cpu().to(torch.int32).to(torch.int64), want), what
 
 
@@ -329,7 +272,7 @@ def test_decode_ignored_bits_extremes_and_repack(kb, dev, w, h, m):
                                   pack(maxed, mc, mc, fmt), pack(maxed, mc, mc, fmt, junk)])
             got, _ = run_decode(kb, dev, fmt, frames.to(dev), w, h, len(frames), m)
             g = got.cpu().to(torch.int32).to(torch.int64)
-            assert torch.equal(g, decode(frames, w, h, fmt, m)), fmt
+            assert torch.equal(g, decode_yuv16(frames, w, h, fmt, m)), fmt
             assert torch.equal(g[0], g[1]), f"{fmt}: garbage in the ignored bits changed the output"
             assert torch.equal(g[3], g[4]), fmt
             outs[fmt] = g
@@ -346,7 +289,7 @@ def test_decode_1080p_batch(kb, dev, fmt, m):
     got, kern = run_decode(kb, dev, fmt, raw, w, h, n, m)
     assert kern == decode_kernel(fmt, w, 0, 0)
     for k0 in range(0, n, 16):
-        assert torch.equal(got[k0:k0 + 16].to(torch.int32).to(torch.int64), decode(raw[k0:k0 + 16], w, h, fmt, m)), f"frames {k0}.."
+        assert torch.equal(got[k0:k0 + 16].to(torch.int32).to(torch.int64), decode_yuv16(raw[k0:k0 + 16], w, h, fmt, m)), f"frames {k0}.."
     del got, raw
     torch.cuda.empty_cache()
 
@@ -362,11 +305,6 @@ def expected_preprocess_kernel(fmt, sampling, w, h, dw, dh, mode):
     if (dw, dh) == (w, h) and w % 4 == 0:
         return f"preprocess_{k}_identity_kernel"
     return f"preprocess_{k}_kernel" if dw % 4 == 0 else "preprocess_generic_kernel"
-
-
-def make_pre(kb, fmt, mode, sampling, m):
-    return (kb.Preprocessor.builder().source_format(kb.SourceFormat[fmt]).mode(kb.ResizeMode[mode]).sampling(kb.InterpolationMode[sampling])
-            .normalize(kb.Normalize.imagenet()).pad_value(114).yuv_matrix(kb.YuvMatrix[m]).build_cuda())
 
 
 @pytest.mark.gpu
@@ -392,7 +330,7 @@ def test_preprocess(kb, dev, fmt, m, mode, sampling, f16):
         strided = torch.full_like(got, float("nan"))
         pre.run_raw_strided(ring.view(-1), 2 * (nw + 12), n, w, h, strided, f16=f16)
         assert torch.equal(strided.view(it), got.view(it)), what
-        rgb = decode(raws, w, h, fmt, m).numpy().astype(np.uint16)
+        rgb = decode_yuv16(raws, w, h, fmt, m).numpy().astype(np.uint16)
         for k in range(n):
             o = restated(kb, rgb[k], BITS[fmt], mode, sampling, dw, dh, f16 and sampling != "Lanczos")
             check_against_restatement(got[k], o, sampling, f16, f"{what} frame {k}")
@@ -411,7 +349,7 @@ def test_preprocess_unaligned_frames(kb, dev, fmt):
         want = torch.full((1, 3, dh, dw), float("nan"), device=dev)
         pre.run_raw(raw, w, h, want)
         k_aligned = kb._lib.last_kernel()
-        shifted = offset_u16(dev, nw, 1)
+        shifted = offset_buf(dev, nw, 1, torch.uint16)
         shifted.copy_(raw)
         got = torch.full_like(want, float("nan"))
         pre.run_raw(shifted, w, h, got)
@@ -419,17 +357,6 @@ def test_preprocess_unaligned_frames(kb, dev, fmt):
         assert k_aligned == (f"preprocess_{k}_identity_kernel" if dw == w else f"preprocess_{k}_kernel")
         assert kb._lib.last_kernel() == f"preprocess_{k}_kernel"
         assert torch.equal(got.view(torch.int32), want.view(torch.int32))
-
-
-def torch_identity(raw, w, h, fmt, m, kb):
-    """Config 3a of frames [n, w*h*3/2] on the device: the restatement's decode, then (px / W - mean) * inv_std as
-    separate IEEE f32 operations."""
-    # the divisor is a device tensor: torch turns division by a host scalar into a multiplication by its reciprocal
-    wl = torch.full((1,), float(white(BITS[fmt])), dtype=torch.float32, device=raw.device)
-    rgb = decode(raw, w, h, fmt, m).to(torch.float32) / wl
-    mean = torch.tensor(kb.IMAGENET_MEAN, dtype=torch.float32, device=raw.device)
-    inv = torch.tensor(1.0, dtype=torch.float32) / torch.tensor(kb.IMAGENET_STD, dtype=torch.float32)
-    return ((rgb - mean) * inv.to(raw.device)).permute(0, 3, 1, 2)
 
 
 @pytest.mark.gpu
@@ -450,7 +377,7 @@ def test_preprocess_identity_1080p(kb, dev, fmt, m, n):
     def check(entry):
         assert kb._lib.last_kernel() == kernel, entry
         for k0 in range(0, n, 16):
-            want = torch_identity(frames[k0:k0 + 16], w, h, fmt, m, kb)
+            want = yuv16_identity(frames[k0:k0 + 16], w, h, fmt, m, kb)
             assert torch.equal(got[k0:k0 + 16].view(torch.int32), want.contiguous().view(torch.int32)), f"{entry} frames {k0}.."
 
     pre.run_raw_batch([frames[k] for k in range(n)], w, h, got)
@@ -459,7 +386,7 @@ def test_preprocess_identity_1080p(kb, dev, fmt, m, n):
     pre.run_raw_strided(ring.view(-1), 2 * (nw + 32), n, w, h, got)
     check("strided")
     for k in sorted({0, 255, n - 1}):   # the f32 restatement of the oracle on frames on both sides of the launch split
-        rgb = decode(frames[k].cpu(), w, h, fmt, m).numpy().astype(np.uint16)
+        rgb = decode_yuv16(frames[k].cpu(), w, h, fmt, m).numpy().astype(np.uint16)
         o = restated(kb, rgb, BITS[fmt], "Stretch", "Bilinear", w, h)
         np.testing.assert_array_equal(got[k].cpu().numpy().view(np.uint32), o.view(np.uint32), f"frame {k}")
     del got, ring, frames

@@ -15,47 +15,17 @@ import numpy as np
 import pytest
 import torch
 
-from test_bayer16 import check_against_restatement, offset_u16, restated
-from test_footprint import Case, Guarded, neighbour_frames, poison, run_guarded
-from test_yuv16 import q16, random_words
-from test_yuv_layouts import offset_u8
-from test_yuv_matrix import TABLE, oracle_cfg, q20
+from harness import FootprintCase, Guarded, check_against_restatement, dev, make_pre, neighbour_frames, offset_buf, oracle_cfg, poison, random_bytes, random_words, restated, run_guarded
+from restate import BITS, MATRICES, TABLE, decode_yuv444, decode_yuv444_16, white
+
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
-MATRICES = ("Bt601Limited", "Bt601Full", "Bt709Limited", "Bt709Full")   # kb200_yuv_matrix order
 FORMATS = ("I444", "I410", "I412", "I410Msb", "I412Msb")
 WORDS = FORMATS[1:]
 CODE = {"I444": 11, "I410": 85, "I412": 86, "I410Msb": 87, "I412Msb": 88}
-BITS = {"I444": 8, "I410": 10, "I412": 12, "I410Msb": 10, "I412Msb": 12}
 LAYOUT = {"I410": 0, "I412": 0, "I410Msb": 1, "I412Msb": 1}   # kb200_yuv444_u16_layout: I41X, I41X_MSB
 TWIN420 = {"I410": "I010", "I412": "I012"}
-
-
-def white(bits):
-    return (1 << bits) - 1
-
-
-# ── the restatement ──
-def codes(words, fmt):
-    """16-bit words -> their n-bit codes (int64): the low bits of an I41x word, the high bits of an Msb word."""
-    wd = words.to(torch.int32).to(torch.int64) & 0xFFFF
-    bits = BITS[fmt]
-    return wd >> (16 - bits) if fmt.endswith("Msb") else wd & white(bits)
-
-
-def decode16(raw, w, h, fmt, m):
-    """Frames [..., 3*w*h] of 16-bit words -> [..., h, w, 3] int64, each pixel from its own Y, U, V."""
-    c = codes(raw, fmt)
-    lead = c.shape[:-1]
-    y, u, v = (c[..., k * w * h:(k + 1) * w * h].reshape(*lead, h, w) for k in range(3))
-    return q16(y, u, v, m, BITS[fmt])
-
-
-def decode8(raw, w, h, m):
-    """One I444 frame (numpy bytes, 3*w*h) -> [h, w, 3] RGB8."""
-    y, u, v = (raw[k * w * h:(k + 1) * w * h].reshape(h, w) for k in range(3))
-    return q20(y, u, v, m)
 
 
 def pack16(yc, uc, vc, fmt, junk=None):
@@ -83,10 +53,6 @@ def i01x_to_i41x(raw, w, h):
     q = (w // 2) * (h // 2)
     up = lambda a: a.reshape(h // 2, w // 2).repeat_interleave(2, 0).repeat_interleave(2, 1).reshape(-1)
     return torch.cat([raw[:w * h], up(raw[w * h:w * h + q]), up(raw[w * h + q:])])
-
-
-def raw_bytes(n, seed):
-    return np.random.default_rng(seed).integers(0, 256, n, dtype=np.uint8)
 
 
 # ═══ CPU ═══════════════════════════════════════════════════════════════════════════════════════════════════════
@@ -225,25 +191,19 @@ def test_bt601_full_i444_within_one_level_of_cv2():
     """JPEG's 4:4:4: an I444 frame decoded with Bt601Full is within one level of cv2 on the interleaved (Y, Cr, Cb) image."""
     cv2 = pytest.importorskip("cv2")
     w, h = 256, 192
-    raw = raw_bytes(3 * w * h, 444)
+    raw = random_bytes(3 * w * h, 444)
     y, u, v = (raw[k * w * h:(k + 1) * w * h].reshape(h, w) for k in range(3))
     ref = cv2.cvtColor(np.ascontiguousarray(np.stack([y, v, u], -1)), cv2.COLOR_YCrCb2RGB).astype(np.int64)
-    assert np.abs(decode8(raw, w, h, "Bt601Full").astype(np.int64) - ref).max() <= 1
+    assert np.abs(decode_yuv444(raw, w, h, "Bt601Full").astype(np.int64) - ref).max() <= 1
 
 
 # ═══ GPU ═══════════════════════════════════════════════════════════════════════════════════════════════════════
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
 def run_decode(kb, dev, fmt, src, w, h, n, m, dst_off=0):
     if fmt == "I444":
-        out = offset_u8(dev, n * h * w * 3, dst_off)
+        out = offset_buf(dev, n * h * w * 3, dst_off, torch.uint8)
         out.fill_(0xCD)
     else:
-        out = offset_u16(dev, n * h * w * 3, dst_off)
+        out = offset_buf(dev, n * h * w * 3, dst_off, torch.uint16)
         out.fill_(0xCDCD)
     getattr(kb.imgproc, f"rgb_from_{fmt.lower()}")(src, kb.Image(out.view(n, h, w, 3)), matrix=kb.YuvMatrix[m])
     return out.view(n, h, w, 3), kb._lib.last_kernel()
@@ -275,19 +235,19 @@ def test_decode(kb, dev, fmt, m):
         seed = w * 131 + h + 7 * n + 1000 * MATRICES.index(m) + 17 * CODE[fmt] + soff + 5 * doff
         what = f"{fmt} {m} {(w, h, n, soff, doff)}"
         if fmt == "I444":
-            raws = raw_bytes(n * ne, seed).reshape(n, ne)
-            src = offset_u8(dev, n * ne, soff)
+            raws = random_bytes(n * ne, seed).reshape(n, ne)
+            src = offset_buf(dev, n * ne, soff, torch.uint8)
             src.copy_(torch.from_numpy(raws.reshape(-1)))
             got, kern = run_decode(kb, dev, fmt, src.view(n, ne), w, h, n, m, doff)
             g = got.cpu().numpy()
             for k in range(n):
-                np.testing.assert_array_equal(g[k], decode8(raws[k], w, h, m), f"{what} frame {k}")
+                np.testing.assert_array_equal(g[k], decode_yuv444(raws[k], w, h, m), f"{what} frame {k}")
         else:
             raws = random_words((n, ne), seed)
-            src = offset_u16(dev, n * ne, soff)
+            src = offset_buf(dev, n * ne, soff, torch.uint16)
             src.copy_(raws.reshape(-1).to(dev))
             got, kern = run_decode(kb, dev, fmt, src.view(n, ne), w, h, n, m, doff)
-            assert torch.equal(got.cpu().to(torch.int32).to(torch.int64), decode16(raws, w, h, fmt, m)), what
+            assert torch.equal(got.cpu().to(torch.int32).to(torch.int64), decode_yuv444_16(raws, w, h, fmt, m)), what
         assert kern == decode_kernel(fmt, w, soff, doff), what
 
 
@@ -299,7 +259,7 @@ def test_decode_twins(kb, dev, w, h, m):
     against I01x (random words, garbage in the ignored bits); an Msb frame holding code << (16 - n) with junk in the low
     bits decodes like its low-bit twin."""
     n = 3
-    i420 = raw_bytes(n * w * h * 3 // 2, w + h).reshape(n, -1)
+    i420 = random_bytes(n * w * h * 3 // 2, w + h).reshape(n, -1)
     want = torch.empty(n, h, w, 3, dtype=torch.uint8, device=dev)
     kb.imgproc.rgb_from_i420(torch.from_numpy(i420).to(dev), kb.Image(want), matrix=kb.YuvMatrix[m])
     i444 = np.stack([i420_to_i444(f, w, h) for f in i420])
@@ -336,9 +296,9 @@ def test_decode_1080p_batch(kb, dev, fmt, m):
     assert kern == decode_kernel(fmt, w, 0, 0)
     for k in (0, 13, n - 1):
         if fmt == "I444":
-            np.testing.assert_array_equal(got[k].cpu().numpy(), decode8(raw[k].cpu().numpy(), w, h, m), f"frame {k}")
+            np.testing.assert_array_equal(got[k].cpu().numpy(), decode_yuv444(raw[k].cpu().numpy(), w, h, m), f"frame {k}")
         else:
-            assert torch.equal(got[k].cpu().to(torch.int32).to(torch.int64), decode16(raw[k].cpu(), w, h, fmt, m)), f"frame {k}"
+            assert torch.equal(got[k].cpu().to(torch.int32).to(torch.int64), decode_yuv444_16(raw[k].cpu(), w, h, fmt, m)), f"frame {k}"
     del got, raw
     torch.cuda.empty_cache()
 
@@ -359,15 +319,9 @@ def expected_preprocess_kernel(fmt, sampling, w, h, dw, dh):
     return f"preprocess_{k}_kernel" if dw % 4 == 0 else "preprocess_generic_kernel"
 
 
-def make_pre(kb, fmt, mode, sampling, m=None):
-    b = (kb.Preprocessor.builder().source_format(kb.SourceFormat[fmt]).mode(kb.ResizeMode[mode]).sampling(kb.InterpolationMode[sampling])
-         .normalize(kb.Normalize.imagenet()).pad_value(114))
-    return (b.yuv_matrix(kb.YuvMatrix[m]) if m else b).build_cuda()
-
-
 def frames_of(fmt, w, h, n, seed):
     if fmt == "I444":
-        return [torch.from_numpy(raw_bytes(3 * w * h, seed + k)) for k in range(n)]
+        return [torch.from_numpy(random_bytes(3 * w * h, seed + k)) for k in range(n)]
     return list(random_words((n, 3 * w * h), seed))
 
 
@@ -395,7 +349,7 @@ def test_preprocess(kb, oracle, dev, fmt, m, sampling, f16):
         pre.run_raw_strided(ring, (raws[0].numel() + 12) * raws[0].element_size(), n, w, h, strided, f16=f16)
         assert torch.equal(strided.view(it), got.view(it)), what
         if fmt == "I444":
-            twins = [decode8(r.numpy(), w, h, m) for r in raws]
+            twins = [decode_yuv444(r.numpy(), w, h, m) for r in raws]
             twin_pre = make_pre(kb, "Rgb8", mode, sampling)
             want = torch.full_like(got, float("nan"))
             (twin_pre.run_raw_batch_f16 if f16 else twin_pre.run_raw_batch)([torch.from_numpy(t.reshape(-1)).to(dev) for t in twins], w, h, want)
@@ -409,7 +363,7 @@ def test_preprocess(kb, oracle, dev, fmt, m, sampling, f16):
                 else:
                     np.testing.assert_array_equal(g.view(np.uint16 if f16 else np.uint32), o.view(np.uint16 if f16 else np.uint32), what)
         else:
-            rgb = decode16(torch.stack(raws), w, h, fmt, m).numpy().astype(np.uint16)
+            rgb = decode_yuv444_16(torch.stack(raws), w, h, fmt, m).numpy().astype(np.uint16)
             for k in range(n):
                 o = restated(kb, rgb[k], BITS[fmt], mode, sampling, dw, dh, f16 and sampling != "Lanczos")
                 check_against_restatement(got[k], o, sampling, f16, f"{what} frame {k}")
@@ -425,7 +379,7 @@ def test_preprocess_twins(kb, dev, sampling, f16):
     for mode, w, h, dw, dh in GEOMS[:4]:
         for fmt, twin in (("I444", "I420"), ("I410", "I010"), ("I412Msb", None)):
             if fmt == "I444":
-                small = torch.from_numpy(raw_bytes(w * h * 3 // 2, w + dw))
+                small = torch.from_numpy(random_bytes(w * h * 3 // 2, w + dw))
                 big = torch.from_numpy(i420_to_i444(small.numpy(), w, h))
             elif twin:
                 small = random_words((w * h * 3 // 2,), w + dw)
@@ -458,7 +412,7 @@ def test_preprocess_unaligned_frames(kb, dev, fmt):
         want = torch.full((1, 3, dh, dw), float("nan"), device=dev)
         pre.run_raw(raw, w, h, want)
         assert kb._lib.last_kernel() == (f"preprocess_{k}_identity_kernel" if dw == w else f"preprocess_{k}_kernel")
-        shifted = offset_u8(dev, raw.numel(), 2) if b == 1 else offset_u16(dev, raw.numel(), 1)
+        shifted = offset_buf(dev, raw.numel(), 2, torch.uint8) if b == 1 else offset_buf(dev, raw.numel(), 1, torch.uint16)
         shifted.copy_(raw)
         got = torch.full_like(want, float("nan"))
         pre.run_raw(shifted, w, h, got)
@@ -482,7 +436,7 @@ def torch_identity(raw, w, h, fmt, m, kb):
         u, v = u - 128, v - 128
         rgb = torch.stack([(yy + cvr * v + (1 << 19)) >> 20, (yy + cug * u + cvg * v + (1 << 19)) >> 20, (yy + cub * u + (1 << 19)) >> 20], -1).clamp(0, 255)
     else:
-        rgb = decode16(raw, w, h, fmt, m)
+        rgb = decode_yuv444_16(raw, w, h, fmt, m)
     rgb = rgb.to(torch.float32) / wl
     mean = torch.tensor(kb.IMAGENET_MEAN, dtype=torch.float32, device=raw.device)
     inv = torch.tensor(1.0, dtype=torch.float32) / torch.tensor(kb.IMAGENET_STD, dtype=torch.float32)
@@ -551,15 +505,15 @@ def test_preprocess_host_pipeline(kb, dev, fmt, mode, dw, dh, f16):
 def _footprint_cases():
     cases = []
     for (w, h), off, v in (((64, 48), False, "vec16"), ((70, 3), False, "generic"), ((64, 16), True, "generic")):
-        cases.append(Case(f"i444-{w}x{h}{'-unaligned' if off else ''}", f"rgb_from_i444_{v}",
-                          lambda k, w=w, h=h: raw_bytes(3 * w * h, 90 + k),
-                          lambda f, w=w, h=h: decode8(f, w, h, "Bt601Limited"),
+        cases.append(FootprintCase(f"i444-{w}x{h}{'-unaligned' if off else ''}", f"rgb_from_i444_{v}",
+                          lambda k, w=w, h=h: random_bytes(3 * w * h, 90 + k),
+                          lambda f, w=w, h=h: decode_yuv444(f, w, h, "Bt601Limited"),
                           lambda lib, s, sl, d, dl, n, aux, a=(w, h): lib.kb200_rgb_from_yuv444_u8(None, s, sl, d, dl, a[0], a[1], n, 0),
                           3 * w * h, 3 * w * h, batch=3, offset=off, row=w * 3))
     for fmt, (w, h), off, v in (("I410", (64, 48), False, "vec"), ("I412Msb", (70, 3), False, "generic"), ("I410Msb", (64, 16), True, "generic")):
-        cases.append(Case(f"i41x-{fmt}-{w}x{h}{'-unaligned' if off else ''}", f"rgb_from_i41x_{v}",
-                          lambda k, w=w, h=h: raw_bytes(6 * w * h, 91 + k).view(np.uint16).copy(),
-                          lambda f, w=w, h=h, fmt=fmt: decode16(torch.from_numpy(f.astype(np.int32)), w, h, fmt, "Bt601Limited").numpy().astype(np.uint16),
+        cases.append(FootprintCase(f"i41x-{fmt}-{w}x{h}{'-unaligned' if off else ''}", f"rgb_from_i41x_{v}",
+                          lambda k, w=w, h=h: random_bytes(6 * w * h, 91 + k).view(np.uint16).copy(),
+                          lambda f, w=w, h=h, fmt=fmt: decode_yuv444_16(torch.from_numpy(f.astype(np.int32)), w, h, fmt, "Bt601Limited").numpy().astype(np.uint16),
                           lambda lib, s, sl, d, dl, n, aux, a=(w, h, LAYOUT[fmt], BITS[fmt]): lib.kb200_rgb_from_yuv444_u16(None, s, sl, d, dl, a[0], a[1], n,
                                                                                                                           a[2], a[3], 0),
                           3 * w * h, 3 * w * h, batch=3, offset=off, row=w * 6))

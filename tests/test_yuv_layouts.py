@@ -13,85 +13,13 @@ import numpy as np
 import pytest
 import torch
 
+from harness import dev, make_pre, offset_buf
+from restate import L420, L422, decode_direct, expected_decode_kernel, layout_bytes, nv12_to_yuv420, to_twin, yuv420_to_nv12, yuv422_swap
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 
-L420 = ("Nv21", "I420", "Yv12")
-L422 = ("Uyvy", "Yvyu")
 LAYOUT_CODE = {"Nv12": 0, "Nv21": 1, "I420": 2, "Yv12": 3, "Yuyv": 0, "Uyvy": 1, "Yvyu": 2}   # kb200_yuv420/422_layout
-# byte positions of (Y0, U, Y1, V) in a 4:2:2 word; YUYV is (0, 1, 2, 3)
-WORD = {"Yuyv": (0, 1, 2, 3), "Uyvy": (1, 0, 3, 2), "Yvyu": (0, 3, 2, 1)}
-
-
-# ── repacking (numpy arrays or torch tensors; the last axis is the frame's bytes) ──
-def _cat(parts):
-    return torch.cat(parts, -1) if isinstance(parts[0], torch.Tensor) else np.concatenate(parts, -1)
-
-
-def _interleave(a, b):
-    st = torch.stack((a, b), -1) if isinstance(a, torch.Tensor) else np.stack((a, b), -1)
-    return st.reshape(*a.shape[:-1], -1)
-
-
-def yuv420_to_nv12(raw, w, h, layout):
-    """A 4:2:0 frame in `layout` -> its NV12 twin."""
-    y, c, q = raw[..., :w * h], raw[..., w * h:], (w // 2) * (h // 2)
-    if layout == "Nv12":
-        return raw
-    if layout == "Nv21":
-        return _cat([y, _interleave(c[..., 1::2], c[..., 0::2])])
-    u, v = (c[..., :q], c[..., q:]) if layout == "I420" else (c[..., q:], c[..., :q])
-    return _cat([y, _interleave(u, v)])
-
-
-def nv12_to_yuv420(nv12, w, h, layout):
-    """An NV12 frame -> the same picture in `layout`."""
-    y, u, v = nv12[..., :w * h], nv12[..., w * h::2], nv12[..., w * h + 1::2]
-    if layout == "Nv21":
-        return _cat([y, _interleave(v, u)])
-    return _cat([y, u, v]) if layout == "I420" else _cat([y, v, u])
-
-
-def yuv422_swap(raw, layout):
-    """YUYV <-> `layout` (each permutation is its own inverse)."""
-    words = raw.reshape(*raw.shape[:-1], -1, 4)
-    idx = list(WORD[layout])
-    return words[..., idx].reshape(raw.shape)
-
-
-def to_twin(raw, w, h, layout):
-    return yuv420_to_nv12(raw, w, h, layout) if layout in L420 + ("Nv12",) else yuv422_swap(raw, layout)
-
-
-def frame_bytes(layout, w, h):
-    return w * h * 3 // 2 if layout in L420 + ("Nv12",) else w * h * 2
-
-
-# ── a numpy restatement of the Q20 decode that reads each layout directly ──
-def q20_rgb(y, u, v):
-    yy = np.maximum(y.astype(np.int64) - 16, 0) * 1220542
-    u, v = u.astype(np.int64) - 128, v.astype(np.int64) - 128
-    r = (yy + 1673527 * v + (1 << 19)) >> 20
-    g = (yy - 409993 * u - 852492 * v + (1 << 19)) >> 20
-    b = (yy + 2116026 * u + (1 << 19)) >> 20
-    return np.clip(np.stack([r, g, b], -1), 0, 255).astype(np.uint8)
-
-
-def decode_direct(raw, w, h, layout):
-    if layout in L420 + ("Nv12",):
-        y, c, q = raw[:w * h].reshape(h, w), raw[w * h:], (w // 2) * (h // 2)
-        if layout in ("Nv12", "Nv21"):
-            pairs = c.reshape(h // 2, w // 2, 2)
-            u, v = (pairs[..., 0], pairs[..., 1]) if layout == "Nv12" else (pairs[..., 1], pairs[..., 0])
-        else:
-            first, second = c[:q].reshape(h // 2, w // 2), c[q:].reshape(h // 2, w // 2)
-            u, v = (first, second) if layout == "I420" else (second, first)
-        up = lambda a: np.repeat(np.repeat(a, 2, 0), 2, 1)
-        return q20_rgb(y, up(u), up(v))
-    words = raw.reshape(h, w // 2, 4)
-    y0, u, y1, v = (words[..., i] for i in WORD[layout])
-    y = np.stack([y0, y1], -1).reshape(h, w)
-    return q20_rgb(y, np.repeat(u, 2, 1), np.repeat(v, 2, 1))
 
 
 def oracle_decode(oracle, raw, w, h, layout):
@@ -109,7 +37,7 @@ def test_cv2_fixture_matches_the_direct_decode_and_the_oracle_twin(oracle):
     for name in names:
         layout = {"nv21": "Nv21", "i420": "I420", "yv12": "Yv12", "uyvy": "Uyvy", "yvyu": "Yvyu"}[name.split("_")[0]]
         raw, want, (w, h) = fx[f"{name}_raw"], fx[f"{name}_rgb"], (int(v) for v in fx[f"{name}_wh"])
-        assert raw.size == frame_bytes(layout, w, h), name
+        assert raw.size == layout_bytes(layout, w, h), name
         np.testing.assert_array_equal(decode_direct(raw, w, h, layout), want, name)
         np.testing.assert_array_equal(oracle_decode(oracle, raw, w, h, layout).reshape(h, w, 3), want, name)
 
@@ -200,29 +128,8 @@ def test_validation_without_a_gpu(kb):
 
 
 # ═══ GPU ═══════════════════════════════════════════════════════════════════════════════════════════════════════
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-def offset_u8(dev, n, off):
-    """A u8 device buffer of n bytes whose data pointer is `off` bytes past the start of a fresh (aligned) allocation."""
-    return torch.empty(n + off, dtype=torch.uint8, device=dev)[off:]
-
-
-def expected_decode_kernel(layout, w, h, n, src_off, dst_off):
-    name = layout.lower()
-    aligned = src_off % 16 == 0 and dst_off % 16 == 0
-    if layout in L420 + ("Nv12",):
-        vec = w % 16 == 0 and aligned and (w * h * 3 // 2) % 16 == 0
-    else:
-        vec = aligned and (w * h * n) % 16 == 0   # otherwise the generic kernel runs last (for the tail, or for all)
-    return f"rgb_from_{name}_{'vec16' if vec else 'generic'}"
-
-
 def run_decode(kb, dev, layout, raw_dev, w, h, n, dst_off=0):
-    out = offset_u8(dev, n * h * w * 3, dst_off)
+    out = offset_buf(dev, n * h * w * 3, dst_off, torch.uint8)
     out.fill_(0xCD)
     img = kb.Image(out.view(n, h, w, 3))
     getattr(kb.imgproc, f"rgb_from_{layout.lower()}")(raw_dev, img)
@@ -248,13 +155,13 @@ def test_decode_layout(kb, oracle, dev, layout, case):
     """Every layout on both paths: equal to the numpy restatement, to the oracle's decode of the twin and to the device
     decode of the twin."""
     w, h, n, soff, doff = case
-    nb = frame_bytes(layout, w, h)
+    nb = layout_bytes(layout, w, h)
     raws = np.random.default_rng(w * 7919 + h * 31 + n + 1000 * LAYOUT_CODE[layout]).integers(0, 256, (n, nb), dtype=np.uint8)
-    src = offset_u8(dev, n * nb, soff)
+    src = offset_buf(dev, n * nb, soff, torch.uint8)
     src.copy_(torch.from_numpy(raws.reshape(-1)))
     got, kern = run_decode(kb, dev, layout, src.view(n, nb), w, h, n, doff)
     assert kern == expected_decode_kernel(layout, w, h, n, soff, doff)
-    twin = offset_u8(dev, n * nb, soff)
+    twin = offset_buf(dev, n * nb, soff, torch.uint8)
     twin.copy_(torch.from_numpy(to_twin(raws, w, h, layout).reshape(-1)))
     twin_out, twin_kern = run_decode(kb, dev, "Nv12" if layout in L420 else "Yuyv", twin.view(n, nb), w, h, n, doff)
     assert twin_kern.endswith(kern.rsplit("_", 1)[1])   # the twin took the same path
@@ -269,7 +176,7 @@ def test_decode_layout(kb, oracle, dev, layout, case):
 @pytest.mark.parametrize("layout", L420 + L422)
 def test_decode_layout_1080p_batch(kb, oracle, dev, layout):
     w, h, n = 1920, 1080, 8
-    nb = frame_bytes(layout, w, h)
+    nb = layout_bytes(layout, w, h)
     g = torch.Generator(device=dev).manual_seed(0x1080)
     raw = torch.randint(0, 256, (n, nb), dtype=torch.uint8, device=dev, generator=g)
     got, kern = run_decode(kb, dev, layout, raw, w, h, n)
@@ -295,11 +202,6 @@ def expected_preprocess_kernel(layout, sampling, w, h, dw, dh):
     if (dw, dh) == (w, h) and w % 4 == 0:
         return f"preprocess_{layout.lower()}_identity_kernel"
     return f"preprocess_{layout.lower()}_kernel" if dw % 4 == 0 else "preprocess_generic_kernel"
-
-
-def make_pre(kb, fmt, mode, sampling):
-    return (kb.Preprocessor.builder().source_format(kb.SourceFormat[fmt]).mode(kb.ResizeMode[mode])
-            .sampling(kb.InterpolationMode[sampling]).normalize(kb.Normalize.imagenet()).pad_value(114).build_cuda())
 
 
 def oracle_cfg(kb, oracle, twin_fmt, mode, sampling):
@@ -383,7 +285,7 @@ def test_preprocess_host_pipeline_layout(kb, dev, layout, mode, dw, dh, f16):
     """run_raw_host sizes frames from the format alone: host frames in / host tensor out equal the device path, and the
     transfers are exactly the frames' and the outputs' bytes."""
     w, h, n = 192, 108, 7
-    nbytes = frame_bytes(layout, w, h)
+    nbytes = layout_bytes(layout, w, h)
     host = torch.from_numpy(np.stack([raw_bytes(nbytes, k) for k in range(n)])).pin_memory()
     pre = make_pre(kb, layout, mode, "Bilinear")
     want = torch.zeros((n, 3, dh, dw), dtype=torch.float16 if f16 else torch.float32, device=dev)

@@ -15,25 +15,16 @@ import numpy as np
 import pytest
 import torch
 
-from test_yuv_layouts import L420, L422, WORD, expected_decode_kernel, frame_bytes, nv12_to_yuv420, offset_u8, raw_bytes, yuv422_swap
+from harness import dev, make_pre, offset_buf, oracle_cfg, raw_bytes
+from restate import KR_KB, L420, L422, MATRICES, TABLE, YUV420, decode_yuv8, expected_decode_kernel, layout_bytes, nv12_to_yuv420, q20, yuv422_swap
+
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 
-MATRICES = ("Bt601Limited", "Bt601Full", "Bt709Limited", "Bt709Full")   # kb200_yuv_matrix order
 FORMATS = ("Nv12",) + L420 + ("Yuyv",) + L422
-YUV420 = ("Nv12",) + L420
 LAYOUT_CODE = {"Nv12": 0, "Nv21": 1, "I420": 2, "Yv12": 3, "Yuyv": 0, "Uyvy": 1, "Yvyu": 2}
 FMT_CODE = {"Nv12": 3, "Yuyv": 4, "Nv21": 5, "I420": 6, "Yv12": 7, "Uyvy": 8, "Yvyu": 9}
-
-# ── the specification: (y_off, cy, cvr, cub, cug, cvg) per matrix ──
-TABLE = {
-    "Bt601Limited": (16, 1220542, 1673527, 2116026, -409993, -852492),
-    "Bt601Full": (0, 1048576, 1470104, 1858077, -360853, -748826),
-    "Bt709Limited": (16, 1220945, 1879825, 2215014, -223607, -558796),
-    "Bt709Full": (0, 1048576, 1651297, 1945738, -196424, -490864),
-}
-KR_KB = {"Bt601": (0.299, 0.114), "Bt709": (0.2126, 0.0722)}
 
 
 def float_coeffs(m):
@@ -43,34 +34,6 @@ def float_coeffs(m):
     full = m.endswith("Full")
     sy, sc = (1.0, 1.0) if full else (255.0 / 219.0, 255.0 / 224.0)
     return (0 if full else 16, sy, 2 * (1 - kr) * sc, 2 * (1 - kb_) * sc, -2 * kb_ * (1 - kb_) / kg * sc, -2 * kr * (1 - kr) / kg * sc)
-
-
-def q20(y, u, v, m):
-    """The Q20 decode of byte arrays y, u, v with matrix m -> [..., 3] RGB8."""
-    yo, cy, cvr, cub, cug, cvg = TABLE[m]
-    yy = np.maximum(y.astype(np.int64) - yo, 0) * cy
-    u, v = u.astype(np.int64) - 128, v.astype(np.int64) - 128
-    r = (yy + cvr * v + (1 << 19)) >> 20
-    g = (yy + cug * u + cvg * v + (1 << 19)) >> 20
-    b = (yy + cub * u + (1 << 19)) >> 20
-    return np.clip(np.stack([r, g, b], -1), 0, 255).astype(np.uint8)
-
-
-def decode(raw, w, h, layout, m):
-    """One frame in `layout` -> [h, w, 3] RGB8 through q20, reading the layout directly (chroma replicated)."""
-    if layout in YUV420:
-        y, c, q = raw[:w * h].reshape(h, w), raw[w * h:], (w // 2) * (h // 2)
-        if layout in ("Nv12", "Nv21"):
-            pairs = c.reshape(h // 2, w // 2, 2)
-            u, v = (pairs[..., 0], pairs[..., 1]) if layout == "Nv12" else (pairs[..., 1], pairs[..., 0])
-        else:
-            first, second = c[:q].reshape(h // 2, w // 2), c[q:].reshape(h // 2, w // 2)
-            u, v = (first, second) if layout == "I420" else (second, first)
-        up = lambda a: np.repeat(np.repeat(a, 2, 0), 2, 1)
-        return q20(y, up(u), up(v), m)
-    words = raw.reshape(h, w // 2, 4)
-    y0, u, y1, v = (words[..., i] for i in WORD.get(layout, (0, 1, 2, 3)))
-    return q20(np.stack([y0, y1], -1).reshape(h, w), np.repeat(u, 2, 1), np.repeat(v, 2, 1), m)
 
 
 # ═══ CPU ═══════════════════════════════════════════════════════════════════════════════════════════════════════
@@ -104,7 +67,7 @@ def test_matrix0_reproduces_the_cv2_fixtures():
         fx = np.load(os.path.join(GOLDEN, path))
         for name in sorted({k.rsplit("_", 1)[0] for k in fx.files}):
             w, h = (int(v) for v in fx[f"{name}_wh"])
-            np.testing.assert_array_equal(decode(fx[f"{name}_raw"], w, h, layout, "Bt601Limited"), fx[f"{name}_rgb"], f"{path} {name}")
+            np.testing.assert_array_equal(decode_yuv8(fx[f"{name}_raw"], w, h, layout, "Bt601Limited"), fx[f"{name}_rgb"], f"{path} {name}")
 
 
 def all_triples(y_lo, y_hi):
@@ -212,14 +175,8 @@ def test_builder_rejects_a_matrix_on_other_formats(kb):
 
 
 # ═══ GPU ═══════════════════════════════════════════════════════════════════════════════════════════════════════
-@pytest.fixture(scope="module")
-def dev():
-    assert torch.cuda.is_available(), "gpu tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
 def run_decode(kb, dev, layout, src, w, h, n, m, dst_off=0):
-    out = offset_u8(dev, n * h * w * 3, dst_off)
+    out = offset_buf(dev, n * h * w * 3, dst_off, torch.uint8)
     out.fill_(0xCD)
     getattr(kb.imgproc, f"rgb_from_{layout.lower()}")(src, kb.Image(out.view(n, h, w, 3)), matrix=kb.YuvMatrix[m])
     return out.view(n, h, w, 3), kb._lib.last_kernel()
@@ -240,38 +197,25 @@ def test_decode_matrix(kb, dev, layout, m):
     from kornia_rs_b200 import _lib
 
     for w, h, n, soff, doff in DECODE_CASES["420" if layout in YUV420 else "422"]:
-        nb = frame_bytes(layout, w, h)
+        nb = layout_bytes(layout, w, h)
         raws = np.random.default_rng(w * 131 + h + 7 * n + 1000 * MATRICES.index(m)).integers(0, 256, (n, nb), dtype=np.uint8)
-        src = offset_u8(dev, n * nb, soff)
+        src = offset_buf(dev, n * nb, soff, torch.uint8)
         src.copy_(torch.from_numpy(raws.reshape(-1)))
         got, kern = run_decode(kb, dev, layout, src.view(n, nb), w, h, n, m, doff)
         what = f"{layout} {m} {(w, h, n, soff, doff)}"
         assert kern == expected_decode_kernel(layout, w, h, n, soff, doff), what
         g = got.cpu().numpy()
         for k in range(n):
-            np.testing.assert_array_equal(g[k], decode(raws[k], w, h, layout, m), f"{what} frame {k}")
+            np.testing.assert_array_equal(g[k], decode_yuv8(raws[k], w, h, layout, m), f"{what} frame {k}")
         if m == "Bt601Limited":
-            old = offset_u8(dev, n * h * w * 3, doff)
+            old = offset_buf(dev, n * h * w * 3, doff, torch.uint8)
             fn = "kb200_rgb_from_yuv420_u8" if layout in YUV420 else "kb200_rgb_from_yuv422_u8"
             st = getattr(_lib.lib(), fn)(torch.cuda.current_stream(dev).cuda_stream, src.data_ptr(), src.numel(), old.data_ptr(), old.numel(),
                                          w, h, n, LAYOUT_CODE[layout])
             assert st == _lib.OK and _lib.last_kernel() == kern
             assert torch.equal(old.view(n, h, w, 3), got), what
         else:
-            assert not np.array_equal(g[0], decode(raws[0], w, h, layout, "Bt601Limited")), what
-
-
-def pre_for(kb, fmt, mode, sampling, m=None):
-    b = (kb.Preprocessor.builder().source_format(kb.SourceFormat[fmt]).mode(kb.ResizeMode[mode]).sampling(kb.InterpolationMode[sampling])
-         .normalize(kb.Normalize.imagenet()).pad_value(114))
-    return (b.yuv_matrix(kb.YuvMatrix[m]) if m else b).build_cuda()
-
-
-def oracle_cfg(kb, oracle, mode, sampling):
-    inv = tuple(float(np.float32(1.0) / np.float32(s)) for s in kb.IMAGENET_STD)
-    return oracle.PreprocessCfg(mode=oracle.LETTERBOX if mode == "Letterbox" else oracle.STRETCH, fmt=oracle.FMT_RGB, mean=kb.IMAGENET_MEAN,
-                                inv_std=inv, pad_value=114.0,
-                                sampling={"Bilinear": oracle.BILINEAR, "Nearest": oracle.NEAREST, "Lanczos": oracle.LANCZOS}[sampling])
+            assert not np.array_equal(g[0], decode_yuv8(raws[0], w, h, layout, "Bt601Limited")), what
 
 
 def expected_preprocess_kernel(fmt, sampling, w, h, dw, dh):
@@ -305,9 +249,9 @@ def test_preprocess_matrix(kb, oracle, dev, fmt, m, sampling, f16):
     n = 2
     for mode, w, h, dw, dh in PRE_GEOMS:
         what = f"{fmt} {m} {sampling} {mode} {(w, h, dw, dh)} {'f16' if f16 else 'f32'}"
-        pre, twin_pre = pre_for(kb, fmt, mode, sampling, m), pre_for(kb, "Rgb8", mode, sampling)
+        pre, twin_pre = make_pre(kb, fmt, mode, sampling, m), make_pre(kb, "Rgb8", mode, sampling)
         raws = [raw_frame(fmt, w, h, k) for k in range(n)]
-        twins = [decode(r, w, h, fmt, m) for r in raws]
+        twins = [decode_yuv8(r, w, h, fmt, m) for r in raws]
         got = torch.full((n, 3, dh, dw), float("nan"), dtype=dt, device=dev)
         (pre.run_raw_batch_f16 if f16 else pre.run_raw_batch)([torch.from_numpy(r).to(dev) for r in raws], w, h, got)
         assert kb._lib.last_kernel() == expected_preprocess_kernel(fmt, sampling, w, h, dw, dh), what
@@ -335,9 +279,9 @@ def test_preprocess_host_pipeline_matrix(kb, dev, f16):
     """run_raw_host with BT.709 limited equals run_raw_batch on the same frames."""
     for fmt, mode, dw, dh in (("Nv12", "Letterbox", 64, 64), ("Yuyv", "Stretch", 100, 60), ("I420", "Stretch", 192, 108)):
         w, h, n = 192, 108, 5
-        nbytes = frame_bytes(fmt, w, h)
+        nbytes = layout_bytes(fmt, w, h)
         host = torch.from_numpy(np.stack([raw_frame(fmt, w, h, k) for k in range(n)])).pin_memory()
-        pre = pre_for(kb, fmt, mode, "Bilinear", "Bt709Limited")
+        pre = make_pre(kb, fmt, mode, "Bilinear", "Bt709Limited")
         want = torch.zeros((n, 3, dh, dw), dtype=torch.float16 if f16 else torch.float32, device=dev)
         (pre.run_raw_batch_f16 if f16 else pre.run_raw_batch)([host[i].to(dev) for i in range(n)], w, h, want)
         pipe = kb.imgproc.HostPipeline(dev, src_chunk_bytes=2 * ((nbytes + 15) // 16 * 16), dst_chunk_bytes=2 * 3 * dw * dh * 4, depth=2)
@@ -348,7 +292,7 @@ def test_preprocess_host_pipeline_matrix(kb, dev, f16):
         assert h2d == n * nbytes
         it = torch.int16 if f16 else torch.int32
         assert torch.equal(got.view(it), want.cpu().view(it)), fmt
-        base = pre_for(kb, fmt, mode, "Bilinear")
+        base = make_pre(kb, fmt, mode, "Bilinear")
         other = torch.zeros_like(want)
         (base.run_raw_batch_f16 if f16 else base.run_raw_batch)([host[i].to(dev) for i in range(n)], w, h, other)
         assert not torch.equal(other, want)
@@ -362,14 +306,14 @@ def test_config3a_shape_bt709(kb, oracle, dev):
     nb = w * h * 3 // 2
     g = torch.Generator(device=dev).manual_seed(0x709)
     frames = torch.randint(0, 256, (n, nb), dtype=torch.uint8, device=dev, generator=g)
-    pre = pre_for(kb, "Nv12", "Stretch", "Bilinear", "Bt709Limited")
+    pre = make_pre(kb, "Nv12", "Stretch", "Bilinear", "Bt709Limited")
     got = torch.full((n, 3, h, w), float("nan"), dtype=torch.float32, device=dev)
     pre.run_raw_batch([frames[k] for k in range(n)], w, h, got)
     assert kb._lib.last_kernel() == "preprocess_nv12_identity_kernel"
-    twin_pre = pre_for(kb, "Rgb8", "Stretch", "Bilinear")
+    twin_pre = make_pre(kb, "Rgb8", "Stretch", "Bilinear")
     cfg = oracle_cfg(kb, oracle, "Stretch", "Bilinear")
     for k in (0, 101, n - 1):
-        twin = decode(frames[k].cpu().numpy(), w, h, "Nv12", "Bt709Limited")
+        twin = decode_yuv8(frames[k].cpu().numpy(), w, h, "Nv12", "Bt709Limited")
         want = torch.full((1, 3, h, w), float("nan"), dtype=torch.float32, device=dev)
         twin_pre.run_raw(torch.from_numpy(twin.reshape(-1)).to(dev), w, h, want)
         assert torch.equal(got[k:k + 1].view(torch.int32), want.view(torch.int32)), k

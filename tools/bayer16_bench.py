@@ -14,7 +14,7 @@ Every arm is timed with CUDA events over --iters launches after warm-up, the arm
 (Bayer12 2 B/px, Bayer8 1 B/px, NV12 1.5 B/px; for 3b NV12 counts the distinct bytes its sampler taps, as in
 tools/bayer_bench.py, while a Bayer tap's 3x3 neighbourhood covers every source sample at 3b's exact 3:1 ratio) plus the
 output (6 / 3 / 3 B/px RGB for the decodes, 12 / 6 B/px for f32 / f16 CHW).
-Every Bayer output is checked on the device: the 12-bit decode against the restatement of tests/test_bayer16.py, the
+Every Bayer output is checked on the device: the 12-bit decode against the restatement of tests/restate.py, the
 12-bit 3a preprocess against that restatement's demosaic normalised in torch (separate IEEE f32 operations), the 12-bit
 3b preprocess against the f32 restatement of the oracle on three frames, the 8-bit arms as tools/bayer_bench.py checks
 them, and end to end against the device run.
@@ -59,8 +59,8 @@ def main():
 
     import kornia_rs_b200 as kb
     from oracle import oracle as o
-    from test_bayer import demosaic as demosaic8
-    from test_bayer16 import demosaic as demosaic16, restated, to_np16, torch_identity
+    from harness import bayer16_identity, restated, to_np16
+    from restate import demosaic
 
     if not torch.cuda.is_available():
         raise SystemExit("bayer16_bench.py needs a CUDA device")
@@ -90,8 +90,8 @@ def main():
         times, kernels = time_arms(bench, fns, args.iters, args.warmup, args.reps, st, kb)
         same = {"Nv12": None,
                 "Bayer12": all(bool(torch.equal(outs["Bayer12"].data[k:k + 16].view(torch.int16),
-                                                demosaic16(src["Bayer12"][k:k + 16].view(-1, h, w), "RGGB").view(torch.int16))) for k in range(0, n, 16)),
-                "Bayer8": all(bool(torch.equal(outs["Bayer8"].data[k:k + 16], demosaic8(src["Bayer8"][k:k + 16].view(-1, h, w), "RGGB")))
+                                                demosaic(src["Bayer12"][k:k + 16].view(-1, h, w), "RGGB").view(torch.int16))) for k in range(0, n, 16)),
+                "Bayer8": all(bool(torch.equal(outs["Bayer8"].data[k:k + 16], demosaic(src["Bayer8"][k:k + 16].view(-1, h, w), "RGGB")))
                               for k in range(0, n, 16))}
         alg = {k: int(n * w * h * (bpp[k] + (6 if k == "Bayer12" else 3))) for k in ARMS}
         decode[tag] = {"batch": n, "src": [w, h], **row(times, kernels, alg, same)}
@@ -120,11 +120,11 @@ def main():
             same = {"Nv12": None}
             if cfg == "cfg3a":
                 same["Bayer12"] = all(bool(torch.equal(outs["Bayer12"][k:k + 16].view(it),
-                                                       torch_identity(src["Bayer12"][k:k + 16].view(-1, h, w), "RGGB", 12, kb).to(dt).contiguous().view(it)))
+                                                       bayer16_identity(src["Bayer12"][k:k + 16].view(-1, h, w), "RGGB", 12, kb).to(dt).contiguous().view(it)))
                                       for k in range(0, n, 16))
             else:
                 same["Bayer12"] = all(np.array_equal(outs["Bayer12"][k].cpu().numpy().view(np.uint16 if f16 else np.uint32),
-                                                     restated(kb, demosaic16(to_np16(src["Bayer12"][k]).reshape(h, w), "RGGB"), 12, mode, "Bilinear",
+                                                     restated(kb, demosaic(to_np16(src["Bayer12"][k]).reshape(h, w), "RGGB"), 12, mode, "Bilinear",
                                                               dw, dh, f16).view(np.uint16 if f16 else np.uint32)) for k in (0, n // 2, n - 1))
             twin_pre = builder(kb.SourceFormat.Rgb8)
             rgb = kb.Image.zeros_cuda(kb.ImageSize(w, h), 3, torch.uint8, dev, batch=32)
@@ -132,7 +132,7 @@ def main():
             ok = True
             for k0 in range(0, n, 32):
                 kb.imgproc.rgb_from_bayer(src["Bayer8"][k0:k0 + 32], rgb, kb.imgproc.BayerPattern.RGGB)
-                ok = ok and bool(torch.equal(rgb.data, demosaic8(src["Bayer8"][k0:k0 + 32].view(-1, h, w), "RGGB")))
+                ok = ok and bool(torch.equal(rgb.data, demosaic(src["Bayer8"][k0:k0 + 32].view(-1, h, w), "RGGB")))
                 (twin_pre.run_raw_batch_f16 if f16 else twin_pre.run_raw_batch)([rgb.data[i].view(-1) for i in range(32)], w, h, want)
                 ok = ok and bool(torch.equal(outs["Bayer8"][k0:k0 + 32].view(it), want.view(it)))
             same["Bayer8"] = ok

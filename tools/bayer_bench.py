@@ -62,7 +62,7 @@ def main():
 
     import kornia_rs_b200 as kb
     from oracle import oracle as o
-    from test_bayer import demosaic
+    from restate import demosaic
 
     if not torch.cuda.is_available():
         raise SystemExit("bayer_bench.py needs a CUDA device")

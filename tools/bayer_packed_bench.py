@@ -59,7 +59,7 @@ def main():
     import torch
 
     import kornia_rs_b200 as kb
-    from test_bayer_packed import unpack
+    from restate import unpack
 
     if not torch.cuda.is_available():
         raise SystemExit("bayer_packed_bench.py needs a CUDA device")

@@ -88,9 +88,8 @@ def main():
     a = ap.parse_args()
     import kornia_rs_b200 as kb
     from kornia_rs_b200._lib import PreprocessDesc, RemapRoi
-    from test_preprocess_remap import remap_reference
-    from test_preprocess_roi import RCase, compare, picture
-    from test_preprocess_sweep import Case
+    from harness import compare_region
+    from restate import Case, RCase, picture, remap_reference
 
     assert torch.cuda.is_available(), "the benchmark needs a GPU"
     lib = kb._lib.lib()
@@ -165,7 +164,7 @@ def main():
             k, j = regs[i]
             raw = base[k * need:(k + 1) * need].cpu().numpy()
             want = remap_reference(picture(c, raw), maps_x[j], maps_y[j], 1, "imagenet", 114.0, out)
-            compare(dst[i].contiguous().view(torch.uint8).cpu().numpy().reshape(-1), want, rc, f"{wl} {fmt} {out} region {i}")
+            compare_region(dst[i].contiguous().view(torch.uint8).cpu().numpy().reshape(-1), want, rc, f"{wl} {fmt} {out} region {i}")
         return picked
 
     def frames_of(fmt, w, h, n, key):

@@ -82,8 +82,8 @@ def main():
     import kornia_rs_b200 as kb
     from kornia_rs_b200._lib import PreprocessDesc, Roi
     from oracle.oracle import preprocess_affine
-    from test_preprocess_roi import RCase, picture, region_reference, compare
-    from test_preprocess_sweep import Case
+    from harness import compare_region
+    from restate import Case, RCase, picture, region_reference
 
     assert torch.cuda.is_available(), "the benchmark needs a GPU"
     lib = kb._lib.lib()
@@ -192,7 +192,7 @@ def main():
                     k = flat[i][0]
                     pic = picture(c, host[k * need:(k + 1) * need])
                     got = dst[i].contiguous().view(torch.uint8).cpu().numpy().reshape(-1)
-                    compare(got, region_reference(rc, pic, flat[i]), rc, f"{wl} region {i}")
+                    compare_region(got, region_reference(rc, pic, flat[i]), rc, f"{wl} region {i}")
                 check["regions_checked_against_crop_reference"] = picked
             arms = {"rois": lambda: roi_call(d, mode, ptrs, lens, rois, dst, out), "existing": other}
             if wl == "W1":   # the batch entry in the region entry's launches: 80 frames per call

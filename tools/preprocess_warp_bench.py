@@ -48,7 +48,7 @@ def frame_len(fmt, w, h):
 
 def tapped_bytes(fmt, w, h, regions, inverse, dw, dh):
     """Distinct source bytes the bilinear sampler reads over `regions` ([(k, forward map)]): see the module docstring."""
-    from test_preprocess_warp import warp_coords
+    from restate import warp_coords
     per_frame = {}
     for k, fwd in regions:
         inv, persp = inverse(fwd)
@@ -88,9 +88,8 @@ def main():
     a = ap.parse_args()
     import kornia_rs_b200 as kb
     from kornia_rs_b200._lib import PreprocessDesc, Roi, WarpRoi
-    from test_preprocess_roi import RCase, compare, picture
-    from test_preprocess_sweep import Case
-    from test_preprocess_warp import forward_of, inverse, warp_reference
+    from harness import compare_region, inverse
+    from restate import Case, RCase, forward_of, picture, warp_reference
 
     assert torch.cuda.is_available(), "the benchmark needs a GPU"
     lib = kb._lib.lib()
@@ -235,7 +234,7 @@ def main():
                 k, fwd = regs[i]
                 inv, persp = inverse(lib, fwd)
                 got = dst[i].contiguous().view(torch.uint8).cpu().numpy().reshape(-1)
-                compare(got, warp_reference(picture(c, host[k * need:(k + 1) * need]), inv, persp, dw, dh, 1, "imagenet", 114.0, out), rc,
+                compare_region(got, warp_reference(picture(c, host[k * need:(k + 1) * need]), inv, persp, dw, dh, 1, "imagenet", 114.0, out), rc,
                         f"{wl} {fmt} region {i}")
             check["regions_checked_against_reference"] = picked
         if wl == "W1":

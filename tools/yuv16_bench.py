@@ -68,9 +68,8 @@ def main():
 
     import kornia_rs_b200 as kb
     from oracle import oracle as o
-    from test_bayer16 import demosaic as demosaic16, restated, to_np16, torch_identity as bayer_identity
-    from test_yuv16 import BITS, decode as decode16, torch_identity as yuv16_identity
-    from test_yuv_matrix import decode as decode8
+    from harness import bayer16_identity, restated, to_np16, yuv16_identity
+    from restate import BITS, decode_yuv16, decode_yuv8, demosaic
 
     if not torch.cuda.is_available():
         raise SystemExit("yuv16_bench.py needs a CUDA device")
@@ -113,13 +112,13 @@ def main():
             fns[k]()
             got = outs[k].data
             if k in YUV16:
-                same[k] = all(bool(torch.equal(got[i:i + 8].to(torch.int32).to(torch.int64), decode16(src[k][i:i + 8], w, h, k, MATRIX)))
+                same[k] = all(bool(torch.equal(got[i:i + 8].to(torch.int32).to(torch.int64), decode_yuv16(src[k][i:i + 8], w, h, k, MATRIX)))
                               for i in range(0, n, 8))
             elif k == "Bayer12":
-                same[k] = all(bool(torch.equal(got[i:i + 16].view(torch.int16), demosaic16(src[k][i:i + 16].view(-1, h, w), "RGGB").view(torch.int16)))
+                same[k] = all(bool(torch.equal(got[i:i + 16].view(torch.int16), demosaic(src[k][i:i + 16].view(-1, h, w), "RGGB").view(torch.int16)))
                               for i in range(0, n, 16))
             else:
-                same[k] = all(np.array_equal(got[i].cpu().numpy(), decode8(src[k][i].cpu().numpy(), w, h, "Nv12", "Bt601Limited"))
+                same[k] = all(np.array_equal(got[i].cpu().numpy(), decode_yuv8(src[k][i].cpu().numpy(), w, h, "Nv12", "Bt601Limited"))
                               for i in sorted({0, n // 2, n - 1}))
         alg = {k: int(n * w * h * (src_bpp[k] + (3 if k == "Nv12" else 6))) for k in ARMS}
         decode[tag] = {"batch": n, "src": [w, h], **row(times, kernels, alg, same)}
@@ -167,14 +166,14 @@ def main():
                                   for i in range(0, n, 8))
                 elif k in YUV16:
                     same[k] = all(np.array_equal(out[i].cpu().numpy().view(np.uint16 if f16 else np.uint32),
-                                                 restated(kb, decode16(src[k][i].cpu(), w, h, k, MATRIX).numpy().astype(np.uint16), BITS[k], mode,
+                                                 restated(kb, decode_yuv16(src[k][i].cpu(), w, h, k, MATRIX).numpy().astype(np.uint16), BITS[k], mode,
                                                           "Bilinear", dw, dh, f16).view(np.uint16 if f16 else np.uint32)) for i in (0, n // 2, n - 1))
                 elif k in ("Bayer12", "Bayer12_zeros") and cfg == "cfg3a":
-                    same[k] = all(bool(torch.equal(out[i:i + 16].view(it), bayer_identity(src[k][i:i + 16].view(-1, h, w), "RGGB", 12, kb).to(dt).contiguous().view(it)))
+                    same[k] = all(bool(torch.equal(out[i:i + 16].view(it), bayer16_identity(src[k][i:i + 16].view(-1, h, w), "RGGB", 12, kb).to(dt).contiguous().view(it)))
                                   for i in range(0, n, 16))
                 elif k == "Bayer12":
                     same[k] = all(np.array_equal(out[i].cpu().numpy().view(np.uint16 if f16 else np.uint32),
-                                                 restated(kb, demosaic16(to_np16(src[k][i]).reshape(h, w), "RGGB"), 12, mode, "Bilinear", dw, dh,
+                                                 restated(kb, demosaic(to_np16(src[k][i]).reshape(h, w), "RGGB"), 12, mode, "Bilinear", dw, dh,
                                                           f16).view(np.uint16 if f16 else np.uint32)) for i in (0, n // 2, n - 1))
                 else:
                     same[k] = all(np.array_equal(out[i].cpu().numpy().view(np.uint16 if f16 else np.uint32),

@@ -66,9 +66,8 @@ def main():
 
     import kornia_rs_b200 as kb
     from oracle import oracle as o
-    from test_bayer16 import restated
-    from test_yuv16 import decode as decode16, torch_identity as yuv16_identity
-    from test_yuv_matrix import decode as decode8
+    from harness import restated, yuv16_identity
+    from restate import decode_yuv16, decode_yuv8
 
     if not torch.cuda.is_available():
         raise SystemExit("yuv444_bench.py needs a CUDA device")
@@ -101,9 +100,9 @@ def main():
         for k in ARMS:
             fns[k]()
         torch.cuda.synchronize()
-        same = {"Nv12": all(np.array_equal(outs["Nv12"].data[i].cpu().numpy(), decode8(src["Nv12"][i].cpu().numpy(), w, h, "Nv12", MATRIX))
+        same = {"Nv12": all(np.array_equal(outs["Nv12"].data[i].cpu().numpy(), decode_yuv8(src["Nv12"][i].cpu().numpy(), w, h, "Nv12", MATRIX))
                             for i in sorted({0, n // 2, n - 1})),
-                "P010": all(bool(torch.equal(outs["P010"].data[i:i + 8].to(torch.int32).to(torch.int64), decode16(src["P010"][i:i + 8], w, h, "P010", MATRIX)))
+                "P010": all(bool(torch.equal(outs["P010"].data[i:i + 8].to(torch.int32).to(torch.int64), decode_yuv16(src["P010"][i:i + 8], w, h, "P010", MATRIX)))
                             for i in range(0, n, 8))}
         for k, sib in SIBLING.items():
             same[k] = bool(torch.equal(outs[k].data, outs[sib].data))
@@ -151,11 +150,11 @@ def main():
                                   for i in range(0, n, 8))
                 elif k == "P010":
                     same[k] = all(np.array_equal(out[i].cpu().numpy().view(np.uint16 if f16 else np.uint32),
-                                                 restated(kb, decode16(src[k][i].cpu(), w, h, k, MATRIX).numpy().astype(np.uint16), 10, mode,
+                                                 restated(kb, decode_yuv16(src[k][i].cpu(), w, h, k, MATRIX).numpy().astype(np.uint16), 10, mode,
                                                           "Bilinear", dw, dh, f16).view(np.uint16 if f16 else np.uint32)) for i in (0, n // 2, n - 1))
                 else:   # the oracle on the RGB8 twin of the BT.709 picture
                     same[k] = all(np.array_equal(out[i].cpu().numpy().view(np.uint16 if f16 else np.uint32),
-                                                 o.preprocess_frame(decode8(src[k][i].cpu().numpy(), w, h, "Nv12", MATRIX).reshape(-1), rcfg, w, h, dw, dh,
+                                                 o.preprocess_frame(decode_yuv8(src[k][i].cpu().numpy(), w, h, "Nv12", MATRIX).reshape(-1), rcfg, w, h, dw, dh,
                                                                     f16=f16).view(np.uint16 if f16 else np.uint32)) for i in (0, n - 1))
                 ref[k] = out.clone()
             for k in arms:

@@ -60,7 +60,7 @@ def main():
 
     import kornia_rs_b200 as kb
     from oracle import oracle as o
-    from test_yuv_matrix import decode
+    from restate import decode_yuv8
 
     if not torch.cuda.is_available():
         raise SystemExit("yuv_matrix_bench.py needs a CUDA device")
@@ -81,7 +81,7 @@ def main():
             times, kernels = time_arms(bench, fns, args.iters, args.warmup, args.reps, st, kb)
             ok = {}
             for m in MATRICES:
-                ok[m] = all(bool((outs[m].data[k].cpu().numpy() == decode(src[k].cpu().numpy(), w, h, layout, m)).all()) for k in (0, n - 1))
+                ok[m] = all(bool((outs[m].data[k].cpu().numpy() == decode_yuv8(src[k].cpu().numpy(), w, h, layout, m)).all()) for k in (0, n - 1))
             decode_rows[f"{layout.lower()}_{tag}"] = {"batch": n, "src": [w, h], **row_for(times, kernels, n * (fb + 3 * w * h), ok)}
             print(f"[yuv_matrix_bench] decode {layout} {tag}: " + "  ".join(f"{m} {min(times[m]):.4f}" for m in MATRICES), file=sys.stderr, flush=True)
             del src, outs
@@ -114,7 +114,7 @@ def main():
             for m in MATRICES:
                 good = True
                 for k in (0, n - 1):
-                    twin = torch.from_numpy(decode(frames_t[k].cpu().numpy(), w, h, "Nv12", m).reshape(-1)).to(dev)
+                    twin = torch.from_numpy(decode_yuv8(frames_t[k].cpu().numpy(), w, h, "Nv12", m).reshape(-1)).to(dev)
                     want = torch.full((1, 3, dh, dw), float("nan"), dtype=dt, device=dev)
                     run(twin_pre, [twin], want)
                     good = good and bool(torch.equal(dsts[m][k:k + 1].view(it), want.view(it)))
