@@ -14,45 +14,29 @@ Every arm is timed with CUDA events over --iters launches after warm-up, the arm
 (Bayer12 2 B/px, Bayer8 1 B/px, NV12 1.5 B/px; for 3b NV12 counts the distinct bytes its sampler taps, as in
 tools/bayer_bench.py, while a Bayer tap's 3x3 neighbourhood covers every source sample at 3b's exact 3:1 ratio) plus the
 output (6 / 3 / 3 B/px RGB for the decodes, 12 / 6 B/px for f32 / f16 CHW).
-Every Bayer output is checked on the device: the 12-bit decode against the restatement of tests/restate.py, the
-12-bit 3a preprocess against that restatement's demosaic normalised in torch (separate IEEE f32 operations), the 12-bit
-3b preprocess against the f32 restatement of the oracle on three frames, the 8-bit arms as tools/bayer_bench.py checks
-them, and end to end against the device run.
+Every Bayer output is checked on the device: the 12-bit decode against restate.demosaic, the 12-bit 3a preprocess
+against that demosaic normalised in torch (harness.bayer16_identity: separate IEEE f32 operations), the 12-bit 3b
+preprocess against the f32 restatement of the oracle (harness.restated) on three frames, the 8-bit arms as
+tools/bayer_bench.py checks them, and end to end against the device run.
 
 Writes one JSON line to DIR/bayer16_bench.jsonl (and stdout), with the card's name, power limit and max SM clock read
 in the same run.
 """
 from __future__ import annotations
 
-import argparse
-import json
-import os
 import sys
 import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-
-from bayer_bench import row  # noqa: E402
-from half_bench import PEAK_GBS, _bench_module, gpu_facts  # noqa: E402
-from yuv_bench import time_arms  # noqa: E402
+from benchkit import PEAK_GBS, arg_parser, e2e_result, parse_args, row, start, time_arms, write_line
 
 ARMS = ("Bayer12", "Bayer8", "Nv12")
 
 
 def main():
-    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
-    ap.add_argument("--out", required=True, help="directory for bayer16_bench.jsonl")
-    ap.add_argument("--iters", type=int, default=20)
-    ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--reps", type=int, default=3)
+    ap = arg_parser(__doc__, "bayer16_bench")
     ap.add_argument("--e2e-frames", type=int, default=64)
     ap.add_argument("--e2e-steps", type=int, default=5)
-    args = ap.parse_args()
-    if args.iters < 20 or args.reps < 3:
-        ap.error("--iters >= 20 and --reps >= 3: fewer cannot show the spread")
+    args = parse_args(ap)
 
     import numpy as np
     import torch
@@ -62,10 +46,7 @@ def main():
     from harness import bayer16_identity, restated, to_np16
     from restate import demosaic
 
-    if not torch.cuda.is_available():
-        raise SystemExit("bayer16_bench.py needs a CUDA device")
-    bench = _bench_module()
-    facts = gpu_facts()
+    bench, facts = start("bayer16_bench")
     dev = torch.device("cuda:0")
     st = torch.cuda.current_stream(dev)
     gen = torch.Generator(device=dev).manual_seed(0xB16)
@@ -94,7 +75,7 @@ def main():
                 "Bayer8": all(bool(torch.equal(outs["Bayer8"].data[k:k + 16], demosaic(src["Bayer8"][k:k + 16].view(-1, h, w), "RGGB")))
                               for k in range(0, n, 16))}
         alg = {k: int(n * w * h * (bpp[k] + (6 if k == "Bayer12" else 3))) for k in ARMS}
-        decode[tag] = {"batch": n, "src": [w, h], **row(times, kernels, alg, same)}
+        decode[tag] = {"batch": n, "src": [w, h], **row(times, kernels, alg, same, "output_checked")}
         print(f"[bayer16_bench] decode {tag}: " + "  ".join(f"{k} {min(times[k]):.4f}" for k in times), file=sys.stderr, flush=True)
         del src, outs
         torch.cuda.empty_cache()
@@ -139,7 +120,8 @@ def main():
             src_b = {"Bayer12": 2 * w * h, "Bayer8": w * h, "Nv12": nv12_bytes}
             alg = {k: n * (src_b[k] + out_b * dw * dh) for k in ARMS}
             key = f"{cfg}_{'f16' if f16 else 'f32'}"
-            preprocess[key] = {"batch": n, "src": [w, h], "dst": [dw, dh], "nv12_src_bytes_per_frame": nv12_bytes, **row(times, kernels, alg, same)}
+            preprocess[key] = {"batch": n, "src": [w, h], "dst": [dw, dh], "nv12_src_bytes_per_frame": nv12_bytes,
+                               **row(times, kernels, alg, same, "output_checked")}
             print(f"[bayer16_bench] {key}: " + "  ".join(f"{k} {min(times[k]):.4f}" for k in times), file=sys.stderr, flush=True)
             del outs, want, rgb
             torch.cuda.empty_cache()
@@ -160,30 +142,16 @@ def main():
     frame_bytes = {k: host[k].shape[1] * host[k].element_size() for k in ARMS}
     pipes = {k: kb.imgproc.HostPipeline(dev, src_chunk_bytes=chunk * ((frame_bytes[k] + 15) // 16 * 16), dst_chunk_bytes=chunk * 12 * w * h,
                                         depth=nstreams) for k in ARMS}
-    steps = {k: [] for k in ARMS}
-    for _ in range(args.reps):
-        for k in ARMS:
-            fn = lambda k=k: pres[k].run_raw_host(host[k], w, h, (w, h), out=outs[k], pipeline=pipes[k])
-            fn()
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record(st)
-            for _ in range(args.e2e_steps):
-                fn()
-            e1.record(st)
-            torch.cuda.synchronize()
-            steps[k].append(e0.elapsed_time(e1) / args.e2e_steps)
+    fns = {k: (lambda k=k: pres[k].run_raw_host(host[k], w, h, (w, h), out=outs[k], pipeline=pipes[k])) for k in ARMS}
+    steps, _ = time_arms(bench, fns, args.e2e_steps, 1, args.reps, st, kb)
     e2e = {}
     for k in ARMS:
-        up, down = pipes[k].last_transfer()
+        transfer = pipes[k].last_transfer()
         pipes[k].close()
         want = torch.empty((n, 3, h, w), dtype=torch.float32, device=dev)
         dev_frames = host[k].to(dev)
         pres[k].run_raw_batch([dev_frames[i] for i in range(n)], w, h, want)
-        best = min(steps[k])
-        e2e[k] = {"ms_per_step": [round(t, 3) for t in steps[k]], "ms_min": round(best, 3), "h2d_bytes": up, "d2h_bytes": down,
-                  "h2d_gbs": round(up / (best * 1e-3) / 1e9, 1), "d2h_gbs": round(down / (best * 1e-3) / 1e9, 1),
-                  "matches_device_result": bool(torch.equal(outs[k].to(dev).view(torch.int32), want.view(torch.int32)))}
+        e2e[k] = e2e_result(steps[k], transfer, bool(torch.equal(outs[k].to(dev).view(torch.int32), want.view(torch.int32))))
         print(f"[bayer16_bench] e2e cfg3a {k}: {e2e[k]['ms_per_step']} ms/step", file=sys.stderr, flush=True)
         del want, dev_frames
         torch.cuda.empty_cache()
@@ -191,10 +159,7 @@ def main():
     line = {"tool": "tools/bayer16_bench.py", "gpu": facts, "date": time.strftime("%Y-%m-%d"), "iters": args.iters, "warmup": args.warmup,
             "reps": args.reps, "peak_gbs": PEAK_GBS, "peak_source": "H100 SXM data sheet, 3.35 TB/s", "decode": decode, "preprocess": preprocess,
             "e2e_cfg3a": {"batch": n, "chunk_frames": chunk, "streams": nstreams, "steps_per_rep": args.e2e_steps, **e2e}}
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "bayer16_bench.jsonl"), "a") as f:
-        f.write(json.dumps(line) + "\n")
-    print(json.dumps(line))
+    write_line(args.out, "bayer16_bench", line)
 
 
 if __name__ == "__main__":

@@ -12,7 +12,7 @@ Every arm is timed with CUDA events over --iters launches after warm-up, the arm
 --reps times to show the spread.  Bandwidth uses algorithmic bytes over the H100 SXM data-sheet 3.35 TB/s: the frame
 (Bayer 1 B/px; NV12 1.5 B/px, for 3b the distinct bytes its sampler taps, counted by the oracle — at 3b's exact 3:1
 ratio a Bayer tap's 3x3 neighbourhood covers every source byte) plus the output (3 B/px RGB8, 12 B/px f32 CHW).
-Every Bayer output is checked: decode against the restatement of tests/test_bayer.py (on the device), preprocess
+Every Bayer output is checked: decode against restate.demosaic (on the device), preprocess
 against the run on its RGB twin (the checked decode's output as SourceFormat.Rgb8), end to end against the device run.
 
 Writes one JSON line to DIR/bayer_bench.jsonl (and stdout), with the card's name, power limit and max SM clock read in
@@ -20,42 +20,19 @@ the same run.
 """
 from __future__ import annotations
 
-import argparse
-import json
-import os
 import sys
 import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-
-from half_bench import PEAK_GBS, _bench_module, gpu_facts  # noqa: E402
-from yuv_bench import row_for, time_arms  # noqa: E402
+from benchkit import PEAK_GBS, arg_parser, e2e_result, parse_args, row, start, time_arms, write_line
 
 PATTERNS = ("RGGB", "BGGR", "GRBG", "GBRG")
 
 
-def row(times, kernels, alg_bytes, checked):
-    """yuv_bench's row, with the outcome of each arm's output check (None: the NV12 arm, a speed reference only)."""
-    r = row_for(times, kernels, alg_bytes, checked)
-    for v in r.values():
-        v["output_checked"] = v.pop("bit_identical_to_sibling")
-    return r
-
-
 def main():
-    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
-    ap.add_argument("--out", required=True, help="directory for bayer_bench.jsonl")
-    ap.add_argument("--iters", type=int, default=20)
-    ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--reps", type=int, default=3)
+    ap = arg_parser(__doc__, "bayer_bench")
     ap.add_argument("--e2e-frames", type=int, default=64)
     ap.add_argument("--e2e-steps", type=int, default=5)
-    args = ap.parse_args()
-    if args.iters < 20 or args.reps < 3:
-        ap.error("--iters >= 20 and --reps >= 3: fewer cannot show the spread")
+    args = parse_args(ap)
 
     import numpy as np
     import torch
@@ -64,10 +41,7 @@ def main():
     from oracle import oracle as o
     from restate import demosaic
 
-    if not torch.cuda.is_available():
-        raise SystemExit("bayer_bench.py needs a CUDA device")
-    bench = _bench_module()
-    facts = gpu_facts()
+    bench, facts = start("bayer_bench")
     dev = torch.device("cuda:0")
     st = torch.cuda.current_stream(dev)
     gen = torch.Generator(device=dev).manual_seed(0xBA7E)
@@ -89,7 +63,7 @@ def main():
         for p in PATTERNS:
             same[p] = all(bool(torch.equal(outs[p].data[k0:k0 + 16], demosaic(bayer[k0:k0 + 16].view(-1, h, w), p))) for k0 in range(0, n, 16))
         alg = {"Nv12": n * (w * h * 3 // 2 + 3 * w * h), **{p: n * (w * h + 3 * w * h) for p in PATTERNS}}
-        decode[tag] = {"batch": n, "src": [w, h], **row(times, kernels, alg, same)}
+        decode[tag] = {"batch": n, "src": [w, h], **row(times, kernels, alg, same, "output_checked")}
         print(f"[bayer_bench] decode {tag}: " + "  ".join(f"{k} {min(times[k]):.4f}" for k in times), file=sys.stderr, flush=True)
         del bayer, nv12, outs
         torch.cuda.empty_cache()
@@ -125,7 +99,7 @@ def main():
             same[p] = ok
         alg = {"Nv12": n * (nv12_bytes + 12 * dw * dh), **{p: n * (w * h + 12 * dw * dh) for p in PATTERNS}}
         preprocess[cfg] = {"batch": n, "src": [w, h], "dst": [dw, dh], "nv12_src_bytes_per_frame": nv12_bytes,
-                           **row(times, kernels, alg, same)}
+                           **row(times, kernels, alg, same, "output_checked")}
         print(f"[bayer_bench] {cfg}: " + "  ".join(f"{k} {min(times[k]):.4f}" for k in times), file=sys.stderr, flush=True)
         del outs, want, rgb
         torch.cuda.empty_cache()
@@ -144,30 +118,16 @@ def main():
     outs = {k: torch.empty((n, 3, h, w), dtype=torch.float32, pin_memory=True) for k in host}
     pipes = {k: kb.imgproc.HostPipeline(dev, src_chunk_bytes=chunk * ((host[k].shape[1] + 15) // 16 * 16), dst_chunk_bytes=chunk * 12 * w * h,
                                         depth=nstreams) for k in host}
-    steps = {k: [] for k in host}
-    for _ in range(args.reps):
-        for k in host:
-            fn = lambda k=k: pres[k].run_raw_host(host[k], w, h, (w, h), out=outs[k], pipeline=pipes[k])
-            fn()
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record(st)
-            for _ in range(args.e2e_steps):
-                fn()
-            e1.record(st)
-            torch.cuda.synchronize()
-            steps[k].append(e0.elapsed_time(e1) / args.e2e_steps)
+    fns = {k: (lambda k=k: pres[k].run_raw_host(host[k], w, h, (w, h), out=outs[k], pipeline=pipes[k])) for k in host}
+    steps, _ = time_arms(bench, fns, args.e2e_steps, 1, args.reps, st, kb)
     e2e = {}
     for k in host:
-        up, down = pipes[k].last_transfer()
+        transfer = pipes[k].last_transfer()
         pipes[k].close()
         want = torch.empty((n, 3, h, w), dtype=torch.float32, device=dev)
         dev_frames = host[k].to(dev)
         pres[k].run_raw_batch([dev_frames[i] for i in range(n)], w, h, want)
-        best = min(steps[k])
-        e2e[k] = {"ms_per_step": [round(t, 3) for t in steps[k]], "ms_min": round(best, 3), "h2d_bytes": up, "d2h_bytes": down,
-                  "h2d_gbs": round(up / (best * 1e-3) / 1e9, 1), "d2h_gbs": round(down / (best * 1e-3) / 1e9, 1),
-                  "matches_device_result": bool(torch.equal(outs[k].to(dev).view(torch.int32), want.view(torch.int32)))}
+        e2e[k] = e2e_result(steps[k], transfer, bool(torch.equal(outs[k].to(dev).view(torch.int32), want.view(torch.int32))))
         print(f"[bayer_bench] e2e cfg3a {k}: {e2e[k]['ms_per_step']} ms/step", file=sys.stderr, flush=True)
         del want, dev_frames
         torch.cuda.empty_cache()
@@ -175,10 +135,7 @@ def main():
     line = {"tool": "tools/bayer_bench.py", "gpu": facts, "date": time.strftime("%Y-%m-%d"), "iters": args.iters, "warmup": args.warmup,
             "reps": args.reps, "peak_gbs": PEAK_GBS, "peak_source": "H100 SXM data sheet, 3.35 TB/s", "decode": decode, "preprocess": preprocess,
             "e2e_cfg3a": {"batch": n, "chunk_frames": chunk, "streams": nstreams, "steps_per_rep": args.e2e_steps, **e2e}}
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "bayer_bench.jsonl"), "a") as f:
-        f.write(json.dumps(line) + "\n")
-    print(json.dumps(line))
+    write_line(args.out, "bayer_bench", line)
 
 
 if __name__ == "__main__":

@@ -25,46 +25,27 @@ read in the same run.
 """
 from __future__ import annotations
 
-import argparse
-import json
-import os
 import sys
 import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-
-from bayer_bench import row  # noqa: E402
-from half_bench import PEAK_GBS, _bench_module, gpu_facts  # noqa: E402
-from yuv_bench import time_arms  # noqa: E402
+from benchkit import PEAK_GBS, arg_parser, e2e_result, parse_args, row, start, time_arms, write_line
 
 PACKED = {"Raw10p": 10, "Raw12p": 12, "Raw14p": 14}
 ARMS = ("Raw10p", "Raw12p", "Raw14p", "Bayer12", "Raw12p_generic")
 
 
 def main():
-    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
-    ap.add_argument("--out", required=True, help="directory for bayer_packed_bench.jsonl")
-    ap.add_argument("--iters", type=int, default=20)
-    ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--reps", type=int, default=3)
+    ap = arg_parser(__doc__, "bayer_packed_bench")
     ap.add_argument("--e2e-frames", type=int, default=64)
     ap.add_argument("--e2e-steps", type=int, default=5)
-    args = ap.parse_args()
-    if args.iters < 20 or args.reps < 3:
-        ap.error("--iters >= 20 and --reps >= 3: fewer cannot show the spread")
+    args = parse_args(ap)
 
     import torch
 
     import kornia_rs_b200 as kb
     from restate import unpack
 
-    if not torch.cuda.is_available():
-        raise SystemExit("bayer_packed_bench.py needs a CUDA device")
-    bench = _bench_module()
-    facts = gpu_facts()
+    bench, facts = start("bayer_packed_bench")
     dev = torch.device("cuda:0")
     st = torch.cuda.current_stream(dev)
     gen = torch.Generator(device=dev).manual_seed(0xBAC)
@@ -75,7 +56,7 @@ def main():
     bpp = {"Raw10p": 1.25, "Raw12p": 1.5, "Raw14p": 1.75, "Bayer12": 2.0, "Raw12p_generic": 1.5}
 
     def pack_dev(samples, bits):
-        """[n, h, w] int32 samples -> [n, h * w * bits / 8] uint8 on the device (the inverse of test_bayer_packed.unpack)."""
+        """[n, h, w] int32 samples -> [n, h * w * bits / 8] uint8 on the device (the inverse of restate.unpack)."""
         g, gb, lo = (2, 3, 4) if bits == 12 else (4, bits // 2, bits - 8)
         n, h, w = samples.shape
         v = samples.view(n, h, w // g, g)
@@ -122,7 +103,7 @@ def main():
         same = {k: bool(torch.equal(outs[k].data.view(torch.int16), outs["Bayer12"].data.view(torch.int16))) for k in ARMS if k != "Bayer12"}
         same["Bayer12"] = None
         alg = {k: int(n * (frame_bytes(k, w, h) + 6 * w * h)) for k in ARMS}
-        decode[tag] = {"batch": n, "src": [w, h], **row(times, kernels, alg, same)}
+        decode[tag] = {"batch": n, "src": [w, h], **row(times, kernels, alg, same, "output_checked")}
         print(f"[bayer_packed_bench] decode {tag}: " + "  ".join(f"{k} {min(times[k]):.4f}" for k in times), file=sys.stderr, flush=True)
         del src, outs, gsrc
         torch.cuda.empty_cache()
@@ -156,7 +137,7 @@ def main():
                 same[k] = ok
             alg = {k: n * (frame_bytes(k, w, h) + out_b * dw * dh) for k in arms}
             key = f"{cfg}_{'f16' if f16 else 'f32'}"
-            preprocess[key] = {"batch": n, "src": [w, h], "dst": [dw, dh], **row(times, kernels, alg, same)}
+            preprocess[key] = {"batch": n, "src": [w, h], "dst": [dw, dh], **row(times, kernels, alg, same, "output_checked")}
             print(f"[bayer_packed_bench] {key}: " + "  ".join(f"{k} {min(times[k]):.4f}" for k in times), file=sys.stderr, flush=True)
             del outs, want
             torch.cuda.empty_cache()
@@ -178,29 +159,15 @@ def main():
     for f16 in (False, True):
         dt, it = (torch.float16, torch.int16) if f16 else (torch.float32, torch.int32)
         outs = {k: torch.empty((n, 3, h, w), dtype=dt, pin_memory=True) for k in e2e_arms}
-        steps = {k: [] for k in e2e_arms}
-        for _ in range(args.reps):
-            for k in e2e_arms:
-                fn = lambda k=k: pres[k].run_raw_host(host[k], w, h, (w, h), out=outs[k], f16=f16, pipeline=pipes[k])
-                fn()
-                torch.cuda.synchronize()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record(st)
-                for _ in range(args.e2e_steps):
-                    fn()
-                e1.record(st)
-                torch.cuda.synchronize()
-                steps[k].append(e0.elapsed_time(e1) / args.e2e_steps)
+        fns = {k: (lambda k=k: pres[k].run_raw_host(host[k], w, h, (w, h), out=outs[k], f16=f16, pipeline=pipes[k])) for k in e2e_arms}
+        steps, _ = time_arms(bench, fns, args.e2e_steps, 1, args.reps, st, kb)
         res = {}
         for k in e2e_arms:
-            up, down = pipes[k].last_transfer()
+            transfer = pipes[k].last_transfer()
             want = torch.empty((n, 3, h, w), dtype=dt, device=dev)
             dev_frames = host[k].to(dev)
             (pres[k].run_raw_batch_f16 if f16 else pres[k].run_raw_batch)([dev_frames[i] for i in range(n)], w, h, want)
-            best = min(steps[k])
-            res[k] = {"ms_per_step": [round(t, 3) for t in steps[k]], "ms_min": round(best, 3), "h2d_bytes": up, "d2h_bytes": down,
-                      "h2d_gbs": round(up / (best * 1e-3) / 1e9, 1), "d2h_gbs": round(down / (best * 1e-3) / 1e9, 1),
-                      "matches_device_result": bool(torch.equal(outs[k].to(dev).view(it), want.view(it)))}
+            res[k] = e2e_result(steps[k], transfer, bool(torch.equal(outs[k].to(dev).view(it), want.view(it))))
             print(f"[bayer_packed_bench] e2e cfg3a {'f16' if f16 else 'f32'} {k}: {res[k]['ms_per_step']} ms/step", file=sys.stderr, flush=True)
             del want, dev_frames
             torch.cuda.empty_cache()
@@ -212,10 +179,7 @@ def main():
     line = {"tool": "tools/bayer_packed_bench.py", "gpu": facts, "date": time.strftime("%Y-%m-%d"), "iters": args.iters, "warmup": args.warmup,
             "reps": args.reps, "peak_gbs": PEAK_GBS, "peak_source": "H100 SXM data sheet, 3.35 TB/s", "decode": decode, "preprocess": preprocess,
             "e2e_cfg3a": {"batch": n, "chunk_frames": chunk, "streams": nstreams, "steps_per_rep": args.e2e_steps, **e2e}}
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "bayer_packed_bench.jsonl"), "a") as f:
-        f.write(json.dumps(line) + "\n")
-    print(json.dumps(line))
+    write_line(args.out, "bayer_packed_bench", line)
 
 
 if __name__ == "__main__":

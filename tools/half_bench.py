@@ -15,32 +15,10 @@ same run.
 """
 from __future__ import annotations
 
-import argparse
-import importlib.util
-import json
-import os
-import subprocess
 import sys
 import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-PEAK_GBS = 3350.0   # H100 SXM data sheet HBM3
-
-
-def _bench_module():
-    spec = importlib.util.spec_from_file_location("bench_mod", os.path.join(ROOT, "bench.py"))
-    m = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(m)
-    return m
-
-
-def gpu_facts() -> dict:
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
-    name, power, clock = (s.strip() for s in q.split(","))
-    return {"name": name, "power_limit": power, "clocks_max_sm": clock}
+from benchkit import PEAK_GBS, arg_parser, e2e_result, parse_args, start, time_arms, write_line
 
 
 def tapped_pixels(sw, sh, dw, dh):
@@ -56,24 +34,15 @@ def tapped_pixels(sw, sh, dw, dh):
 
 
 def main():
-    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
-    ap.add_argument("--out", required=True, help="directory for half_bench.jsonl")
-    ap.add_argument("--iters", type=int, default=20)
-    ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--reps", type=int, default=3)
+    ap = arg_parser(__doc__, "half_bench")
     ap.add_argument("--e2e-steps", type=int, default=10)
-    args = ap.parse_args()
-    if args.iters < 20 or args.reps < 3:
-        ap.error("--iters >= 20 and --reps >= 3: fewer cannot show the spread")
+    args = parse_args(ap)
 
     import torch
 
     import kornia_rs_b200 as kb
 
-    if not torch.cuda.is_available():
-        raise SystemExit("half_bench.py needs a CUDA device")
-    bench = _bench_module()
-    facts = gpu_facts()
+    bench, facts = start("half_bench")
     dev = torch.device("cuda:0")
     st = torch.cuda.current_stream(dev)
     p = kb.imgproc.NormalizeParams.from_mean_std(bench.IMAGENET_MEAN, bench.IMAGENET_STD)
@@ -95,12 +64,7 @@ def main():
         s = src[:n]
         outs = {k: torch.empty((n, 3, dh, dw), dtype=t, device=dev) for k, t in dtypes.items()}
         fns = {k: (lambda k=k: op(s, dw, dh, scale, bias, dtypes[k], out=outs[k])) for k in dtypes}
-        times = {k: [] for k in dtypes}
-        kernels = {}
-        for _ in range(args.reps):
-            for k in dtypes:
-                times[k].append(bench.time_launches(fns[k], args.iters, args.warmup, st))
-                kernels[k] = kb._lib.last_kernel()
+        times, kernels = time_arms(bench, fns, args.iters, args.warmup, args.reps, st, kb)
         same = {k: bool(torch.equal(outs[k].view(torch.int16), outs["f32"].to(dtypes[k]).view(torch.int16))) for k in ("f16", "bf16")}
         tapped = tapped_pixels(SW, SH, dw, dh)
         row = {"batch": n, "dst": [dw, dh], "tapped_src_bytes_per_frame": tapped * 3, "bit_identical_to_f32_cast": same}
@@ -126,37 +90,18 @@ def main():
     for k in dtypes:
         pipes[k] = kb.imgproc.HostPipeline(dev, src_chunk_bytes=chunk * SW * SH * 3, dst_chunk_bytes=chunk * 3 * DW * DH * esize[k], depth=nstreams)
         hosts[k] = torch.empty((N, 3, DH, DW), dtype=dtypes[k], pin_memory=True)
-    steps = {k: [] for k in dtypes}
-    for _ in range(args.reps):
-        for k in dtypes:
-            fn = lambda: op(host_src, DW, DH, scale, bias, dtypes[k], out=hosts[k], pipeline=pipes[k])
-            fn(); fn()
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record(st)
-            for _ in range(args.e2e_steps):
-                fn()
-            e1.record(st)
-            torch.cuda.synchronize()
-            steps[k].append(e0.elapsed_time(e1) / args.e2e_steps)
+    fns = {k: (lambda k=k: op(host_src, DW, DH, scale, bias, dtypes[k], out=hosts[k], pipeline=pipes[k])) for k in dtypes}
+    steps, _ = time_arms(bench, fns, args.e2e_steps, 2, args.reps, st, kb)
     for k in dtypes:
-        up, down = pipes[k].last_transfer()
-        best = min(steps[k])
-        e2e[k] = {"ms_per_step": [round(t, 3) for t in steps[k]], "ms_min": round(best, 3), "h2d_bytes": up, "d2h_bytes": down,
-                  "h2d_gbs": round(up / (best * 1e-3) / 1e9, 1), "d2h_gbs": round(down / (best * 1e-3) / 1e9, 1),
-                  "gpix_s": round(N * DW * DH / (best * 1e-3) / 1e9, 3),
-                  "matches_device_result": bool(torch.equal(hosts[k].to(dev).view(torch.int16 if esize[k] == 2 else torch.int32),
-                                                            ref[k].view(torch.int16 if esize[k] == 2 else torch.int32)))}
+        it = torch.int16 if esize[k] == 2 else torch.int32
+        e2e[k] = e2e_result(steps[k], pipes[k].last_transfer(), bool(torch.equal(hosts[k].to(dev).view(it), ref[k].view(it))), pixels=N * DW * DH)
         pipes[k].close()
         print(f"[half_bench] e2e {k}: {e2e[k]['ms_per_step']} ms/step", file=sys.stderr, flush=True)
 
     line = {"tool": "tools/half_bench.py", "gpu": facts, "date": time.strftime("%Y-%m-%d"), "iters": args.iters, "warmup": args.warmup,
             "reps": args.reps, "peak_gbs": PEAK_GBS, "peak_source": "H100 SXM data sheet, 3.35 TB/s", "device": device,
             "e2e_cfg2": {"batch": N, "chunk_frames": chunk, "streams": nstreams, "steps_per_rep": args.e2e_steps, **e2e}}
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "half_bench.jsonl"), "a") as f:
-        f.write(json.dumps(line) + "\n")
-    print(json.dumps(line))
+    write_line(args.out, "half_bench", line)
 
 
 if __name__ == "__main__":

@@ -23,8 +23,6 @@ from __future__ import annotations
 
 import argparse
 import ctypes as C
-import importlib.util
-import json
 import os
 import shutil
 import statistics
@@ -33,24 +31,9 @@ import sys
 import tempfile
 import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from benchkit import ROOT, start, write_line
 
 PERIOD, FIRST = 3, 1          # the headline's tapped rows and columns: 3d + 1
-
-
-def _bench_module():
-    spec = importlib.util.spec_from_file_location("bench_mod", os.path.join(ROOT, "bench.py"))
-    m = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(m)
-    return m
-
-
-def gpu_facts() -> dict:
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
-    name, power, clock = (s.strip() for s in q.split(","))
-    return {"name": name, "power_limit": power, "clocks_max_sm": clock}
 
 
 def build_probes(tmp: str) -> C.CDLL:
@@ -85,10 +68,7 @@ def main():
 
     import kornia_rs_b200 as kb
 
-    if not torch.cuda.is_available():
-        raise SystemExit("point_ceiling.py needs a CUDA device")
-    bench = _bench_module()
-    facts = gpu_facts()
+    bench, facts = start("point_ceiling")
     dev = torch.device("cuda:0")
     st = torch.cuda.current_stream(dev)
     sp = C.c_void_p(st.cuda_stream)
@@ -178,10 +158,7 @@ def main():
             "twin_faster_than_tiled": round(1.0 - res["c_twin"]["ms_mean"] / res["e_tiled"]["ms_mean"], 4),
             "rows_faster_than_tiled": round(1.0 - res["f_rows"]["ms_mean"] / res["e_tiled"]["ms_mean"], 4),
             "twin_output_ok": twin_ok, "rows_bits_equal_tiled": same}
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "point_ceiling.jsonl"), "a") as f:
-        f.write(json.dumps(line) + "\n")
-    print(json.dumps(line))
+    write_line(args.out, "point_ceiling", line)
 
 
 if __name__ == "__main__":

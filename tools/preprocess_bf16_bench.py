@@ -21,19 +21,10 @@ clock read in the same run.
 """
 from __future__ import annotations
 
-import argparse
-import json
-import os
 import sys
 import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-
-from half_bench import PEAK_GBS, _bench_module, gpu_facts  # noqa: E402
-from yuv_bench import time_arms  # noqa: E402
+from benchkit import PEAK_GBS, arg_parser, e2e_result, parse_args, start, time_arms, write_line
 
 OUTS = ("f32", "f16", "bf16")
 FAST = ("Nv12", "P010", "BayerRggb12", "I444")
@@ -42,16 +33,10 @@ TAP_BPP = {"Nv12": None, "P010": None, "BayerRggb12": 2, "I444": 3, "Yuyv": 2}  
 
 
 def main():
-    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
-    ap.add_argument("--out", required=True, help="directory for preprocess_bf16_bench.jsonl")
-    ap.add_argument("--iters", type=int, default=20)
-    ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--reps", type=int, default=3)
+    ap = arg_parser(__doc__, "preprocess_bf16_bench")
     ap.add_argument("--e2e-frames", type=int, default=64)
     ap.add_argument("--e2e-steps", type=int, default=5)
-    args = ap.parse_args()
-    if args.iters < 20 or args.reps < 3:
-        ap.error("--iters >= 20 and --reps >= 3: fewer cannot show the spread")
+    args = parse_args(ap)
 
     import numpy as np
     import torch
@@ -59,10 +44,7 @@ def main():
     import kornia_rs_b200 as kb
     from oracle import oracle as o
 
-    if not torch.cuda.is_available():
-        raise SystemExit("preprocess_bf16_bench.py needs a CUDA device")
-    bench = _bench_module()
-    facts = gpu_facts()
+    bench, facts = start("preprocess_bf16_bench")
     dev = torch.device("cuda:0")
     st = torch.cuda.current_stream(dev)
     gen = torch.Generator(device=dev).manual_seed(0xBF16)
@@ -136,38 +118,25 @@ def main():
     outs = {k: torch.empty((ne, 3, h, w), dtype=dtypes[k], pin_memory=True) for k in OUTS}
     pipe = kb.imgproc.HostPipeline(dev, src_chunk_bytes=chunk * ((host.shape[1] + 15) // 16 * 16), dst_chunk_bytes=chunk * 12 * w * h, depth=nstreams)
     steps, transfer = {k: [] for k in OUTS}, {}
-    for _ in range(args.reps):
+    for _ in range(args.reps):   # one pipeline for the three arms: each arm's link bytes are read right after its turn
         for k in OUTS:
             fn = lambda k=k: pre.run_raw_host(host, w, h, (w, h), out=outs[k], pipeline=pipe, dtype=dtypes[k])
-            fn()
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record(st)
-            for _ in range(args.e2e_steps):
-                fn()
-            e1.record(st)
-            torch.cuda.synchronize()
-            steps[k].append(e0.elapsed_time(e1) / args.e2e_steps)
+            steps[k].append(bench.time_launches(fn, args.e2e_steps, 1, st))
             transfer[k] = pipe.last_transfer()
     pipe.close()
     want = outs["f32"].to(torch.bfloat16)
     e2e_ok = bool(torch.equal(outs["bf16"].view(torch.int16), want.view(torch.int16)))
     e2e = {}
     for k in OUTS:
-        best = min(steps[k])
-        up, down = transfer[k]
-        e2e[k] = {"ms_per_step": [round(t, 3) for t in steps[k]], "ms_min": round(best, 3), "h2d_bytes": up, "d2h_bytes": down,
-                  "h2d_gbs": round(up / (best * 1e-3) / 1e9, 1), "d2h_gbs": round(down / (best * 1e-3) / 1e9, 1)}
-        print(f"[preprocess_bf16_bench] e2e cfg3a {k}: {e2e[k]['ms_per_step']} ms/step, {up} B up, {down} B down", file=sys.stderr, flush=True)
+        e2e[k] = e2e_result(steps[k], transfer[k])
+        print(f"[preprocess_bf16_bench] e2e cfg3a {k}: {e2e[k]['ms_per_step']} ms/step, {transfer[k][0]} B up, {transfer[k][1]} B down",
+              file=sys.stderr, flush=True)
     e2e["bf16"]["equals_f32_rounded"] = e2e_ok
 
     line = {"tool": "tools/preprocess_bf16_bench.py", "gpu": facts, "date": time.strftime("%Y-%m-%d"), "iters": args.iters, "warmup": args.warmup,
             "reps": args.reps, "peak_gbs": PEAK_GBS, "peak_source": "H100 SXM data sheet, 3.35 TB/s", "preprocess": preprocess,
             "e2e_cfg3a": {"batch": ne, "chunk_frames": chunk, "streams": nstreams, "steps_per_rep": args.e2e_steps, **e2e}}
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "preprocess_bf16_bench.jsonl"), "a") as f:
-        f.write(json.dumps(line) + "\n")
-    print(json.dumps(line))
+    write_line(args.out, "preprocess_bf16_bench", line)
 
 
 if __name__ == "__main__":

@@ -14,7 +14,7 @@ results/h100_preprocess_remap_bench.jsonl (or --out).
   R3  a rig of 6 cameras x 16 NV12 1080p frames, each camera with its own 640 x 384 map, f32: one call (96 regions,
       6 maps) against 6 shared-map calls (`per_map`).
 
-Three regions of every output are checked in the same run against tests/test_preprocess_remap.remap_reference.
+Three regions of every output are checked in the same run against restate.remap_reference.
 Arms alternate: 20 launches after warm-up, 3 repeats, minima given with the repeat spread.  Algorithmic bytes: the
 distinct source bytes the bilinear taps read in each frame (per tapped luma pixel of NV12 / P010 the chroma pair it decodes
 with, per tapped Bayer pixel its 3 x 3 demosaic neighbourhood), each distinct map once (8 bytes per output pixel) and the
@@ -24,52 +24,23 @@ import argparse
 import ctypes as C
 import json
 import os
-import sys
 import zlib
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-from preprocess_roi_bench import HBM, gpu_facts  # noqa: E402
+from benchkit import (FORMATS, OUT_CODES, PEAK_GBS, ROOT, append_lines, frame_len, gpu_facts, mask_bytes, preprocess_desc, stream,
+                      tap_mask, time_alternating)
 
 F32 = np.float32
-OUT_CODES = {"f32": 0, "bf16": 2}
 DTYPES = {"f32": torch.float32, "bf16": torch.bfloat16}
-FMT = {"NV12": (3, 1), "P010": (80, 2), "RGGB12": (36, 2)}   # format code, bytes per sample
-
-
-def frame_len(fmt, w, h):
-    return w * h * 3 // 2 * FMT[fmt][1] if fmt != "RGGB12" else w * h * 2
 
 
 def tapped_bytes(fmt, w, h, mx, my):
     """Distinct source bytes of one frame the bilinear sampler reads through the map (mx, my): see the module docstring."""
     with np.errstate(invalid="ignore"):
         inside = (mx >= 0) & (mx < F32(w)) & (my >= 0) & (my < F32(h))
-    sx, sy = mx[inside], my[inside]
-    x0, y0 = np.floor(sx).astype(np.int64), np.floor(sy).astype(np.int64)
-    nx, ny = sx != x0, sy != y0
-    x1, y1 = np.minimum(x0 + 1, w - 1), np.minimum(y0 + 1, h - 1)
-    m = np.zeros((h, w), bool)
-    m[y0, x0] = True
-    m[y0[nx], x1[nx]] = True
-    m[y1[ny], x0[ny]] = True
-    m[y1[nx & ny], x1[nx & ny]] = True
-    if fmt == "RGGB12":
-        p = np.pad(m, 1)
-        m = np.zeros_like(m)
-        for dy in range(3):
-            for dx in range(3):
-                m |= p[dy:dy + h, dx:dx + w]
-        return int(m.sum()) * 2
-    ys, xs = np.nonzero(m)
-    chroma = np.zeros((h // 2, w // 2), bool)
-    chroma[ys >> 1, xs >> 1] = True
-    return (int(m.sum()) + 2 * int(chroma.sum())) * FMT[fmt][1]
+    return mask_bytes(fmt, tap_mask(mx[inside], my[inside], w, h))
 
 
 def camera(w, h, rng):
@@ -87,7 +58,7 @@ def main():
     ap.add_argument("--region-major-lib", default=None, help="a scratch build whose remap kernels walk regions slowest (R1 only)")
     a = ap.parse_args()
     import kornia_rs_b200 as kb
-    from kornia_rs_b200._lib import PreprocessDesc, RemapRoi
+    from kornia_rs_b200._lib import RemapRoi
     from harness import compare_region
     from restate import Case, RCase, picture, remap_reference
 
@@ -99,39 +70,7 @@ def main():
         alt.kb200_preprocess_remap.argtypes = lib.kb200_preprocess_remap.argtypes
         alt.kb200_preprocess_remap.restype = C.c_int
     dev = torch.device("cuda:0")
-    facts = gpu_facts()
-    inv_std = tuple(float(F32(1) / F32(s)) for s in kb.IMAGENET_STD)
-
-    def desc(fmt, w, h, dw, dh, code=None, bpp=1, pitch=None):
-        d = PreprocessDesc()
-        d.scale_x, d.scale_y, d.pad_x, d.pad_y = 1.0, 1.0, 0.0, 0.0
-        d.src_w, d.src_h, d.src_bpp = w, h, bpp
-        d.src_pitch = pitch if pitch is not None else w * FMT[fmt][1]
-        d.fmt = FMT[fmt][0] if code is None else code
-        d.dst_w, d.dst_h = dw, dh
-        d.mean, d.inv_std = (C.c_float * 3)(*kb.IMAGENET_MEAN), (C.c_float * 3)(*inv_std)
-        d.pad_value, d.sampling = 114.0, 1
-        return d
-
-    def time_arms(arms):
-        """{name: fn}: alternate, `iters` calls each, `repeats` times; ms per call, min and max over repeats."""
-        for fn in arms.values():
-            fn(); fn()
-        torch.cuda.synchronize()
-        res = {k: [] for k in arms}
-        for _ in range(a.repeats):
-            for k, fn in arms.items():
-                s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                s.record()
-                for _ in range(a.iters):
-                    fn()
-                e.record()
-                torch.cuda.synchronize()
-                res[k].append(s.elapsed_time(e) / a.iters)
-        return {k: (min(v), max(v)) for k, v in res.items()}
-
-    def stream():
-        return torch.cuda.current_stream().cuda_stream
+    facts = dict(zip(("gpu", "power_limit", "max_sm_clock"), gpu_facts().values()))
 
     def gen_map(intr, dist, new, dw, dh):
         mx = torch.empty((dh, dw), dtype=torch.float32, device=dev)
@@ -156,7 +95,7 @@ def main():
 
     def check_regions(wl, fmt, w, h, dw, dh, out, base, need, regs, maps_x, maps_y, dst):
         torch.cuda.synchronize()
-        c = Case(wl, 0, FMT[fmt][0], 0, 1, w, h, w * FMT[fmt][1], "remap", 1.0, 1.0, 0.0, 0.0, dw, dh, 1, False, "table", 1, (), None, 0,
+        c = Case(wl, 0, FORMATS[fmt][0], 0, 1, w, h, w * FORMATS[fmt][1], "remap", 1.0, 1.0, 0.0, 0.0, dw, dh, 1, False, "table", 1, (), None, 0,
                  "imagenet", 114.0)
         rc = RCase(c, 1, out, 1, (), ())
         picked = [0, len(regs) // 2, len(regs) - 1]
@@ -185,7 +124,7 @@ def main():
         row["algorithmic_bytes"] = nbytes
         for k in t:
             if k in (main_arm, "batch_entry", "remap_region_major"):
-                row[f"{k}_share_of_3.35TBps"] = round(nbytes / (t[k][0] * 1e-3) / HBM, 3)
+                row[f"{k}_share_of_3.35TBps"] = round(nbytes / (t[k][0] * 1e-3) / (PEAK_GBS * 1e9), 3)
         row.update(iters=a.iters, repeats=a.repeats, **check, **facts)
         print(json.dumps(row), flush=True)
         lines.append(row)
@@ -201,10 +140,10 @@ def main():
     hx, hy = mx.cpu().numpy(), my.cpu().numpy()
     src_bytes = tapped_bytes("NV12", w, h, hx, hy) * n
     regs = [(k, 0) for k in range(n)]
-    d = desc("NV12", w, h, w, h)
+    d = preprocess_desc(*FORMATS["NV12"], w, h, w, h)
     rgb = torch.empty((n, h, w, 3), dtype=torch.uint8, device=dev)
     rgb2 = torch.empty_like(rgb)
-    dn = desc("NV12", w, h, w, h, code=0, bpp=3, pitch=3 * w)
+    dn = preprocess_desc(0, 3, w, h, w, h, bpp=3)   # RGB8
     for out in ("f32", "bf16"):
         dst = torch.empty((n, 3, h, w), dtype=DTYPES[out], device=dev)
         run = remap_call(lib.kb200_preprocess_remap, d, ptrs, lens, n, mx, my, 1, regs, dst, out)
@@ -231,7 +170,7 @@ def main():
             assert entry(s, C.byref(dn), rgb2.data_ptr(), rgb2.numel(), w * h * 3, n, edst.data_ptr(), edst.numel()) == 0
 
         arms["existing"] = existing
-        t = time_arms(arms)
+        t = time_alternating(arms, a.iters, a.repeats)
         nbytes = src_bytes + 8 * w * h + dst.numel() * dst.element_size()
         row = {"workload": "R1", "src": f"NV12 {w}x{h}", "out": out, "frames": n, "regions": n, "maps": 1, "dst": [3, h, w], "sampling": "Bilinear",
                "kernel": kern, "launches": -(-n // 192), "tapped_src_bytes": src_bytes}
@@ -257,7 +196,7 @@ def main():
         torch.cuda.synchronize()
         check = {"batch_entry_kernel": kb._lib.last_kernel(), "identical_to_batch_entry": bool(torch.equal(dst.view(torch.uint8), ref.view(torch.uint8)))}
         assert check["identical_to_batch_entry"], "R1 identity differs from the batch entry"
-        t = time_arms({"remap": run, "batch_entry": batch})
+        t = time_alternating({"remap": run, "batch_entry": batch}, a.iters, a.repeats)
         src_b = (w * h * 3 // 2) * n
         nbytes = src_b + 8 * w * h + dst.numel() * dst.element_size()
         row = {"workload": "R1-identity", "src": f"NV12 {w}x{h}", "out": out, "frames": n, "regions": n, "maps": 1, "dst": [3, h, w],
@@ -277,7 +216,7 @@ def main():
     regs = [(k, 0) for k in range(n)]
     for fmt in ("NV12", "P010", "RGGB12"):
         base, need, ptrs, lens = frames_of(fmt, w, h, n, "R2" + fmt)
-        d = desc(fmt, w, h, dw, dh)
+        d = preprocess_desc(*FORMATS[fmt], w, h, dw, dh)
         src_bytes = tapped_bytes(fmt, w, h, hx, hy) * n
         for out in ("f32", "bf16"):
             dst = torch.empty((n, 3, dh, dw), dtype=DTYPES[out], device=dev)
@@ -285,7 +224,7 @@ def main():
             run()
             kern = kb._lib.last_kernel()
             check = {"regions_checked_against_reference": check_regions("R2", fmt, w, h, dw, dh, out, base, need, regs, [hx], [hy], dst)}
-            t = time_arms({"remap": run})
+            t = time_alternating({"remap": run}, a.iters, a.repeats)
             nbytes = src_bytes + 8 * dw * dh + dst.numel() * dst.element_size()
             row = {"workload": "R2", "src": f"{fmt} {w}x{h}", "out": out, "frames": n, "regions": n, "maps": 1, "dst": [3, dh, dw],
                    "sampling": "Bilinear", "kernel": kern, "tapped_src_bytes": src_bytes}
@@ -307,7 +246,7 @@ def main():
     my = torch.stack([m[1] for m in maps]).contiguous()
     hx, hy = mx.cpu().numpy(), my.cpu().numpy()
     regs = [(k, k % cams) for k in range(n)]   # frame k comes from camera k % 6
-    d = desc("NV12", w, h, dw, dh)
+    d = preprocess_desc(*FORMATS["NV12"], w, h, dw, dh)
     src_bytes = sum(tapped_bytes("NV12", w, h, hx[k % cams], hy[k % cams]) for k in range(n))
     out = "f32"
     dst = torch.empty((n, 3, dh, dw), dtype=DTYPES[out], device=dev)
@@ -330,16 +269,13 @@ def main():
     torch.cuda.synchronize()
     check["identical_to_per_map_calls"] = bool(torch.equal(pdst.transpose(0, 1).reshape(n, 3, dh, dw).view(torch.uint8), dst.view(torch.uint8)))
     assert check["identical_to_per_map_calls"], "R3 differs from the per-map calls"
-    t = time_arms({"remap": run, "per_map": six_calls})
+    t = time_alternating({"remap": run, "per_map": six_calls}, a.iters, a.repeats)
     nbytes = src_bytes + 8 * dw * dh * cams + dst.numel() * dst.element_size()
     row = {"workload": "R3", "src": f"NV12 {w}x{h}", "out": out, "frames": n, "regions": n, "maps": cams, "dst": [3, dh, dw], "sampling": "Bilinear",
            "kernel": kern, "tapped_src_bytes": src_bytes}
     emit(row, t, nbytes, "remap", check)
 
-    os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-    with open(a.out, "a") as f:
-        for r in lines:
-            f.write(json.dumps(r) + "\n")
+    append_lines(a.out, lines)
 
 
 if __name__ == "__main__":

@@ -11,7 +11,7 @@ preprocess call per region.  Appends one JSON line per workload and output type 
 The W2 / W3 comparison arm is one kb200_preprocess_* call per region with a zoom descriptor over the whole frame (the only
 way to crop a YUV frame without this entry).  Its taps clamp at the frame's edges, not the region's, so its outputs differ
 at region borders: it is for timing only.  Three regions of each W2 / W3 output are checked in the same run against the
-crop reference of tests/test_preprocess_roi.py (the oracle on the w x h crop of the decoded frame).
+crop reference restate.region_reference (the oracle on the w x h crop of the decoded frame).
 
 W1 has a third arm: the batch entry called once per 80 frames (80, 80, 80, 16), the launches the region entry makes for 256
 regions, which tells the cost of that split from the rest of the gap.
@@ -25,24 +25,13 @@ import argparse
 import ctypes as C
 import json
 import os
-import subprocess
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-HBM = 3.35e12
-OUT_CODES = {"f32": 0, "bf16": 2}
+from benchkit import FORMATS, OUT_CODES, PEAK_GBS, ROOT, append_lines, gpu_facts, preprocess_desc, stream, time_alternating
+
 DTYPES = {"f32": torch.float32, "bf16": torch.bfloat16}
-
-
-def gpu_facts():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
-    name, power, clock = [v.strip() for v in q.stdout.strip().splitlines()[0].split(",")]
-    return {"gpu": name, "power_limit": power, "max_sm_clock": clock}
 
 
 def taps_1d(n_out, scale, pad, n, origin):
@@ -80,7 +69,7 @@ def main():
     ap.add_argument("--repeats", type=int, default=3)
     a = ap.parse_args()
     import kornia_rs_b200 as kb
-    from kornia_rs_b200._lib import PreprocessDesc, Roi
+    from kornia_rs_b200._lib import Roi
     from oracle.oracle import preprocess_affine
     from harness import compare_region
     from restate import Case, RCase, picture, region_reference
@@ -88,37 +77,10 @@ def main():
     assert torch.cuda.is_available(), "the benchmark needs a GPU"
     lib = kb._lib.lib()
     dev = torch.device("cuda:0")
-    facts = gpu_facts()
-    inv = tuple(float(np.float32(1) / np.float32(s)) for s in kb.IMAGENET_STD)
-
-    def desc(w, h, dw, dh, affine=(1.0, 1.0, 0.0, 0.0)):
-        d = PreprocessDesc()
-        d.scale_x, d.scale_y, d.pad_x, d.pad_y = affine
-        d.src_w, d.src_h, d.src_pitch, d.src_bpp, d.fmt = w, h, w, 1, 3
-        d.dst_w, d.dst_h = dw, dh
-        d.mean, d.inv_std = (C.c_float * 3)(*kb.IMAGENET_MEAN), (C.c_float * 3)(*inv)
-        d.pad_value, d.sampling = 114.0, 1
-        return d
-
-    def time_arms(arms):
-        """{name: fn}: alternate, `iters` calls each, `repeats` times; ms per call, min and max over repeats."""
-        for fn in arms.values():
-            fn(); fn()
-        torch.cuda.synchronize()
-        res = {k: [] for k in arms}
-        for _ in range(a.repeats):
-            for k, fn in arms.items():
-                s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                s.record()
-                for _ in range(a.iters):
-                    fn()
-                e.record()
-                torch.cuda.synchronize()
-                res[k].append(s.elapsed_time(e) / a.iters)
-        return {k: (min(v), max(v)) for k, v in res.items()}
+    facts = dict(zip(("gpu", "power_limit", "max_sm_clock"), gpu_facts().values()))
 
     def roi_call(d, mode, ptrs, lens, rois, dst, out):
-        st = lib.kb200_preprocess_rois(torch.cuda.current_stream().cuda_stream, C.byref(d), mode, ptrs, lens, len(lens), rois, len(rois),
+        st = lib.kb200_preprocess_rois(stream(), C.byref(d), mode, ptrs, lens, len(lens), rois, len(rois),
                                        dst.data_ptr(), dst.numel(), OUT_CODES[out])
         assert st == 0, kb._lib.last_error()
         return lib.kb200_last_kernel().decode()
@@ -151,7 +113,7 @@ def main():
         lens = (C.c_size_t * n)(*[need] * n)
         flat = [r for rs in per for r in rs]
         rois = (Roi * len(flat))(*[Roi(*r) for r in flat])
-        d = desc(w, h, dw, dh)
+        d = preprocess_desc(*FORMATS["NV12"], w, h, dw, dh)
         m = len(flat)
         for out in ("f32", "bf16"):
             dst = torch.empty((m, 3, dh, dw), dtype=DTYPES[out], device=dev)
@@ -159,21 +121,21 @@ def main():
             kern = roi_call(d, mode, ptrs, lens, rois, dst, out)
             entry = getattr(lib, f"kb200_preprocess_strided_{out}")
             if wl == "W1":
-                dfull = desc(w, h, dw, dh, preprocess_affine(mode, w, h, dw, dh))
+                dfull = preprocess_desc(*FORMATS["NV12"], w, h, dw, dh, preprocess_affine(mode, w, h, dw, dh))
 
                 def other():
-                    assert entry(torch.cuda.current_stream().cuda_stream, C.byref(dfull), base.data_ptr(), base.numel(), need, n, ref.data_ptr(),
+                    assert entry(stream(), C.byref(dfull), base.data_ptr(), base.numel(), need, n, ref.data_ptr(),
                                  ref.numel()) == 0
             else:
                 # one call per region: a zoom descriptor on the whole frame (taps clamp at the frame's edges)
                 calls = []
                 for i, (k, x, y, rw, rh) in enumerate(flat):
                     sx, sy, px, py = preprocess_affine(mode, rw, rh, dw, dh)
-                    dz = desc(w, h, dw, dh, (sx, sy, px - x * sx, py - y * sy))
+                    dz = preprocess_desc(*FORMATS["NV12"], w, h, dw, dh, (sx, sy, px - x * sx, py - y * sy))
                     calls.append((dz, frames[k].data_ptr(), ref[i].data_ptr()))
 
                 def other():
-                    s = torch.cuda.current_stream().cuda_stream
+                    s = stream()
                     for dz, fp, op in calls:
                         entry(s, C.byref(dz), fp, need, need, 1, op, 3 * dw * dh)
             other()
@@ -197,13 +159,13 @@ def main():
             arms = {"rois": lambda: roi_call(d, mode, ptrs, lens, rois, dst, out), "existing": other}
             if wl == "W1":   # the batch entry in the region entry's launches: 80 frames per call
                 def split():
-                    st = torch.cuda.current_stream().cuda_stream
+                    st = stream()
                     for f0 in range(0, n, 80):
                         nb = min(80, n - f0)
                         assert entry(st, C.byref(dfull), base.data_ptr() + f0 * need, nb * need, need, nb,
                                      ref.data_ptr() + f0 * 3 * dw * dh * ref.element_size(), nb * 3 * dw * dh) == 0
                 arms["existing_80_per_launch"] = split
-            t = time_arms(arms)
+            t = time_alternating(arms, a.iters, a.repeats)
             esz = dst.element_size()
             nbytes = src_bytes_tapped(w, h, per, dw, dh, mode, preprocess_affine) + dst.numel() * esz
             row = {"workload": wl, "out": out, "frames": n, "regions": m, "src": f"NV12 {w}x{h}", "dst": [3, dh, dw], "mode": ["Letterbox", "Stretch"][mode],
@@ -211,16 +173,14 @@ def main():
                    "rois_ms_min": round(t["rois"][0], 4), "rois_ms_max": round(t["rois"][1], 4),
                    "existing_arm": "kb200_preprocess_strided (one call)" if wl == "W1" else f"{m} x kb200_preprocess_strided (zoom descriptor, timing only)",
                    "existing_ms_min": round(t["existing"][0], 4), "existing_ms_max": round(t["existing"][1], 4),
-                   "algorithmic_bytes": nbytes, "rois_share_of_3.35TBps": round(nbytes / (t["rois"][0] * 1e-3) / HBM, 3),
-                   "existing_share_of_3.35TBps": round(nbytes / (t["existing"][0] * 1e-3) / HBM, 3),
+                   "algorithmic_bytes": nbytes, "rois_share_of_3.35TBps": round(nbytes / (t["rois"][0] * 1e-3) / (PEAK_GBS * 1e9), 3),
+                   "existing_share_of_3.35TBps": round(nbytes / (t["existing"][0] * 1e-3) / (PEAK_GBS * 1e9), 3),
                    **({"existing_80_per_launch_ms_min": round(t["existing_80_per_launch"][0], 4),
                        "existing_80_per_launch_ms_max": round(t["existing_80_per_launch"][1], 4)} if wl == "W1" else {}),
                    "iters": a.iters, "repeats": a.repeats, **check, **facts}
             print(json.dumps(row), flush=True)
             lines.append(row)
-    with open(a.out, "a") as f:
-        for r in lines:
-            f.write(json.dumps(r) + "\n")
+    append_lines(a.out, lines)
 
 
 if __name__ == "__main__":

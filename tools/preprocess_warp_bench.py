@@ -13,7 +13,7 @@ whole frames.  Appends one JSON line per workload, source format and output type
   W4  identity: 256 NV12 1080p frames through identity maps to 1920 x 1080, f32, against the batch entry
       (kb200_preprocess_strided_f32 at scale 1, its identity kernel) in the same run: the outputs must be identical.
 
-W1-W3 check three regions of each `warps` output in the same run against tests/test_preprocess_warp.warp_reference.
+W1-W3 check three regions of each `warps` output in the same run against restate.warp_reference.
 Arms alternate: 20 launches after warm-up, 3 repeats, minima given with the repeat spread.  Algorithmic bytes: the distinct
 source bytes the sampler taps in each frame over the union of its regions plus the output bytes.  The taps come from the
 same float32 coordinate rule as the reference (warp_coords): for each inside pixel the tap (x0, y0), and x0 + 1 / y0 + 1
@@ -24,26 +24,16 @@ import argparse
 import ctypes as C
 import json
 import os
-import sys
 import zlib
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-from preprocess_roi_bench import HBM, gpu_facts  # noqa: E402
+from benchkit import (FORMATS, OUT_CODES, PEAK_GBS, ROOT, append_lines, frame_len, gpu_facts, mask_bytes, preprocess_desc, stream,
+                      tap_mask, time_alternating)
 
 F32 = np.float32
-OUT_CODES = {"f32": 0, "bf16": 2}
 DTYPES = {"f32": torch.float32, "bf16": torch.bfloat16}
-FMT = {"NV12": (3, 1), "P010": (80, 2), "RGGB": (16, 1)}   # format code, bytes per sample
-
-
-def frame_len(fmt, w, h):
-    return w * h * 3 // 2 * FMT[fmt][1] if fmt != "RGGB" else w * h
 
 
 def tapped_bytes(fmt, w, h, regions, inverse, dw, dh):
@@ -55,29 +45,8 @@ def tapped_bytes(fmt, w, h, regions, inverse, dw, dh):
         sx, sy, inside, _ = warp_coords(inv, persp, dw, dh, w, h)
         sx = np.minimum(np.maximum(sx[inside], F32(0)), np.nextafter(F32(w), F32(0)))
         sy = np.minimum(np.maximum(sy[inside], F32(0)), np.nextafter(F32(h), F32(0)))
-        x0, y0 = np.floor(sx).astype(np.int64), np.floor(sy).astype(np.int64)
-        nx, ny = sx != x0, sy != y0
-        x1, y1 = np.minimum(x0 + 1, w - 1), np.minimum(y0 + 1, h - 1)
-        m = per_frame.setdefault(k, np.zeros((h, w), bool))
-        m[y0, x0] = True
-        m[y0[nx], x1[nx]] = True
-        m[y1[ny], x0[ny]] = True
-        m[y1[nx & ny], x1[nx & ny]] = True
-    total = 0
-    for m in per_frame.values():
-        if fmt == "RGGB":   # the 3 x 3 demosaic neighbourhood of every tap
-            p = np.pad(m, 1)
-            m = np.zeros_like(m)
-            for dy in range(3):
-                for dx in range(3):
-                    m |= p[dy:dy + h, dx:dx + w]
-            total += int(m.sum())
-            continue
-        ys, xs = np.nonzero(m)
-        chroma = np.zeros((h // 2, w // 2), bool)
-        chroma[ys >> 1, xs >> 1] = True
-        total += (int(m.sum()) + 2 * int(chroma.sum())) * FMT[fmt][1]
-    return total
+        tap_mask(sx, sy, w, h, per_frame.setdefault(k, np.zeros((h, w), bool)))
+    return sum(mask_bytes(fmt, m) for m in per_frame.values())
 
 
 def main():
@@ -87,49 +56,17 @@ def main():
     ap.add_argument("--repeats", type=int, default=3)
     a = ap.parse_args()
     import kornia_rs_b200 as kb
-    from kornia_rs_b200._lib import PreprocessDesc, Roi, WarpRoi
+    from kornia_rs_b200._lib import Roi, WarpRoi
     from harness import compare_region, inverse
     from restate import Case, RCase, forward_of, picture, warp_reference
 
     assert torch.cuda.is_available(), "the benchmark needs a GPU"
     lib = kb._lib.lib()
     dev = torch.device("cuda:0")
-    facts = gpu_facts()
-    inv_std = tuple(float(F32(1) / F32(s)) for s in kb.IMAGENET_STD)
-
-    def desc(fmt, w, h, dw, dh, code=None, bpp=1, pitch=None):
-        d = PreprocessDesc()
-        d.scale_x, d.scale_y, d.pad_x, d.pad_y = 1.0, 1.0, 0.0, 0.0
-        d.src_w, d.src_h, d.src_bpp = w, h, bpp
-        d.src_pitch = pitch if pitch is not None else w * FMT[fmt][1]
-        d.fmt = FMT[fmt][0] if code is None else code
-        d.dst_w, d.dst_h = dw, dh
-        d.mean, d.inv_std = (C.c_float * 3)(*kb.IMAGENET_MEAN), (C.c_float * 3)(*inv_std)
-        d.pad_value, d.sampling = 114.0, 1
-        return d
-
-    def time_arms(arms):
-        """{name: fn}: alternate, `iters` calls each, `repeats` times; ms per call, min and max over repeats."""
-        for fn in arms.values():
-            fn(); fn()
-        torch.cuda.synchronize()
-        res = {k: [] for k in arms}
-        for _ in range(a.repeats):
-            for k, fn in arms.items():
-                s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                s.record()
-                for _ in range(a.iters):
-                    fn()
-                e.record()
-                torch.cuda.synchronize()
-                res[k].append(s.elapsed_time(e) / a.iters)
-        return {k: (min(v), max(v)) for k, v in res.items()}
+    facts = dict(zip(("gpu", "power_limit", "max_sm_clock"), gpu_facts().values()))
 
     def lib_inverse(fwd):
         return inverse(lib, fwd)
-
-    def stream():
-        return torch.cuda.current_stream().cuda_stream
 
     lines = []
 
@@ -199,7 +136,7 @@ def main():
         ptrs = (C.c_void_p * n)(*[f.data_ptr() for f in frames])
         lens = (C.c_size_t * n)(*[need] * n)
         warps = (WarpRoi * m)(*[WarpRoi(k, (C.c_float * 9)(*f)) for k, f in regs])
-        d = desc(fmt, w, h, dw, dh)
+        d = preprocess_desc(*FORMATS[fmt], w, h, dw, dh)
         dst = torch.empty((m, 3, dh, dw), dtype=DTYPES[out], device=dev)
 
         def run_warps():
@@ -226,7 +163,7 @@ def main():
         else:
             torch.cuda.synchronize()
             host = base.cpu().numpy()
-            c = Case(wl, 0, FMT[fmt][0], 0, 1, w, h, w * FMT[fmt][1], "warp", 1.0, 1.0, 0.0, 0.0, dw, dh, 1, False, "table", n, (), None, 0,
+            c = Case(wl, 0, FORMATS[fmt][0], 0, 1, w, h, w * FORMATS[fmt][1], "warp", 1.0, 1.0, 0.0, 0.0, dw, dh, 1, False, "table", n, (), None, 0,
                      "imagenet", 114.0)
             rc = RCase(c, 1, out, n, (), ())
             picked = [0, m // 2, m - 1]
@@ -251,7 +188,7 @@ def main():
                 rgb = torch.empty((n, h, w, 3), dtype=torch.uint8, device=dev)
                 crops = torch.empty((m, dh, dw, 3), dtype=torch.uint8, device=dev)
                 ms = [(C.c_float * 6)(*f[:6]) for _, f in regs]
-                dn = desc(fmt, dw, dh, dw, dh, code=0, bpp=3, pitch=3 * dw)
+                dn = preprocess_desc(0, 3, dw, dh, dw, dh, bpp=3)   # RGB8
                 entry = getattr(lib, f"kb200_preprocess_strided_{out}")
                 edst = torch.empty_like(dst)
 
@@ -267,23 +204,21 @@ def main():
                     assert entry(s, C.byref(dn), crops.data_ptr(), crops.numel(), cb, m, edst.data_ptr(), edst.numel()) == 0
 
                 arms["existing"] = existing
-        t = time_arms(arms)
+        t = time_alternating(arms, a.iters, a.repeats)
         nbytes = src_bytes + dst.numel() * dst.element_size()
         row = {"workload": wl, "src": f"{fmt} {w}x{h}", "out": out, "frames": n, "regions": m, "dst": [3, dh, dw], "sampling": "Bilinear",
                "kernel": kern, "launches": -(-m // 72), "tapped_src_bytes": src_bytes, "algorithmic_bytes": nbytes}
         for k, (lo, hi) in t.items():
             row[f"{k}_ms_min"], row[f"{k}_ms_max"] = round(lo, 4), round(hi, 4)
-        row["warps_share_of_3.35TBps"] = round(nbytes / (t["warps"][0] * 1e-3) / HBM, 3)
+        row["warps_share_of_3.35TBps"] = round(nbytes / (t["warps"][0] * 1e-3) / (PEAK_GBS * 1e9), 3)
         if "batch_entry" in t:
-            row["batch_entry_share_of_3.35TBps"] = round(nbytes / (t["batch_entry"][0] * 1e-3) / HBM, 3)
+            row["batch_entry_share_of_3.35TBps"] = round(nbytes / (t["batch_entry"][0] * 1e-3) / (PEAK_GBS * 1e9), 3)
         row.update(iters=a.iters, repeats=a.repeats, **check, **facts)
         print(json.dumps(row), flush=True)
         lines.append(row)
         del dst
         torch.cuda.empty_cache()
-    with open(a.out, "a") as f:
-        for r in lines:
-            f.write(json.dumps(r) + "\n")
+    append_lines(a.out, lines)
 
 
 if __name__ == "__main__":

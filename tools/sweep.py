@@ -9,31 +9,23 @@ import json
 import os
 import sys
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from benchkit import PEAK_GBS, ROOT, bench_module
 import torch
 
 import kornia_rs_b200 as kb
 
-PEAK = 6580.3
+PEAK = PEAK_GBS
 try:
-    PEAK = float(json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")))["hbm_gbs"])
+    PEAK = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
 except Exception:
     pass
 dev = torch.device("cuda:0")
 st = torch.cuda.current_stream(dev)
+time_launches = bench_module().time_launches
 
 
-def timeit(fn, it=10, wu=3):
-    for _ in range(wu):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record(st)
-    for _ in range(it):
-        fn()
-    e1.record(st)
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / it
+def timeit(fn):
+    return time_launches(fn, 10, 3, st)
 
 
 def setk(**kw):

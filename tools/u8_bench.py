@@ -1,17 +1,9 @@
 """u8 twins quick timing (GPU box): python tools/u8_bench.py — word-granular sampler on/off (knob b=1 disables)."""
-import os, sys
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from benchkit import PEAK_GBS, bench_module
 import torch
 import kornia_rs_b200 as kb
 dev = torch.device("cuda:0"); st = torch.cuda.current_stream(dev)
-def timeit(fn, it=10, wu=3):
-    for _ in range(wu): fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record(st)
-    for _ in range(it): fn()
-    e1.record(st); torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / it
+time_launches = bench_module().time_launches
 w, h, n = 3840, 2160, 16
 g = torch.Generator(device=dev).manual_seed(1)
 s8 = kb.Image(torch.randint(0, 256, (n, h, w, 3), dtype=torch.uint8, device=dev, generator=g))
@@ -26,5 +18,5 @@ ops = {"warp_perspective_u8": lambda: kb.imgproc.warp_perspective_u8(s8, d8, H),
 for b in (1, 0):
     kb._lib.set_knob("b", b)
     for name, fn in ops.items():
-        ms = timeit(fn)
-        print(f"words={'off' if b else 'on '} {name:24s} {ms:.4f} ms  {n*w*h/ms/1e6:.0f} Gpix/s  frac {n*w*h*6/ms/1e6/6580.3:.3f}", flush=True)
+        ms = time_launches(fn, 10, 3, st)
+        print(f"words={'off' if b else 'on '} {name:24s} {ms:.4f} ms  {n*w*h/ms/1e6:.0f} Gpix/s  frac {n*w*h*6/ms/1e6/PEAK_GBS:.3f}", flush=True)

@@ -19,8 +19,8 @@ Every arm is timed with CUDA events over --iters launches after warm-up, the arm
 frame (I444 3 B/px, I41x 6 B/px, NV12 1.5 B/px, P010 3 B/px; for 3b the distinct bytes the sampler taps, counted by the
 oracle on the RGB8 twin for 4:4:4 and on the NV12 frame for 4:2:0, doubled for 16-bit words) plus the output (3 / 6 B/px
 RGB for the decodes, 12 / 6 B/px for f32 / f16 CHW).  Afterwards every arm runs once more and its output is checked bit
-for bit: the 4:4:4 arms against their 4:2:0 sibling on every frame (the twin identity), NV12 and P010 against the
-restatements of tests/test_yuv_matrix.py and tests/test_yuv16.py and the oracle, the generic 3b arm against the fast one,
+for bit: the 4:4:4 arms against their 4:2:0 sibling on every frame (the twin identity), NV12 and P010 against
+restate.decode_yuv8, restate.decode_yuv16 and the oracle, the generic 3b arm against the fast one,
 and end to end against the device run.
 
 Writes one JSON line to DIR/yuv444_bench.jsonl (and stdout), with the card's name, power limit and max SM clock read in
@@ -28,20 +28,10 @@ the same run.
 """
 from __future__ import annotations
 
-import argparse
-import json
-import os
 import sys
 import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-
-from bayer_bench import row  # noqa: E402
-from half_bench import PEAK_GBS, _bench_module, gpu_facts  # noqa: E402
-from yuv_bench import time_arms  # noqa: E402
+from benchkit import PEAK_GBS, arg_parser, e2e_result, parse_args, row, start, time_arms, write_line
 
 ARMS = ("I444", "I410", "I410Msb", "Nv12", "P010")
 SIBLING = {"I444": "Nv12", "I410": "P010", "I410Msb": "P010"}   # the 4:2:0 arm each 4:4:4 arm must equal bit for bit
@@ -50,16 +40,10 @@ MATRIX = "Bt709Limited"
 
 
 def main():
-    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
-    ap.add_argument("--out", required=True, help="directory for yuv444_bench.jsonl")
-    ap.add_argument("--iters", type=int, default=20)
-    ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--reps", type=int, default=3)
+    ap = arg_parser(__doc__, "yuv444_bench")
     ap.add_argument("--e2e-frames", type=int, default=64)
     ap.add_argument("--e2e-steps", type=int, default=5)
-    args = ap.parse_args()
-    if args.iters < 20 or args.reps < 3:
-        ap.error("--iters >= 20 and --reps >= 3: fewer cannot show the spread")
+    args = parse_args(ap)
 
     import numpy as np
     import torch
@@ -69,10 +53,7 @@ def main():
     from harness import restated, yuv16_identity
     from restate import decode_yuv16, decode_yuv8
 
-    if not torch.cuda.is_available():
-        raise SystemExit("yuv444_bench.py needs a CUDA device")
-    bench = _bench_module()
-    facts = gpu_facts()
+    bench, facts = start("yuv444_bench")
     dev = torch.device("cuda:0")
     st = torch.cuda.current_stream(dev)
     gen = torch.Generator(device=dev).manual_seed(0x444)
@@ -107,7 +88,7 @@ def main():
         for k, sib in SIBLING.items():
             same[k] = bool(torch.equal(outs[k].data, outs[sib].data))
         alg = {k: int(n * w * h * (src_bpp[k] + (6 if k in WORDS else 3))) for k in ARMS}
-        decode[tag] = {"batch": n, "src": [w, h], **row(times, kernels, alg, same)}
+        decode[tag] = {"batch": n, "src": [w, h], **row(times, kernels, alg, same, "output_checked")}
         print(f"[yuv444_bench] decode {tag}: " + "  ".join(f"{k} {min(times[k]):.4f}" for k in times), file=sys.stderr, flush=True)
         del src, outs
         torch.cuda.empty_cache()
@@ -168,7 +149,7 @@ def main():
             alg = {k: n * (src_b[k] + out_b * dw * dh) for k in arms}
             key = f"{cfg}_{'f16' if f16 else 'f32'}"
             preprocess[key] = {"batch": n, "src": [w, h], "dst": [dw, dh], "i444_src_bytes_per_frame": rgb_bytes, "nv12_src_bytes_per_frame": nv12_bytes,
-                               **row(times, kernels, alg, same)}
+                               **row(times, kernels, alg, same, "output_checked")}
             print(f"[yuv444_bench] {key}: " + "  ".join(f"{k} {min(times[k]):.4f}" for k in times), file=sys.stderr, flush=True)
             del out, off, flat
             torch.cuda.empty_cache()
@@ -189,30 +170,16 @@ def main():
     frame_bytes = {k: host[k].shape[1] * host[k].element_size() for k in ARMS}
     pipes = {k: kb.imgproc.HostPipeline(dev, src_chunk_bytes=chunk * ((frame_bytes[k] + 15) // 16 * 16), dst_chunk_bytes=chunk * 12 * w * h,
                                         depth=nstreams) for k in ARMS}
-    steps = {k: [] for k in ARMS}
-    for _ in range(args.reps):
-        for k in ARMS:
-            fn = lambda k=k: pres[k].run_raw_host(host[k], w, h, (w, h), out=outs[k], pipeline=pipes[k])
-            fn()
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record(st)
-            for _ in range(args.e2e_steps):
-                fn()
-            e1.record(st)
-            torch.cuda.synchronize()
-            steps[k].append(e0.elapsed_time(e1) / args.e2e_steps)
+    fns = {k: (lambda k=k: pres[k].run_raw_host(host[k], w, h, (w, h), out=outs[k], pipeline=pipes[k])) for k in ARMS}
+    steps, _ = time_arms(bench, fns, args.e2e_steps, 1, args.reps, st, kb)
     e2e = {}
     for k in ARMS:
-        up, down = pipes[k].last_transfer()
+        transfer = pipes[k].last_transfer()
         pipes[k].close()
         want = torch.empty((n, 3, h, w), dtype=torch.float32, device=dev)
         dev_frames = host[k].to(dev)
         pres[k].run_raw_batch([dev_frames[i] for i in range(n)], w, h, want)
-        best = min(steps[k])
-        e2e[k] = {"ms_per_step": [round(t, 3) for t in steps[k]], "ms_min": round(best, 3), "h2d_bytes": up, "d2h_bytes": down,
-                  "h2d_gbs": round(up / (best * 1e-3) / 1e9, 1), "d2h_gbs": round(down / (best * 1e-3) / 1e9, 1),
-                  "matches_device_result": bool(torch.equal(outs[k].to(dev).view(torch.int32), want.view(torch.int32)))}
+        e2e[k] = e2e_result(steps[k], transfer, bool(torch.equal(outs[k].to(dev).view(torch.int32), want.view(torch.int32))))
         print(f"[yuv444_bench] e2e cfg3a {k}: {e2e[k]['ms_per_step']} ms/step", file=sys.stderr, flush=True)
         del want, dev_frames
         torch.cuda.empty_cache()
@@ -220,10 +187,7 @@ def main():
     line = {"tool": "tools/yuv444_bench.py", "gpu": facts, "date": time.strftime("%Y-%m-%d"), "iters": args.iters, "warmup": args.warmup,
             "reps": args.reps, "matrix": MATRIX, "peak_gbs": PEAK_GBS, "peak_source": "H100 SXM data sheet, 3.35 TB/s", "decode": decode,
             "preprocess": preprocess, "e2e_cfg3a": {"batch": n, "chunk_frames": chunk, "streams": nstreams, "steps_per_rep": args.e2e_steps, **e2e}}
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "yuv444_bench.jsonl"), "a") as f:
-        f.write(json.dumps(line) + "\n")
-    print(json.dumps(line))
+    write_line(args.out, "yuv444_bench", line)
 
 
 if __name__ == "__main__":

@@ -17,17 +17,10 @@ same run.
 """
 from __future__ import annotations
 
-import argparse
-import json
-import os
 import sys
 import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-from half_bench import PEAK_GBS, _bench_module, gpu_facts  # noqa: E402
+from benchkit import PEAK_GBS, arg_parser, parse_args, row, start, time_arms, write_line
 
 FAMILIES = {"yuv420": ("Nv12", ("Nv21", "I420", "Yv12")), "yuv422": ("Yuyv", ("Uyvy", "Yvyu"))}
 
@@ -47,35 +40,8 @@ def from_sibling(t, w, h, layout):
     return torch.cat([y, u, v] if layout == "I420" else [y, v, u], 1).contiguous()
 
 
-def time_arms(bench, fns, iters, warmup, reps, stream, kb):
-    times = {k: [] for k in fns}
-    kernels = {}
-    for _ in range(reps):
-        for k, fn in fns.items():
-            times[k].append(bench.time_launches(fn, iters, warmup, stream))
-            kernels[k] = kb._lib.last_kernel()
-    return times, kernels
-
-
-def row_for(times, kernels, alg_bytes, same):
-    row = {}
-    for k in times:
-        best = min(times[k])
-        gbs = alg_bytes[k] / (best * 1e-3) / 1e9
-        row[k] = {"ms": [round(t, 4) for t in times[k]], "ms_min": round(best, 4), "alg_bytes": alg_bytes[k], "gbs": round(gbs, 1),
-                  "frac_of_3350": round(gbs / PEAK_GBS, 3), "kernel": kernels[k], "bit_identical_to_sibling": same[k]}
-    return row
-
-
 def main():
-    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
-    ap.add_argument("--out", required=True, help="directory for yuv_bench.jsonl")
-    ap.add_argument("--iters", type=int, default=20)
-    ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--reps", type=int, default=3)
-    args = ap.parse_args()
-    if args.iters < 20 or args.reps < 3:
-        ap.error("--iters >= 20 and --reps >= 3: fewer cannot show the spread")
+    args = parse_args(arg_parser(__doc__, "yuv_bench"))
 
     import numpy as np
     import torch
@@ -83,10 +49,7 @@ def main():
     import kornia_rs_b200 as kb
     from oracle import oracle as o
 
-    if not torch.cuda.is_available():
-        raise SystemExit("yuv_bench.py needs a CUDA device")
-    bench = _bench_module()
-    facts = gpu_facts()
+    bench, facts = start("yuv_bench")
     dev = torch.device("cuda:0")
     st = torch.cuda.current_stream(dev)
     gen = torch.Generator(device=dev).manual_seed(0x7E11)
@@ -102,7 +65,8 @@ def main():
             fns = {k: (lambda k=k: getattr(kb.imgproc, f"rgb_from_{k.lower()}")(srcs[k], outs[k])) for k in srcs}
             times, kernels = time_arms(bench, fns, args.iters, args.warmup, args.reps, st, kb)
             same = {k: bool(torch.equal(outs[k].data, outs[sib].data)) for k in srcs}
-            decode[f"{fam}_{tag}"] = {"batch": n, "src": [w, h], **row_for(times, kernels, {k: n * (fb + 3 * w * h) for k in srcs}, same)}
+            decode[f"{fam}_{tag}"] = {"batch": n, "src": [w, h],
+                                      **row(times, kernels, {k: n * (fb + 3 * w * h) for k in srcs}, same, "bit_identical_to_sibling")}
             print(f"[yuv_bench] decode {fam} {tag}: " + "  ".join(f"{k} {min(times[k]):.4f}" for k in times), file=sys.stderr, flush=True)
             del base, srcs, outs
             torch.cuda.empty_cache()
@@ -136,7 +100,8 @@ def main():
                 pres[k].run_raw_batch(frames[k], w, h, dst)
                 same[k] = bool(torch.equal(dst.view(torch.int32), want.view(torch.int32)))
             preprocess[f"{cfg}_{fam}"] = {"batch": n, "src": [w, h], "dst": [dw, dh], "src_bytes_per_frame": src_bytes,
-                                          **row_for(times, kernels, {k: n * (src_bytes + 12 * dw * dh) for k in srcs}, same)}
+                                          **row(times, kernels, {k: n * (src_bytes + 12 * dw * dh) for k in srcs}, same,
+                                                "bit_identical_to_sibling")}
             print(f"[yuv_bench] {cfg} {fam}: " + "  ".join(f"{k} {min(times[k]):.4f}" for k in times), file=sys.stderr, flush=True)
             del dst, want, frames
             torch.cuda.empty_cache()
@@ -144,10 +109,7 @@ def main():
 
     line = {"tool": "tools/yuv_bench.py", "gpu": facts, "date": time.strftime("%Y-%m-%d"), "iters": args.iters, "warmup": args.warmup,
             "reps": args.reps, "peak_gbs": PEAK_GBS, "peak_source": "H100 SXM data sheet, 3.35 TB/s", "decode": decode, "preprocess": preprocess}
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "yuv_bench.jsonl"), "a") as f:
-        f.write(json.dumps(line) + "\n")
-    print(json.dumps(line))
+    write_line(args.out, "yuv_bench", line)
 
 
 if __name__ == "__main__":

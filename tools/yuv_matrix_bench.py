@@ -17,19 +17,10 @@ in the same run.
 """
 from __future__ import annotations
 
-import argparse
-import json
-import os
 import sys
 import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-
-from half_bench import PEAK_GBS, _bench_module, gpu_facts  # noqa: E402
-from yuv_bench import time_arms  # noqa: E402
+from benchkit import PEAK_GBS, arg_parser, parse_args, start, time_arms, write_line
 
 MATRICES = ("Bt601Limited", "Bt601Full", "Bt709Limited", "Bt709Full")
 
@@ -45,14 +36,7 @@ def row_for(times, kernels, alg_bytes, ok):
 
 
 def main():
-    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
-    ap.add_argument("--out", required=True, help="directory for yuv_matrix_bench.jsonl")
-    ap.add_argument("--iters", type=int, default=20)
-    ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--reps", type=int, default=3)
-    args = ap.parse_args()
-    if args.iters < 20 or args.reps < 3:
-        ap.error("--iters >= 20 and --reps >= 3: fewer cannot show the spread")
+    args = parse_args(arg_parser(__doc__, "yuv_matrix_bench"))
 
     import torch
 
@@ -62,10 +46,7 @@ def main():
     from oracle import oracle as o
     from restate import decode_yuv8
 
-    if not torch.cuda.is_available():
-        raise SystemExit("yuv_matrix_bench.py needs a CUDA device")
-    bench = _bench_module()
-    facts = gpu_facts()
+    bench, facts = start("yuv_matrix_bench")
     dev = torch.device("cuda:0")
     st = torch.cuda.current_stream(dev)
     gen = torch.Generator(device=dev).manual_seed(0x709)
@@ -130,10 +111,7 @@ def main():
     line = {"tool": "tools/yuv_matrix_bench.py", "gpu": facts, "date": time.strftime("%Y-%m-%d"), "iters": args.iters, "warmup": args.warmup,
             "reps": args.reps, "peak_gbs": PEAK_GBS, "peak_source": "H100 SXM data sheet, 3.35 TB/s", "decode": decode_rows,
             "preprocess": preprocess}
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "yuv_matrix_bench.jsonl"), "a") as f:
-        f.write(json.dumps(line) + "\n")
-    print(json.dumps(line))
+    write_line(args.out, "yuv_matrix_bench", line)
 
 
 if __name__ == "__main__":
