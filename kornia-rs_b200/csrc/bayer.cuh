@@ -1,6 +1,6 @@
 // bayer.cuh — bilinear demosaic of Bayer mosaics, 8-bit, 16-bit or MIPI-packed 10/12/14-bit samples, shared by the
 // standalone decoders (color.cu: rgb_from_bayer_vec<T, P>, rgb_from_bayer_generic<T, P>) and the camera preprocess
-// (preprocess.cu: preprocess_bayer_identity_kernel<F16, PTRS, T, P> and the Bayer taps of the generic kernel).  Everything
+// (preprocess.cu: preprocess_bayer_identity_kernel<OUT, T, P> and the Bayer taps of the generic kernel).  Everything
 // here is generic over the sample type T; BayerSample<T> holds the few facts of T the kernels above it need.  Packed
 // samples (T = BayerPacked<BITS>) only change the loads: they are unpacked into the words of the 16-bit kernels
 // (bayer_unpack, bayer_load_rows_packed, bayer_px_packed), and everything after that is the uint16_t path.

@@ -33,8 +33,9 @@
 
 namespace kb200 {
 
-// One thread per output pixel of frame frame0 + blockIdx.y; SAMP: kb200_interp (generic_pixel).
-template <int OUT, int SAMP, bool PTRS, int TAP>
+// One thread per output pixel of frame frame0 + blockIdx.y; SAMP: kb200_interp (generic_pixel).  STRIDED: the frame is
+// fr.base + (frame0 + f) * fr.stride rather than fr.ptr[f]; only the packed-Bayer tap is instantiated so (launch_preprocess).
+template <int OUT, int SAMP, int TAP, bool STRIDED = false>
 __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                  const __grid_constant__ PreFrames fr, void* __restrict__ dst,
                                                                  uint32_t frame0, const SrcFormat sf, const TapCoeffs<TAP> yc) {
@@ -42,7 +43,7 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= pixels) return;
     const uint32_t f = blockIdx.y;
-    const uint8_t* src = PTRS ? fr.ptr[f] : fr.base + (size_t)(frame0 + f) * fr.stride;
+    const uint8_t* src = STRIDED ? fr.base + (size_t)(frame0 + f) * fr.stride : fr.ptr[f];
     const int ox = i % d.dst_w, oy = i / d.dst_w;
     float o[3];
     generic_pixel<SAMP, TAP>(src, ox, oy, d, sf, yc, FrameGeom{d}, o);
@@ -69,7 +70,7 @@ __global__ void __launch_bounds__(256) preprocess_generic_kernel(const __grid_co
 // 16-bit words (T = uint16_t): LDG.64 of 4 Y words per row; P01x one LDG.64 of the 2 chroma pairs, I01x 2 U words and
 // 2 V words (LDG.32 each; w % 4 == 0 and even h keep them 4-B aligned in an 8-B aligned frame).  A pixel is normalised
 // as (px / W - mean) * inv_std with the IEEE division, like a 16-bit Bayer tap.
-template <int OUT, bool PTRS, int L, typename T>
+template <int OUT, int L, typename T>
 __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                          const __grid_constant__ PreFrames fr, void* __restrict__ dst,
                                                                          uint32_t frame0, uint32_t groups_per_row, uint32_t items,
@@ -79,7 +80,7 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const _
     const uint32_t rp = item / groups_per_row, g = item - rp * groups_per_row;
     const uint32_t w = (uint32_t)d.src_w, h = (uint32_t)d.src_h;
     const uint32_t f = blockIdx.y;
-    const uint8_t* src = PTRS ? fr.ptr[f] : fr.base + (size_t)(frame0 + f) * fr.stride;
+    const uint8_t* src = fr.ptr[f];
     const uint32_t x = g * 4u;
     if constexpr (sizeof(T) == 2) {
         const uint16_t* s = reinterpret_cast<const uint16_t*>(src);
@@ -167,7 +168,7 @@ __global__ void __launch_bounds__(128) preprocess_yuv420_identity_kernel(const _
 // Every pixel has its own chroma, so one thread = 4 columns of one row: one lane-contiguous load from each of the Y, U
 // and V planes (LDG.32 of 4 bytes, LDG.64 of 4 words: w % 4 == 0 and a frame aligned to that load align every plane's
 // rows), 3 x nv12_store4.  Bytes are normalised as in the 4:2:0 kernel (norm_int_px), words by W through div_white.
-template <int OUT, bool PTRS, typename T>
+template <int OUT, typename T>
 __global__ void __launch_bounds__(128) preprocess_yuv444_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                          const __grid_constant__ PreFrames fr, void* __restrict__ dst,
                                                                          uint32_t frame0, uint32_t groups_per_row, uint32_t items,
@@ -177,7 +178,7 @@ __global__ void __launch_bounds__(128) preprocess_yuv444_identity_kernel(const _
     const uint32_t y = item / groups_per_row, g = item - y * groups_per_row;
     const uint32_t w = (uint32_t)d.src_w, h = (uint32_t)d.src_h;
     const uint32_t f = blockIdx.y;
-    const uint8_t* src = PTRS ? fr.ptr[f] : fr.base + (size_t)(frame0 + f) * fr.stride;
+    const uint8_t* src = fr.ptr[f];
     const size_t plane = (size_t)w * h, p = (size_t)y * w + g * 4u;
     const float m0 = d.mean[0], m1 = d.mean[1], m2 = d.mean[2], i0 = d.inv_std[0], i1 = d.inv_std[1], i2 = d.inv_std[2];
     float r4[4], g4[4], b4[4];
@@ -226,7 +227,7 @@ __global__ void __launch_bounds__(128) preprocess_yuv444_identity_kernel(const _
 // Packed samples (T = BayerPacked<BITS>): a thread's 4 columns are BITS / 2 bytes of a row, read as the aligned 8-byte
 // word that holds their first byte and, when they run past it, the next one (L1-allocating: the neighbouring lanes read
 // the same words), then unpacked into the words of the 16-bit kernel (bayer_unpack).  Rows and frames 16-B aligned.
-template <int OUT, bool PTRS, typename T, int P>
+template <int OUT, typename T, int P>
 __global__ void __launch_bounds__(128) preprocess_bayer_identity_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                                         const __grid_constant__ PreFrames fr, void* __restrict__ dst,
                                                                         uint32_t frame0, uint32_t groups_per_row, uint32_t items, uint32_t bits) {
@@ -238,7 +239,7 @@ __global__ void __launch_bounds__(128) preprocess_bayer_identity_kernel(const __
     const uint32_t rp = it / groups_per_row, g = it - rp * groups_per_row;
     const uint32_t w = (uint32_t)d.src_w, h = (uint32_t)d.src_h;
     const uint32_t f = blockIdx.y;
-    const T* src = reinterpret_cast<const T*>(PTRS ? fr.ptr[f] : fr.base + (size_t)(frame0 + f) * fr.stride);
+    const T* src = reinterpret_cast<const T*>(fr.ptr[f]);
     const uint32_t x = g * 4u, ya = 1u + 2u * rp, yb = ya + 1u;
     uint32_t rows[4][NW];
     int hl[4], hr[4];
@@ -314,14 +315,14 @@ __global__ void __launch_bounds__(128) preprocess_bayer_identity_kernel(const __
 //   * a pixel that was not interpolated is an integer 0..255, whose `px / 255.0f` is the 3-instruction exact
 //     form (norm_int_px); interpolated pixels use the IEEE division.
 // The sampler is yuv_resample (preprocess.cuh), here over frame frame0 + blockIdx.z.
-template <int OUT, bool BILINEAR, bool PTRS, int L, typename T>
+template <int OUT, bool BILINEAR, int L, typename T>
 __global__ void __launch_bounds__(128) preprocess_yuv_kernel(const __grid_constant__ kb200_preprocess_desc d,
                                                              const __grid_constant__ PreFrames fr, const __grid_constant__ Nv12Args na,
                                                              void* __restrict__ dst, uint32_t frame0, const typename YuvSample<T>::Coeffs yc) {
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= na.groups) return;
     const uint32_t f = blockIdx.z;
-    const uint8_t* src = PTRS ? fr.ptr[f] : fr.base + (size_t)(frame0 + f) * fr.stride;
+    const uint8_t* src = fr.ptr[f];
     yuv_resample<OUT, BILINEAR, L, T>(FrameGeom{d}, src, d, na, dst, frame0 + f, (int)g * 4, yc);
 }
 
@@ -475,47 +476,38 @@ int check_region_frame(uint32_t i, int32_t frame, uint32_t n_frames) {
 // The fast kernels of layout L (4:2:0, or YUV444) and sample type T, for one launch of <= 256 frames.
 template <int OUT, int L, typename T = uint8_t>
 static void launch_yuv_fast(cudaStream_t s, bool identity, bool bil, const kb200_preprocess_desc& d, const typename YuvSample<T>::Coeffs& yc,
-                            const PreFrames& fr, bool ptrs, const Nv12Args& nv, void* dst, uint32_t f0, uint32_t nb, uint32_t id_groups,
-                            size_t id_items) {
+                            const PreFrames& fr, const Nv12Args& nv, void* dst, uint32_t f0, uint32_t nb, uint32_t id_groups, size_t id_items) {
     if (identity) {
         dim3 grid(div_up(id_items, 128), nb);
-        if constexpr (L == YUV444) {
-            if (ptrs) preprocess_yuv444_identity_kernel<OUT, true, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
-            else preprocess_yuv444_identity_kernel<OUT, false, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
-        } else {
-            if (ptrs) preprocess_yuv420_identity_kernel<OUT, true, L, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
-            else preprocess_yuv420_identity_kernel<OUT, false, L, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
-        }
+        if constexpr (L == YUV444) preprocess_yuv444_identity_kernel<OUT, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
+        else preprocess_yuv420_identity_kernel<OUT, L, T><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, yc);
         return;
     }
     dim3 grid(div_up(nv.groups, 128), div_up((size_t)d.dst_h, NV12_ROWS), nb);
-#define KB200_YUV_LAUNCH(BIL, PT) preprocess_yuv_kernel<OUT, BIL, PT, L, T><<<grid, 128, 0, s>>>(d, fr, nv, dst, f0, yc)
-    if (bil) { if (ptrs) KB200_YUV_LAUNCH(true, true); else KB200_YUV_LAUNCH(true, false); }
-    else     { if (ptrs) KB200_YUV_LAUNCH(false, true); else KB200_YUV_LAUNCH(false, false); }
-#undef KB200_YUV_LAUNCH
+    if (bil) preprocess_yuv_kernel<OUT, true, L, T><<<grid, 128, 0, s>>>(d, fr, nv, dst, f0, yc);
+    else preprocess_yuv_kernel<OUT, false, L, T><<<grid, 128, 0, s>>>(d, fr, nv, dst, f0, yc);
 }
 
 // The Bayer identity kernel of sample type T and pattern P, for one launch of <= 256 frames.
 template <int OUT, typename T, int P>
-static void launch_bayer_identity(cudaStream_t s, const kb200_preprocess_desc& d, const PreFrames& fr, bool ptrs, void* dst, uint32_t f0,
-                                  uint32_t nb, uint32_t id_groups, size_t id_items, uint32_t bits) {
+static void launch_bayer_identity(cudaStream_t s, const kb200_preprocess_desc& d, const PreFrames& fr, void* dst, uint32_t f0, uint32_t nb,
+                                  uint32_t id_groups, size_t id_items, uint32_t bits) {
     dim3 grid(div_up(id_items, 128), nb);
-    if (ptrs) preprocess_bayer_identity_kernel<OUT, true, T, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, bits);
-    else preprocess_bayer_identity_kernel<OUT, false, T, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, bits);
+    preprocess_bayer_identity_kernel<OUT, T, P><<<grid, 128, 0, s>>>(d, fr, dst, f0, id_groups, (uint32_t)id_items, bits);
 }
 
-template <int OUT, bool PTRS, int TAP>
+template <int OUT, int TAP, bool STRIDED = false>
 static void launch_generic(cudaStream_t s, dim3 grid, const kb200_preprocess_desc& d, const SrcFormat& f, const TapCoeffs<TAP>& yc,
                            const PreFrames& fr, void* dst, uint32_t f0) {
-    if (d.sampling == KB200_INTERP_LANCZOS) preprocess_generic_kernel<OUT, KB200_INTERP_LANCZOS, PTRS, TAP><<<grid, 256, 0, s>>>(d, fr, dst, f0, f, yc);
-    else if (d.sampling == KB200_INTERP_BILINEAR) preprocess_generic_kernel<OUT, KB200_INTERP_BILINEAR, PTRS, TAP><<<grid, 256, 0, s>>>(d, fr, dst, f0, f, yc);
-    else preprocess_generic_kernel<OUT, KB200_INTERP_NEAREST, PTRS, TAP><<<grid, 256, 0, s>>>(d, fr, dst, f0, f, yc);
+    if (d.sampling == KB200_INTERP_LANCZOS) preprocess_generic_kernel<OUT, KB200_INTERP_LANCZOS, TAP, STRIDED><<<grid, 256, 0, s>>>(d, fr, dst, f0, f, yc);
+    else if (d.sampling == KB200_INTERP_BILINEAR) preprocess_generic_kernel<OUT, KB200_INTERP_BILINEAR, TAP, STRIDED><<<grid, 256, 0, s>>>(d, fr, dst, f0, f, yc);
+    else preprocess_generic_kernel<OUT, KB200_INTERP_NEAREST, TAP, STRIDED><<<grid, 256, 0, s>>>(d, fr, dst, f0, f, yc);
 }
 
-template <int OUT, bool PTRS>
+template <int OUT>
 static void launch_generic_for(cudaStream_t s, dim3 grid, const kb200_preprocess_desc& d, const SrcFormat& f, const YuvCoeffs& yc,
                                const Yuv16Coeffs& yc16, const PreFrames& fr, void* dst, uint32_t f0) {
-    with_tap(f, yc, yc16, [&](auto tap, const auto& c) { launch_generic<OUT, PTRS, decltype(tap)::value>(s, grid, d, f, c, fr, dst, f0); });
+    with_tap(f, yc, yc16, [&](auto tap, const auto& c) { launch_generic<OUT, decltype(tap)::value>(s, grid, d, f, c, fr, dst, f0); });
 }
 
 // d: a validated descriptor with the plain format code; matrix: its kb200_yuv_matrix
@@ -547,16 +539,15 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, int
         const uint32_t nb = std::min<uint32_t>(256, batch - f0);
         PreFrames fr{};
         fr.base = base; fr.stride = stride;
-        if (frames) for (uint32_t k = 0; k < nb; ++k) fr.ptr[k] = frames[f0 + k];
-        const bool p = frames != nullptr;
+        for (uint32_t k = 0; k < nb; ++k) fr.ptr[k] = frames ? frames[f0 + k] : base + (size_t)(f0 + k) * stride;
         if (identity && bayer) {
             auto launch = [&](auto sample) {   // the kernel of the format's pattern for samples of the type of `sample`
                 using T = decltype(sample);
                 switch (f.pattern) {
-                    case KB200_BAYER_RGGB: launch_bayer_identity<OUT, T, KB200_BAYER_RGGB>(s, d, fr, p, dst, f0, nb, id_groups, id_items, f.bits); break;
-                    case KB200_BAYER_BGGR: launch_bayer_identity<OUT, T, KB200_BAYER_BGGR>(s, d, fr, p, dst, f0, nb, id_groups, id_items, f.bits); break;
-                    case KB200_BAYER_GRBG: launch_bayer_identity<OUT, T, KB200_BAYER_GRBG>(s, d, fr, p, dst, f0, nb, id_groups, id_items, f.bits); break;
-                    default: launch_bayer_identity<OUT, T, KB200_BAYER_GBRG>(s, d, fr, p, dst, f0, nb, id_groups, id_items, f.bits); break;
+                    case KB200_BAYER_RGGB: launch_bayer_identity<OUT, T, KB200_BAYER_RGGB>(s, d, fr, dst, f0, nb, id_groups, id_items, f.bits); break;
+                    case KB200_BAYER_BGGR: launch_bayer_identity<OUT, T, KB200_BAYER_BGGR>(s, d, fr, dst, f0, nb, id_groups, id_items, f.bits); break;
+                    case KB200_BAYER_GRBG: launch_bayer_identity<OUT, T, KB200_BAYER_GRBG>(s, d, fr, dst, f0, nb, id_groups, id_items, f.bits); break;
+                    default: launch_bayer_identity<OUT, T, KB200_BAYER_GBRG>(s, d, fr, dst, f0, nb, id_groups, id_items, f.bits); break;
                 }
             };
             if (!f.packed && f.words) launch(uint16_t{});
@@ -569,14 +560,16 @@ static int launch_preprocess(cudaStream_t s, const kb200_preprocess_desc& d, int
         }
         if (identity || yuv420_fast) {
             with_yuv_layout(f, yc, yc16, [&](auto l, auto t, const auto& c) {
-                launch_yuv_fast<OUT, decltype(l)::value, decltype(t)>(s, identity, bil, d, c, fr, p, nv, dst, f0, nb, id_groups, id_items);
+                launch_yuv_fast<OUT, decltype(l)::value, decltype(t)>(s, identity, bil, d, c, fr, nv, dst, f0, nb, id_groups, id_items);
             });
             KB200_TRY(check_launch(identity ? f.identity_kernel : f.fast_kernel));
             continue;
         }
         dim3 grid(div_up(pixels, 256), nb);
-        if (p) launch_generic_for<OUT, true>(s, grid, d, f, yc, yc16, fr, dst, f0);
-        else launch_generic_for<OUT, false>(s, grid, d, f, yc, yc16, fr, dst, f0);
+        // The packed-Bayer generic kernel reading base + i * stride compiles shorter than the one reading the table (its
+        // tap addresses in 64-bit adds, not IMAD.WIDE) and runs about 1.5 % faster on a strided batch, so it is kept
+        if (f.packed && !frames) launch_generic<OUT, TAP_BAYER_PACKED, true>(s, grid, d, f, yc, fr, dst, f0);
+        else launch_generic_for<OUT>(s, grid, d, f, yc, yc16, fr, dst, f0);
         KB200_TRY(check_launch("preprocess_generic_kernel"));
     }
     return KB200_OK;

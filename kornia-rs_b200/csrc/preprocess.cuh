@@ -16,10 +16,13 @@
 
 namespace kb200 {
 
+// The frames of one batch launch, by value in the kernel parameter block.  A strided call's frames are written into the
+// table by the host (base + i * stride), so every batch kernel reads its frame from ptr[], except the packed-Bayer
+// generic kernel of a strided call, which reads base and stride (see launch_preprocess).
 struct PreFrames {
-    const uint8_t* base;  // strided mode
+    const uint8_t* base;
     size_t stride;
-    const uint8_t* ptr[256];  // pointer-table mode
+    const uint8_t* ptr[256];
 };
 
 // preprocess.rs:461-484 — manual RNE f32 -> binary16 (kept bit-identical, including its rule that
