@@ -1,6 +1,7 @@
 """The benchmarks under tools/: no tool imports another (shared code lives in tools/benchkit.py), every tool with a
-command line starts without a GPU, and benchkit's shared arithmetic gives the numbers each tool computed on its own
-before it was shared (literals taken from those functions on the inputs below)."""
+command line starts without a GPU, benchkit's shared arithmetic gives the numbers each tool computed on its own before
+it was shared (literals taken from those functions on the inputs below), and format_bench's table names real formats
+and decoders and counts the algorithmic bytes the per-format scripts it replaced wrote."""
 import ast
 import glob
 import os
@@ -50,6 +51,17 @@ def test_tool_help_without_gpu(script):
     r = subprocess.run([sys.executable, os.path.join(TOOLS, script), "--help"], capture_output=True, text=True, env=env, timeout=300)
     assert r.returncode == 0, r.stderr
     assert "--out" in r.stdout
+
+
+@pytest.mark.parametrize("name", ["yuv", "yuv_matrix", "yuv16", "yuv444", "bayer", "bayer16", "bayer_packed", "bf16"])
+def test_format_bench_set_without_gpu(name, tmp_path):
+    """Each set the per-format scripts ran is a --set of format_bench.py, which refuses to run it without a GPU and writes
+    nothing."""
+    env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
+    r = subprocess.run([sys.executable, os.path.join(TOOLS, "format_bench.py"), "--out", str(tmp_path), "--set", name],
+                       capture_output=True, text=True, env=env, timeout=300)
+    assert r.returncode == 1 and "needs a CUDA device" in r.stderr, r.stderr
+    assert not os.listdir(tmp_path)
 
 
 def np_inverse(fwd):
@@ -128,3 +140,97 @@ def test_share_of_peak_rounding():
     for nbytes, ms in zip(rng.integers(1, 10**11, 2000), rng.uniform(0.01, 100.0, 2000)):
         nbytes = int(nbytes)
         assert round(nbytes / (ms * 1e-3) / (benchkit.PEAK_GBS * 1e9), 3) == round(nbytes / (ms * 1e-3) / 3.35e12, 3)
+
+
+def test_format_bench_arms():
+    import format_bench as fb
+    import kornia_rs_b200 as kb
+
+    for name, s in fb.SETS.items():
+        for section in (s.decode, s.pre, (("", s.e2e),)):
+            for _, arms in section:
+                for a in arms:
+                    assert a.fmt in kb.SourceFormat.__members__, (name, a.label, a.fmt)
+                    assert a.matrix is None or a.matrix in kb.YuvMatrix.__members__, (name, a.label, a.matrix)
+        for _, arms in s.decode:
+            for a in arms:
+                assert callable(getattr(kb.imgproc, fb.decoder(fb.FMT[a.fmt]), None)), (name, a.label)
+
+
+MATRICES = ("Bt601Limited", "Bt601Full", "Bt709Limited", "Bt709Full")
+# the algorithmic bytes the eight per-format scripts this tool replaced wrote at 1080p, from results/h100_*_bench.jsonl
+ALG_BYTES = {
+    "yuv": {
+        "yuv420_1080p_x256": {"Nv12": 2388787200, "Nv21": 2388787200, "I420": 2388787200, "Yv12": 2388787200},
+        "yuv422_1080p_x256": {"Yuyv": 2654208000, "Uyvy": 2654208000, "Yvyu": 2654208000},
+        "cfg3a_yuv420": {"Nv12": 7166361600, "I420": 7166361600, "Nv21": 7166361600, "Yv12": 7166361600},
+        "cfg3b_yuv420": {"Nv12": 1759641600, "I420": 1759641600, "Nv21": 1759641600, "Yv12": 1759641600},
+        "cfg3a_yuv422": {"Yuyv": 7431782400, "Uyvy": 7431782400},
+        "cfg3b_yuv422": {"Yuyv": 1848115200, "Uyvy": 1848115200},
+    },
+    "yuv_matrix": {   # its line records no alg_bytes: n * (frame + 3 * w * h), n * (src + out bytes * dw * dh), 3b src = 1958400
+        "nv12_1080p_x256": dict.fromkeys(MATRICES, 256 * (1920 * 1080 * 3 // 2 + 3 * 1920 * 1080)),
+        "yuyv_1080p_x256": dict.fromkeys(MATRICES, 256 * (1920 * 1080 * 2 + 3 * 1920 * 1080)),
+        "cfg3a_f32": dict.fromkeys(MATRICES, 256 * (1920 * 1080 * 3 // 2 + 12 * 1920 * 1080)),
+        "cfg3a_f16": dict.fromkeys(MATRICES, 256 * (1920 * 1080 * 3 // 2 + 6 * 1920 * 1080)),
+        "cfg3b_f32": dict.fromkeys(MATRICES, 256 * (1958400 + 12 * 640 * 640)),
+        "cfg3b_f16": dict.fromkeys(MATRICES, 256 * (1958400 + 6 * 640 * 640)),
+    },
+    "yuv16": {
+        "1080p_x256": {"P010": 4777574400, "P012": 4777574400, "I010": 4777574400, "I012": 4777574400, "Nv12": 2388787200, "Bayer12": 4246732800},
+        "cfg3a_f32": {"P010": 7962624000, "P012": 7962624000, "I010": 7962624000, "I012": 7962624000, "Nv12": 7166361600, "Bayer12": 7431782400, "Bayer12_zeros": 7431782400},
+        "cfg3a_f16": {"P010": 4777574400, "P012": 4777574400, "I010": 4777574400, "I012": 4777574400, "Nv12": 3981312000, "Bayer12": 4246732800, "Bayer12_zeros": 4246732800},
+        "cfg3b_f32": {"P010": 2260992000, "P012": 2260992000, "I010": 2260992000, "I012": 2260992000, "Nv12": 1759641600, "Bayer12": 2319974400, "P010_generic": 2260992000},
+        "cfg3b_f16": {"P010": 1631846400, "P012": 1631846400, "I010": 1631846400, "I012": 1631846400, "Nv12": 1130496000, "Bayer12": 1690828800, "P010_generic": 1631846400},
+    },
+    "yuv444": {
+        "1080p_x256": {"I444": 3185049600, "I410": 6370099200, "I410Msb": 6370099200, "Nv12": 2388787200, "P010": 4777574400},
+        "cfg3a_f32": {"I444": 7962624000, "I410": 9555148800, "I410Msb": 9555148800, "Nv12": 7166361600, "P010": 7962624000},
+        "cfg3a_f16": {"I444": 4777574400, "I410": 6370099200, "I410Msb": 6370099200, "Nv12": 3981312000, "P010": 4777574400},
+        "cfg3b_f32": {"I444": 1966080000, "I410": 2673868800, "I410Msb": 2673868800, "Nv12": 1759641600, "P010": 2260992000, "I444_generic": 1966080000},
+        "cfg3b_f16": {"I444": 1336934400, "I410": 2044723200, "I410Msb": 2044723200, "Nv12": 1130496000, "P010": 1631846400, "I444_generic": 1336934400},
+    },
+    "bayer": {
+        "1080p_x256": {"Nv12": 2388787200, "RGGB": 2123366400, "BGGR": 2123366400, "GRBG": 2123366400, "GBRG": 2123366400},
+        "cfg3a": {"Nv12": 7166361600, "RGGB": 6900940800, "BGGR": 6900940800, "GRBG": 6900940800, "GBRG": 6900940800},
+        "cfg3b": {"Nv12": 1759641600, "RGGB": 1789132800, "BGGR": 1789132800, "GRBG": 1789132800, "GBRG": 1789132800},
+    },
+    "bayer16": {
+        "1080p_x256": {"Bayer12": 4246732800, "Bayer8": 2123366400, "Nv12": 2388787200},
+        "cfg3a_f32": {"Bayer12": 7431782400, "Bayer8": 6900940800, "Nv12": 7166361600},
+        "cfg3a_f16": {"Bayer12": 4246732800, "Bayer8": 3715891200, "Nv12": 3981312000},
+        "cfg3b_f32": {"Bayer12": 2319974400, "Bayer8": 1789132800, "Nv12": 1759641600},
+        "cfg3b_f16": {"Bayer12": 1690828800, "Bayer8": 1159987200, "Nv12": 1130496000},
+    },
+    "bayer_packed": {
+        "1080p_x256": {"Raw10p": 3848601600, "Raw12p": 3981312000, "Raw14p": 4114022400, "Bayer12": 4246732800, "Raw12p_generic": 3981312000},
+        "cfg3a_f32": {"Raw10p": 7033651200, "Raw12p": 7166361600, "Raw14p": 7299072000, "Bayer12": 7431782400, "Raw12p_generic": 7166361600},
+        "cfg3a_f16": {"Raw10p": 3848601600, "Raw12p": 3981312000, "Raw14p": 4114022400, "Bayer12": 4246732800, "Raw12p_generic": 3981312000},
+        "cfg3b_f32": {"Raw10p": 1921843200, "Raw12p": 2054553600, "Raw14p": 2187264000, "Bayer12": 2319974400},
+        "cfg3b_f16": {"Raw10p": 1292697600, "Raw12p": 1425408000, "Raw14p": 1558118400, "Bayer12": 1690828800},
+    },
+    "bf16": {
+        "Nv12_cfg3a": {"f32": 7166361600, "f16": 3981312000, "bf16": 3981312000},
+        "Nv12_cfg3b": {"f32": 1759641600, "f16": 1130496000, "bf16": 1130496000},
+        "P010_cfg3a": {"f32": 7962624000, "f16": 4777574400, "bf16": 4777574400},
+        "P010_cfg3b": {"f32": 2260992000, "f16": 1631846400, "bf16": 1631846400},
+        "BayerRggb12_cfg3a": {"f32": 7431782400, "f16": 4246732800, "bf16": 4246732800},
+        "BayerRggb12_cfg3b": {"f32": 1730150400, "f16": 1101004800, "bf16": 1101004800},
+        "I444_cfg3a": {"f32": 7962624000, "f16": 4777574400, "bf16": 4777574400},
+        "I444_cfg3b": {"f32": 1966080000, "f16": 1336934400, "bf16": 1336934400},
+        "Yuyv_cfg3a": {"f32": 7431782400, "f16": 4246732800, "bf16": 4246732800},
+        "Yuyv_cfg3b": {"f32": 1730150400, "f16": 1101004800, "bf16": 1101004800},
+        "Nv12_cfg3b_lanczos": {"f32": 2054553600, "f16": 1425408000, "bf16": 1425408000},
+    },
+}
+
+
+@pytest.mark.parametrize("name", sorted(ALG_BYTES))
+def test_format_bench_alg_bytes(name):
+    import format_bench as fb
+
+    s = fb.SETS[name]
+    got = {key: {a.label: fb.decode_bytes(a, w, h, n) for a in arms} for key, w, h, n, arms in fb.decode_sections(s) if w == 1920}
+    for group, arms in s.pre:
+        got.update({key: {a.label: fb.pre_bytes(a, cfg, out) for a in arms_c} for key, cfg, out, arms_c in fb.pre_sections(s, group, arms)})
+    assert got == ALG_BYTES[name]

@@ -82,17 +82,17 @@ def write_line(out_dir: str, name: str, line: dict) -> None:
     print(json.dumps(line))
 
 
-def time_arms(bench, fns, iters, warmup, reps, stream, kb):
+def time_arms(bench, fns, iters, warmup, reps, stream, kb, probe=None):
     """{arm: fn}, the arms alternating, the set repeated `reps` times; each arm's turn is bench.time_launches (`warmup`
     calls, a synchronise, CUDA events around `iters` calls, a synchronise).  Returns ({arm: [ms per call, one per rep]},
-    {arm: the kernel its last call launched})."""
+    {arm: probe(arm) after its last turn}); the default probe is the kernel the arm's last call launched."""
     times = {k: [] for k in fns}
-    kernels = {}
+    probed = {}
     for _ in range(reps):
         for k, fn in fns.items():
             times[k].append(bench.time_launches(fn, iters, warmup, stream))
-            kernels[k] = kb._lib.last_kernel()
-    return times, kernels
+            probed[k] = probe(k) if probe else kb._lib.last_kernel()
+    return times, probed
 
 
 def time_alternating(arms, iters, repeats):
@@ -141,6 +141,14 @@ def e2e_result(steps, transfer, matches=None, pixels=None):
     if matches is not None:
         r["matches_device_result"] = matches
     return r
+
+
+def words(t, shift):
+    """Samples as 16-bit words, each shifted left by `shift` bits: a P01x / I41xMsb code in the high bits, an I01x / I41x
+    code in the low ones."""
+    import torch
+
+    return (t.to(torch.int32) << shift).to(torch.uint16)
 
 
 # ── the region benchmarks (preprocess_roi / _warp / _remap_bench) ──
